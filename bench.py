@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- RNN-T loss+grad throughput on B200 (BASELINE.json metric), one JSON line on stdout.
+"""bench.py -- RNN-T loss+grad throughput on H100 (BASELINE.json metric), one JSON line on stdout.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c2|c3|c4|c5mb]
+                    [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch of synthetic input: loss + dense gradient
 w.r.t. log_probs for all lattices of the batch (what the reference's forward call produces,
@@ -9,21 +10,28 @@ pytorch_binding/benchmark.py:36-43), log_softmax excluded.
 
   value      lattices/s, inputs resident in HBM, CUDA events over exactly K steps, max over ranks.
              Buffers rotate over R input sets and R live outputs so that consecutive steps never
-             touch the same lines (aggregate footprint >> 126 MB L2).
+             touch the same lines (aggregate footprint >> the H100's 50 MB L2).
   e2e        same metric through the public Python API (warp_rnnt_b200.rnnt_loss + backward) with
              HOST (pinned) inputs: H2D copy of the step's inputs and a D2H read of the loss inside
              the timed region.
   roofline   algorithmic bytes per launch (SURVEY.md 8d: 4*N*T*U*V grad write + 8*N*T*U log-prob
-             reads + 4*N*(U-1) + 12*N) / measured step time, against MEASURED_PEAKS.json hbm_gbs.
+             reads + 4*N*(U-1) + 12*N) / measured step time, against MEASURED_PEAKS.json hbm_gbs when present,
+             else the H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s).
   cpu_baseline  the CPU oracle port (oracle/rnnt_oracle.c, f32 flavour, OpenMP over lattices) timed on
              this box's host cores on a bounded sample of the same workload (rank 0, N=1 only).
 
 Multi-GPU (launched by torchrun): every rank runs the same per-GPU workload on its own shard
 (weak scaling, no data-path collective) and the scalar loss is all-reduced over NCCL each step.
 
---impl reference: the UNMODIFIED reference kernels (oracle/_ref/warp_rnnt_ref_C.so, built from
-/root/reference by oracle/build_ref.py) through the reference's own operator API on the GPU, same
+--impl reference: the UNMODIFIED reference kernels (oracle/_ref/warp_rnnt_ref_C.so, built from the
+reference's sources by oracle/build_ref.py) through the reference's own operator API on the GPU, same
 harness; falls back to the CPU oracle port when that extension or a GPU is not available.
+
+--dump-outputs DIR: after the timed steps, write what the last timed step returned to its caller -- the loss
+(loss.npy) and the gradient w.r.t. the step's input (grad.npy, or above 48 MB a fixed, seeded sample of whole
+lattice rows, grad_rows_sample.npy, with their row numbers in grad_rows_sample_index.npy) -- as float32 .npy
+files (with --impl reference: the reference's outputs, on the GPU only).  The inputs depend only on the arguments,
+so two builds can be compared output for output.
 """
 import argparse
 import contextlib
@@ -87,7 +95,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 def make_host_inputs(N, T, U, V, seed, ragged=False, compact=False, dtype=None):
@@ -192,6 +200,20 @@ def cpu_oracle_rate(N, T, U, V, budget_s=8.0, threads=None):
             "numpy_ref_transduce_ms_per_lattice": np_ms, "host_cpus": os.cpu_count()}
 
 
+def dump_outputs(out_dir, loss, grad, budget=48 << 20):
+    """The loss and the gradient one step returned, as float32 .npy files (see the module docstring)."""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().cpu().numpy())
+    g = grad.detach().reshape(-1, grad.shape[-1])
+    if g.numel() * 4 <= budget:
+        np.save(os.path.join(out_dir, "grad.npy"), g.float().cpu().numpy().reshape(tuple(grad.shape)))
+        return
+    k = budget // (4 * g.shape[1])
+    idx = np.sort(np.random.RandomState(0).choice(g.shape[0], k, replace=False))
+    np.save(os.path.join(out_dir, "grad_rows_sample.npy"), g[torch.from_numpy(idx).to(g.device)].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "grad_rows_sample_index.npy"), idx.astype(np.float64))
+
+
 def config_dict(workload, desc, N, T, U, V, world, R, footprint_mb):
     """Identical for both arms (the driver compares the dicts)."""
     return {"workload": "%s: %s" % (workload, desc), "lattices_per_gpu": N, "T": T, "U": U, "V": V,
@@ -239,6 +261,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true", help="time the eager python API instead of CUDA-graph replays")
     ap.add_argument("--no-c5", action="store_true", help="skip the cfg-5 block of multi-GPU runs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the loss and gradient of the last timed step to DIR as .npy files")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -339,14 +363,19 @@ def main():
             graphs, graph_note = None, "eager python API (graph capture failed: %s)" % (str(e).splitlines()[0][:120])
             torch.cuda.synchronize()
 
+    last = {}                                             # loss and input set of the latest step
+
     if graphs is not None:
         def step(i):
             g, loss, _ = graphs[i % R]
             g.replay()
             reduce_async(loss)
+            last.update(loss=loss, set=i % R)
     else:
         def step(i):
-            reduce_async(api_step(sets[i % R]))
+            loss = api_step(sets[i % R])
+            reduce_async(loss)
+            last.update(loss=loss, set=i % R)
 
     for i in range(args.warmup):
         step(i)
@@ -356,6 +385,8 @@ def main():
     launches = (launches_per_step * args.steps) if graphs is not None else int(w._C.launch_count() - n0)
     ms_per_step = ms / args.steps
     value = N * world * args.steps / (ms * 1e-3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["loss"], sets[last["set"]][0].grad)
 
     # ---- extra information (N=1): eager API, operator-level call, the opt-in short LSE chain
     extra = {}
@@ -459,20 +490,7 @@ def main():
                "compact": "k_prefix + k_gather + k_wavefront + k_grads_pairs + k_expand<2>",
                "bf16": "k_fused<exact,dense,bf16>" if args.workload == "c2b" else "k_gather<bf16> + k_wavefront + k_expand<0,bf16>",
                "logits": "k_lse_pairs + k_fused<exact,pairs> + k_expand_logits"}[mode]
-    # dram__bytes_read + dram__bytes_write of the dominant kernel: from the committed ncu --set full capture of the same
-    # workload (profiles/), labelled as such -- it is NOT measured in this run
-    traffic, traffic_note = None, "not measured in this run; ncu dram__bytes per launch are in profiles/"
-    key = {"c2": "c2", "c4d": "c4"}.get(args.workload)
-    summ = os.path.join(ROOT, "profiles", "r2_summary.json")
-    if key and world == 1 and os.path.exists(summ):
-        try:
-            ent = json.load(open(summ)).get(key)
-            if ent:
-                traffic = ent["dram_bytes_per_launch"]
-                traffic_note = ("from the committed ncu --set full capture of this workload (profiles/r2_summary.json, kernel %s), "
-                                "not measured in this run" % ent.get("kernel", "?")[:60])
-        except Exception:
-            pass
+    traffic, traffic_note = None, "not measured (DRAM byte counters need a profiler)"
     out = {
         "metric": "RNN-T loss+grad lattices/sec", "value": value, "unit": "lattices/s",
         "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_per_step,
@@ -520,7 +538,7 @@ def finish(world, dist):
 
 def run_c5(w, parallel, dist, dev, world, rank, steps=4, warm=2):
     """N=2048 T=600 U=150 V=1024 over 8 GPUs = 256 lattices per GPU; log_probs + gradient of one GPU's share are
-    2 x 94 GB > 180 GB, so each rank runs 8 micro-batches of 32 (the joint network upstream would be micro-batched the
+    2 x 94 GB > 80 GB, so each rank runs 8 micro-batches of 32 (the joint network upstream would be micro-batched the
     same way) and the step ends with ONE all-reduce of the scalar loss.  Synthetic log-probs are made on the device;
     one 11.8 GB input buffer serves all micro-batches (far larger than L2)."""
     N, T, U, V, MB = 32, 600, 150, 1024, 8
@@ -610,6 +628,8 @@ def run_reference(args, rank, world, N, T, U, V, mode, ragged, desc, have_cuda):
             ref = build_ref.load()
         except Exception:
             ref = None
+    if args.dump_outputs and ref is None:
+        raise SystemExit("bench.py: --dump-outputs with --impl reference needs a GPU and oracle/_ref/warp_rnnt_ref_C.so")
     cpu = None if args.no_cpu_baseline and ref is not None else cpu_oracle_rate(N, T, U, V)
     per_set = 2 * 4 * N * T * U * V
     R = rotation(per_set)
@@ -649,7 +669,13 @@ def run_reference(args, rank, world, N, T, U, V, mode, ragged, desc, have_cuda):
         api_step(sets[i % R])
     for i in range(args.warmup):
         api_step(sets[i % R])
-    ms = timed(lambda i: api_step(sets[(args.warmup + i) % R]), steps, 1, None, dev)
+    last = {}
+
+    def ref_step(i):
+        last.update(loss=api_step(sets[(args.warmup + i) % R]), set=(args.warmup + i) % R)
+    ms = timed(ref_step, steps, 1, None, dev)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, last["loss"], sets[last["set"]][0].grad)
     ke = args.e2e_steps or min(steps, 20)
 
     def e2e_step(i):
@@ -681,7 +707,7 @@ def run_reference(args, rank, world, N, T, U, V, mode, ragged, desc, have_cuda):
                  "e2e": {"value": N * ke / e2e_s, "unit": "lattices/s", "h2d_bytes_per_step": hb,
                          "d2h_bytes_per_step": 4, "steps": ke, "ms_per_step": e2e_s / ke * 1e3},
                  "gpu_launches": None, "clocks": sampler.stop(),
-                 "reference_kind": "unmodified reference kernels (oracle/_ref/warp_rnnt_ref_C.so) on the same B200"})
+                 "reference_kind": "unmodified reference kernels (oracle/_ref/warp_rnnt_ref_C.so) on the same GPU"})
     print(json.dumps(base), flush=True)
 
 

@@ -1,17 +1,18 @@
-"""Build the UNMODIFIED reference (1ytic/warp-rnnt) for sm_100a into oracle/_ref/ -- checker only.
+"""Build the UNMODIFIED reference (1ytic/warp-rnnt) for sm_90a into oracle/_ref/ -- checker only.
 
-    python oracle/build_ref.py
+    python oracle/build_ref.py        # RNNT_REFERENCE_DIR=<checkout of 1ytic/warp-rnnt> overrides the default
 
-Compiles the reference's own sources where they lie under /root/reference (core.cu,
+Compiles the reference's own sources in $RNNT_REFERENCE_DIR, default /root/reference (core.cu,
 core_gather.cu, core_compact.cu, pytorch_binding/binding.cpp) with nvcc / g++ directly; nothing
 is copied into this repository and the reference's setup.py (which refuses to run without a
 visible GPU, setup.py:21-22) is not used.  Output: oracle/_ref/warp_rnnt_ref_C.so, a torch
 extension exposing the reference's `_C` API (rnnt_loss / rnnt_loss_compact /
-rnnt_loss_compact_backward).  oracle/_ref/ is git-ignored but travels to the GPU box with gpurun,
-where /root/reference does not exist.
+rnnt_loss_compact_backward).  oracle/_ref/ is git-ignored; without a reference checkout nothing is built and a
+prebuilt oracle/_ref/ is used if there is one.
 
-TEST INFRASTRUCTURE ONLY: used by tests/ (parity against the real reference on the GPU) and by
-bench.py --impl reference.  The product never loads it.
+TEST INFRASTRUCTURE ONLY: used by tests/golden/make_reference_outputs.py (which records the reference's outputs
+that the GPU tests compare with), by tests/test_gpu_parity.py (the reference's binding.cpp on our C ABI, when
+present) and by bench.py --impl reference.  The product never loads it.
 """
 import os
 import subprocess
@@ -27,7 +28,7 @@ NAME = "warp_rnnt_ref_C"
 
 def build(force=False):
     if not os.path.isdir(REF):
-        return None                      # GPU box: use the prebuilt file if it travelled
+        return None                      # no reference checkout: use a prebuilt file if there is one
     if os.path.exists(OUT) and not force:
         return OUT
     os.makedirs(OUT_DIR, exist_ok=True)
@@ -36,7 +37,7 @@ def build(force=False):
     objs = []
     for cu in ("core.cu", "core_gather.cu", "core_compact.cu"):
         o = os.path.join(OUT_DIR, cu.replace(".cu", ".o"))
-        subprocess.check_call(["nvcc", "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a",
+        subprocess.check_call(["nvcc", "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a",
                                "-Xcompiler", "-fPIC", "-I" + REF, "-c", os.path.join(REF, cu), "-o", o])
         objs.append(o)
     cmd = ["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-w",

@@ -4,7 +4,7 @@ TEST INFRASTRUCTURE ONLY -- this is the checker, never the product.  Only tests/
 __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs import it.
 The product package (warp_rnnt_b200) never imports anything from oracle/.
 
-Reference citations (/root/reference/...): core.cu:41-370 (alpha, beta, grads, costs),
+Reference citations (the reference's files): core.cu:41-370 (alpha, beta, grads, costs),
 core_gather.cu (V=2 form), core_compact.cu:29-484 (ragged form), pytorch_binding/warp_rnnt/
 __init__.py:57-143 (python-level gather / average_frames / reduction).
 """

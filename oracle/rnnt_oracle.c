@@ -4,7 +4,7 @@
  * Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may
  * load it.  The product path (warp_rnnt_b200) never links or calls anything in oracle/.
  *
- * What it restates (all citations are /root/reference/<file>:<line>):
+ * What it restates (all citations are the reference's <file>:<line>):
  *   alpha recurrence      core.cu:41-141   (row 0 :80-90, column 0 :92-110, interior :112-134)
  *   beta recurrence       core.cu:143-246  (corner :171-173, last row :185-195, last col :197-215,
  *                                           interior :217-239)
@@ -20,7 +20,7 @@
  * The reference has no CPU implementation; the per-sample double loop is the awni
  * ref_transduce.py style the reference README names as the algorithm's origin (README.md:6,11).
  * Pinned against the golden vectors of pytorch_binding/warp_rnnt/test.py (tests/golden/) and,
- * on the GPU box, against the compiled unmodified reference (oracle/_ref).
+ * on the GPU, against the recorded outputs of the compiled unmodified reference (tests/golden/).
  *
  * Two arithmetic flavours are generated from one body: f64 (truth) and f32 (same operation
  * order as the reference kernels, CPU libm expf/log1pf -- close to, not bit-equal with, CUDA's).

@@ -1,4 +1,6 @@
-"""Shared helpers for the tests: golden vectors, synthetic inputs (the reference's recipe)."""
+"""Shared helpers for the tests: golden vectors, stored outputs of the reference, synthetic inputs (the reference's
+recipe)."""
+import hashlib
 import json
 import os
 
@@ -6,6 +8,59 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLDEN = json.load(open(os.path.join(HERE, "golden", "reference_vectors.json")))
+REF_OUTPUTS = os.path.join(HERE, "golden", "reference_outputs.npz")
+_ref_out = None
+
+# Outputs of the unmodified reference kernels (1ytic/warp-rnnt built for sm_90a) on the inputs of the tests below,
+# recorded on an H100 by tests/golden/make_reference_outputs.py.  A tensor of at most FULL_MAX elements is stored
+# whole; a larger one as the SHA-256 of its bytes plus its values at SAMPLE seeded positions (mostly non-zero ones),
+# which name the first differing elements when the digest does not match.
+FULL_MAX = 4096
+SAMPLE = 64
+
+
+def _host(t):
+    a = t.detach().cpu().numpy() if hasattr(t, "detach") else np.asarray(t)
+    return np.ascontiguousarray(a)
+
+
+def digest(t):
+    return hashlib.sha256(_host(t).tobytes()).hexdigest()
+
+
+def record(rec, key, t):
+    """Store tensor `t` under `key` in the dict `rec` (the writer side of same_as_reference)."""
+    a = _host(t)
+    if a.size <= FULL_MAX:
+        rec[key] = a
+        return
+    flat = a.reshape(-1)
+    nz = np.flatnonzero(flat)
+    rng = np.random.RandomState(a.size % (2 ** 31))
+    pick = np.concatenate([rng.choice(nz, min(SAMPLE - 8, nz.size), replace=False) if nz.size else nz,
+                           rng.randint(0, flat.size, 8)]).astype(np.int64)
+    rec[key + ".idx"] = pick
+    rec[key + ".val"] = flat[pick]
+    rec[key + ".shape"] = np.asarray(a.shape, dtype=np.int64)
+    rec[key + ".sha256"] = np.asarray(digest(a))
+
+
+def same_as_reference(key, t):
+    """Assert that `t` equals the reference's stored output `key` bit for bit."""
+    global _ref_out
+    if _ref_out is None:
+        _ref_out = dict(np.load(REF_OUTPUTS))
+    a = _host(t)
+    if key in _ref_out:
+        r = _ref_out[key]
+        assert a.shape == r.shape and a.dtype == r.dtype, (key, a.shape, a.dtype, r.shape, r.dtype)
+        np.testing.assert_array_equal(a, r, err_msg=key)
+        assert a.tobytes() == r.tobytes(), "%s differs from the reference (signed zeros)" % key
+        return
+    assert tuple(a.shape) == tuple(_ref_out[key + ".shape"]), (key, a.shape)
+    idx, val = _ref_out[key + ".idx"], _ref_out[key + ".val"]
+    np.testing.assert_array_equal(a.reshape(-1)[idx], val, err_msg=key)
+    assert digest(a) == str(_ref_out[key + ".sha256"]), "%s differs from the reference" % key
 
 
 def log_softmax(x, axis=-1):
@@ -69,3 +124,10 @@ def from_compact(flat, xn, yn, T, U):
         out[i, :xn[i], :yn[i] + 1] = flat[o:o + c].reshape(xn[i], yn[i] + 1, V)
         o += c
     return out
+
+
+def input_sample(xs, k=32):
+    """Fingerprint of a (device-synthesised) input tensor: its values at k fixed positions."""
+    import torch
+    idx = torch.from_numpy(np.random.RandomState(12345).randint(0, xs.numel(), k)).to(xs.device)
+    return xs.reshape(-1)[idx]

@@ -1,13 +1,13 @@
 """Extract the known-answer vectors of the reference's own tests into reference_vectors.json.
 
-Run in the build container (needs /root/reference, which the GPU box does not have):
+Run with a checkout of the reference (1ytic/warp-rnnt):
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py REFERENCE_DIR
 
-Source: /root/reference/pytorch_binding/warp_rnnt/test.py (test_one_to_many :34-62,
+Source: the reference's pytorch_binding/warp_rnnt/test.py (test_one_to_many :34-62,
 test_one_to_empty :64-85, test_forward_single :87-121, test_forward_batch :123-188,
 test_forward_single_gather :214-257, test_forward_batch_compact :259-336) and
-/root/reference/tensorflow_binding/warp_rnnt_tf/test.py (test_forward_single_inner_gather :227-252).
+the reference's tensorflow_binding/warp_rnnt_tf/test.py (test_forward_single_inner_gather :227-252).
 
 Only literal data (logits, labels, lengths, expected costs / gradients) is read, via the AST --
 no reference code is executed or copied.  Logits are stored raw; the tests apply log_softmax
@@ -16,9 +16,10 @@ exactly as the reference tests do (test.py:42, 68, 98, 147, 225, 283).
 import ast
 import json
 import os
+import sys
 
-REF_PT = "/root/reference/pytorch_binding/warp_rnnt/test.py"
-REF_TF = "/root/reference/tensorflow_binding/warp_rnnt_tf/test.py"
+REF_PT = "pytorch_binding/warp_rnnt/test.py"
+REF_TF = "tensorflow_binding/warp_rnnt_tf/test.py"
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "reference_vectors.json")
 
 WANTED = {"xs", "ys", "xn", "yn", "expected_cost", "expected_costs", "expected_grads"}
@@ -38,8 +39,8 @@ def _literal(node):
     return None
 
 
-def extract(path, names):
-    tree = ast.parse(open(path).read())
+def extract(root, path, names):
+    tree = ast.parse(open(os.path.join(root, path)).read())
     out = {}
     for cls in [n for n in tree.body if isinstance(n, ast.ClassDef)]:
         for fn in [n for n in cls.body if isinstance(n, ast.FunctionDef)]:
@@ -59,11 +60,11 @@ def extract(path, names):
     return out
 
 
-def main():
-    vec = extract(REF_PT, {"test_one_to_many", "test_one_to_empty", "test_forward_single",
+def main(root):
+    vec = extract(root, REF_PT, {"test_one_to_many", "test_one_to_empty", "test_forward_single",
                            "test_forward_batch", "test_forward_single_gather",
                            "test_forward_batch_compact"})
-    tf = extract(REF_TF, {"test_forward_single_inner_gather"})
+    tf = extract(root, REF_TF, {"test_forward_single_inner_gather"})
     vec.update(tf)
     for k, r in vec.items():
         missing = {"xs", "ys", "xn", "yn", "expected_grads"} - set(r)
@@ -75,4 +76,4 @@ def main():
 
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1])

@@ -1,5 +1,6 @@
-"""GPU, BASELINE.json's full sizes: size-independent properties of the domain + the compiled
-reference where it finishes in seconds.
+"""GPU, BASELINE.json's full sizes: size-independent properties of the domain + what the compiled reference computes
+where it finishes in seconds (recorded on an H100 in tests/golden/reference_outputs.npz; the inputs are synthesised
+on the device, and their fingerprint is checked first).
 
 Properties (all follow from alpha/beta being a flow on the lattice, SURVEY.md section 0):
   * every anti-diagonal t+u = d < Tn+Un-2 carries total flow 1:  -sum_{t+u=d}(g_blank + g_label) == 1
@@ -14,6 +15,8 @@ import numpy as np
 import pytest
 import torch
 
+from tests.common import input_sample, same_as_reference
+
 pytestmark = pytest.mark.gpu
 
 
@@ -21,12 +24,6 @@ pytestmark = pytest.mark.gpu
 def w():
     import warp_rnnt_b200
     return warp_rnnt_b200
-
-
-@pytest.fixture(scope="module")
-def ref():
-    from oracle import build_ref
-    return build_ref.load()
 
 
 def synth(N, T, U, V, seed, random_lengths=False):
@@ -72,26 +69,27 @@ def check_properties(xs, ys, xn, yn, costs, grads, flow_tol):
     assert per[~live].abs().max().item() <= flow_tol if (~live).any() else True
 
 
-def test_cfg2_full(w, ref):
+def test_cfg2_full(w):
     xs, ys, xn, yn = synth(128, 150, 40, 28, seed=128)
+    same_as_reference("cfg2_full/xs_sample", input_sample(xs))
     w.set_lse_mode("fast")
     cf, gf = w._C.rnnt_loss(xs, ys, xn, yn)
     check_properties(xs, ys, xn, yn, cf, gf, flow_tol=2e-3)
     w.set_lse_mode("exact")
     ce, ge = w._C.rnnt_loss(xs, ys, xn, yn)
-    if ref is not None:
-        cr, gr = ref.rnnt_loss(xs, ys, xn, yn)
-        assert torch.equal(ce, cr) and torch.equal(ge, gr)          # bit-identical at full size
-        # the opt-in fast LSE: fp32 noise against the reference (measured 1.2e-4 on one of 21.5M
-        # gradient elements -- the reference itself is 1.25e-4 from the fp64 oracle at this shape).
-        # This is why the library default is the exact flavour.
-        assert ((cf - cr).abs() / cr.abs()).max().item() <= 1e-5
-        assert (gf - gr).abs().max().item() <= 2.5e-4
+    same_as_reference("cfg2_full/costs", ce)                       # bit-identical to the reference at full size
+    same_as_reference("cfg2_full/grads", ge)
+    # the opt-in fast LSE: fp32 noise against the reference (ce, ge) (up to ~1.2e-4 on single gradient elements --
+    # the reference itself is about as far from the fp64 oracle at this shape).  This is why the library default is
+    # the exact flavour.
+    assert ((cf - ce).abs() / ce.abs()).max().item() <= 1e-5
+    assert (gf - ge).abs().max().item() <= 2.5e-4
     w.set_lse_mode("auto")
 
 
-def test_cfg2_random_lengths_python_api(w, ref):
+def test_cfg2_random_lengths_python_api(w):
     xs, ys, xn, yn = synth(128, 150, 40, 28, seed=7, random_lengths=True)
+    same_as_reference("cfg2_rl/xs_sample", input_sample(xs))
     w.set_lse_mode("exact")
     x = xs.clone().requires_grad_(True)
     loss = w.rnnt_loss(x, ys, xn, yn, reduction="sum", gather=True)
@@ -99,25 +97,24 @@ def test_cfg2_random_lengths_python_api(w, ref):
     costs, grads = w._C.rnnt_loss(xs, ys, xn, yn)
     assert torch.equal(x.grad, grads)                              # deferred emit == eager emit, bit for bit
     check_properties(xs, ys, xn, yn, costs, grads, flow_tol=2e-3)
-    if ref is not None:
-        cr, gr = ref.rnnt_loss(xs, ys, xn, yn)
-        assert torch.equal(costs, cr) and torch.equal(grads, gr)
+    same_as_reference("cfg2_rl/costs", costs)
+    same_as_reference("cfg2_rl/grads", grads)
     w.set_lse_mode("auto")
 
 
-def test_cfg3_full(w, ref):
+def test_cfg3_full(w):
     xs, ys, xn, yn = synth(32, 150, 20, 5000, seed=32)
+    same_as_reference("cfg3_full/xs_sample", input_sample(xs))
     w.set_lse_mode("exact")
     ce, ge = w._C.rnnt_loss(xs, ys, xn, yn)
     check_properties(xs, ys, xn, yn, ce, ge, flow_tol=2e-3)
-    if ref is not None:
-        cr, gr = ref.rnnt_loss(xs, ys, xn, yn)
-        assert torch.equal(ce, cr) and torch.equal(ge, gr)
+    same_as_reference("cfg3_full/costs", ce)
+    same_as_reference("cfg3_full/grads", ge)
     w.set_lse_mode("auto")
 
 
 def test_cfg4_full_dense_and_compact(w):
-    """N=64 T=1500 U=300 V=50 (the reference needs 14 s per call on B200 here; properties instead)."""
+    """N=64 T=1500 U=300 V=50 (the reference needs many seconds per call here; properties instead)."""
     N, T, U, V = 64, 1500, 300, 50
     xs, ys, xn, yn = synth(N, T, U, V, seed=64, random_lengths=True)
     w.set_lse_mode("fast")
@@ -140,11 +137,12 @@ def test_cfg4_full_dense_and_compact(w):
     w.set_lse_mode("auto")
 
 
-def test_cfg5_microbatch_independence_and_64bit(w, ref):
+def test_cfg5_microbatch_independence_and_64bit(w):
     """N=32 T=600 U=150 V=1024: 2.9e9 gradient elements (> 2^31, the reference's int idx4 overflows
     beyond 23 lattices, core.cu:22-24).  A batch must equal its sub-batches bit for bit."""
     N, T, U, V = 32, 600, 150, 1024
     xs, ys, xn, yn = synth(N, T, U, V, seed=5, random_lengths=True)
+    same_as_reference("cfg5_last4/xs_sample", input_sample(xs))
     w.set_lse_mode("exact")
     costs, grads = w._C.rnnt_loss(xs, ys, xn, yn)
     for lo, hi in ((0, 16), (16, 32)):
@@ -152,9 +150,6 @@ def test_cfg5_microbatch_independence_and_64bit(w, ref):
                                 yn[lo:hi].contiguous())
         assert torch.equal(costs[lo:hi], c2) and torch.equal(grads[lo:hi], g2)
         del c2, g2
-    if ref is not None:
-        k = 4                                                          # the reference on the last 4 lattices
-        cr, gr = ref.rnnt_loss(xs[N - k:].contiguous(), ys[N - k:].contiguous(), xn[N - k:].contiguous(),
-                               yn[N - k:].contiguous())
-        assert torch.equal(costs[N - k:], cr) and torch.equal(grads[N - k:], gr)
+    same_as_reference("cfg5_last4/costs", costs[N - 4:])             # the reference on the last 4 lattices
+    same_as_reference("cfg5_last4/grads", grads[N - 4:])
     w.set_lse_mode("auto")

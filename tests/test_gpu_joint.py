@@ -1,5 +1,5 @@
 """GPU: compact packing of the joint network's input (SURVEY.md 8(f)3) against the reference's own recipe
-(/root/reference/pytorch_binding/benchmark2.py:37-50: a python loop over the batch + cat) and its autograd backward.
+(the reference's pytorch_binding/benchmark2.py:37-50: a python loop over the batch + cat) and its autograd backward.
 Forward is exact (one fp32 add per element); the backward sums in a fixed order, compared to 1e-5 relative."""
 import numpy as np
 import pytest

@@ -1,6 +1,6 @@
 """CPU, world_size 2 (gloo): the batch-sharding + scalar all-reduce host logic of
 warp_rnnt_b200.parallel.  The local loss is injected (an autograd wrapper around the fp64 oracle),
-so no GPU is needed; on the GPU box the same code path runs with the CUDA op over NCCL."""
+so no GPU is needed; on a GPU the same code path runs with the CUDA op over NCCL."""
 import os
 import socket
 

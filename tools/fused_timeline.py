@@ -14,7 +14,7 @@ import torch  # noqa: E402
 
 import warp_rnnt_b200 as w  # noqa: E402
 
-SHAPES = {"c2": (128, 150, 40, 28), "c2n32": (32, 150, 40, 28), "c2n148": (148, 150, 40, 28), "c3": (32, 150, 20, 5000), "c1": (1, 150, 40, 28)}
+SHAPES = {"c2": (128, 150, 40, 28), "c2n32": (32, 150, 40, 28), "c2n132": (132, 150, 40, 28), "c3": (32, 150, 20, 5000), "c1": (1, 150, 40, 28)}
 NAMES = ["start", "sentinels", "gather_done", "sweep_start", "alpha_done", "beta_done", "fill_issued", "end", "chase_done",
          "zeros_landed", "patch_start"]
 

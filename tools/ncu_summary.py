@@ -1,5 +1,5 @@
 """Summarise ncu captures (run here, no GPU needed):
-    python tools/ncu_summary.py <name> <rep.ncu-rep> [launch_list.csv]  ->  profiles/r2_<name>.md (+ r2_summary.json entry)
+    python tools/ncu_summary.py <name> <rep.ncu-rep> [launch_list.csv]  ->  profiles/ncu_<name>.md (+ ncu_summary.json entry)
 """
 import csv, io, json, os, subprocess, sys
 
@@ -91,8 +91,8 @@ def main():
             lines.append("| %s | %d | %.2f | %.1f%% |" % (kn, c, ns / c / 1e3, 100 * ns / tot))
         lines.append("")
     os.makedirs(os.path.join(ROOT, "profiles"), exist_ok=True)
-    open(os.path.join(ROOT, "profiles", "r2_%s.md" % name), "w").write("\n".join(lines))
-    sj = os.path.join(ROOT, "profiles", "r2_summary.json")
+    open(os.path.join(ROOT, "profiles", "ncu_%s.md" % name), "w").write("\n".join(lines))
+    sj = os.path.join(ROOT, "profiles", "ncu_summary.json")
     allj = json.load(open(sj)) if os.path.exists(sj) else {}
     allj[name.split("_")[-1] if name.split("_")[-1] in ("c2", "c3", "c4", "c5mb") else name] = summ
     json.dump(allj, open(sj, "w"), indent=1)

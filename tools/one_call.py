@@ -1,4 +1,4 @@
-"""Scratch: a few calls of one config for ncu."""
+"""Scratch: a few calls of one config (for a profiler run)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -49,10 +49,9 @@ for name, (N, T, U, V) in {"c2": (128, 150, 40, 28), "c3": (32, 150, 20, 5000), 
     r["ours_gather_fwd_us"] = time_fn(lambda s: w._C.rnnt_gather_forward(*s, 0, 0.0, True, 0), sets)
     if ref is not None and N * T * U * V < 2**31:
         r["ref_us"] = time_fn(lambda s: ref.rnnt_loss(*s), sets, iters=5, warm=2)
-    r["frac_fast"] = r["B_alg_MB"] * 1e6 / (r["ours_fast_us"] * 1e-6) / 6567.4e9
+    r["frac_fast"] = r["B_alg_MB"] * 1e6 / (r["ours_fast_us"] * 1e-6) / 3350e9   # H100 SXM data-sheet HBM3 bandwidth
     out[name] = r
     print(name, json.dumps(r), flush=True)
     del sets
     torch.cuda.empty_cache()
-os.makedirs("gpurun_out", exist_ok=True)
-json.dump(out, open("gpurun_out/quick_time.json", "w"), indent=1)
+print(json.dumps(out, indent=1))

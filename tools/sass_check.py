@@ -1,9 +1,9 @@
 """Scheduling lint for the fused kernel's recurrence loop (no GPU needed; needs cuobjdump).
 
-ptxas sometimes runs a lane's two exact-LSE chains one after the other instead of interleaved (160 vs 125 ns per
-anti-diagonal at cfg 2).  In a well-scheduled step the two MUFU.EX2 of the two chains are a few instructions apart;
-serialised, they are ~40 apart.  Prints the distances for every k_fused<exact, *, C=2> kernel and exits 1 if a loop
-step is serialised.
+ptxas sometimes runs a lane's two exact-LSE chains one after the other instead of interleaved, which lengthens the
+dependent chain of every anti-diagonal.  In a well-scheduled step the two MUFU.EX2 of the two chains are a few
+instructions apart; serialised, they are ~40 apart.  Prints the distances for every k_fused<exact, *, C=2> kernel and
+exits 1 if a loop step is serialised.
 
     python tools/sass_check.py [path/to/librnnt_b200.so]
 """

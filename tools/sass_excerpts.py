@@ -1,4 +1,4 @@
-"""Regenerate profiles/r2_sass_k_fused.txt from the built library (run here, no GPU needed):
+"""Write profiles/r<round>_sass_k_fused.txt from the built library (no GPU needed):
 
     python tools/sass_excerpts.py [round]
 
@@ -34,7 +34,7 @@ def main():
             if o == key or o.startswith(key + "."):
                 census[key] += 1
                 break
-    out = ["# SASS excerpts of rnnt::k_fused<exact, dense, C=2, float> (sm_100a), cuobjdump -sass of warp_rnnt_b200/lib/librnnt_b200.so",
+    out = ["# SASS excerpts of rnnt::k_fused<exact, dense, C=2, float> (sm_90a), cuobjdump -sass of warp_rnnt_b200/lib/librnnt_b200.so",
            "# (regenerate with tools/sass_excerpts.py)  %d instructions in the kernel.  Mnemonic census:" % len(lines),
            "#   " + ", ".join("%s %d" % kv for kv in census.items()), ""]
     out.append("## bulk-copy (TMA engine) sites: row gather (global->shared, mbarrier completion) and zero-fill (shared->global)")

@@ -1,5 +1,5 @@
-"""warp_rnnt_b200 -- B200-native RNN-Transducer loss, drop-in for 1ytic/warp-rnnt's
-``warp_rnnt.rnnt_loss`` (reference: /root/reference/pytorch_binding/warp_rnnt/__init__.py).
+"""warp_rnnt_b200 -- H100-native RNN-Transducer loss, drop-in for 1ytic/warp-rnnt's
+``warp_rnnt.rnnt_loss`` (reference: the reference's pytorch_binding/warp_rnnt/__init__.py).
 
 Same public surface as the reference module (``__init__.py:9-143``):
 
@@ -9,7 +9,7 @@ Same public surface as the reference module (``__init__.py:9-143``):
     (rnnt_loss / rnnt_loss_compact / rnnt_loss_compact_backward, same kwargs and error strings).
 
 Host code here is plumbing only (argument handling, autograd wiring); all arithmetic runs in the
-hand-written sm_100a kernels of ``lib/librnnt_b200.so`` through ``lib/_C.so``.  There is no CPU or
+hand-written sm_90a kernels of ``lib/librnnt_b200.so`` through ``lib/_C.so``.  There is no CPU or
 eager-PyTorch fallback: importing this package without the built extension raises ImportError.
 """
 import contextlib

@@ -3,10 +3,10 @@
     python -m warp_rnnt_b200.build            # both
     python -m warp_rnnt_b200.build --lib      # librnnt_b200.so only (no torch needed)
 
-Artifacts (git-ignored, shipped to the GPU box by gpurun):
-    warp_rnnt_b200/lib/librnnt_b200.so   nvcc -gencode arch=compute_100a,code=sm_100a  (C ABI)
+Artifacts (git-ignored):
+    warp_rnnt_b200/lib/librnnt_b200.so   nvcc -gencode arch=compute_90a,code=sm_90a  (C ABI)
     warp_rnnt_b200/lib/_C.so             g++ binding.cpp against torch + librnnt_b200.so
-sm_100a only: no other arch, no PTX fallback, no CPU path.
+sm_90a (H100) only: no other arch, no PTX fallback, no CPU path.
 """
 import os
 import shutil
@@ -77,7 +77,7 @@ def build_lib(force=False, verbose=False):
     deps = srcs + [d if os.path.isabs(d) else os.path.join(CSRC, d) for d in CU_HEADERS]
     if not (force or _stale(LIB, deps)):
         return LIB
-    cmd = [_nvcc(), "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    cmd = [_nvcc(), "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
            "-Xcompiler", "-fPIC", "-shared", "-Xlinker", "-soname=librnnt_b200.so", "-o", LIB] + srcs
     if verbose:
         cmd += ["-Xptxas", "-v"]

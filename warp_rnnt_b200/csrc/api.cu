@@ -1,7 +1,7 @@
 // api.cu -- the extern "C" surface of librnnt_b200.so (declared in include/rnnt_b200.h).
 //
 // (A) rnnt_b200_*: native interface bound by csrc/binding.cpp.
-// (B) run_warp_rnnt & co: the reference's C ABI (/root/reference/core.h:29-60) implemented on top
+// (B) run_warp_rnnt & co: the reference's C ABI (the reference's core.h:29-60) implemented on top
 //     of (A)'s kernels so the reference's own bindings link against this library unchanged.
 #include <atomic>
 #include <cstdio>
@@ -41,10 +41,10 @@ static int default_lse_mode() {
 
 // AUTO policy (DESIGN.md "numerics"): AUTO = exact, i.e. results are bit-identical to the reference
 // kernels unless the caller opts out.  Parity is the first gate: at BASELINE cfg 2 the fast flavour
-// differs from the reference by up to 1.2e-4 on a gradient (pure fp32 noise -- the reference itself is
-// 1.25e-4 away from fp64 there), which is outside the stated 1e-4.  The exact chain is ~2x longer per
-// anti-diagonal; it costs ~10 us at cfg 2 and nothing measurable where the dense write dominates
-// (cfg 3-5).  RNNT_LSE_FAST / RNNT_B200_LSE=fast selects the short chain.
+// differs from the reference by fp32 noise that can exceed the stated 1e-4 on single gradient elements (the
+// full-size test bounds it at 2.5e-4).  The exact chain is ~2x longer per anti-diagonal, but on an H100
+// (700 W) the dense cfg-2 call takes 110 us in both flavours: the dense gradient write dominates.
+// RNNT_LSE_FAST / RNNT_B200_LSE=fast selects the short chain.
 static int resolve_kind(int lse_mode, bool compact) {
     if (lse_mode == RNNT_LSE_AUTO) lse_mode = default_lse_mode();
     if (lse_mode == RNNT_LSE_FAST) return kFast;
@@ -114,10 +114,9 @@ struct Pipeline {
     int device;
 };
 static bool pipeline_enabled() {
-    // on by default (RNNT_B200_PIPELINE=0 disables).  Measured on B200, same box: cfg 5 micro-batch
-    // 2.23 ms pipelined vs 2.38 ms serial, cfg 4 2.85 vs 2.94 ms.  It only pays off with the
-    // early-retiring emit grid (launch_expand retire_early): persistent emit CTAs hold every SM
-    // until their kernel ends and the high-priority wavefront CTAs never get in (2.96 vs 2.90 ms).
+    // on by default (RNNT_B200_PIPELINE=0 disables).  It only pays off with the early-retiring emit grid
+    // (launch_expand retire_early): persistent emit CTAs hold every SM until their kernel ends and the
+    // high-priority wavefront CTAs never get in.
     static const bool on = !env_is("RNNT_B200_PIPELINE", '0');
     return on;
 }
@@ -238,9 +237,10 @@ static int loss_dense_any(void *stream, void *workspace, size_t workspace_bytes,
     const int kind = resolve_kind(lse_mode, false);
     // Large batches of large lattices: software-pipeline lattice groups over internal streams so that the
     // latency-bound wavefront of group g overlaps the bandwidth-bound gather of g+1 and emit of g-1.
-    // ... which only pays when the wavefront (a per-lattice latency chain of T+U-1 steps, ~0.45 us each, that does not
-    // shrink with the group) is short against the bandwidth-bound emit: measured on B200, cfg 5 micro-batch (chain
-    // 0.34 ms, emit 2.1 ms) 2.14 ms pipelined vs 2.39 ms serial; cfg 4 (chain 0.8 ms, emit 1.05 ms) 2.96 vs 2.70 ms.
+    // ... which only pays when the wavefront (a per-lattice latency chain of T+U-1 steps that does not shrink with the
+    // group) is short against the bandwidth-bound emit: cfg 5's micro-batch takes the pipeline, cfg 4 does not.
+    // The two estimates (0.45 us per anti-diagonal, an emit at 5.5 TB/s) were measured on a B200 and have not been
+    // re-derived for the H100 (3.35 TB/s HBM3): there the emit is slower, so the true break-even favours the pipeline more often than this estimate.
     const double wave_us = 0.45 * (T + U), emit_us = (double)cells * V * (io_bf16 ? 2 : 4) / 5.5e6;
     const int groups = (grads && N >= 8 && (int64_t)cells * V * 4 >= ((int64_t)512 << 20) && pipeline_enabled() &&
                         wave_us < 0.4 * emit_us)
@@ -306,7 +306,7 @@ static int loss_dense_any(void *stream, void *workspace, size_t workspace_bytes,
 
 extern "C" {
 
-const char *rnnt_b200_version(void) { return "0.1.0 (sm_100a)"; }
+const char *rnnt_b200_version(void) { return "0.1.0 (sm_90a)"; }
 
 const char *rnnt_b200_status_string(int s) {
     switch (s) {
@@ -335,7 +335,7 @@ void rnnt_b200_debug_guard_poison(int n, float delta) {
 }
 int rnnt_b200_debug_lse_selfcheck(void *stream, unsigned long long *mismatches) {
     if (!mismatches) return RNNT_STATUS_INVALID_ARGUMENT;
-    rnnt::k_lse_selfcheck<<<148 * 8, 256, 0, (cudaStream_t)stream>>>(mismatches);
+    rnnt::k_lse_selfcheck<<<sm_count(current_device()) * 8, 256, 0, (cudaStream_t)stream>>>(mismatches);
     return cudaGetLastError() == cudaSuccess ? RNNT_STATUS_SUCCESS : RNNT_STATUS_WARP_FAILED;
 }
 void rnnt_b200_debug_fused_trace(void *buf) { rnnt::set_fused_trace(static_cast<long long *>(buf)); }

@@ -1,6 +1,6 @@
 // binding.cpp -- the `_C` operator module: PyTorch tensors in, librnnt_b200.so (C ABI) underneath.
 //
-// Mirrors the reference's operator boundary /root/reference/pytorch_binding/binding.cpp:
+// Mirrors the reference's operator boundary the reference's pytorch_binding/binding.cpp:
 //   rnnt_loss                  (:28-106, pybind :250-254)   same kwargs, checks, messages, returns
 //   rnnt_loss_compact          (:109-207, pybind :256-262)
 //   rnnt_loss_compact_backward (:209-247, pybind :264-268)
@@ -416,13 +416,13 @@ at::Tensor rnnt_gather_backward(const at::Tensor &pair_grads, const at::Tensor &
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     namespace py = pybind11;
-    m.def("rnnt_loss", &rnnt_loss, "B200 RNN-Transducer loss (forward and gradients).", py::arg("xs"), py::arg("ys"),
+    m.def("rnnt_loss", &rnnt_loss, "H100 RNN-Transducer loss (forward and gradients).", py::arg("xs"), py::arg("ys"),
           py::arg("xn"), py::arg("yn"), py::arg("blank") = 0, py::arg("fastemit_lambda") = 0.0);
-    m.def("rnnt_loss_compact", &rnnt_loss_compact, "B200 RNN-Transducer loss in compact layout.", py::arg("xs"),
+    m.def("rnnt_loss_compact", &rnnt_loss_compact, "H100 RNN-Transducer loss in compact layout.", py::arg("xs"),
           py::arg("ys"), py::arg("xn"), py::arg("yn"), py::arg("blank") = 0, py::arg("fastemit_lambda") = 0.0,
           py::arg("required_grad") = true, py::arg("max_T") = 0, py::arg("max_U") = 0);
     m.def("rnnt_loss_compact_backward", &rnnt_loss_compact_backward,
-          "B200 RNN-Transducer loss backward for compact layout", py::arg("grad_costs"), py::arg("grad_xs"),
+          "H100 RNN-Transducer loss backward for compact layout", py::arg("grad_costs"), py::arg("grad_xs"),
           py::arg("cumSum"), py::arg("loc"), py::arg("V"), py::arg("blank") = 0);
     m.def("rnnt_loss_dense", &rnnt_loss_dense, py::arg("xs"), py::arg("ys"), py::arg("xn"), py::arg("yn"),
           py::arg("blank") = 0, py::arg("fastemit_lambda") = 0.0, py::arg("grad_scale") = py::none(),

@@ -1,7 +1,7 @@
 // expand.cu -- dense gradient emit: every element of the (cells, V) output is written exactly once
 // (zeros + the <= 2 non-zeros of each row), with 128-bit streaming stores.
 //
-// What it replaces in the reference (/root/reference):
+// What it replaces in the reference (1ytic/warp-rnnt):
 //   at::zeros_like(xs) dense memset                 pytorch_binding/binding.cpp:58
 //   kernel_grads_blank / kernel_grads_label         core.cu:260-332  (4-byte stores at stride U*V)
 //   RNNTLoss.backward grads.mul_(grad_output)       pytorch_binding/warp_rnnt/__init__.py:21-24
@@ -194,7 +194,7 @@ k_expand(Problem p, ExpandSrc src, OUT *__restrict__ out, int64_t cells, int V, 
             if ((V & (VEC - 1)) == 0) {
                 // rows are whole vectors: one staged-row fetch, four compare/selects.  (Kernel-uniform
                 // test on purpose: a per-vector "does it straddle a row end" branch makes nearly every
-                // warp run both paths -- measured 15 % slower at V = 50.  Also tried and dropped: composing
+                // warp run both paths -- slower at V = 50.  Also tried and dropped: composing
                 // 16 KB tiles in shared memory and streaming them out, 40 % slower at V = 50 because the
                 // per-chunk barriers and staging latency are amortised over too few bytes.)
                 const float2 g = s_g[row];

@@ -18,7 +18,7 @@
 //                        the recurrence (replaces kernel_warp + the global-memory counts scheduler, core.cu:41-258)
 //            zero-fill   when the gather is done, two warps' lane 0 issue TMA bulk stores of a zeroed shared-memory
 //                        buffer (evict_last) over this CTA's slice of the dense gradient (replaces at::zeros_like,
-//                        binding.cpp:58); fallback: 256-bit stores
+//                        binding.cpp:58); fallback: 128-bit evict_last stores
 //            chase       the other free warps follow the two wavefronts from the middle anti-diagonal outwards and
 //                        replace each staged log-prob by (alpha + beta) + log-prob: all of the gradient that does not
 //                        need beta[0,0]
@@ -41,11 +41,13 @@ namespace rnnt {
 constexpr int kFusedThreads = 512;
 constexpr float kBigF = -1.0e30f;   // finite stand-in for -inf (see wavefront.cu)
 
-// L2 residency control (B200: 126 MB L2).  The dense gradient slab is zero-filled while the
+// L2 residency control (H100: 50 MB L2).  The dense gradient slab is zero-filled while the
 // wavefront runs and patched afterwards; the patch is a partial-sector write, so it must still HIT
 // in L2 or ECC forces a DRAM read-modify-write per touched sector.  Filled lines are therefore
-// stored evict_last (TMA bulk stores with an evict_last policy, or 256-bit STG.E.ELL2.256), and the
-// one-pass log-prob gather is loaded evict_first so that it cannot displace them.
+// stored evict_last (TMA bulk stores with an evict_last policy, or 128-bit stores with the same policy), and the
+// one-pass log-prob gather is loaded evict_first so that it cannot displace them.  This order was chosen for a
+// 126 MB L2 (B200); at cfg 2 the gradient (86 MB) exceeds the H100's 50 MB L2, and how many patch stores still hit
+// there has not been measured.  The kernel is correct either way; only the patch's cost depends on it.
 __device__ __forceinline__ uint64_t policy_evict_first() {
     uint64_t p;
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
@@ -68,19 +70,21 @@ __device__ __forceinline__ float2 ldg_hint2(const float2 *ptr, uint64_t pol) {
     asm volatile("ld.global.nc.L2::cache_hint.v2.f32 {%0, %1}, [%2], %3;" : "=f"(v.x), "=f"(v.y) : "l"(ptr), "l"(pol));
     return v;
 }
-__device__ __forceinline__ void stg_zero256_evict_last(float *ptr) {
-    asm volatile("st.global.L2::evict_last.v8.b32 [%0], {%1,%1,%1,%1,%1,%1,%1,%1};" ::"l"(ptr), "r"(0) : "memory");
-}
 
 // Zero-fill through the TMA engine: bulk shared->global copies of a zeroed shared-memory buffer,
 // evict_last in L2.  One thread issues 8 KB per instruction, so the fill costs the SM no LSU / MIO
 // queue slots -- with STG fills the queue stays full of back-pressured stores and the wavefront
-// warps' LDS/STS wait behind them (measured: exact-LSE step 330 ns with STG fill running, 160 ns alone).
+// warps' LDS/STS wait behind them (an exact-LSE step took about twice as long with an STG fill running).
 constexpr int kZeroBytes = 8192;
 __device__ __forceinline__ uint64_t policy_evict_last() {
     uint64_t p;
     asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
     return p;
+}
+// 32 zero bytes as two 128-bit stores (sm_90 has no 256-bit STG), evict_last in L2
+__device__ __forceinline__ void stg_zero32_evict_last(float *ptr, uint64_t pol) {
+    asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1,%1,%1,%1}, %2;" ::"l"(ptr), "r"(0), "l"(pol) : "memory");
+    asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1,%1,%1,%1}, %2;" ::"l"(ptr + 4), "r"(0), "l"(pol) : "memory");
 }
 __device__ __forceinline__ void bulk_store(void *gdst, uint32_t ssrc, uint32_t bytes, uint64_t pol) {
     asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;"
@@ -252,7 +256,7 @@ struct FusedArgs {
 // __shfl_up_sync(full, v, 1) as a volatile asm: keeps the shuffle in program order with the (volatile)
 // shared-memory loads/stores of the loop.  Left free, the compiler batches three steps' LDS/STS in front of
 // the fourth shuffle and then copies the freshly loaded operands into place -- register moves that wait
-// for the load they follow, on the dependent chain (exact LSE: 158 vs 125 ns per step).
+// for the load they follow, on the dependent chain.
 __device__ __forceinline__ float shfl_up1_ordered(float v) {
     float r;
     asm volatile("shfl.sync.up.b32 %0, %1, 1, 0, 0xffffffff;" : "=f"(r) : "f"(v) : "memory");
@@ -312,8 +316,8 @@ __device__ __forceinline__ void sweep_diag(uint32_t wb, uint32_t wl, uint32_t ou
     // exact mode: the first real column is taken from the reference-order prefix scan (core.cu:92-110)
     const int l0 = first_col / C, c0 = first_col - l0 * C;
     // Predicate registers are scarce (7 per thread) and each exact-LSE chain keeps 3 alive; with more in the
-    // loop ptxas runs the lane's C chains one after the other instead of interleaved (160 vs 125 ns per step
-    // at C = 2).  So the column override is a bitwise select on a mask, and lanes past the staged row store to a
+    // loop ptxas runs the lane's C chains one after the other instead of interleaved (on an H100, the (cells,2)
+    // kernel at cfg 2 took 65 instead of 57 us).  So the column override is a bitwise select on a mask, and lanes past the staged row store to a
     // scratch slot instead of being predicated off.
     uint32_t own[C];                                          // all-ones where this register holds the first real column
 #pragma unroll
@@ -341,7 +345,7 @@ __device__ __forceinline__ void sweep_diag(uint32_t wb, uint32_t wl, uint32_t ou
     }
     // Exact LSE: ptxas interleaves the lane's C chains in every step of the unrolled body except the last one
     // before the back-edge (and in none of them if the loop also contains a conditional store, e.g. a trace
-    // stamp) -- so the body is 2P steps long: 7 of 8 steps run at ~125 ns instead of 160 ns.
+    // stamp) -- so the body is 2P steps long.
     // tools/sass_check.py watches this.
     constexpr int H = (KIND != kFast) ? 2 : 1;                 // groups of P steps per iteration
     for (int d00 = 0; d00 < ndiag; d00 += H * P) {
@@ -361,7 +365,9 @@ __device__ __forceinline__ void sweep_diag(uint32_t wb, uint32_t wl, uint32_t ou
             lse_vec<KIND, C>(xs, ys, nv);
             if (KIND != kFast) {
                 const int i = d0 + k - first_col;              // row of the first real column on this diagonal
-                const uint32_t in = ((i >= 1) && (i < pre_rows)) ? 0xffffffffu : 0u;
+                // all-ones for i in [1, pre_rows), from sign bits: as a compare it costs two more predicates per step,
+                // and ptxas for sm_90a then serialises the lane's chains
+                const uint32_t in = (uint32_t)(((i - pre_rows) >> 31) & ~((i - 1) >> 31));
 #pragma unroll
                 for (int c = 0; c < C; ++c) {
                     const uint32_t m = own[c] & in;
@@ -464,7 +470,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
     // Roles go by a rotated warp index: the two wavefront warps are the HIGHEST-numbered hardware
     // warps (14 and 15, on different sub-partitions).  The SM's issue arbiter favours higher warp
     // ids, so the latency-critical recurrence is never starved by the fill / gather warps sharing its
-    // scheduler (with the sweep on warps 0/1 the exact flavour measured anywhere from 65 to 250 us).
+    // scheduler (with the sweep on warps 0/1 the exact flavour's time varied several-fold from run to run).
     //   logical warp 0 / 1      alpha / beta wavefront, chasing the gather chunk by chunk
     //   logical warps [2,2+GW)  gather, then (MODE 0) zero-fill
     //   the rest (MODE 0)       zero-fill from the start: HBM reads (gather) and writes (fill) overlap
@@ -619,7 +625,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
     }
     if (MODE == 0) {
         // zero-fill rows [t0,t1) of this lattice's slab: elements [f0,f1); 32 KB chunks handed out by
-        // s_next; 256-bit evict_last stores (or bulk copies) on the 32-byte aligned interior
+        // s_next; 2 x 128-bit evict_last stores per 32 bytes (or bulk copies) on the 32-byte aligned interior
         const int64_t f0 = (slab + (int64_t)t0 * U) * V, f1 = (slab + (int64_t)t1 * U) * V;
         IO *g = static_cast<IO *>(A.grads);
         constexpr int EPV = 32 / ESZ;                   // elements per 32 bytes
@@ -647,6 +653,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
             }
             __syncwarp();
         } else {
+            const uint64_t pol = policy_evict_last();
             for (;;) {
                 int c = 0;
                 if (lane == 0) c = atomicAdd(&s_next, 1);
@@ -655,7 +662,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
                 const int64_t b = a0 + (int64_t)c * kChunk;
                 const int64_t e = min(a1, b + kChunk);
 #pragma unroll 4
-                for (int64_t f = b + EPV * lane; f < e; f += 32 * EPV) stg_zero256_evict_last(reinterpret_cast<float *>(g + f));
+                for (int64_t f = b + EPV * lane; f < e; f += 32 * EPV) stg_zero32_evict_last(reinterpret_cast<float *>(g + f), pol);
             }
         }
         if (lw == kFusedThreads / 32 - 1) {             // unaligned head / tail (< 32 bytes each, or everything if !vec)
@@ -944,7 +951,7 @@ cudaError_t launch_fused(cudaStream_t s, int kind, const FusedPlan &plan, const 
         }
     }
     {
-        static const bool tma = !env_is("RNNT_B200_FILL", 's');   // RNNT_B200_FILL=stg selects the 256-bit store fill
+        static const bool tma = !env_is("RNNT_B200_FILL", 's');   // RNNT_B200_FILL=stg selects the 128-bit store fill
         a.tma_fill = tma ? 1 : 0;
         static const int fw = env_int("RNNT_B200_FILL_WARPS", 2);
         a.fill_warps = max(1, min(fw, kFusedThreads / 32 - 2));

@@ -1,7 +1,7 @@
 // joint.cu -- compact packing of the joint network's input (SURVEY.md 8(f)3): the caller side of compact=True.
 //
 // The reference's benchmark builds the ragged joint input with a python loop over the batch
-// (/root/reference/pytorch_binding/benchmark2.py:37-50):
+// (the reference's pytorch_binding/benchmark2.py:37-50):
 //     x = cat([ (f[i, :lf[i]].unsqueeze(1) + g[i, :lg[i]+1].unsqueeze(0)).view(-1, H)  for i in range(N) ])
 // i.e. 2N host syncs (lf[i], lg[i] index tensors), N small kernels + a cat, and autograd replays the same pieces
 // backwards.  Here: one kernel forward (rows at mem_pref[n] + t*(lg[n]+1) + u, the layout rnnt_loss(compact=True)

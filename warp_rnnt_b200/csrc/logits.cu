@@ -1,7 +1,7 @@
 // logits.cu -- the step BEFORE the reference's path, fused in: the loss straight from un-normalised joint-network
 // logits (SURVEY.md 8(f)1).
 //
-// The reference requires log-softmaxed input (/root/reference/README.md:59) and its benchmark times F.log_softmax with
+// The reference requires log-softmaxed input (the reference's README.md:59) and its benchmark times F.log_softmax with
 // the loss (pytorch_binding/benchmark.py:65): log_softmax forward (read + write of (N,T,U,V)), the loss (read + dense
 // gradient write, + mul_) and log_softmax backward (two reads + one write) -- seven dense passes.  Here:
 //

@@ -1,7 +1,7 @@
 // wavefront.cu -- general (any-size) path: prefix sums, log-prob gather, the alpha/beta wavefront
 // and the (cells,2) gradient kernel.
 //
-// What it replaces in the reference (/root/reference):
+// What it replaces in the reference (1ytic/warp-rnnt):
 //   k_prefix      : host-side cumsum + 4 .item() syncs        pytorch_binding/binding.cpp:132-158
 //   k_gather      : kernel_fill_gather                        core_compact.cu:403-436
 //                   python-level gather (index tensor + torch.gather)   warp_rnnt/__init__.py:118-128
@@ -588,7 +588,7 @@ static cudaError_t launch_wavefront_kp(cudaStream_t s, const Problem &p, const f
 // The unroll factor of the recurrence loop = its operand prefetch distance.  The exact-LSE body is ~150 instructions
 // per step; unrolled 8x, the two instantiations a CTA runs (ring-fed warps + the column-0 warp) are ~40 KB of SASS,
 // more than the 32 KB instruction cache behind an SM's schedulers (ncu r1: "no instruction" was the top stall reason).
-// Measured at cfg 4 (us): exact 1027 / 797 / 986 for unroll 8 / 4 / 2, fast 634 / 687 / 855 -> 4 for exact, 8 for fast.
+// At cfg 4 unroll 4 was fastest for the exact flavour and unroll 8 for the fast one.
 template <int KIND>
 static cudaError_t launch_wavefront_kind(cudaStream_t s, const Problem &p, const float2 *pairs, float *alphas,
                                          float *betas, float *ws_ll, int *bad, float *costs, int beta_only,
