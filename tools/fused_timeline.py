@@ -1,6 +1,8 @@
 """Phase timeline of the fused small-lattice kernel (k_fused) from its optional clock64 stamps
 (rnnt_b200_debug_fused_trace, include/rnnt_b200.h).  Prints, per LSE mode, the median over CTAs of each
-phase's end time relative to the CTA's start, in microseconds.
+phase's end time relative to the CTA's start, in microseconds.  Phases the launch's dense-gradient emit order does
+not have are left out: fill_issued / zeros_landed belong to zero-fill + patch, store_start (composed rows staged,
+the stores begin) to the composed emit; emit_start is where beta[0,0] is known and either emit begins.
 
     python tools/fused_timeline.py [c2|c3] [out.json]
 """
@@ -16,7 +18,7 @@ import warp_rnnt_b200 as w  # noqa: E402
 
 SHAPES = {"c2": (128, 150, 40, 28), "c2n32": (32, 150, 40, 28), "c2n132": (132, 150, 40, 28), "c3": (32, 150, 20, 5000), "c1": (1, 150, 40, 28)}
 NAMES = ["start", "sentinels", "gather_done", "sweep_start", "alpha_done", "beta_done", "fill_issued", "end", "chase_done",
-         "zeros_landed", "patch_start"]
+         "zeros_landed", "emit_start", "store_start"]
 
 
 def sm_mhz():
@@ -64,9 +66,10 @@ def main():
         rel = (tr[:, :len(NAMES)] - tr[:, :1]).clamp(min=0).double() / mhz          # cycles / MHz = us
         med = rel.median(dim=0).values.tolist()
         mx = rel.max(dim=0).values.tolist()
+        seen = [i == 0 or bool((tr[:, i] > 0).any()) for i in range(len(NAMES))]
         out[mode] = {"ctas": int(tr.shape[0]), "sm_mhz": mhz, "event_us": e0.elapsed_time(e1) * 1e3,
-                     "median_us": dict(zip(NAMES, [round(x, 2) for x in med])),
-                     "max_us": dict(zip(NAMES, [round(x, 2) for x in mx]))}
+                     "median_us": {k: round(x, 2) for k, x, s in zip(NAMES, med, seen) if s},
+                     "max_us": {k: round(x, 2) for k, x, s in zip(NAMES, mx, seen) if s}}
         print(mode, json.dumps(out[mode]))
     if len(sys.argv) > 2:
         json.dump(out, open(sys.argv[2], "w"), indent=1)

@@ -42,8 +42,9 @@ static int default_lse_mode() {
 // AUTO policy (DESIGN.md "numerics"): AUTO = exact, i.e. results are bit-identical to the reference
 // kernels unless the caller opts out.  Parity is the first gate: at BASELINE cfg 2 the fast flavour
 // differs from the reference by fp32 noise that can exceed the stated 1e-4 on single gradient elements (the
-// full-size test bounds it at 2.5e-4).  The exact chain is ~2x longer per anti-diagonal, but on an H100
-// (700 W) the dense cfg-2 call takes 110 us in both flavours: the dense gradient write dominates.
+// full-size test bounds it at 2.5e-4).  The exact chain is ~2x longer per anti-diagonal; on an H100 (700 W) the dense
+// cfg-2 call's gradient write follows the recurrence (composed emit, fused.cu), so the recurrence is on its critical
+// path: the timeline (tools/fused_timeline.py) shows beta[0,0] at ~51 us exact and ~46 us fast, of a ~80 us kernel.
 // RNNT_LSE_FAST / RNNT_B200_LSE=fast selects the short chain.
 static int resolve_kind(int lse_mode, bool compact) {
     if (lse_mode == RNNT_LSE_AUTO) lse_mode = default_lse_mode();

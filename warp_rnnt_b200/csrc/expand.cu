@@ -88,20 +88,6 @@ __device__ __forceinline__ void stage_row(const Problem &p, const ExpandSrc &src
 // MODE 0: dense layout, source = alpha/beta/pairs (forward)            label overrides blank
 // MODE 1: dense layout, source = pair grads (gather=True backward)     label adds to blank (scatter_add)
 // MODE 2: compact layout, source = pair grads + loc (compact backward) label written iff loc != blank
-// 16-byte streaming store of VEC output elements (4 floats or 8 bf16)
-__device__ __forceinline__ void st_vec(float *p, const float (&e)[4]) { st_cs_v4(p, make_float4(e[0], e[1], e[2], e[3])); }
-__device__ __forceinline__ void st_vec(__nv_bfloat16 *p, const float (&e)[8]) {
-    uint32_t w[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const __nv_bfloat162 h = __floats2bfloat162_rn(e[2 * k], e[2 * k + 1]);
-        w[k] = *reinterpret_cast<const uint32_t *>(&h);
-    }
-    asm volatile("st.global.cs.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]) : "memory");
-}
-__device__ __forceinline__ void st_one(float *p, float v) { st_cs(p, v); }
-__device__ __forceinline__ void st_one(__nv_bfloat16 *p, float v) { *p = __float2bfloat16_rn(v); }
-
 // OUT: element type of the dense output (float; __nv_bfloat16 for the bf16 i/o forward, MODE 0)
 template <int MODE, typename OUT = float>
 __global__ void __launch_bounds__(kExpandThreads)
@@ -142,13 +128,12 @@ k_expand(Problem p, ExpandSrc src, OUT *__restrict__ out, int64_t cells, int V, 
         // ---- phase 2: sweep the chunk's floats [f0, f1)
         const int64_t f0 = r0 * (int64_t)V;
         const int64_t f1 = f0 + (int64_t)rows * V;
-        auto value = [&](int row, int v) -> float {
-            const float2 g = s_g[row];
-            const int lab = s_lab[row];
-            float x = (v == blank) ? g.x : 0.0f;
-            // override mode: a zero label gradient marks "no label transition here" (padded labels may equal blank)
-            if (v == lab) x = (MODE == 1 && src.label_adds) ? x + g.y : ((MODE == 1 && !p.yn && g.y == 0.0f) ? x : g.y);
-            return x;
+        // override mode: a zero label gradient marks "no label transition here" (padded labels may equal blank)
+        const bool adds = (MODE == 1) && src.label_adds;
+        auto row_at = [&](int row) -> GradRow {
+            GradRow r{s_g[row], s_lab[row]};
+            if (MODE == 1 && !adds && !p.yn && r.g.y == 0.0f) r.lab = -1;
+            return r;
         };
         int64_t a0 = vec_ok ? min(f1, (f0 + VEC - 1) & ~(int64_t)(VEC - 1)) : f1;
         int64_t a1 = vec_ok ? max(a0, f1 & ~(int64_t)(VEC - 1)) : f1;
@@ -156,12 +141,12 @@ k_expand(Problem p, ExpandSrc src, OUT *__restrict__ out, int64_t cells, int V, 
         for (int64_t f = f0 + threadIdx.x; f < a0; f += kExpandThreads) {
             const uint32_t local = (uint32_t)(f - f0);
             const uint32_t row = divV.div(local);
-            st_one(out + f, value((int)row, (int)(local - row * V)));
+            st_one(out + f, grad_row_elem(row_at((int)row), blank, (int)(local - row * V), adds));
         }
         for (int64_t f = a1 + threadIdx.x; f < f1; f += kExpandThreads) {
             const uint32_t local = (uint32_t)(f - f0);
             const uint32_t row = divV.div(local);
-            st_one(out + f, value((int)row, (int)(local - row * V)));
+            st_one(out + f, grad_row_elem(row_at((int)row), blank, (int)(local - row * V), adds));
         }
         if (VEC == 4 && pair_path) {
             // rows come in pairs of G = V/2 vectors (r0 is even, so a0 == f0): vector k of pair q covers positions
@@ -188,33 +173,13 @@ k_expand(Problem p, ExpandSrc src, OUT *__restrict__ out, int64_t cells, int V, 
         } else
         for (int64_t f = a0 + VEC * (int64_t)threadIdx.x; f < a1; f += VEC * kExpandThreads) {
             const uint32_t local = (uint32_t)(f - f0);
-            uint32_t row = divV.div(local);
-            int v = (int)(local - row * V);
+            const uint32_t row = divV.div(local);
             float e[VEC];
-            if ((V & (VEC - 1)) == 0) {
-                // rows are whole vectors: one staged-row fetch, four compare/selects.  (Kernel-uniform
-                // test on purpose: a per-vector "does it straddle a row end" branch makes nearly every
-                // warp run both paths -- slower at V = 50.  Also tried and dropped: composing
-                // 16 KB tiles in shared memory and streaming them out, 40 % slower at V = 50 because the
-                // per-chunk barriers and staging latency are amortised over too few bytes.)
-                const float2 g = s_g[row];
-                const int lab = s_lab[row];
-                const int pb = blank - v, pl = lab - v;
-                const bool adds = (MODE == 1) && src.label_adds;
-                const bool lab_live = (MODE != 1) || adds || p.yn || (g.y != 0.0f);
-#pragma unroll
-                for (int k = 0; k < VEC; ++k) {
-                    float x = (k == pb) ? g.x : 0.0f;
-                    if (k == pl && lab_live) x = adds ? x + g.y : g.y;
-                    e[k] = x;
-                }
-            } else {
-#pragma unroll
-                for (int k = 0; k < VEC; ++k) {
-                    e[k] = value((int)row, v);
-                    if (++v == V) { v = 0; ++row; }
-                }
-            }
+            // (rows_whole is kernel-uniform on purpose: a per-vector "does it straddle a row end" branch makes nearly
+            // every warp run both paths -- slower at V = 50.  Also tried and dropped: composing 16 KB tiles in shared
+            // memory and streaming them out, 40 % slower at V = 50 because the per-chunk barriers and staging latency
+            // are amortised over too few bytes.)
+            compose_vec<VEC>(e, (int)row, (int)(local - row * V), V, blank, adds, (V & (VEC - 1)) == 0, row_at);
             st_vec(out + f, e);
         }
     }

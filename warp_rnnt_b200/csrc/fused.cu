@@ -16,17 +16,20 @@
 //                        move as C-wide vector LDS/STS (a diagonal's cells are contiguous in the staged layout; alpha
 //                        walks the same planes as beta, backwards).  No inter-warp hand-off, no barrier, no atomics on
 //                        the recurrence (replaces kernel_warp + the global-memory counts scheduler, core.cu:41-258)
-//            zero-fill   when the gather is done, two warps' lane 0 issue TMA bulk stores of a zeroed shared-memory
-//                        buffer (evict_last) over this CTA's slice of the dense gradient (replaces at::zeros_like,
-//                        binding.cpp:58); fallback: 128-bit evict_last stores
+//            zero-fill   (MODE 0, patch order) when the gather is done, two warps' lane 0 issue TMA bulk stores of a
+//                        zeroed shared-memory buffer (evict_last) over this CTA's slice of the dense gradient (replaces
+//                        at::zeros_like, binding.cpp:58); fallback: 128-bit evict_last stores
 //            chase       the other free warps follow the two wavefronts from the middle anti-diagonal outwards and
 //                        replace each staged log-prob by (alpha + beta) + log-prob: all of the gradient that does not
 //                        need beta[0,0]
 //   phase 2  cost/guard  kernel_fill_costs (core.cu:334-370) + the reduced loss sum_n costs[n]*scale[n] by the last CTA
-//            patch       expf(x - beta00) and <= 2 four-byte stores per cell into the freshly zeroed, still L2-resident
-//                        lines (kernel_grads_blank/label, core.cu:260-332), or -- MODE 1 -- the gradients are emitted
-//                        in (N,T,U,2) form for the deferred dense backward (+ loc for the compact layout, whose
-//                        lattices are addressed through mem_pref / lab_pref).
+//            emit        MODE 0, two orders (chosen per launch, see launch_fused):
+//                          compose: expf(x - beta00) of every cell in place, then every element of the CTA's rows is
+//                                   written once as 16-byte streaming stores (replaces zeros_like + kernel_grads_*)
+//                          patch:   expf(x - beta00) and <= 2 four-byte stores per cell into the zeroed lines
+//                                   (kernel_grads_blank/label, core.cu:260-332)
+//                        MODE 1: the gradients are emitted in (N,T,U,2) form for the deferred dense backward (+ loc for
+//                        the compact layout, whose lattices are addressed through mem_pref / lab_pref).
 //
 // grid (S, N): S CTAs per lattice recompute the (cheap) wavefront redundantly and split the
 // (bandwidth-bound) fill/patch of the lattice's rows, so small batches still use every SM.
@@ -41,13 +44,13 @@ namespace rnnt {
 constexpr int kFusedThreads = 512;
 constexpr float kBigF = -1.0e30f;   // finite stand-in for -inf (see wavefront.cu)
 
-// L2 residency control (H100: 50 MB L2).  The dense gradient slab is zero-filled while the
+// L2 residency control (H100: 50 MB L2).  In the patch order the dense gradient slab is zero-filled while the
 // wavefront runs and patched afterwards; the patch is a partial-sector write, so it must still HIT
 // in L2 or ECC forces a DRAM read-modify-write per touched sector.  Filled lines are therefore
 // stored evict_last (TMA bulk stores with an evict_last policy, or 128-bit stores with the same policy), and the
-// one-pass log-prob gather is loaded evict_first so that it cannot displace them.  This order was chosen for a
-// 126 MB L2 (B200); at cfg 2 the gradient (86 MB) exceeds the H100's 50 MB L2, and how many patch stores still hit
-// there has not been measured.  The kernel is correct either way; only the patch's cost depends on it.
+// one-pass log-prob gather is loaded evict_first so that it cannot displace them.  A gradient larger than L2 (cfg 2:
+// 86 MB) loses many zeroed lines before the patch reaches them, so the dense emit composes such gradients after
+// beta[0,0] instead and writes every line once, as whole sectors (launch_fused; DESIGN.md 3.1).
 __device__ __forceinline__ uint64_t policy_evict_first() {
     uint64_t p;
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
@@ -234,8 +237,10 @@ struct FusedArgs {
     int Wd;                 // staged row stride (floats) = C * ceil(U / C), even
     int nd;                 // staged rows (diagonals) allocated = T + Wd + 16
     int gw;                 // warps that gather (of the 14 non-wavefront warps); MODE 0: the rest start the zero-fill at once
-    int tma_fill;           // MODE 0: zero-fill with bulk shared->global copies (else 256-bit STG)
+    int compose;            // MODE 0: emit order -- 1: composed rows after beta[0,0]; 0: zero-fill + patch
+    int tma_fill;           // MODE 0, zero-fill: bulk shared->global copies (else 128-bit STG)
     int fill_warps;         // MODE 0, bulk fill: how many of the 14 free warps issue it (the others chase at once)
+    FastDiv divV, divU;     // MODE 0, composed emit: element -> cell, cell -> (row, column)
     long long *trace;       // optional per-CTA phase stamps (clock64), 8 per CTA; null = off
     float *loss_sum;        // optional: sum_n costs[n] * (scale ? scale[n] : 1), written by the last CTA to finish
     unsigned *sync_counter; // with loss_sum: device counter, 0 on entry, left 0 (self-resetting)
@@ -389,7 +394,7 @@ __device__ __forceinline__ void sweep_diag(uint32_t wb, uint32_t wl, uint32_t ou
     asm volatile("st.release.cta.shared.u32 [%0], %1;" ::"r"(a_prog), "r"(0x3fffffff) : "memory");
 }
 
-// MODE 0: dense gradients (zero-fill + patch).  MODE 1: (N,T,U,2) gradients.  Both write costs.
+// MODE 0: dense gradients (composed, or zero-fill + patch).  MODE 1: (N,T,U,2) gradients.  Both write costs.
 // IO: element type of log_probs and of the dense gradient (float, or __nv_bfloat16 with MODE 0).
 template <int KIND, int MODE, int C, typename IO = float>
 __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
@@ -450,7 +455,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
-    if (MODE == 0 && A.tma_fill) {
+    if (MODE == 0 && !A.compose && A.tma_fill) {
         for (int k = tid; k < kZeroBytes / 4; k += kFusedThreads) zbuf[k] = 0.0f;
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy zeros -> async-proxy reads
     }
@@ -525,7 +530,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
             stamp(2);
         }
         // the zero-fill starts when the whole gather is done (HBM serves the critical reads first)
-        if (MODE == 0 && lw >= 2) asm volatile("bar.sync 1, %0;" ::"r"(kFusedThreads - 64) : "memory");
+        if (MODE == 0 && !A.compose && lw >= 2) asm volatile("bar.sync 1, %0;" ::"r"(kFusedThreads - 64) : "memory");
     } else if (ok && lw >= 2 && lw < 2 + GW) {
         const float inv = 1.0f / (float)Un;
         const uint64_t pol_first = policy_evict_first();
@@ -623,7 +628,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
         else sweep_diag<KIND, C, true>(wb_a, wl_a, out_a, Wd, ndiag, lane, first_col, pre, Tn, gwait, scr, &s_prog[0], T1 + Wd);
         stamp(beta ? 5 : 4);
     }
-    if (MODE == 0) {
+    if (MODE == 0 && !A.compose) {
         // zero-fill rows [t0,t1) of this lattice's slab: elements [f0,f1); 32 KB chunks handed out by
         // s_next; 2 x 128-bit evict_last stores per 32 bytes (or bulk copies) on the 32-byte aligned interior
         const int64_t f0 = (slab + (int64_t)t0 * U) * V, f1 = (slab + (int64_t)t1 * U) * V;
@@ -670,6 +675,8 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
             for (int64_t f = a1 + lane; f < f1; f += 32) g[f] = io_from_float<IO>(0.0f);
         }
         stamp(6);
+    }
+    if (MODE == 0) {
         // ---- chase: while the zeros drain and the two wavefronts run their last diagonals, the 14 free warps follow
         // them from the MIDDLE anti-diagonal outwards (alpha has passed it from above, beta from below: the cells of
         // diagonal e are final once alpha is past e+1 and beta past e+1 from the other side) and replace each staged
@@ -707,11 +714,11 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
             }
             stamp(8);
         }
-        if (A.tma_fill && lane == 0) {
+        if (!A.compose && A.tma_fill && lane == 0) {
             asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // the zeros have landed ...
             asm volatile("fence.proxy.async;" ::: "memory");            // ... before anyone patches them
         }
-        stamp(9);
+        if (!A.compose) stamp(9);
     }
     __syncthreads();
 
@@ -766,7 +773,91 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
         if (A.scale) { gb *= sc; gl *= sc; }
         return make_float2(gb, gl);
     };
-    if (MODE == 0) {
+    if (MODE == 0 && A.compose) {
+        // Composed emit: every element of rows [t0,t1) is written once, as whole 16-byte vectors.
+        // Pass 1 turns the chase's x = alpha + beta + lp of the rows this CTA emits into the final values in place, with
+        // the patch's arithmetic (expf(x - beta00), FastEmit, scale): WBb = gradient at the blank's column, +0 where the
+        // reference writes none (the last row's inner cells, or label == blank: there the label gradient wins);
+        // WLb = gradient at the label's column.
+        const int r0 = t0, r1 = min(t1, Tn);
+        if (live) {
+            // thread i takes cells i, i + 512, ... of the rows (row-major), K at a time: all loads first, so that one
+            // thread's K cells overlap their shared-memory and MUFU latencies (one CTA per SM leaves few warps to hide them)
+            constexpr int K = 4;
+            const double lam1 = 1.0 + (double)A.lam;
+            const int dq = kFusedThreads / Un, dr = kFusedThreads - dq * Un;   // one step: dq rows down, dr columns right
+            int t = r0 + tid / Un, u = tid % Un;
+            while (t < r1) {
+                int ib[K];
+                bool in[K], go_b[K], go_l[K];
+                float xb[K], xl[K];
+#pragma unroll
+                for (int k = 0; k < K; ++k) {
+                    in[k] = t < r1;
+                    const bool last_t = (t == T1), last_u = (u == U1);
+                    ib[k] = idxB(t, u);
+                    go_b[k] = in[k] && !(last_t && !last_u) && (last_u || s_lab[u] != A.blank);
+                    go_l[k] = in[k] && !last_u;
+                    if (in[k]) { xb[k] = WBb[ib[k]]; xl[k] = WLb[ib[k]]; }
+                    u += dr; t += dq;
+                    if (u >= Un) { u -= Un; ++t; }
+                }
+#pragma unroll
+                for (int k = 0; k < K; ++k) {
+                    float gb = 0.0f, gl = 0.0f;
+                    if (go_b[k]) {
+                        gb = -expf(xb[k] - b00);
+                        if (A.scale) gb *= sc;
+                    }
+                    if (go_l[k]) {
+                        float a = expf(xl[k] - b00);
+                        if (has_lam) a = (float)(lam1 * (double)a);   // see the patch below
+                        gl = -a;
+                        if (A.scale) gl *= sc;
+                    }
+                    if (in[k]) { WBb[ib[k]] = gb; WLb[ib[k]] = gl; }
+                }
+            }
+        }
+        __syncthreads();
+        stamp(11);
+        // Pass 2: all 16 warps sweep the slab's elements [f0,f1) with streaming stores, each vector composed from the
+        // staged values of the cells it covers; padding rows / columns and a dead lattice (invalid lengths, guard
+        // fired) are zeros.  Unaligned head and tail: scalar stores.
+        constexpr int VEC = 16 / ESZ;
+        IO *const g = static_cast<IO *>(A.grads);
+        const int64_t f0 = (slab + (int64_t)t0 * U) * V, f1 = (slab + (int64_t)t1 * U) * V;
+        const bool vec = ((reinterpret_cast<uintptr_t>(g) & 15u) == 0);
+        const int64_t a0 = vec ? min(f1, (f0 + VEC - 1) & ~(int64_t)(VEC - 1)) : f1;
+        const int64_t a1 = vec ? max(a0, f1 & ~(int64_t)(VEC - 1)) : f1;
+        auto row_at = [&](int c) -> GradRow {          // c: cell of rows [t0,t1), row-major
+            uint32_t tt, u;
+            A.divU.divmod((uint32_t)c, tt, u);
+            const int t = t0 + (int)tt;
+            GradRow r{make_float2(0.0f, 0.0f), -1};
+            if (live && t < Tn && (int)u < Un) {
+                const int ib = idxB(t, (int)u);
+                r.g = make_float2(WBb[ib], WLb[ib]);
+                if ((int)u < U1) r.lab = s_lab[u];
+            }
+            return r;
+        };
+        auto scalar = [&](int64_t f) {
+            uint32_t c, v;
+            A.divV.divmod((uint32_t)(f - f0), c, v);
+            st_one(g + f, grad_row_elem(row_at((int)c), A.blank, (int)v, false));
+        };
+        for (int64_t f = f0 + tid; f < a0; f += kFusedThreads) scalar(f);
+        for (int64_t f = a1 + tid; f < f1; f += kFusedThreads) scalar(f);
+        const bool rows_whole = (V & (VEC - 1)) == 0;
+        for (int64_t f = a0 + VEC * tid; f < a1; f += VEC * kFusedThreads) {
+            uint32_t c, v;
+            A.divV.divmod((uint32_t)(f - f0), c, v);
+            float e[VEC];
+            compose_vec<VEC>(e, (int)c, (int)v, V, A.blank, false, rows_whole, row_at);
+            st_vec(g + f, e);
+        }
+    } else if (MODE == 0) {
         if (live) {
             // Items (t, u, blank|label) of rows [r0,r1) in row-major order, thread i takes items i, i+512, ...: lanes
             // (2k,2k+1) = (blank,label) of one cell, a store instruction covers 16 adjacent cells.  The chase has left
@@ -831,6 +922,12 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
 constexpr int kFusedMaxDynSmem = 223 * 1024;           // 227 KB per CTA minus the kernel's static shared memory
 static long long *g_fused_trace = nullptr;             // diagnostics: see rnnt_b200_debug_fused_trace
 void set_fused_trace(long long *buf) { g_fused_trace = buf; }
+
+// Largest gradient row (V * element size, bytes) that the dense emit composes after beta[0,0] instead of
+// zero-filling under the recurrence and patching.  On an H100 the composed order is faster at every row size up to
+// this one (whole 16-byte vectors) once the gradient exceeds L2 (profiles/h100_emit_sweep.json); larger rows were
+// not measured.
+constexpr size_t kComposeMaxRowBytes = 4096;
 
 static size_t fused_zero_offset(int T, int U, int Wd, int nd) {
     const size_t used = sizeof(float) * ((size_t)4 * nd * Wd + (size_t)2 * T) + sizeof(int) * (size_t)U;
@@ -924,10 +1021,25 @@ cudaError_t launch_fused(cudaStream_t s, int kind, const FusedPlan &plan, const 
         a.gw = gw_env ? gw_env : kFusedThreads / 32 - 2;
         if (!grads) a.gw = kFusedThreads / 32 - 2;      // nothing to fill: everyone gathers
     }
+    {
+        // dense emit order (DESIGN.md 3.1): a gradient of small rows of whole 16-byte vectors that does not fit in L2
+        // is composed and written once after beta[0,0]; otherwise it is zero-filled under the recurrence and patched --
+        // large rows keep the fill overlapped, a gradient that fits in L2 is patched there, and rows that are not whole
+        // vectors compose slower (bf16 V=28) (RNNT_B200_EMIT=compose|patch overrides, for A/B measurements)
+        static const int emit_env = env_is("RNNT_B200_EMIT", 'c') ? 1 : env_is("RNNT_B200_EMIT", 'p') ? 0 : -1;
+        const size_t row_bytes = (size_t)V * (io_bf16 ? 2 : sizeof(float));
+        const bool rows_fit = row_bytes <= kComposeMaxRowBytes && row_bytes % 16 == 0;
+        const bool over_l2 = (size_t)N * T * U * row_bytes > l2_bytes(current_device());
+        a.compose = grads ? (emit_env >= 0 ? emit_env : (rows_fit && over_l2 ? 1 : 0)) : 0;
+        a.divV = FastDiv((uint32_t)V);
+        a.divU = FastDiv((uint32_t)U);
+    }
     a.zoff = (int)(plan.smem - kZeroBytes);
     // TMA row gather when a lattice row (U*V floats) is a 16-byte multiple at a 16-byte aligned address and
-    // at least four row buffers fit behind the planes (RNNT_B200_GATHER=ldg forces the LDG gather)
-    size_t smem = plan.smem;
+    // at least four row buffers fit behind the planes (RNNT_B200_GATHER=ldg forces the LDG gather); the composed
+    // emit needs no zero buffer, so they start where it would be
+    const size_t base = a.compose ? plan.smem - kZeroBytes : plan.smem;
+    size_t smem = base;
     a.nbuf = 0; a.row_off = 0; a.row_stride = 0; a.gwn = 0; a.nb_per = 1;
     {
         static const bool want_tma = !env_is("RNNT_B200_GATHER", 'l');
@@ -937,17 +1049,17 @@ cudaError_t launch_fused(cudaStream_t s, int kind, const FusedPlan &plan, const 
         // keep two CTAs per SM where the plan counted on them
         const size_t cap = (plan.smem <= 110 * 1024) ? (size_t)113 * 1024 : (size_t)kFusedMaxDynSmem;
         if (want_tma && !pairs_in && (row % 16) == 0 && (reinterpret_cast<uintptr_t>(lp) % 16) == 0 && row <= 32 * 1024 &&
-            plan.smem + 4 * stride <= cap) {
-            const int fit = (int)((cap - plan.smem) / stride);
+            base + 4 * stride <= cap) {
+            const int fit = (int)((cap - base) / stride);
             // two buffers per gather warp once at least 8 fit (the copy of the next row overlaps the picking of this one
             // and more bytes stay in flight per SM: the gather is bound by that, not by HBM, up to ~20 rows); else one
             a.nb_per = (nb_env == 1 || nb_env == 2) ? nb_env : (fit >= 8 ? 2 : 1);
             if (a.nb_per == 2 && fit < 2) a.nb_per = 1;
             a.gwn = min(kMaxRowBufs, fit / a.nb_per);
             a.nbuf = a.gwn * a.nb_per;
-            a.row_off = (int)(plan.smem);
+            a.row_off = (int)base;
             a.row_stride = (int)stride;
-            smem = plan.smem + (size_t)a.nbuf * stride;
+            smem = base + (size_t)a.nbuf * stride;
         }
     }
     {
