@@ -22,6 +22,7 @@ import torch  # noqa: E402
 
 from oracle import build_ref  # noqa: E402
 from tests import test_gpu_fullsize as F, test_gpu_holes as H, test_gpu_logits as L, test_gpu_parity as P  # noqa: E402
+from tests import test_gpu_nonfinite as NF  # noqa: E402
 from tests.common import REF_OUTPUTS, input_sample, make_inputs, record, to_compact  # noqa: E402
 
 
@@ -112,6 +113,8 @@ def main(out):
         x, ys, xn, yn = L.make(N, T, U, V, seed=11 + V, blank=blank)
         lp = torch.log_softmax(cu(x), -1)
         dense(rec, "logits_%d" % k, ref, (lp.contiguous(), cu(ys), cu(xn), cu(yn)), blank=blank, fastemit_lambda=lam)
+    # tests/test_gpu_nonfinite.py: masked and non-finite log-probs
+    NF.record_reference(rec, ref)
     torch.cuda.synchronize()
     np.savez_compressed(out, **rec)
     print("wrote %s: %d arrays, %d bytes" % (out, len(rec), os.path.getsize(out)))

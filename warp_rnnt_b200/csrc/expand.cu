@@ -77,7 +77,7 @@ __device__ __forceinline__ void stage_row(const Problem &p, const ExpandSrc &src
             const Lattice L = get_lattice(p, (int)n);
             const bool live = L.ok && !(src.bad && src.bad[n]);
             if (live && (int)t < L.Tn && (int)u < L.Un) {
-                g = cell_grads_ab(L, src, (int)t, (int)u, src.betas[L.base]);
+                g = cell_grads_ab(L, src, (int)t, (int)u, dead_b00(src.betas[L.base]));   // dead lattice: NaN
                 if (src.scale) { const float sc = src.scale[n]; g.x *= sc; g.y *= sc; }
                 if ((int)u < L.Un - 1) lab = src.labels[L.lab_base + u];
             }

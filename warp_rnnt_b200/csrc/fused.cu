@@ -42,7 +42,7 @@
 namespace rnnt {
 
 constexpr int kFusedThreads = 512;
-constexpr float kBigF = -1.0e30f;   // finite stand-in for -inf (see wavefront.cu)
+constexpr float kBigF = kBig;       // finite stand-in for -inf (see common.cuh, wavefront.cu)
 
 // L2 residency control (H100: 50 MB L2).  In the patch order the dense gradient slab is zero-filled while the
 // wavefront runs and patched afterwards; the patch is a partial-sector write, so it must still HIT
@@ -727,7 +727,11 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
         float cost = NAN;
         if (ok) {
             float b = BE[idxB(0, 0)];                   // beta[0,0]
-            if (A.guard) {
+            if (lattice_dead(b)) {
+                // no alignment of finite log-probability: the reference's class (common.cuh), no mismatch guard.
+                // (The layout is re-read from the argument: a flag kept live since phase 0 costs the recurrence a register.)
+                b = -dead_cost(Tn, Un, MODE == 1 && A.mem_pref != nullptr);
+            } else if (A.guard) {
                 // alpha-side ll = alpha[T-1,U-1] + blank[T-1,U-1] (core.cu:346); MODE 0: the chase has left exactly this sum
                 float a = (MODE == 0 && t0 <= T1 && T1 < t1) ? WBb[idxB(T1, U1)] : AL[idxA(T1, U1)] + WBb[idxB(T1, U1)];
                 if (n == A.poison_n) a += A.poison_delta;              // test hook, see rnnt_b200_debug_guard_poison
@@ -747,7 +751,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
     __syncthreads();
     stamp(10);
     const bool live = ok && !s_bad;
-    const float b00 = live ? BE[idxB(0, 0)] : 0.0f;
+    const float b00 = live ? dead_b00(BE[idxB(0, 0)]) : 0.0f;   // dead lattice: NaN, in every emit order and MODE 1
     const float sc = A.scale ? A.scale[n] : 1.0f;
     const bool has_lam = (A.lam != 0.0f);
     auto cell_grad = [&](int t, int u) -> float2 {

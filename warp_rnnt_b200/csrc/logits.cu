@@ -13,7 +13,8 @@
 //                    i.e. log_softmax's backward applied to the loss' (blank, label) gradient on the fly, times grad_out[n]
 //
 // three dense passes in total.  A label equal to blank: the two gradients add (what autograd through torch.gather /
-// log_softmax does).  Padded cells carry zero pair gradients and get exact zeros.
+// log_softmax does).  Padded cells carry zero pair gradients and get exact zeros (NaN where the row's normaliser is
+// NaN, as log_softmax's backward gives).
 #include "common.cuh"
 #include "kernels.cuh"
 
@@ -34,9 +35,13 @@ k_lse_pairs(const float *__restrict__ x, const int *__restrict__ labels, int64_t
         const int64_t cell = min(base + threadIdx.x / SUB, cells - 1);          // surplus groups redo the last cell (shuffles need every lane)
         const float *row = x + cell * V;
         float m = -INFINITY, s = 0.0f;
+        // The online sums below subtract the running max m, which stays -inf while every logit seen so far is -inf
+        // (a masked vocabulary entry): exp(-inf - (-inf)) would be NaN.  Until a finite logit arrives they subtract 0
+        // instead -- exp(-inf) = 0, and a NaN logit still makes the sum NaN; with a finite m nothing changes.
+        auto off = [&]() { return m == -INFINITY ? 0.0f : m; };
         auto add = [&](float a) {
-            if (a > m) { s = s * expf(m - a); m = a; }        // (m == -inf: s is 0, exp(-inf) = 0)
-            s += expf(a - m);
+            if (a > m) { s = s * expf(m - a); m = a; }        // (m == -inf: s is 0 or NaN, exp(-inf) = 0)
+            s += expf(a - off());
         };
         if (VEC4 && (V >> 2) <= SUB) {
             // the whole row is one float4 per lane: max first (shuffles only), then ONE exp per element -- the online
@@ -55,7 +60,8 @@ k_lse_pairs(const float *__restrict__ x, const int *__restrict__ labels, int64_t
                 const float4 a = __ldg(row4 + q);
                 const float mx = fmaxf(fmaxf(a.x, a.y), fmaxf(a.z, a.w));
                 if (mx > m) { s = s * expf(m - mx); m = mx; }
-                s += (expf(a.x - m) + expf(a.y - m)) + (expf(a.z - m) + expf(a.w - m));
+                const float mo = off();
+                s += (expf(a.x - mo) + expf(a.y - mo)) + (expf(a.z - mo) + expf(a.w - mo));
             }
         } else if (SUB == 1) {
             // short unaligned rows: one thread per cell; neighbouring threads' rows share cache lines, so the pass over
@@ -75,7 +81,8 @@ k_lse_pairs(const float *__restrict__ x, const int *__restrict__ labels, int64_t
             }
         }
         if (sub == 0) {
-            const float l = m + logf(s);
+            // every logit -inf: NaN, as torch.log_softmax gives (and as the max-first paths above compute it)
+            const float l = (m == -INFINITY) ? NAN : m + logf(s);
             uint32_t n, rem, t, u;
             divTU.divmod((uint32_t)cell, n, rem);
             divU.divmod(rem, t, u);
@@ -107,8 +114,11 @@ k_expand_logits(const float *__restrict__ x, const float *__restrict__ lse, cons
         const float2 q = pg[row];
         float e[VEC];
         if (q.x == 0.0f && q.y == 0.0f) {
+            // padding (or a cell without gradient): exact zeros -- (0 - softmax * 0), as log_softmax's backward gives,
+            // which is NaN when the row's normaliser is NaN (a NaN or +inf logit, or every logit -inf)
+            const float z = (lse[row] == lse[row]) ? 0.0f : NAN;
 #pragma unroll
-            for (int k = 0; k < VEC; ++k) e[k] = 0.0f;            // padding (or a dead cell): exact zeros
+            for (int k = 0; k < VEC; ++k) e[k] = z;
         } else {
             uint32_t n, rem, t, u;
             divTU.divmod((uint32_t)row, n, rem);

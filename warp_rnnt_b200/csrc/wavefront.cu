@@ -226,11 +226,14 @@ struct Sweep {
     bool col_ok, publish, backpressure, override0;
 };
 
-// "Minus infinity" that stays finite: cells outside the lattice carry kBig so that the one uniform
-// step below needs no per-lane control flow.  LSE(x, kBig) == x and LSE(kBig, kBig) == kBig (+ln 2,
-// absorbed) exactly, in every LSE flavour, and kBig + (any log-prob) stays ~kBig without ever
-// producing inf - inf.
-constexpr float kBig = -1.0e30f;
+// "Minus infinity" that stays finite: cells outside the lattice carry kBig (common.cuh) so that the one
+// uniform step below needs no per-lane control flow.  LSE(kBig, kBig) == kBig (+ln 2, absorbed) and
+// kBig + (a finite log-prob) stays ~kBig without ever producing inf - inf.  LSE(x, kBig) == x exactly, in
+// every LSE flavour, only while x is well above kBig: for x = -inf, or any x at or below about -1e30, the
+// sentinel wins and the result is ~kBig.  Row 0 of alpha and the last row of beta, which the reference
+// computes as plain sums, therefore hold ~kBig where the reference has -inf, and a lattice with no alignment
+// of finite log-probability ends with beta[0,0] ~ kBig (or NaN) instead of -inf / NaN.  The epilogue
+// (k_wavefront) and the gradient kernels map that to the reference's classes: lattice_dead, common.cuh.
 
 // One direction of one lattice.  "Primed" coordinates (i,j): alpha uses (t,u); beta uses
 // (Tn-1-t, Un-1-u), so both are the same recurrence
@@ -455,7 +458,11 @@ __global__ void __launch_bounds__(512, 1) k_wavefront(Problem p, const float2 *_
         int isbad = 0;
         if (L.ok) {
             float b = __ldcg(ws_ll + p.N + n);
-            if (!beta_only && guard) {
+            if (lattice_dead(b)) {
+                // no alignment of finite log-probability: the reference's class, and no mismatch guard (its ratio
+                // is NaN in the reference)
+                b = -dead_cost(L.Tn, L.Un, p.compact);
+            } else if (!beta_only && guard) {
                 // forward/backward mismatch guard, core.cu:346-367
                 float a = __ldcg(ws_ll + n);
                 if (n == poison.n) a += poison.delta;      // test hook, see rnnt_b200_debug_guard_poison
@@ -518,7 +525,7 @@ k_grads_pairs(Problem p, const float2 *__restrict__ pairs, const float *__restri
     const int64_t slab = p.compact ? L.base : (int64_t)n * p.T * p.U;
     const int stride = p.compact ? L.stride : p.U;
     const bool live = L.ok && !(bad && bad[n]);
-    const float b00 = live ? betas[L.base] : 0.0f;
+    const float b00 = live ? dead_b00(betas[L.base]) : 0.0f;   // dead lattice: NaN gradients
     for (int r = blockIdx.x * kGradThreads + threadIdx.x; r < total; r += gridDim.x * kGradThreads) {
         const int t = r / stride, u = r - t * stride;
         float2 g = make_float2(0.0f, 0.0f);
