@@ -304,6 +304,52 @@ static int loss_dense_any(void *stream, void *workspace, size_t workspace_bytes,
     return RNNT_STATUS_SUCCESS;
 }
 
+// loss from logits of 4-byte (f32) or 2-byte (bf16) elements: the normaliser pass reads them, the recurrence and
+// everything after it run on the f32 (cells,2) pairs and do not see the element type
+static int logits_forward_any(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                              const int *labels, const int *xn, const int *yn, float *costs, float *lse,
+                              float *pair_grads, int N, int T, int U, int V, int blank, float fastemit_lambda,
+                              int lse_mode, int io_bf16) {
+    if (!dense_args_ok(N, T, U, V) || blank < 0 || blank >= V || !lse) return RNNT_STATUS_INVALID_ARGUMENT;
+    if (reinterpret_cast<uintptr_t>(pair_grads) & 7u) return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    cudaStream_t s = (cudaStream_t)stream;
+    const int64_t cells = (int64_t)N * T * U;
+    const Workspace w = carve(workspace, cells, N);
+    if (!workspace || workspace_bytes < w.bytes) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    // one pass over the logits: normaliser per cell + the two normalised log-probs the recurrence needs
+    RNNT_TRY(launch_lse_pairs(s, logits, labels, N, T, U, V, blank, w.pairs, lse, io_bf16), RNNT_STATUS_GATHER_FAILED);
+    // the (cells,2) layout from here on: same kernels as rnnt_b200_loss_pairs
+    const int kind = resolve_kind(lse_mode, false);
+    FusedPlan plan;
+    if (want_fused(N, T, U, &plan)) {
+        RNNT_TRY(launch_fused(s, kind, plan, reinterpret_cast<const float *>(w.pairs), nullptr, xn, yn, costs, nullptr,
+                              reinterpret_cast<float2 *>(pair_grads), nullptr, N, T, U, 2, 0, fastemit_lambda, 1, 1),
+                 RNNT_STATUS_WARP_FAILED);
+        return RNNT_STATUS_SUCCESS;
+    }
+    Problem p = {xn, yn, nullptr, nullptr, N, T, U, 0};
+    RNNT_TRY(launch_wavefront(s, kind, p, w.pairs, w.alphas, w.betas, w.ll, w.bad, costs, pair_grads == nullptr, 1, T, U),
+             RNNT_STATUS_WARP_FAILED);
+    if (pair_grads)
+        RNNT_TRY(launch_grads_pairs(s, p, w.pairs, w.alphas, w.betas, w.bad, fastemit_lambda,
+                                    reinterpret_cast<float2 *>(pair_grads), cells),
+                 RNNT_STATUS_GRADS_BLANK_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+static int logits_backward_any(void *stream, const void *logits, const float *lse, const float *pair_grads,
+                               const int *labels, const float *grad_out, void *out, int N, int T, int U, int V,
+                               int blank, int io_bf16) {
+    if (!dense_args_ok(N, T, U, V) || blank < 0 || blank >= V) return RNNT_STATUS_INVALID_ARGUMENT;
+    if (reinterpret_cast<uintptr_t>(pair_grads) & 7u) return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    RNNT_TRY(launch_expand_logits((cudaStream_t)stream, logits, lse, reinterpret_cast<const float2 *>(pair_grads), labels,
+                                  grad_out, out, N, T, U, V, blank, io_bf16),
+             RNNT_STATUS_GRADS_BLANK_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
 
 extern "C" {
 
@@ -443,44 +489,31 @@ int rnnt_b200_logits_forward(void *stream, void *workspace, size_t workspace_byt
                               const int *labels, const int *xn, const int *yn, float *costs, float *lse,
                               float *pair_grads, int N, int T, int U, int V, int blank, float fastemit_lambda,
                               int lse_mode) {
-    if (!dense_args_ok(N, T, U, V) || blank < 0 || blank >= V || !lse) return RNNT_STATUS_INVALID_ARGUMENT;
-    if (reinterpret_cast<uintptr_t>(pair_grads) & 7u) return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0) return RNNT_STATUS_SUCCESS;
-    cudaStream_t s = (cudaStream_t)stream;
-    const int64_t cells = (int64_t)N * T * U;
-    const Workspace w = carve(workspace, cells, N);
-    if (!workspace || workspace_bytes < w.bytes) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
-    // one pass over the logits: normaliser per cell + the two normalised log-probs the recurrence needs
-    RNNT_TRY(launch_lse_pairs(s, logits, labels, N, T, U, V, blank, w.pairs, lse), RNNT_STATUS_GATHER_FAILED);
-    // the (cells,2) layout from here on: same kernels as rnnt_b200_loss_pairs
-    const int kind = resolve_kind(lse_mode, false);
-    FusedPlan plan;
-    if (want_fused(N, T, U, &plan)) {
-        RNNT_TRY(launch_fused(s, kind, plan, reinterpret_cast<const float *>(w.pairs), nullptr, xn, yn, costs, nullptr,
-                              reinterpret_cast<float2 *>(pair_grads), nullptr, N, T, U, 2, 0, fastemit_lambda, 1, 1),
-                 RNNT_STATUS_WARP_FAILED);
-        return RNNT_STATUS_SUCCESS;
-    }
-    Problem p = {xn, yn, nullptr, nullptr, N, T, U, 0};
-    RNNT_TRY(launch_wavefront(s, kind, p, w.pairs, w.alphas, w.betas, w.ll, w.bad, costs, pair_grads == nullptr, 1, T, U),
-             RNNT_STATUS_WARP_FAILED);
-    if (pair_grads)
-        RNNT_TRY(launch_grads_pairs(s, p, w.pairs, w.alphas, w.betas, w.bad, fastemit_lambda,
-                                    reinterpret_cast<float2 *>(pair_grads), cells),
-                 RNNT_STATUS_GRADS_BLANK_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    return logits_forward_any(stream, workspace, workspace_bytes, logits, labels, xn, yn, costs, lse, pair_grads, N, T,
+                              U, V, blank, fastemit_lambda, lse_mode, 0);
 }
 
 int rnnt_b200_logits_backward(void *stream, const float *logits, const float *lse, const float *pair_grads,
                               const int *labels, const float *grad_out, float *out, int N, int T, int U, int V,
                               int blank) {
-    if (!dense_args_ok(N, T, U, V) || blank < 0 || blank >= V) return RNNT_STATUS_INVALID_ARGUMENT;
-    if (reinterpret_cast<uintptr_t>(pair_grads) & 7u) return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0) return RNNT_STATUS_SUCCESS;
-    RNNT_TRY(launch_expand_logits((cudaStream_t)stream, logits, lse, reinterpret_cast<const float2 *>(pair_grads), labels,
-                                  grad_out, out, N, T, U, V, blank),
-             RNNT_STATUS_GRADS_BLANK_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    return logits_backward_any(stream, logits, lse, pair_grads, labels, grad_out, out, N, T, U, V, blank, 0);
+}
+
+int rnnt_b200_logits_forward_bf16(void *stream, void *workspace, size_t workspace_bytes, const void *logits_bf16,
+                                  const int *labels, const int *xn, const int *yn, float *costs, float *lse,
+                                  float *pair_grads, int N, int T, int U, int V, int blank, float fastemit_lambda,
+                                  int lse_mode) {
+    if (reinterpret_cast<uintptr_t>(logits_bf16) & 1u) return RNNT_STATUS_INVALID_ARGUMENT;
+    return logits_forward_any(stream, workspace, workspace_bytes, logits_bf16, labels, xn, yn, costs, lse, pair_grads,
+                              N, T, U, V, blank, fastemit_lambda, lse_mode, 1);
+}
+
+int rnnt_b200_logits_backward_bf16(void *stream, const void *logits_bf16, const float *lse, const float *pair_grads,
+                                   const int *labels, const float *grad_out, void *out_bf16, int N, int T, int U, int V,
+                                   int blank) {
+    if ((reinterpret_cast<uintptr_t>(logits_bf16) | reinterpret_cast<uintptr_t>(out_bf16)) & 1u)
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    return logits_backward_any(stream, logits_bf16, lse, pair_grads, labels, grad_out, out_bf16, N, T, U, V, blank, 1);
 }
 
 int rnnt_b200_gather_backward(void *stream, const float *pair_grads, const int *labels, const float *grad_out,

@@ -15,6 +15,12 @@
 // three dense passes in total.  A label equal to blank: the two gradients add (what autograd through torch.gather /
 // log_softmax does).  Padded cells carry zero pair gradients and get exact zeros (NaN where the row's normaliser is
 // NaN, as log_softmax's backward gives).
+//
+// Both dense kernels take float or bf16 logits (SURVEY.md 8(f)2); the bf16 gradient is bf16 too.  Everything between
+// the load and the store is fp32 and the same for both types: k_lse_pairs sums a bf16 row in the order it sums the
+// float row of the same V (same SUB, same lanes, same groups of 4 -- a bf16 group is one 8-byte load where a float
+// group is a float4), so lse and pairs are bit for bit those of the float path on the widened logits; k_expand_logits
+// computes every element as the float kernel does and rounds it to bf16 once, on the store.
 #include "common.cuh"
 #include "kernels.cuh"
 
@@ -22,18 +28,27 @@ namespace rnnt {
 
 constexpr int kLogitThreads = 256;
 
+// group q of 4 consecutive logits of a row whose groups are aligned (4 * sizeof(IN) bytes)
+__device__ __forceinline__ float4 ld_group4(const float *row, int q) { return __ldg(reinterpret_cast<const float4 *>(row) + q); }
+__device__ __forceinline__ float4 ld_group4(const __nv_bfloat16 *row, int q) {
+    const uint2 r = __ldg(reinterpret_cast<const uint2 *>(row) + q);
+    return make_float4(__uint_as_float(r.x << 16), __uint_as_float(r.x & 0xffff0000u), __uint_as_float(r.y << 16),
+                       __uint_as_float(r.y & 0xffff0000u));
+}
+
 // SUB lanes cooperate on one cell (SUB in {1, 8, 32}); online max / sum so the row is read once.  VEC4: rows are whole
-// float4s at 16-byte aligned addresses -> the SUB lanes stride over float4s (V = 28: 7 of 8 lanes load one vector each,
-// a warp reads 4 consecutive rows = 448 contiguous bytes).
-template <int SUB, bool VEC4>
+// groups of 4 at group-aligned addresses -> the SUB lanes stride over groups (float V = 28: 7 of 8 lanes load one float4
+// each, a warp reads 4 consecutive rows = 448 contiguous bytes).  The choice of SUB and VEC4 depends on V and the
+// alignment only, never on IN: a bf16 row is summed exactly like the float row of the same values.
+template <typename IN, int SUB, bool VEC4>
 __global__ void __launch_bounds__(kLogitThreads)
-k_lse_pairs(const float *__restrict__ x, const int *__restrict__ labels, int64_t cells, int V, int blank, int U,
+k_lse_pairs(const IN *__restrict__ x, const int *__restrict__ labels, int64_t cells, int V, int blank, int U,
             FastDiv divU, FastDiv divTU, float2 *__restrict__ pairs, float *__restrict__ lse_out) {
     const int sub = threadIdx.x % SUB;
     const int64_t per_block = kLogitThreads / SUB;
     for (int64_t base = (int64_t)blockIdx.x * per_block; base < cells; base += (int64_t)gridDim.x * per_block) {   // block-uniform trip count
         const int64_t cell = min(base + threadIdx.x / SUB, cells - 1);          // surplus groups redo the last cell (shuffles need every lane)
-        const float *row = x + cell * V;
+        const IN *row = x + cell * V;
         float m = -INFINITY, s = 0.0f;
         // The online sums below subtract the running max m, which stays -inf while every logit seen so far is -inf
         // (a masked vocabulary entry): exp(-inf - (-inf)) would be NaN.  Until a finite logit arrives they subtract 0
@@ -44,10 +59,10 @@ k_lse_pairs(const float *__restrict__ x, const int *__restrict__ labels, int64_t
             s += expf(a - off());
         };
         if (VEC4 && (V >> 2) <= SUB) {
-            // the whole row is one float4 per lane: max first (shuffles only), then ONE exp per element -- the online
+            // the whole row is one group per lane: max first (shuffles only), then ONE exp per element -- the online
             // merge below would spend two more exp per lane and shuffle round
             const bool has = sub < (V >> 2);
-            const float4 a = has ? __ldg(reinterpret_cast<const float4 *>(row) + sub) : make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
+            const float4 a = has ? ld_group4(row, sub) : make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
             m = fmaxf(fmaxf(a.x, a.y), fmaxf(a.z, a.w));
 #pragma unroll
             for (int o = SUB / 2; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
@@ -55,9 +70,8 @@ k_lse_pairs(const float *__restrict__ x, const int *__restrict__ labels, int64_t
 #pragma unroll
             for (int o = SUB / 2; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
         } else if (VEC4) {
-            const float4 *row4 = reinterpret_cast<const float4 *>(row);
             for (int q = sub; q < (V >> 2); q += SUB) {
-                const float4 a = __ldg(row4 + q);
+                const float4 a = ld_group4(row, q);
                 const float mx = fmaxf(fmaxf(a.x, a.y), fmaxf(a.z, a.w));
                 if (mx > m) { s = s * expf(m - mx); m = mx; }
                 const float mo = off();
@@ -66,10 +80,10 @@ k_lse_pairs(const float *__restrict__ x, const int *__restrict__ labels, int64_t
         } else if (SUB == 1) {
             // short unaligned rows: one thread per cell; neighbouring threads' rows share cache lines, so the pass over
             // v is served from L1 after the first touch
-            for (int v = 0; v < V; ++v) m = fmaxf(m, __ldg(row + v));
-            for (int v = 0; v < V; ++v) s += expf(__ldg(row + v) - m);
+            for (int v = 0; v < V; ++v) m = fmaxf(m, io_load(row + v));
+            for (int v = 0; v < V; ++v) s += expf(io_load(row + v) - m);
         } else {
-            for (int v = sub; v < V; v += SUB) add(__ldg(row + v));
+            for (int v = sub; v < V; v += SUB) add(io_load(row + v));
         }
         if (SUB > 1 && !(VEC4 && (V >> 2) <= SUB)) {
 #pragma unroll
@@ -87,25 +101,89 @@ k_lse_pairs(const float *__restrict__ x, const int *__restrict__ labels, int64_t
             divTU.divmod((uint32_t)cell, n, rem);
             divU.divmod(rem, t, u);
             const int lab = ((int)u < U - 1) ? labels[(int64_t)n * (U - 1) + u] : blank;
-            pairs[cell] = make_float2(__ldg(row + blank) - l, __ldg(row + lab) - l);
+            pairs[cell] = make_float2(io_load(row + blank) - l, io_load(row + lab) - l);
             lse_out[cell] = l;
         }
     }
 }
 
-// flat stream of the (cells, V) output in vectors of VEC floats (VEC = 4 when V % 4 == 0, 2 when V % 2 == 0, else 1):
-// a vector never straddles a row, so one (gb, gl, lse, label) fetch serves it.
+// VEC consecutive elements at p (VEC * sizeof(T) bytes, aligned to that) <-> fp32
 template <int VEC>
+__device__ __forceinline__ void ld_logits(const float *p, float (&v)[VEC]) {
+    if constexpr (VEC == 4) {
+        const float4 t4 = __ldg(reinterpret_cast<const float4 *>(p));
+        v[0] = t4.x; v[1] = t4.y; v[2] = t4.z; v[3] = t4.w;
+    } else if constexpr (VEC == 2) {
+        const float2 t2 = __ldg(reinterpret_cast<const float2 *>(p));
+        v[0] = t2.x; v[1] = t2.y;
+    } else {
+        v[0] = __ldg(p);
+    }
+}
+template <int VEC>
+__device__ __forceinline__ void ld_logits(const __nv_bfloat16 *p, float (&v)[VEC]) {
+    if constexpr (VEC == 1) {
+        v[0] = io_load(p);
+    } else {
+        uint32_t w[VEC / 2];                                 // element 2k in the low half of word k
+        if constexpr (VEC == 8) {
+            const uint4 t = __ldg(reinterpret_cast<const uint4 *>(p));
+            w[0] = t.x; w[1] = t.y; w[2] = t.z; w[3] = t.w;
+        } else if constexpr (VEC == 4) {
+            const uint2 t = __ldg(reinterpret_cast<const uint2 *>(p));
+            w[0] = t.x; w[1] = t.y;
+        } else {
+            w[0] = __ldg(reinterpret_cast<const unsigned int *>(p));
+        }
+#pragma unroll
+        for (int k = 0; k < VEC / 2; ++k) {
+            v[2 * k] = __uint_as_float(w[k] << 16);
+            v[2 * k + 1] = __uint_as_float(w[k] & 0xffff0000u);
+        }
+    }
+}
+template <int VEC>
+__device__ __forceinline__ void st_logit_grads(float *p, const float (&e)[VEC]) {
+    if constexpr (VEC == 4) st_cs_v4(p, make_float4(e[0], e[1], e[2], e[3]));
+    else if constexpr (VEC == 2) st_cs_v2(p, make_float2(e[0], e[1]));
+    else st_cs(p, e[0]);
+}
+// bf16: every element rounded once (round to nearest even), streaming stores of the vector's width
+template <int VEC>
+__device__ __forceinline__ void st_logit_grads(__nv_bfloat16 *p, const float (&e)[VEC]) {
+    if constexpr (VEC == 8) {
+        st_vec(p, e);
+    } else if constexpr (VEC == 1) {
+        const unsigned short h = __bfloat16_as_ushort(__float2bfloat16_rn(e[0]));
+        asm volatile("st.global.cs.b16 [%0], %1;" ::"l"(p), "h"(h) : "memory");
+    } else {
+        uint32_t w[VEC / 2];
+#pragma unroll
+        for (int k = 0; k < VEC / 2; ++k) {
+            const __nv_bfloat162 h = __floats2bfloat162_rn(e[2 * k], e[2 * k + 1]);
+            w[k] = *reinterpret_cast<const uint32_t *>(&h);
+        }
+        if constexpr (VEC == 4)
+            asm volatile("st.global.cs.v2.b32 [%0], {%1, %2};" ::"l"(p), "r"(w[0]), "r"(w[1]) : "memory");
+        else
+            asm volatile("st.global.cs.b32 [%0], %1;" ::"l"(p), "r"(w[0]) : "memory");
+    }
+}
+
+// flat stream of the (cells, V) output in vectors of VEC elements (float: 4 when V % 4 == 0, 2 when V % 2 == 0, else
+// 1; bf16 also 8): a vector never straddles a row, so one (gb, gl, lse, label) fetch serves it.  IO is the element
+// type of the logits and of the gradient.
+template <typename IO, int VEC>
 __global__ void __launch_bounds__(kLogitThreads)
-k_expand_logits(const float *__restrict__ x, const float *__restrict__ lse, const float2 *__restrict__ pg,
-                const int *__restrict__ labels, const float *__restrict__ grad_out, float *__restrict__ out,
+k_expand_logits(const IO *__restrict__ x, const float *__restrict__ lse, const float2 *__restrict__ pg,
+                const int *__restrict__ labels, const float *__restrict__ grad_out, IO *__restrict__ out,
                 int64_t cells, int V, int blank, int U, FastDiv divU, FastDiv divTU, int64_t stride_rows,
                 int stride_v) {
     const int64_t total = cells * (int64_t)V;
     int64_t f = ((int64_t)blockIdx.x * kLogitThreads + threadIdx.x) * VEC;
     if (f >= total) return;
     // (row, v0) of the thread's vector: one 64-bit division here, then a running cursor (the grid stride is
-    // stride_rows whole rows + stride_v floats)
+    // stride_rows whole rows + stride_v elements)
     int64_t row = f / V;
     int v0 = (int)(f - row * V);
     const int64_t stride = stride_rows * V + stride_v;
@@ -127,15 +205,7 @@ k_expand_logits(const float *__restrict__ x, const float *__restrict__ lse, cons
             const float sc = grad_out ? grad_out[n] : 1.0f;
             const float l = lse[row], tot = q.x + q.y;
             float xv[VEC];
-            if (VEC == 4) {
-                const float4 t4 = __ldg(reinterpret_cast<const float4 *>(x + f));
-                xv[0] = t4.x; xv[1] = t4.y; xv[2 % VEC] = t4.z; xv[3 % VEC] = t4.w;
-            } else if (VEC == 2) {
-                const float2 t2 = __ldg(reinterpret_cast<const float2 *>(x + f));
-                xv[0] = t2.x; xv[1 % VEC] = t2.y;
-            } else {
-                xv[0] = __ldg(x + f);
-            }
+            ld_logits<VEC>(x + f, xv);
 #pragma unroll
             for (int k = 0; k < VEC; ++k) {
                 float gsel = (v0 + k == blank) ? q.x : 0.0f;
@@ -143,23 +213,23 @@ k_expand_logits(const float *__restrict__ x, const float *__restrict__ lse, cons
                 e[k] = (gsel - expf(xv[k] - l) * tot) * sc;
             }
         }
-        if (VEC == 4) st_cs_v4(out + f, make_float4(e[0], e[1 % VEC], e[2 % VEC], e[3 % VEC]));
-        else if (VEC == 2) st_cs_v2(out + f, make_float2(e[0], e[1 % VEC]));
-        else st_cs(out + f, e[0]);
+        st_logit_grads<VEC>(out + f, e);
     }
 }
 
-cudaError_t launch_lse_pairs(cudaStream_t s, const float *x, const int *labels, int N, int T, int U, int V, int blank,
-                             float2 *pairs, float *lse) {
+template <typename IN>
+static cudaError_t lse_pairs_as(cudaStream_t s, const IN *x, const int *labels, int N, int T, int U, int V, int blank,
+                                float2 *pairs, float *lse) {
     const int64_t cells = (int64_t)N * T * U;
     if (cells <= 0) return cudaSuccess;
     const FastDiv divU((uint32_t)U), divTU((uint32_t)(T * U));
     const int sms = sm_count(current_device());
-    const bool vec4 = (V % 4 == 0) && ((reinterpret_cast<uintptr_t>(x) & 15u) == 0);
+    // groups of 4 elements: float4 (16 bytes) or 4 bf16 (8 bytes) per load
+    const bool vec4 = (V % 4 == 0) && ((reinterpret_cast<uintptr_t>(x) & (4 * sizeof(IN) - 1)) == 0);
     const int sub = vec4 ? (V <= 32 ? 8 : 32) : (V <= 12 ? 1 : (V <= 512 ? 8 : 32));
     const int64_t per_block = kLogitThreads / sub;
     const int grid = (int)min((cells + per_block - 1) / per_block, (int64_t)sms * 16);
-#define RNNT_LSE_LAUNCH(SUB, VEC) k_lse_pairs<SUB, VEC><<<grid, kLogitThreads, 0, s>>>(x, labels, cells, V, blank, U, divU, divTU, pairs, lse)
+#define RNNT_LSE_LAUNCH(SUB, VEC) k_lse_pairs<IN, SUB, VEC><<<grid, kLogitThreads, 0, s>>>(x, labels, cells, V, blank, U, divU, divTU, pairs, lse)
     if (vec4) { if (sub == 8) RNNT_LSE_LAUNCH(8, true); else RNNT_LSE_LAUNCH(32, true); }
     else if (sub == 1) RNNT_LSE_LAUNCH(1, false);
     else if (sub == 8) RNNT_LSE_LAUNCH(8, false);
@@ -169,25 +239,53 @@ cudaError_t launch_lse_pairs(cudaStream_t s, const float *x, const int *labels, 
     return cudaGetLastError();
 }
 
-cudaError_t launch_expand_logits(cudaStream_t s, const float *x, const float *lse, const float2 *pg, const int *labels,
-                                 const float *grad_out, float *out, int N, int T, int U, int V, int blank) {
+cudaError_t launch_lse_pairs(cudaStream_t s, const void *x, const int *labels, int N, int T, int U, int V, int blank,
+                             float2 *pairs, float *lse, int io_bf16) {
+    if (io_bf16) return lse_pairs_as(s, static_cast<const __nv_bfloat16 *>(x), labels, N, T, U, V, blank, pairs, lse);
+    return lse_pairs_as(s, static_cast<const float *>(x), labels, N, T, U, V, blank, pairs, lse);
+}
+
+template <typename IO>
+static cudaError_t expand_logits_as(cudaStream_t s, const IO *x, const float *lse, const float2 *pg, const int *labels,
+                                    const float *grad_out, IO *out, int N, int T, int U, int V, int blank) {
     const int64_t cells = (int64_t)N * T * U;
     if (cells <= 0) return cudaSuccess;
     const FastDiv divU((uint32_t)U), divTU((uint32_t)(T * U));
     const int sms = sm_count(current_device());
-    const bool al16 = ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out)) & 15u) == 0;
-    const bool al8 = ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out)) & 7u) == 0;
-    const int vec = (V % 4 == 0 && al16) ? 4 : ((V % 2 == 0 && al8) ? 2 : 1);
+    // the widest vector (at most 16 bytes) that V and the alignment of both tensors allow
+    const uintptr_t al = reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out);
+    const int vmax = 16 / (int)sizeof(IO);
+    int vec = 1;
+    for (int c = vmax; c > 1; c >>= 1)
+        if (V % c == 0 && (al & (c * sizeof(IO) - 1)) == 0) { vec = c; break; }
     const int64_t total = cells * (int64_t)V / vec;
     const int grid = (int)min((total + kLogitThreads - 1) / kLogitThreads, (int64_t)sms * 32);
     const int64_t stride = (int64_t)grid * kLogitThreads * vec;
     const int64_t srows = stride / V;
     const int sv = (int)(stride - srows * V);
-    if (vec == 4) k_expand_logits<4><<<grid, kLogitThreads, 0, s>>>(x, lse, pg, labels, grad_out, out, cells, V, blank, U, divU, divTU, srows, sv);
-    else if (vec == 2) k_expand_logits<2><<<grid, kLogitThreads, 0, s>>>(x, lse, pg, labels, grad_out, out, cells, V, blank, U, divU, divTU, srows, sv);
-    else k_expand_logits<1><<<grid, kLogitThreads, 0, s>>>(x, lse, pg, labels, grad_out, out, cells, V, blank, U, divU, divTU, srows, sv);
+#define RNNT_EXPAND_LAUNCH(VEC) k_expand_logits<IO, VEC><<<grid, kLogitThreads, 0, s>>>(x, lse, pg, labels, grad_out, out, cells, V, blank, U, divU, divTU, srows, sv)
+    if constexpr (sizeof(IO) == 2) {
+        if (vec == 8) RNNT_EXPAND_LAUNCH(8);
+        else if (vec == 4) RNNT_EXPAND_LAUNCH(4);
+        else if (vec == 2) RNNT_EXPAND_LAUNCH(2);
+        else RNNT_EXPAND_LAUNCH(1);
+    } else {
+        if (vec == 4) RNNT_EXPAND_LAUNCH(4);
+        else if (vec == 2) RNNT_EXPAND_LAUNCH(2);
+        else RNNT_EXPAND_LAUNCH(1);
+    }
+#undef RNNT_EXPAND_LAUNCH
     count_launch();
     return cudaGetLastError();
+}
+
+cudaError_t launch_expand_logits(cudaStream_t s, const void *x, const float *lse, const float2 *pg, const int *labels,
+                                 const float *grad_out, void *out, int N, int T, int U, int V, int blank, int io_bf16) {
+    if (io_bf16)
+        return expand_logits_as(s, static_cast<const __nv_bfloat16 *>(x), lse, pg, labels, grad_out,
+                                static_cast<__nv_bfloat16 *>(out), N, T, U, V, blank);
+    return expand_logits_as(s, static_cast<const float *>(x), lse, pg, labels, grad_out, static_cast<float *>(out), N, T,
+                            U, V, blank);
 }
 
 }  // namespace rnnt
