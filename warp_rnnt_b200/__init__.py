@@ -160,8 +160,33 @@ class RNNTLossFromLogits(torch.autograd.Function):
         return _C.rnnt_logits_backward(logits, lse, pg, labels, go, ctx.blank), None, None, None, None, None
 
 
+class RNNTLossFromLogitsCompact(torch.autograd.Function):
+    """``RNNTLossFromLogits`` on compact (STU,V) logits in ``joint_pack``'s row order: a packed joint network feeds
+    the fused loss without padding.  Forward keeps lse (4 bytes per row), the (STU,2) pair gradients (8 bytes per row)
+    and the compact prefix sums (16 bytes per lattice); backward writes d loss / d logits, of the logits' dtype.  Inside
+    ``compact_hints`` the forward has no host sync (CUDA-graph capturable), as ``rnnt_loss(compact=True)``."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, frames_lengths, labels_lengths, blank=0, fastemit_lambda=0.0):
+        need = ctx.needs_input_grad[0]
+        hints = getattr(_tls, "hints", None) or (0, 0)
+        costs, lse, pg, prefix = _C.rnnt_logits_compact_forward(logits, labels, frames_lengths, labels_lengths, blank,
+                                                                fastemit_lambda, need, 0, hints[0], hints[1])
+        if need:
+            ctx.save_for_backward(logits, lse, pg, labels, frames_lengths, labels_lengths, prefix)
+            ctx.blank = blank
+        return costs
+
+    @staticmethod
+    def backward(ctx, grads_output):
+        logits, lse, pg, labels, xn, yn, prefix = ctx.saved_tensors
+        go = grads_output.contiguous().to(torch.float32)
+        g = _C.rnnt_logits_compact_backward(logits, lse, pg, labels, xn, yn, prefix, go, ctx.blank)
+        return g, None, None, None, None, None
+
+
 def rnnt_loss_from_logits(logits, labels, frames_lengths, labels_lengths, average_frames=False, reduction="none",
-                          blank=0, fastemit_lambda=0.0):
+                          blank=0, fastemit_lambda=0.0, compact=False):
     """``rnnt_loss(log_softmax(logits, -1), ...)`` in three dense passes instead of seven; the gradient is w.r.t. the
     LOGITS.  Dense (N,T,U,V) layout, float32 or bfloat16 (what ``torch.autocast(dtype=torch.bfloat16)`` makes of the
     joint network's output); other arguments as in ``rnnt_loss``.  Agrees with ``torch.log_softmax`` + the reference
@@ -169,12 +194,19 @@ def rnnt_loss_from_logits(logits, labels, frames_lengths, labels_lengths, averag
 
     bfloat16 logits: costs and the loss are float32, ``logits.grad`` is bfloat16, all arithmetic is float32.  The costs
     equal those of float32 logits with the same values bit for bit, and the gradient is their float32 gradient rounded
-    to bfloat16 once (logits at 8-byte aligned addresses, as torch allocates them; include/rnnt_b200.h)."""
+    to bfloat16 once (logits at 8-byte aligned addresses, as torch allocates them; include/rnnt_b200.h).
+
+    ``compact=True``: ``logits`` is (STU, V), float32 or bfloat16, rows in ``joint_pack``'s order
+    (STU = sum frames_lengths * (labels_lengths + 1)); ``labels`` is (sum labels_lengths,) int32, as for
+    ``rnnt_loss(compact=True)``, and so are the shape checks and ``compact_hints``.  Costs are float32, the gradient is
+    w.r.t. the packed logits and has their dtype."""
     assert average_frames is None or isinstance(average_frames, bool)
     assert reduction is None or reduction in ("none", "mean", "sum")
     assert isinstance(blank, int)
+    assert isinstance(compact, bool)
     assert not labels.requires_grad and not frames_lengths.requires_grad and not labels_lengths.requires_grad
-    costs = RNNTLossFromLogits.apply(logits, labels, frames_lengths, labels_lengths, blank, fastemit_lambda)
+    fn = RNNTLossFromLogitsCompact if compact else RNNTLossFromLogits
+    costs = fn.apply(logits, labels, frames_lengths, labels_lengths, blank, fastemit_lambda)
     if average_frames:
         costs = costs / frames_lengths.to(costs.dtype)      # float32: bf16 would round frame counts (601 -> 600)
     if reduction == "sum":
@@ -334,5 +366,6 @@ def rnnt_loss(log_probs, labels, frames_lengths, labels_lengths, average_frames=
             f"Unknown reduction method: {reduction}, expected to be one of ['mean', 'sum', 'none']")
 
 
-__all__ = ["rnnt_loss", "rnnt_loss_from_logits", "joint_pack", "JointPack", "RNNTLossFromLogits", "RNNTLoss", "RNNTLossGather", "RNNTLossEager", "RNNTLossCompact", "compact_hints", "set_lse_mode", "core", "_C",
+__all__ = ["rnnt_loss", "rnnt_loss_from_logits", "joint_pack", "JointPack", "RNNTLossFromLogits",
+           "RNNTLossFromLogitsCompact", "RNNTLoss", "RNNTLossGather", "RNNTLossEager", "RNNTLossCompact", "compact_hints", "set_lse_mode", "core", "_C",
            "__version__"]

@@ -350,6 +350,58 @@ static int logits_backward_any(void *stream, const void *logits, const float *ls
     return RNNT_STATUS_SUCCESS;
 }
 
+// compact (STU,V) logits in joint_pack's row order: the normaliser pass over the ragged rows, then the recurrence of
+// rnnt_b200_compact_forward on the (STU,2) pairs -- the fused kernel reading pairs (no gather) when the hints admit it,
+// else the general wavefront -- without the mismatch guard, as the compact layout has none
+static int logits_compact_forward_any(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                      const int *ys, const int *xn, const int *yn, float *costs, float *lse,
+                                      float *pair_grads, int64_t *prefix, int *totals, int64_t STU, int N, int V,
+                                      int blank, float fastemit_lambda, int lse_mode, int max_T, int max_U,
+                                      int io_bf16) {
+    if (N < 0 || STU < 0 || V < 1 || V >= (1 << 22) || blank < 0 || blank >= V || !lse || !prefix)
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (reinterpret_cast<uintptr_t>(pair_grads) & 7u) return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    cudaStream_t s = (cudaStream_t)stream;
+    const Workspace w = carve(workspace, STU, N);
+    if (!workspace || workspace_bytes < w.bytes) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    int64_t *mem_pref = prefix, *lab_pref = prefix + N;
+    RNNT_TRY(launch_prefix(s, xn, yn, N, mem_pref, lab_pref, totals ? totals : w.totals), RNNT_STATUS_GATHER_FAILED);
+    const Problem p = {xn, yn, mem_pref, lab_pref, N, 0, 0, 1};
+    RNNT_TRY(launch_lse_pairs_compact(s, logits, p, ys, STU, V, blank, w.pairs, lse, io_bf16), RNNT_STATUS_GATHER_FAILED);
+    const int kind = resolve_kind(lse_mode, true);
+    FusedPlan fplan;
+    if (max_T > 0 && max_U > 0 && want_fused(N, max_T, max_U, &fplan)) {
+        RNNT_TRY(launch_fused(s, kind, fplan, reinterpret_cast<const float *>(w.pairs), nullptr, xn, yn, costs, nullptr,
+                              reinterpret_cast<float2 *>(pair_grads), nullptr, N, max_T, max_U, 2, 0, fastemit_lambda,
+                              1, 0, mem_pref, lab_pref, nullptr),
+                 RNNT_STATUS_WARP_FAILED);
+        return RNNT_STATUS_SUCCESS;
+    }
+    RNNT_TRY(launch_wavefront(s, kind, p, w.pairs, w.alphas, w.betas, w.ll, w.bad, costs, pair_grads == nullptr, 0,
+                              max_T, max_U),
+             RNNT_STATUS_WARP_FAILED);
+    if (pair_grads)
+        RNNT_TRY(launch_grads_pairs(s, p, w.pairs, w.alphas, w.betas, nullptr, fastemit_lambda,
+                                    reinterpret_cast<float2 *>(pair_grads), STU),
+                 RNNT_STATUS_GRADS_BLANK_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+static int logits_compact_backward_any(void *stream, const void *logits, const float *lse, const float *pair_grads,
+                                       const int *ys, const int *xn, const int *yn, const int64_t *prefix,
+                                       const float *grad_out, void *out, int64_t STU, int N, int V, int blank,
+                                       int io_bf16) {
+    if (N < 0 || STU < 0 || V < 1 || V >= (1 << 22) || blank < 0 || blank >= V || !lse || !prefix)
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (reinterpret_cast<uintptr_t>(pair_grads) & 7u) return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0 || STU == 0) return RNNT_STATUS_SUCCESS;
+    const Problem p = {xn, yn, prefix, prefix + N, N, 0, 0, 1};
+    RNNT_TRY(launch_expand_logits_compact((cudaStream_t)stream, logits, lse, reinterpret_cast<const float2 *>(pair_grads),
+                                          p, ys, grad_out, out, STU, V, blank, io_bf16),
+             RNNT_STATUS_GRADS_BLANK_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
 
 extern "C" {
 
@@ -564,6 +616,42 @@ int rnnt_b200_compact_forward(void *stream, void *workspace, size_t workspace_by
                                     reinterpret_cast<float2 *>(pair_grads), STU),
                  RNNT_STATUS_GRADS_BLANK_FAILED);
     return RNNT_STATUS_SUCCESS;
+}
+
+int rnnt_b200_logits_compact_forward(void *stream, void *workspace, size_t workspace_bytes, const float *logits,
+                                     const int *ys, const int *xn, const int *yn, float *costs, float *lse,
+                                     float *pair_grads, int64_t *prefix, int *totals, int64_t STU, int N, int V,
+                                     int blank, float fastemit_lambda, int lse_mode, int max_T, int max_U) {
+    return logits_compact_forward_any(stream, workspace, workspace_bytes, logits, ys, xn, yn, costs, lse, pair_grads,
+                                      prefix, totals, STU, N, V, blank, fastemit_lambda, lse_mode, max_T, max_U, 0);
+}
+
+int rnnt_b200_logits_compact_forward_bf16(void *stream, void *workspace, size_t workspace_bytes,
+                                          const void *logits_bf16, const int *ys, const int *xn, const int *yn,
+                                          float *costs, float *lse, float *pair_grads, int64_t *prefix, int *totals,
+                                          int64_t STU, int N, int V, int blank, float fastemit_lambda, int lse_mode,
+                                          int max_T, int max_U) {
+    if (reinterpret_cast<uintptr_t>(logits_bf16) & 1u) return RNNT_STATUS_INVALID_ARGUMENT;
+    return logits_compact_forward_any(stream, workspace, workspace_bytes, logits_bf16, ys, xn, yn, costs, lse,
+                                      pair_grads, prefix, totals, STU, N, V, blank, fastemit_lambda, lse_mode, max_T,
+                                      max_U, 1);
+}
+
+int rnnt_b200_logits_compact_backward(void *stream, const float *logits, const float *lse, const float *pair_grads,
+                                      const int *ys, const int *xn, const int *yn, const int64_t *prefix,
+                                      const float *grad_out, float *out, int64_t STU, int N, int V, int blank) {
+    return logits_compact_backward_any(stream, logits, lse, pair_grads, ys, xn, yn, prefix, grad_out, out, STU, N, V,
+                                       blank, 0);
+}
+
+int rnnt_b200_logits_compact_backward_bf16(void *stream, const void *logits_bf16, const float *lse,
+                                           const float *pair_grads, const int *ys, const int *xn, const int *yn,
+                                           const int64_t *prefix, const float *grad_out, void *out_bf16, int64_t STU,
+                                           int N, int V, int blank) {
+    if ((reinterpret_cast<uintptr_t>(logits_bf16) | reinterpret_cast<uintptr_t>(out_bf16)) & 1u)
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    return logits_compact_backward_any(stream, logits_bf16, lse, pair_grads, ys, xn, yn, prefix, grad_out, out_bf16,
+                                       STU, N, V, blank, 1);
 }
 
 int rnnt_b200_compact_totals(void *stream, const int *xn, const int *yn, int N, int64_t *scratch, int *totals) {

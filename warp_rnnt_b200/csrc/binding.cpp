@@ -347,6 +347,96 @@ at::Tensor rnnt_logits_backward(const at::Tensor &xs, const at::Tensor &lse, con
     return out;
 }
 
+// loss from compact (STU,V) logits in joint_pack's row order, float32 or bfloat16: (costs (N), lse (STU),
+// pair_grads (STU,2) or empty, prefix (2N) int64 = {mem_pref, lab_pref} for the backward).  Shapes are validated as in
+// rnnt_loss_compact: one 16-byte device->host copy, or none with hints (max_T, max_U > 0).
+std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor>
+rnnt_logits_compact_forward(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
+                            int blank, float fastemit_lambda, bool want_grads, int lse_mode, int max_T, int max_U) {
+    check4(xs, ys, xn, yn, true);
+    TORCH_CHECK(xs.dim() == 2, "xs must have 2 dimensions");
+    TORCH_CHECK(xn.dim() == 1 && yn.dim() == 1 && xn.size(0) == yn.size(0), "xn and yn shape must be equal (N,)");
+    const c10::cuda::CUDAGuard guard(xs.device());
+    const int64_t N = xn.size(0), STU = xs.size(0), V = xs.size(1);
+    const bool bf16 = xs.scalar_type() == at::ScalarType::BFloat16;
+    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    void *stream = current_stream(xs);
+    const auto f32 = xs.options().dtype(at::kFloat);
+    at::Tensor costs = at::empty({N}, f32);
+    at::Tensor lse = at::empty({STU}, f32);
+    at::Tensor pg = want_grads ? at::empty({STU, 2}, f32) : at::empty({0}, f32);
+    at::Tensor prefix = at::empty({2 * N}, xs.options().dtype(at::kLong));
+    if (N == 0) return std::make_tuple(costs, lse, pg, prefix);
+    if (!(max_T > 0 && max_U > 0)) {
+        at::Tensor totals = at::empty({4}, xs.options().dtype(at::kInt));
+        check_status(rnnt_b200_compact_totals(stream, xn.data_ptr<int>(), yn.data_ptr<int>(), (int)N,
+                                              prefix.data_ptr<int64_t>(), totals.data_ptr<int>()));
+        at::Tensor h = totals.cpu();
+        const int *t = h.data_ptr<int>();
+        TORCH_CHECK(ys.numel() == t[1], "ys shape must be equal to (sum(yn), )");
+        TORCH_CHECK(STU == t[0], "xs shape mismatch with (\\sum{xn*(yn+1)}, )");
+        max_T = t[2];
+        max_U = t[3];
+    }
+    at::Tensor ws = workspace_for(xs, STU, N);
+    float *pgp = want_grads ? pg.data_ptr<float>() : nullptr;
+    if (bf16)
+        check_status(rnnt_b200_logits_compact_forward_bf16(
+            stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(), ys.data_ptr<int>(), xn.data_ptr<int>(),
+            yn.data_ptr<int>(), costs.data_ptr<float>(), lse.data_ptr<float>(), pgp, prefix.data_ptr<int64_t>(), nullptr,
+            STU, (int)N, (int)V, blank, fastemit_lambda, lse_mode, max_T, max_U));
+    else
+        check_status(rnnt_b200_logits_compact_forward(
+            stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr<float>(), ys.data_ptr<int>(), xn.data_ptr<int>(),
+            yn.data_ptr<int>(), costs.data_ptr<float>(), lse.data_ptr<float>(), pgp, prefix.data_ptr<int64_t>(), nullptr,
+            STU, (int)N, (int)V, blank, fastemit_lambda, lse_mode, max_T, max_U));
+    return std::make_tuple(costs, lse, pg, prefix);
+}
+
+// d loss / d compact logits, of the dtype of xs
+at::Tensor rnnt_logits_compact_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &pair_grads,
+                                        const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
+                                        const at::Tensor &prefix, const at::Tensor &grad_out, int blank) {
+    const bool bf16 = xs.scalar_type() == at::ScalarType::BFloat16;
+    TORCH_CHECK(xs.is_contiguous() && (xs.scalar_type() == at::ScalarType::Float || bf16) && xs.device().is_cuda() &&
+                    xs.dim() == 2,
+                "xs must be a contiguous CUDA Float tensor of shape (STU, V)");
+    const int64_t STU = xs.size(0), V = xs.size(1), N = xn.numel();
+    TORCH_CHECK(lse.is_contiguous() && lse.scalar_type() == at::ScalarType::Float && lse.device() == xs.device() &&
+                    lse.numel() == STU,
+                "lse must be a contiguous Float tensor of shape (STU,) on the device of xs");
+    TORCH_CHECK(pair_grads.is_contiguous() && pair_grads.scalar_type() == at::ScalarType::Float &&
+                    pair_grads.device() == xs.device() && pair_grads.numel() == STU * 2,
+                "pair_grads must be a contiguous Float tensor of shape (STU, 2) on the device of xs");
+    TORCH_CHECK(ys.is_contiguous() && ys.scalar_type() == at::ScalarType::Int && ys.device() == xs.device(),
+                "ys must be a contiguous Int tensor on the device of xs");
+    TORCH_CHECK(xn.is_contiguous() && yn.is_contiguous() && xn.scalar_type() == at::ScalarType::Int &&
+                    yn.scalar_type() == at::ScalarType::Int && xn.device() == xs.device() &&
+                    yn.device() == xs.device() && yn.numel() == N,
+                "xn and yn must be contiguous Int tensors of shape (N,) on the device of xs");
+    TORCH_CHECK(prefix.is_contiguous() && prefix.scalar_type() == at::ScalarType::Long && prefix.device() == xs.device() &&
+                    prefix.numel() == 2 * N,
+                "prefix must be a contiguous Long tensor of shape (2N,) on the device of xs");
+    TORCH_CHECK(grad_out.is_contiguous() && grad_out.scalar_type() == at::ScalarType::Float &&
+                    grad_out.device() == xs.device() && grad_out.numel() == N,
+                "grad_out must be a contiguous Float tensor of shape (N,)");
+    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    const c10::cuda::CUDAGuard guard(xs.device());
+    at::Tensor out = at::empty_like(xs);
+    if (N == 0 || STU == 0) return out;                 // empty tensors: nothing to write (and no data pointers)
+    if (bf16)
+        check_status(rnnt_b200_logits_compact_backward_bf16(
+            current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(), pair_grads.data_ptr<float>(), ys.data_ptr<int>(),
+            xn.data_ptr<int>(), yn.data_ptr<int>(), prefix.data_ptr<int64_t>(), grad_out.data_ptr<float>(),
+            out.data_ptr(), STU, (int)N, (int)V, blank));
+    else
+        check_status(rnnt_b200_logits_compact_backward(
+            current_stream(xs), xs.data_ptr<float>(), lse.data_ptr<float>(), pair_grads.data_ptr<float>(),
+            ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(), prefix.data_ptr<int64_t>(),
+            grad_out.data_ptr<float>(), out.data_ptr<float>(), STU, (int)N, (int)V, blank));
+    return out;
+}
+
 // compact packing of the joint input: (x (STU,H), mem_pref (N) int64).  stu < 0: STU is read back from the device
 // (one 16-byte copy); stu >= 0: trusted, no host sync.
 std::tuple<at::Tensor, at::Tensor> rnnt_joint_pack(const at::Tensor &f, const at::Tensor &g, const at::Tensor &lf,
@@ -453,6 +543,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("blank") = 0, py::arg("fastemit_lambda") = 0.0, py::arg("want_grads") = true, py::arg("lse_mode") = 0);
     m.def("rnnt_logits_backward", &rnnt_logits_backward, py::arg("xs"), py::arg("lse"), py::arg("pair_grads"),
           py::arg("ys"), py::arg("grad_out"), py::arg("blank") = 0);
+    m.def("rnnt_logits_compact_forward", &rnnt_logits_compact_forward, py::arg("xs"), py::arg("ys"), py::arg("xn"),
+          py::arg("yn"), py::arg("blank") = 0, py::arg("fastemit_lambda") = 0.0, py::arg("want_grads") = true,
+          py::arg("lse_mode") = 0, py::arg("max_T") = 0, py::arg("max_U") = 0);
+    m.def("rnnt_logits_compact_backward", &rnnt_logits_compact_backward, py::arg("xs"), py::arg("lse"),
+          py::arg("pair_grads"), py::arg("ys"), py::arg("xn"), py::arg("yn"), py::arg("prefix"), py::arg("grad_out"),
+          py::arg("blank") = 0);
     m.def("rnnt_joint_pack", &rnnt_joint_pack, py::arg("f"), py::arg("g"), py::arg("lf"), py::arg("lg"), py::arg("stu") = -1);
     m.def("rnnt_joint_pack_backward", &rnnt_joint_pack_backward, py::arg("dx"), py::arg("lf"), py::arg("lg"),
           py::arg("mem_pref"), py::arg("T"), py::arg("U1"));

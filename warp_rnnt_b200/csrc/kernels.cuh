@@ -47,6 +47,13 @@ cudaError_t launch_lse_pairs(cudaStream_t s, const void *x, const int *labels, i
 cudaError_t launch_expand_logits(cudaStream_t s, const void *x, const float *lse, const float2 *pg, const int *labels,
                                  const float *grad_out, void *out, int N, int T, int U, int V, int blank,
                                  int io_bf16 = 0);
+// ... the same two passes over compact (STU,V) logits in joint_pack's row order: p is the compact Problem (prefix sums
+// on the device), labels (sum yn), grad_out (N) or nullptr
+cudaError_t launch_lse_pairs_compact(cudaStream_t s, const void *x, const Problem &p, const int *labels, int64_t STU,
+                                     int V, int blank, float2 *pairs, float *lse, int io_bf16);
+cudaError_t launch_expand_logits_compact(cudaStream_t s, const void *x, const float *lse, const float2 *pg,
+                                         const Problem &p, const int *labels, const float *grad_out, void *out,
+                                         int64_t STU, int V, int blank, int io_bf16);
 
 // joint.cu -- compact packing of the joint network's input (caller side of compact=True)
 cudaError_t launch_joint_pack(cudaStream_t s, const float *f, const float *g, const int *lf, const int *lg,

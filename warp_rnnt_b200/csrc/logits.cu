@@ -40,10 +40,21 @@ __device__ __forceinline__ float4 ld_group4(const __nv_bfloat16 *row, int q) {
 // groups of 4 at group-aligned addresses -> the SUB lanes stride over groups (float V = 28: 7 of 8 lanes load one float4
 // each, a warp reads 4 consecutive rows = 448 contiguous bytes).  The choice of SUB and VEC4 depends on V and the
 // alignment only, never on IN: a bf16 row is summed exactly like the float row of the same values.
-template <typename IN, int SUB, bool VEC4>
+//
+// COMPACT: the rows are joint_pack's ragged (STU, V) order and the grid is (gx, N): CTA row blockIdx.y streams over the
+// Tn*Un rows of lattice n (Problem `lay`, compact prefix sums), the pointers rebased to its first row.  Only the
+// (lattice, u, label) of a row differs from the dense kernel; a row is summed exactly as the dense row of its values.
+template <typename IN, int SUB, bool VEC4, bool COMPACT = false>
 __global__ void __launch_bounds__(kLogitThreads)
 k_lse_pairs(const IN *__restrict__ x, const int *__restrict__ labels, int64_t cells, int V, int blank, int U,
-            FastDiv divU, FastDiv divTU, float2 *__restrict__ pairs, float *__restrict__ lse_out) {
+            FastDiv divU, FastDiv divTU, float2 *__restrict__ pairs, float *__restrict__ lse_out, Problem lay) {
+    Lattice L;
+    if constexpr (COMPACT) {
+        // `cells` = STU on entry: a lattice never reaches past the rows of the tensor (lengths the hints vouched for)
+        L = get_lattice(lay, blockIdx.y);
+        cells = L.ok ? max(min((int64_t)L.Tn * L.Un, cells - L.base), (int64_t)0) : 0;
+        x += L.base * V; pairs += L.base; lse_out += L.base;
+    }
     const int sub = threadIdx.x % SUB;
     const int64_t per_block = kLogitThreads / SUB;
     for (int64_t base = (int64_t)blockIdx.x * per_block; base < cells; base += (int64_t)gridDim.x * per_block) {   // block-uniform trip count
@@ -97,10 +108,16 @@ k_lse_pairs(const IN *__restrict__ x, const int *__restrict__ labels, int64_t ce
         if (sub == 0) {
             // every logit -inf: NaN, as torch.log_softmax gives (and as the max-first paths above compute it)
             const float l = (m == -INFINITY) ? NAN : m + logf(s);
-            uint32_t n, rem, t, u;
-            divTU.divmod((uint32_t)cell, n, rem);
-            divU.divmod(rem, t, u);
-            const int lab = ((int)u < U - 1) ? labels[(int64_t)n * (U - 1) + u] : blank;
+            int lab;
+            if constexpr (COMPACT) {
+                const int u = (int)cell % L.Un;
+                lab = (u < L.Un - 1) ? labels[L.lab_base + u] : blank;
+            } else {
+                uint32_t n, rem, t, u;
+                divTU.divmod((uint32_t)cell, n, rem);
+                divU.divmod(rem, t, u);
+                lab = ((int)u < U - 1) ? labels[(int64_t)n * (U - 1) + u] : blank;
+            }
             pairs[cell] = make_float2(io_load(row + blank) - l, io_load(row + lab) - l);
             lse_out[cell] = l;
         }
@@ -172,13 +189,20 @@ __device__ __forceinline__ void st_logit_grads(__nv_bfloat16 *p, const float (&e
 
 // flat stream of the (cells, V) output in vectors of VEC elements (float: 4 when V % 4 == 0, 2 when V % 2 == 0, else
 // 1; bf16 also 8): a vector never straddles a row, so one (gb, gl, lse, label) fetch serves it.  IO is the element
-// type of the logits and of the gradient.
-template <typename IO, int VEC>
+// type of the logits and of the gradient.  COMPACT: as in k_lse_pairs, CTA row blockIdx.y streams over the Tn*Un*V
+// elements of lattice n.
+template <typename IO, int VEC, bool COMPACT = false>
 __global__ void __launch_bounds__(kLogitThreads)
 k_expand_logits(const IO *__restrict__ x, const float *__restrict__ lse, const float2 *__restrict__ pg,
                 const int *__restrict__ labels, const float *__restrict__ grad_out, IO *__restrict__ out,
                 int64_t cells, int V, int blank, int U, FastDiv divU, FastDiv divTU, int64_t stride_rows,
-                int stride_v) {
+                int stride_v, Problem lay) {
+    Lattice L;
+    if constexpr (COMPACT) {
+        L = get_lattice(lay, blockIdx.y);
+        cells = L.ok ? max(min((int64_t)L.Tn * L.Un, cells - L.base), (int64_t)0) : 0;
+        x += L.base * V; out += L.base * V; lse += L.base; pg += L.base;
+    }
     const int64_t total = cells * (int64_t)V;
     int64_t f = ((int64_t)blockIdx.x * kLogitThreads + threadIdx.x) * VEC;
     if (f >= total) return;
@@ -198,11 +222,19 @@ k_expand_logits(const IO *__restrict__ x, const float *__restrict__ lse, const f
 #pragma unroll
             for (int k = 0; k < VEC; ++k) e[k] = z;
         } else {
-            uint32_t n, rem, t, u;
-            divTU.divmod((uint32_t)row, n, rem);
-            divU.divmod(rem, t, u);
-            const int lab = ((int)u < U - 1) ? labels[(int64_t)n * (U - 1) + u] : -1;
-            const float sc = grad_out ? grad_out[n] : 1.0f;
+            int lab;
+            float sc;
+            if constexpr (COMPACT) {
+                const int u = (int)row % L.Un;
+                lab = (u < L.Un - 1) ? labels[L.lab_base + u] : -1;
+                sc = grad_out ? grad_out[blockIdx.y] : 1.0f;
+            } else {
+                uint32_t n, rem, t, u;
+                divTU.divmod((uint32_t)row, n, rem);
+                divU.divmod(rem, t, u);
+                lab = ((int)u < U - 1) ? labels[(int64_t)n * (U - 1) + u] : -1;
+                sc = grad_out ? grad_out[n] : 1.0f;
+            }
             const float l = lse[row], tot = q.x + q.y;
             float xv[VEC];
             ld_logits<VEC>(x + f, xv);
@@ -217,19 +249,33 @@ k_expand_logits(const IO *__restrict__ x, const float *__restrict__ lse, const f
     }
 }
 
+// Compact grids are (gx, N): lattice lengths are on the device only, so gx covers twice the average lattice
+// (STU / N rows, as launch_gather sizes its grid) in CTAs of kCompactIters grid-stride iterations each; a larger lattice
+// is finished by the grid stride, the surplus CTAs of a smaller one return at once.
+constexpr int64_t kCompactIters = 4;
+static int compact_gx(int64_t STU, int N, int64_t per_cta_rows) {
+    const int64_t per = (STU / (N > 0 ? N : 1)) * 2 + 1;
+    return (int)max((int64_t)1, min((per + per_cta_rows - 1) / per_cta_rows, (int64_t)65535));
+}
+
+// lay == nullptr: dense (N,T,U,V) logits; else the compact (STU,V) rows of lattices lay->N, lay->T = lay->U = 0.
 template <typename IN>
 static cudaError_t lse_pairs_as(cudaStream_t s, const IN *x, const int *labels, int N, int T, int U, int V, int blank,
-                                float2 *pairs, float *lse) {
-    const int64_t cells = (int64_t)N * T * U;
-    if (cells <= 0) return cudaSuccess;
-    const FastDiv divU((uint32_t)U), divTU((uint32_t)(T * U));
+                                float2 *pairs, float *lse, const Problem *lay, int64_t STU) {
+    const int64_t cells = lay ? STU : (int64_t)N * T * U;
+    if (cells <= 0 || N <= 0) return cudaSuccess;
+    const FastDiv divU((uint32_t)max(U, 1)), divTU((uint32_t)max(T * U, 1));
     const int sms = sm_count(current_device());
     // groups of 4 elements: float4 (16 bytes) or 4 bf16 (8 bytes) per load
     const bool vec4 = (V % 4 == 0) && ((reinterpret_cast<uintptr_t>(x) & (4 * sizeof(IN) - 1)) == 0);
     const int sub = vec4 ? (V <= 32 ? 8 : 32) : (V <= 12 ? 1 : (V <= 512 ? 8 : 32));
     const int64_t per_block = kLogitThreads / sub;
-    const int grid = (int)min((cells + per_block - 1) / per_block, (int64_t)sms * 16);
-#define RNNT_LSE_LAUNCH(SUB, VEC) k_lse_pairs<IN, SUB, VEC><<<grid, kLogitThreads, 0, s>>>(x, labels, cells, V, blank, U, divU, divTU, pairs, lse)
+    const Problem p = lay ? *lay : Problem{};
+    const dim3 grid = lay ? dim3(compact_gx(STU, N, per_block * kCompactIters), N)
+                          : dim3((unsigned)min((cells + per_block - 1) / per_block, (int64_t)sms * 16));
+#define RNNT_LSE_LAUNCH(SUB, VEC)                                                                                          \
+    (lay ? k_lse_pairs<IN, SUB, VEC, true><<<grid, kLogitThreads, 0, s>>>(x, labels, cells, V, blank, U, divU, divTU, pairs, lse, p) \
+         : k_lse_pairs<IN, SUB, VEC><<<grid, kLogitThreads, 0, s>>>(x, labels, cells, V, blank, U, divU, divTU, pairs, lse, p))
     if (vec4) { if (sub == 8) RNNT_LSE_LAUNCH(8, true); else RNNT_LSE_LAUNCH(32, true); }
     else if (sub == 1) RNNT_LSE_LAUNCH(1, false);
     else if (sub == 8) RNNT_LSE_LAUNCH(8, false);
@@ -241,16 +287,25 @@ static cudaError_t lse_pairs_as(cudaStream_t s, const IN *x, const int *labels, 
 
 cudaError_t launch_lse_pairs(cudaStream_t s, const void *x, const int *labels, int N, int T, int U, int V, int blank,
                              float2 *pairs, float *lse, int io_bf16) {
-    if (io_bf16) return lse_pairs_as(s, static_cast<const __nv_bfloat16 *>(x), labels, N, T, U, V, blank, pairs, lse);
-    return lse_pairs_as(s, static_cast<const float *>(x), labels, N, T, U, V, blank, pairs, lse);
+    if (io_bf16)
+        return lse_pairs_as(s, static_cast<const __nv_bfloat16 *>(x), labels, N, T, U, V, blank, pairs, lse, nullptr, 0);
+    return lse_pairs_as(s, static_cast<const float *>(x), labels, N, T, U, V, blank, pairs, lse, nullptr, 0);
+}
+
+cudaError_t launch_lse_pairs_compact(cudaStream_t s, const void *x, const Problem &p, const int *labels, int64_t STU,
+                                     int V, int blank, float2 *pairs, float *lse, int io_bf16) {
+    if (io_bf16)
+        return lse_pairs_as(s, static_cast<const __nv_bfloat16 *>(x), labels, p.N, 0, 0, V, blank, pairs, lse, &p, STU);
+    return lse_pairs_as(s, static_cast<const float *>(x), labels, p.N, 0, 0, V, blank, pairs, lse, &p, STU);
 }
 
 template <typename IO>
 static cudaError_t expand_logits_as(cudaStream_t s, const IO *x, const float *lse, const float2 *pg, const int *labels,
-                                    const float *grad_out, IO *out, int N, int T, int U, int V, int blank) {
-    const int64_t cells = (int64_t)N * T * U;
-    if (cells <= 0) return cudaSuccess;
-    const FastDiv divU((uint32_t)U), divTU((uint32_t)(T * U));
+                                    const float *grad_out, IO *out, int N, int T, int U, int V, int blank,
+                                    const Problem *lay, int64_t STU) {
+    const int64_t cells = lay ? STU : (int64_t)N * T * U;
+    if (cells <= 0 || N <= 0) return cudaSuccess;
+    const FastDiv divU((uint32_t)max(U, 1)), divTU((uint32_t)max(T * U, 1));
     const int sms = sm_count(current_device());
     // the widest vector (at most 16 bytes) that V and the alignment of both tensors allow
     const uintptr_t al = reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out);
@@ -259,11 +314,16 @@ static cudaError_t expand_logits_as(cudaStream_t s, const IO *x, const float *ls
     for (int c = vmax; c > 1; c >>= 1)
         if (V % c == 0 && (al & (c * sizeof(IO) - 1)) == 0) { vec = c; break; }
     const int64_t total = cells * (int64_t)V / vec;
-    const int grid = (int)min((total + kLogitThreads - 1) / kLogitThreads, (int64_t)sms * 32);
-    const int64_t stride = (int64_t)grid * kLogitThreads * vec;
+    const Problem p = lay ? *lay : Problem{};
+    // compact: CTAs per lattice from the rows a CTA covers in kCompactIters iterations (rounded up to whole rows)
+    const dim3 grid = lay ? dim3(compact_gx(STU, N, ((int64_t)kLogitThreads * vec * kCompactIters + V - 1) / V), N)
+                          : dim3((unsigned)min((total + kLogitThreads - 1) / kLogitThreads, (int64_t)sms * 32));
+    const int64_t stride = (int64_t)grid.x * kLogitThreads * vec;
     const int64_t srows = stride / V;
     const int sv = (int)(stride - srows * V);
-#define RNNT_EXPAND_LAUNCH(VEC) k_expand_logits<IO, VEC><<<grid, kLogitThreads, 0, s>>>(x, lse, pg, labels, grad_out, out, cells, V, blank, U, divU, divTU, srows, sv)
+#define RNNT_EXPAND_LAUNCH(VEC)                                                                                            \
+    (lay ? k_expand_logits<IO, VEC, true><<<grid, kLogitThreads, 0, s>>>(x, lse, pg, labels, grad_out, out, cells, V, blank, U, divU, divTU, srows, sv, p) \
+         : k_expand_logits<IO, VEC><<<grid, kLogitThreads, 0, s>>>(x, lse, pg, labels, grad_out, out, cells, V, blank, U, divU, divTU, srows, sv, p))
     if constexpr (sizeof(IO) == 2) {
         if (vec == 8) RNNT_EXPAND_LAUNCH(8);
         else if (vec == 4) RNNT_EXPAND_LAUNCH(4);
@@ -283,9 +343,19 @@ cudaError_t launch_expand_logits(cudaStream_t s, const void *x, const float *lse
                                  const float *grad_out, void *out, int N, int T, int U, int V, int blank, int io_bf16) {
     if (io_bf16)
         return expand_logits_as(s, static_cast<const __nv_bfloat16 *>(x), lse, pg, labels, grad_out,
-                                static_cast<__nv_bfloat16 *>(out), N, T, U, V, blank);
+                                static_cast<__nv_bfloat16 *>(out), N, T, U, V, blank, nullptr, 0);
     return expand_logits_as(s, static_cast<const float *>(x), lse, pg, labels, grad_out, static_cast<float *>(out), N, T,
-                            U, V, blank);
+                            U, V, blank, nullptr, 0);
+}
+
+cudaError_t launch_expand_logits_compact(cudaStream_t s, const void *x, const float *lse, const float2 *pg,
+                                         const Problem &p, const int *labels, const float *grad_out, void *out,
+                                         int64_t STU, int V, int blank, int io_bf16) {
+    if (io_bf16)
+        return expand_logits_as(s, static_cast<const __nv_bfloat16 *>(x), lse, pg, labels, grad_out,
+                                static_cast<__nv_bfloat16 *>(out), p.N, 0, 0, V, blank, &p, STU);
+    return expand_logits_as(s, static_cast<const float *>(x), lse, pg, labels, grad_out, static_cast<float *>(out), p.N,
+                            0, 0, V, blank, &p, STU);
 }
 
 }  // namespace rnnt
