@@ -63,6 +63,31 @@ def test_native_dense_and_gather(lib, shape):
     st = lib.rnnt_b200_loss_dense(stream, p(ws), ctypes.c_size_t(ws.numel()), p(xs), p(y), p(a), p(b), p(costs),
                                   p(grads), None, N, T, U, V, V, ctypes.c_float(0.0), 0)
     assert st == 5
+    # without a workspace (6 = too small): the dense, pairs and gather forwards need none when the fused kernel takes
+    # the shape (700 frames do not fit its shared memory); the from-logits and compact forwards always need one
+    fused_status = 0 if T < 700 else 6
+    no_ws, lam = (stream, p(ws), ctypes.c_size_t(0)), ctypes.c_float(0.0)
+    xb, gb = xs.bfloat16(), torch.empty(N, T, U, V, dtype=torch.bfloat16, device="cuda")
+    pairs, lse = xs[..., :2].contiguous(), torch.empty(N, T, U, device="cuda")
+    assert lib.rnnt_b200_loss_dense(*no_ws, p(xs), p(y), p(a), p(b), p(costs), p(grads), None, N, T, U, V, 1, lam,
+                                    0) == fused_status
+    assert lib.rnnt_b200_loss_dense_bf16(*no_ws, p(xb), p(y), p(a), p(b), p(costs), p(gb), None, None, None, N, T, U,
+                                         V, 1, lam, 0) == fused_status
+    assert lib.rnnt_b200_loss_pairs(*no_ws, p(pairs), p(a), p(b), p(costs), p(pg), N, T, U, lam, 0) == fused_status
+    assert lib.rnnt_b200_gather_forward(*no_ws, p(xs), p(y), p(a), p(b), p(costs), p(pg), N, T, U, V, 1, lam,
+                                        0) == fused_status
+    for fwd, x in ((lib.rnnt_b200_logits_forward, xs), (lib.rnnt_b200_logits_forward_bf16, xb)):
+        assert fwd(*no_ws, p(x), p(y), p(a), p(b), p(costs), p(lse), p(pg), N, T, U, V, 1, lam, 0) == 6
+    xs_c, ys_c = to_compact(lp, ys, xn, yn)
+    STU = xs_c.shape[0]
+    xc, yc = cu(xs_c), cu(ys_c)
+    pgc, lsec = torch.empty(STU, 2, device="cuda"), torch.empty(STU, device="cuda")
+    loc, prefix = torch.empty(STU, dtype=torch.int64, device="cuda"), torch.empty(2 * N, dtype=torch.int64, device="cuda")
+    assert lib.rnnt_b200_compact_forward(*no_ws, p(xc), p(yc), p(a), p(b), p(costs), p(pgc), p(loc), None,
+                                         ctypes.c_int64(STU), N, V, 1, lam, 0, T, U) == 6
+    for fwd, x in ((lib.rnnt_b200_logits_compact_forward, xc), (lib.rnnt_b200_logits_compact_forward_bf16, xc.bfloat16())):
+        assert fwd(*no_ws, p(x), p(yc), p(a), p(b), p(costs), p(lsec), p(pgc), p(prefix), None, ctypes.c_int64(STU), N,
+                   V, 1, lam, 0, T, U) == 6
 
 
 def test_reference_abi_symbols_direct(lib):

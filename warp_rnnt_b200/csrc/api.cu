@@ -46,10 +46,9 @@ static int default_lse_mode() {
 // cfg-2 call's gradient write follows the recurrence (composed emit, fused.cu), so the recurrence is on its critical
 // path: the timeline (tools/fused_timeline.py) shows beta[0,0] at ~51 us exact and ~46 us fast, of a ~80 us kernel.
 // RNNT_LSE_FAST / RNNT_B200_LSE=fast selects the short chain.
-static int resolve_kind(int lse_mode, bool compact) {
+static bool fast_lse(int lse_mode) {
     if (lse_mode == RNNT_LSE_AUTO) lse_mode = default_lse_mode();
-    if (lse_mode == RNNT_LSE_FAST) return kFast;
-    return compact ? kExactCompact : kExactDense;
+    return lse_mode == RNNT_LSE_FAST;
 }
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
@@ -97,13 +96,18 @@ static Workspace carve(void *base, int64_t cells, int N) {
     return w;
 }
 
-static bool dense_args_ok(int N, int T, int U, int V) {
+static bool dense_args_ok(int N, int T, int U, int V, int blank) {
     if (N < 0 || T < 1 || U < 1 || V < 1) return false;
     if ((int64_t)T * U >= (int64_t)1 << 31) return false;
     if ((int64_t)N * T * U >= (int64_t)1 << 31) return false;   // cell ids are 32-bit in the emit kernel
     if (V >= (1 << 22)) return false;
-    return true;
+    return blank >= 0 && blank < V;
 }
+static bool compact_args_ok(int N, int64_t STU, int V, int blank) {
+    return N >= 0 && STU >= 0 && V >= 1 && V < (1 << 22) && blank >= 0 && blank < V;
+}
+// (cells,2) pairs and their gradients are read and written as float2
+static bool pairs_aligned(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 7u) == 0; }
 
 // Internal streams for the pipelined general path: one for gathers, one for emits, four
 // high-priority ones for wavefronts (their CTAs are few and long-lived; priority lets them take the
@@ -210,98 +214,180 @@ __global__ void k_lse_selfcheck(unsigned long long *counts) {
 
 using namespace rnnt;
 
+// One loss call, described on the host; run_loss runs it.
+struct LossCall {
+    Problem p;                   // dense (N,T,U), or compact with its device prefix sums (p.T = p.U = 0)
+    int T, U;                    // lattice bounds: p.T, p.U (dense); max_T, max_U (compact; 0 = unknown)
+    int64_t cells;               // N*T*U (dense) or STU (compact)
+    // source: log-probs of V elements per cell (f32 or bf16) with their labels, or ready-made (cells,2) pairs
+    const void *lp;
+    const int *labels;
+    int V, blank, io_bf16;
+    const float2 *pairs;
+    // outputs: costs, plus the dense gradient (with scale and the reduced loss), or the (cells,2) gradient, or neither
+    float *costs;
+    void *grads;
+    const float *grad_scale;
+    float *loss_sum;
+    unsigned *sync_counter;      // with loss_sum: reduce in the fused kernel, else in a launch of its own
+    float2 *pair_grads;
+    int64_t *loc;                // compact gather: label id per cell, or null
+    float fastemit_lambda;
+    int lse_mode;
+};
+
+static LossCall dense_call(const int *xn, const int *yn, int N, int T, int U, float *costs, float fastemit_lambda,
+                           int lse_mode) {
+    LossCall c = {};
+    c.p = {xn, yn, nullptr, nullptr, N, T, U, 0};
+    c.T = T; c.U = U; c.cells = (int64_t)N * T * U;
+    c.costs = costs; c.fastemit_lambda = fastemit_lambda; c.lse_mode = lse_mode;
+    return c;
+}
+
+static LossCall compact_call(const int *xn, const int *yn, const int64_t *mem_pref, const int64_t *lab_pref, int N,
+                             int64_t STU, int max_T, int max_U, float *costs, float fastemit_lambda, int lse_mode) {
+    LossCall c = {};
+    c.p = {xn, yn, mem_pref, lab_pref, N, 0, 0, 1};
+    c.T = max_T; c.U = max_U; c.cells = STU;
+    c.costs = costs; c.fastemit_lambda = fastemit_lambda; c.lse_mode = lse_mode;
+    return c;
+}
+
+// the workspace carved for a call on `cells` cells; false when the caller's is missing or too small
+static bool carve_ok(void *workspace, size_t workspace_bytes, int64_t cells, int N, Workspace *w) {
+    *w = carve(workspace, cells, N);
+    return workspace && workspace_bytes >= w->bytes;
+}
+
+// Large batches of large lattices: software-pipeline lattice groups over internal streams so that the
+// latency-bound wavefront of group g overlaps the bandwidth-bound gather of g+1 and emit of g-1.
+// ... which only pays when the wavefront (a per-lattice latency chain of T+U-1 steps that does not shrink with the
+// group) is short against the bandwidth-bound emit: cfg 5's micro-batch takes the pipeline, cfg 4 does not.
+// The two estimates (0.45 us per anti-diagonal, an emit at 5.5 TB/s) were measured on a B200 and have not been
+// re-derived for the H100 (3.35 TB/s HBM3): there the emit is slower, so the true break-even favours the pipeline more often than this estimate.
+static int pipeline_groups(const LossCall &c) {
+    const int N = c.p.N;
+    const double wave_us = 0.45 * (c.T + c.U), emit_us = (double)c.cells * c.V * (c.io_bf16 ? 2 : 4) / 5.5e6;
+    return (c.grads && N >= 8 && (int64_t)c.cells * c.V * 4 >= ((int64_t)512 << 20) && pipeline_enabled() &&
+            wave_us < 0.4 * emit_us)
+               ? (N >= 32 ? 8 : 4) : 1;
+}
+
+// the general path of a dense call with dense gradients, one lattice group after another over the pipeline's streams
+static int run_pipelined(cudaStream_t s, Pipeline *pl, const LossCall &c, const Workspace &w, int groups) {
+    const int N = c.p.N, T = c.T, U = c.U, V = c.V;
+    const size_t esz = c.io_bf16 ? 2 : 4;
+    const bool fast = fast_lse(c.lse_mode);
+    int status = RNNT_STATUS_SUCCESS;
+    cudaEventRecord(pl->fork, s);
+    cudaStreamWaitEvent(pl->gather_s, pl->fork, 0);
+    cudaStreamWaitEvent(pl->expand_s, pl->fork, 0);
+    for (int i = 0; i < Pipeline::kWave; ++i) cudaStreamWaitEvent(pl->wave_s[i], pl->fork, 0);
+    for (int g = 0; g < groups && !status; ++g) {
+        const int n0 = (int)((int64_t)N * g / groups), n1 = (int)((int64_t)N * (g + 1) / groups);
+        const int ng = n1 - n0;
+        const int64_t c0 = (int64_t)n0 * T * U, cg = (int64_t)ng * T * U;
+        Problem p = {c.p.xn + n0, c.p.yn + n0, nullptr, nullptr, ng, T, U, 0};
+        const int *lab_g = c.labels + (int64_t)n0 * (U - 1);
+        const void *lp_g = (const char *)c.lp + (size_t)c0 * V * esz;
+        void *grads_g = (char *)c.grads + (size_t)c0 * V * esz;
+        cudaStream_t ws = pl->wave_s[g % Pipeline::kWave];
+        if (launch_gather(pl->gather_s, p, lp_g, lab_g, V, c.blank, w.pairs + c0, nullptr, cg, c.io_bf16) != cudaSuccess)
+            status = RNNT_STATUS_GATHER_FAILED;
+        cudaEventRecord(pl->gathered[g], pl->gather_s);
+        cudaStreamWaitEvent(ws, pl->gathered[g], 0);
+        if (!status && launch_wavefront(ws, fast, p, w.pairs + c0, w.alphas + c0, w.betas + c0, w.ll + 2 * n0,
+                                        w.bad + n0, c.costs + n0, 0, T, U) != cudaSuccess)
+            status = RNNT_STATUS_WARP_FAILED;
+        cudaEventRecord(pl->swept[g], ws);
+        cudaStreamWaitEvent(pl->expand_s, pl->swept[g], 0);
+        ExpandSrc src = {};
+        src.pairs = w.pairs + c0; src.alphas = w.alphas + c0; src.betas = w.betas + c0; src.bad = w.bad + n0;
+        src.scale = c.grad_scale ? c.grad_scale + n0 : nullptr; src.labels = lab_g;
+        src.fastemit_lambda = c.fastemit_lambda;
+        if (!status && launch_expand(pl->expand_s, p, src, grads_g, cg, V, c.blank, true, c.io_bf16) != cudaSuccess)
+            status = RNNT_STATUS_GRADS_BLANK_FAILED;
+    }
+    cudaEventRecord(pl->join[0], pl->gather_s);
+    cudaEventRecord(pl->join[1], pl->expand_s);
+    cudaStreamWaitEvent(s, pl->join[0], 0);
+    cudaStreamWaitEvent(s, pl->join[1], 0);
+    for (int i = 0; i < Pipeline::kWave; ++i) {
+        cudaEventRecord(pl->join[2 + i], pl->wave_s[i]);
+        cudaStreamWaitEvent(s, pl->join[2 + i], 0);
+    }
+    if (!status && c.loss_sum && launch_loss_sum(s, c.costs, c.grad_scale, N, c.loss_sum) != cudaSuccess)
+        status = RNNT_STATUS_COSTS_FAILED;
+    return status;
+}
+
+// Runs one loss call (N > 0, arguments checked): the fused kernel when the lattices fit it, else the general path --
+// gather (unless the pairs are given), wavefront, then the dense emit or the (cells,2) gradients.  Only the general
+// path needs the workspace.
+static int run_loss(cudaStream_t s, void *workspace, size_t workspace_bytes, const LossCall &c) {
+    const Problem &p = c.p;
+    FusedPlan plan;
+    if (c.T > 0 && c.U > 0 && want_fused(p.N, c.T, c.U, &plan)) {
+        FusedCall f = {};
+        f.fast_lse = fast_lse(c.lse_mode);
+        if (c.pairs) {
+            f.lp = c.pairs; f.V = 2; f.pairs_in = 1;
+        } else {
+            f.lp = c.lp; f.labels = c.labels; f.V = c.V; f.blank = c.blank; f.io_bf16 = c.io_bf16;
+        }
+        f.xn = p.xn; f.yn = p.yn; f.mem_pref = p.mem_pref; f.lab_pref = p.lab_pref; f.loc = c.loc;
+        f.costs = c.costs; f.grads = c.grads; f.pair_grads = c.pair_grads; f.scale = c.grad_scale;
+        f.loss_sum = c.loss_sum; f.sync_counter = c.sync_counter;
+        f.N = p.N; f.T = c.T; f.U = c.U; f.lam = c.fastemit_lambda;
+        RNNT_TRY(launch_fused(s, plan, f), RNNT_STATUS_WARP_FAILED);
+        if (c.loss_sum && !c.sync_counter)                  // no counter: reduce in a second, tiny launch
+            RNNT_TRY(launch_loss_sum(s, c.costs, c.grad_scale, p.N, c.loss_sum), RNNT_STATUS_COSTS_FAILED);
+        return RNNT_STATUS_SUCCESS;
+    }
+    Workspace w;
+    if (!carve_ok(workspace, workspace_bytes, c.cells, p.N, &w)) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    const int groups = pipeline_groups(c);
+    if (groups > 1) {
+        std::lock_guard<std::mutex> lock(g_pipe_mu);    // the pipeline's events are shared by all calls on this device
+        if (Pipeline *pl = get_pipeline_locked()) return run_pipelined(s, pl, c, w, groups);
+    }
+    const bool fast = fast_lse(c.lse_mode);
+    const float2 *pairs = c.pairs;
+    if (!pairs) {
+        RNNT_TRY(launch_gather(s, p, c.lp, c.labels, c.V, c.blank, w.pairs, c.loc, c.cells, c.io_bf16),
+                 RNNT_STATUS_GATHER_FAILED);
+        pairs = w.pairs;
+    }
+    RNNT_TRY(launch_wavefront(s, fast, p, pairs, w.alphas, w.betas, w.ll, w.bad, c.costs, !c.grads && !c.pair_grads,
+                              c.T, c.U),
+             RNNT_STATUS_WARP_FAILED);
+    if (c.grads) {
+        ExpandSrc src = {};
+        src.pairs = pairs; src.alphas = w.alphas; src.betas = w.betas; src.bad = w.bad;
+        src.scale = c.grad_scale; src.labels = c.labels; src.fastemit_lambda = c.fastemit_lambda;
+        RNNT_TRY(launch_expand(s, p, src, c.grads, c.cells, c.V, c.blank, false, c.io_bf16),
+                 RNNT_STATUS_GRADS_BLANK_FAILED);
+    }
+    if (c.pair_grads)
+        RNNT_TRY(launch_grads_pairs(s, p, pairs, w.alphas, w.betas, p.compact ? nullptr : w.bad, c.fastemit_lambda,
+                                    c.pair_grads, c.cells),
+                 RNNT_STATUS_GRADS_BLANK_FAILED);
+    if (c.loss_sum) RNNT_TRY(launch_loss_sum(s, c.costs, c.grad_scale, p.N, c.loss_sum), RNNT_STATUS_COSTS_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
 // dense layout, log_probs / grads of 4-byte (f32) or 2-byte (bf16) elements
 static int loss_dense_any(void *stream, void *workspace, size_t workspace_bytes, const void *log_probs,
                           const int *labels, const int *xn, const int *yn, float *costs, void *grads,
                           const float *grad_scale, float *loss_sum, unsigned int *sync_counter, int N, int T,
                           int U, int V, int blank, float fastemit_lambda, int lse_mode, int io_bf16) {
-    const size_t esz = io_bf16 ? 2 : 4;
-    auto lp_at = [&](int64_t cell0) { return (const void *)((const char *)log_probs + (size_t)cell0 * V * esz); };
-    auto g_at = [&](int64_t cell0) { return (void *)((char *)grads + (size_t)cell0 * V * esz); };
-    if (io_bf16 && !grads) return RNNT_STATUS_INVALID_ARGUMENT;
-    if (!dense_args_ok(N, T, U, V) || blank < 0 || blank >= V) return RNNT_STATUS_INVALID_ARGUMENT;
+    if ((io_bf16 && !grads) || !dense_args_ok(N, T, U, V, blank)) return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
-    cudaStream_t s = (cudaStream_t)stream;
-    const int64_t cells = (int64_t)N * T * U;
-    FusedPlan plan;
-    if (want_fused(N, T, U, &plan)) {
-        RNNT_TRY(launch_fused(s, resolve_kind(lse_mode, false), plan, log_probs, labels, xn, yn, costs, grads, nullptr,
-                              grad_scale, N, T, U, V, blank, fastemit_lambda, 0, 1, nullptr, nullptr, nullptr, loss_sum,
-                              sync_counter, io_bf16),
-                 RNNT_STATUS_WARP_FAILED);
-        if (loss_sum && !sync_counter)                  // no counter: reduce in a second, tiny launch
-            RNNT_TRY(launch_loss_sum(s, costs, grad_scale, N, loss_sum), RNNT_STATUS_COSTS_FAILED);
-        return RNNT_STATUS_SUCCESS;
-    }
-    const Workspace w = carve(workspace, cells, N);
-    if (!workspace || workspace_bytes < w.bytes) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
-    const int kind = resolve_kind(lse_mode, false);
-    // Large batches of large lattices: software-pipeline lattice groups over internal streams so that the
-    // latency-bound wavefront of group g overlaps the bandwidth-bound gather of g+1 and emit of g-1.
-    // ... which only pays when the wavefront (a per-lattice latency chain of T+U-1 steps that does not shrink with the
-    // group) is short against the bandwidth-bound emit: cfg 5's micro-batch takes the pipeline, cfg 4 does not.
-    // The two estimates (0.45 us per anti-diagonal, an emit at 5.5 TB/s) were measured on a B200 and have not been
-    // re-derived for the H100 (3.35 TB/s HBM3): there the emit is slower, so the true break-even favours the pipeline more often than this estimate.
-    const double wave_us = 0.45 * (T + U), emit_us = (double)cells * V * (io_bf16 ? 2 : 4) / 5.5e6;
-    const int groups = (grads && N >= 8 && (int64_t)cells * V * 4 >= ((int64_t)512 << 20) && pipeline_enabled() &&
-                        wave_us < 0.4 * emit_us)
-                           ? (N >= 32 ? 8 : 4) : 1;
-    if (groups > 1) {
-        std::lock_guard<std::mutex> lock(g_pipe_mu);    // the pipeline's events are shared by all calls on this device
-        Pipeline *pl = get_pipeline_locked();
-        if (pl) {
-            int status = RNNT_STATUS_SUCCESS;
-            cudaEventRecord(pl->fork, s);
-            cudaStreamWaitEvent(pl->gather_s, pl->fork, 0);
-            cudaStreamWaitEvent(pl->expand_s, pl->fork, 0);
-            for (int i = 0; i < Pipeline::kWave; ++i) cudaStreamWaitEvent(pl->wave_s[i], pl->fork, 0);
-            for (int g = 0; g < groups && !status; ++g) {
-                const int n0 = (int)((int64_t)N * g / groups), n1 = (int)((int64_t)N * (g + 1) / groups);
-                const int ng = n1 - n0;
-                const int64_t c0 = (int64_t)n0 * T * U, cg = (int64_t)ng * T * U;
-                Problem p = {xn + n0, yn + n0, nullptr, nullptr, ng, T, U, 0};
-                const int *lab_g = labels + (int64_t)n0 * (U - 1);
-                cudaStream_t ws = pl->wave_s[g % Pipeline::kWave];
-                if (launch_gather(pl->gather_s, p, lp_at(c0), lab_g, V, blank, w.pairs + c0, nullptr, cg, io_bf16) != cudaSuccess)
-                    status = RNNT_STATUS_GATHER_FAILED;
-                cudaEventRecord(pl->gathered[g], pl->gather_s);
-                cudaStreamWaitEvent(ws, pl->gathered[g], 0);
-                if (!status && launch_wavefront(ws, kind, p, w.pairs + c0, w.alphas + c0, w.betas + c0, w.ll + 2 * n0,
-                                                w.bad + n0, costs + n0, 0, 1, T, U) != cudaSuccess)
-                    status = RNNT_STATUS_WARP_FAILED;
-                cudaEventRecord(pl->swept[g], ws);
-                cudaStreamWaitEvent(pl->expand_s, pl->swept[g], 0);
-                ExpandSrc src = {};
-                src.pairs = w.pairs + c0; src.alphas = w.alphas + c0; src.betas = w.betas + c0; src.bad = w.bad + n0;
-                src.scale = grad_scale ? grad_scale + n0 : nullptr; src.labels = lab_g; src.fastemit_lambda = fastemit_lambda;
-                if (!status && launch_expand(pl->expand_s, p, src, g_at(c0), cg, V, blank, true, io_bf16) != cudaSuccess)
-                    status = RNNT_STATUS_GRADS_BLANK_FAILED;
-            }
-            cudaEventRecord(pl->join[0], pl->gather_s);
-            cudaEventRecord(pl->join[1], pl->expand_s);
-            cudaStreamWaitEvent(s, pl->join[0], 0);
-            cudaStreamWaitEvent(s, pl->join[1], 0);
-            for (int i = 0; i < Pipeline::kWave; ++i) {
-                cudaEventRecord(pl->join[2 + i], pl->wave_s[i]);
-                cudaStreamWaitEvent(s, pl->join[2 + i], 0);
-            }
-            if (!status && loss_sum && launch_loss_sum(s, costs, grad_scale, N, loss_sum) != cudaSuccess)
-                status = RNNT_STATUS_COSTS_FAILED;
-            return status;
-        }
-    }
-    Problem p = {xn, yn, nullptr, nullptr, N, T, U, 0};
-    RNNT_TRY(launch_gather(s, p, log_probs, labels, V, blank, w.pairs, nullptr, cells, io_bf16), RNNT_STATUS_GATHER_FAILED);
-    RNNT_TRY(launch_wavefront(s, kind, p, w.pairs, w.alphas, w.betas, w.ll, w.bad, costs, grads == nullptr, 1, T, U),
-             RNNT_STATUS_WARP_FAILED);
-    if (grads) {
-        ExpandSrc src = {};
-        src.pairs = w.pairs; src.alphas = w.alphas; src.betas = w.betas; src.bad = w.bad;
-        src.scale = grad_scale; src.labels = labels; src.fastemit_lambda = fastemit_lambda;
-        RNNT_TRY(launch_expand(s, p, src, grads, cells, V, blank, false, io_bf16), RNNT_STATUS_GRADS_BLANK_FAILED);
-    }
-    if (loss_sum) RNNT_TRY(launch_loss_sum(s, costs, grad_scale, N, loss_sum), RNNT_STATUS_COSTS_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    LossCall c = dense_call(xn, yn, N, T, U, costs, fastemit_lambda, lse_mode);
+    c.lp = log_probs; c.labels = labels; c.V = V; c.blank = blank; c.io_bf16 = io_bf16;
+    c.grads = grads; c.grad_scale = grad_scale; c.loss_sum = loss_sum; c.sync_counter = sync_counter;
+    return run_loss((cudaStream_t)stream, workspace, workspace_bytes, c);
 }
 
 // loss from logits of 4-byte (f32) or 2-byte (bf16) elements: the normaliser pass reads them, the recurrence and
@@ -310,39 +396,22 @@ static int logits_forward_any(void *stream, void *workspace, size_t workspace_by
                               const int *labels, const int *xn, const int *yn, float *costs, float *lse,
                               float *pair_grads, int N, int T, int U, int V, int blank, float fastemit_lambda,
                               int lse_mode, int io_bf16) {
-    if (!dense_args_ok(N, T, U, V) || blank < 0 || blank >= V || !lse) return RNNT_STATUS_INVALID_ARGUMENT;
-    if (reinterpret_cast<uintptr_t>(pair_grads) & 7u) return RNNT_STATUS_INVALID_ARGUMENT;
+    if (!dense_args_ok(N, T, U, V, blank) || !lse || !pairs_aligned(pair_grads)) return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
     cudaStream_t s = (cudaStream_t)stream;
-    const int64_t cells = (int64_t)N * T * U;
-    const Workspace w = carve(workspace, cells, N);
-    if (!workspace || workspace_bytes < w.bytes) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    LossCall c = dense_call(xn, yn, N, T, U, costs, fastemit_lambda, lse_mode);
+    Workspace w;
+    if (!carve_ok(workspace, workspace_bytes, c.cells, N, &w)) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
     // one pass over the logits: normaliser per cell + the two normalised log-probs the recurrence needs
     RNNT_TRY(launch_lse_pairs(s, logits, labels, N, T, U, V, blank, w.pairs, lse, io_bf16), RNNT_STATUS_GATHER_FAILED);
-    // the (cells,2) layout from here on: same kernels as rnnt_b200_loss_pairs
-    const int kind = resolve_kind(lse_mode, false);
-    FusedPlan plan;
-    if (want_fused(N, T, U, &plan)) {
-        RNNT_TRY(launch_fused(s, kind, plan, reinterpret_cast<const float *>(w.pairs), nullptr, xn, yn, costs, nullptr,
-                              reinterpret_cast<float2 *>(pair_grads), nullptr, N, T, U, 2, 0, fastemit_lambda, 1, 1),
-                 RNNT_STATUS_WARP_FAILED);
-        return RNNT_STATUS_SUCCESS;
-    }
-    Problem p = {xn, yn, nullptr, nullptr, N, T, U, 0};
-    RNNT_TRY(launch_wavefront(s, kind, p, w.pairs, w.alphas, w.betas, w.ll, w.bad, costs, pair_grads == nullptr, 1, T, U),
-             RNNT_STATUS_WARP_FAILED);
-    if (pair_grads)
-        RNNT_TRY(launch_grads_pairs(s, p, w.pairs, w.alphas, w.betas, w.bad, fastemit_lambda,
-                                    reinterpret_cast<float2 *>(pair_grads), cells),
-                 RNNT_STATUS_GRADS_BLANK_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    c.pairs = w.pairs; c.pair_grads = reinterpret_cast<float2 *>(pair_grads);
+    return run_loss(s, workspace, workspace_bytes, c);
 }
 
 static int logits_backward_any(void *stream, const void *logits, const float *lse, const float *pair_grads,
                                const int *labels, const float *grad_out, void *out, int N, int T, int U, int V,
                                int blank, int io_bf16) {
-    if (!dense_args_ok(N, T, U, V) || blank < 0 || blank >= V) return RNNT_STATUS_INVALID_ARGUMENT;
-    if (reinterpret_cast<uintptr_t>(pair_grads) & 7u) return RNNT_STATUS_INVALID_ARGUMENT;
+    if (!dense_args_ok(N, T, U, V, blank) || !pairs_aligned(pair_grads)) return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
     RNNT_TRY(launch_expand_logits((cudaStream_t)stream, logits, lse, reinterpret_cast<const float2 *>(pair_grads), labels,
                                   grad_out, out, N, T, U, V, blank, io_bf16),
@@ -351,50 +420,31 @@ static int logits_backward_any(void *stream, const void *logits, const float *ls
 }
 
 // compact (STU,V) logits in joint_pack's row order: the normaliser pass over the ragged rows, then the recurrence of
-// rnnt_b200_compact_forward on the (STU,2) pairs -- the fused kernel reading pairs (no gather) when the hints admit it,
-// else the general wavefront -- without the mismatch guard, as the compact layout has none
+// rnnt_b200_compact_forward on the (STU,2) pairs
 static int logits_compact_forward_any(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
                                       const int *ys, const int *xn, const int *yn, float *costs, float *lse,
                                       float *pair_grads, int64_t *prefix, int *totals, int64_t STU, int N, int V,
                                       int blank, float fastemit_lambda, int lse_mode, int max_T, int max_U,
                                       int io_bf16) {
-    if (N < 0 || STU < 0 || V < 1 || V >= (1 << 22) || blank < 0 || blank >= V || !lse || !prefix)
+    if (!compact_args_ok(N, STU, V, blank) || !lse || !prefix || !pairs_aligned(pair_grads))
         return RNNT_STATUS_INVALID_ARGUMENT;
-    if (reinterpret_cast<uintptr_t>(pair_grads) & 7u) return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
     cudaStream_t s = (cudaStream_t)stream;
-    const Workspace w = carve(workspace, STU, N);
-    if (!workspace || workspace_bytes < w.bytes) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
-    int64_t *mem_pref = prefix, *lab_pref = prefix + N;
-    RNNT_TRY(launch_prefix(s, xn, yn, N, mem_pref, lab_pref, totals ? totals : w.totals), RNNT_STATUS_GATHER_FAILED);
-    const Problem p = {xn, yn, mem_pref, lab_pref, N, 0, 0, 1};
-    RNNT_TRY(launch_lse_pairs_compact(s, logits, p, ys, STU, V, blank, w.pairs, lse, io_bf16), RNNT_STATUS_GATHER_FAILED);
-    const int kind = resolve_kind(lse_mode, true);
-    FusedPlan fplan;
-    if (max_T > 0 && max_U > 0 && want_fused(N, max_T, max_U, &fplan)) {
-        RNNT_TRY(launch_fused(s, kind, fplan, reinterpret_cast<const float *>(w.pairs), nullptr, xn, yn, costs, nullptr,
-                              reinterpret_cast<float2 *>(pair_grads), nullptr, N, max_T, max_U, 2, 0, fastemit_lambda,
-                              1, 0, mem_pref, lab_pref, nullptr),
-                 RNNT_STATUS_WARP_FAILED);
-        return RNNT_STATUS_SUCCESS;
-    }
-    RNNT_TRY(launch_wavefront(s, kind, p, w.pairs, w.alphas, w.betas, w.ll, w.bad, costs, pair_grads == nullptr, 0,
-                              max_T, max_U),
-             RNNT_STATUS_WARP_FAILED);
-    if (pair_grads)
-        RNNT_TRY(launch_grads_pairs(s, p, w.pairs, w.alphas, w.betas, nullptr, fastemit_lambda,
-                                    reinterpret_cast<float2 *>(pair_grads), STU),
-                 RNNT_STATUS_GRADS_BLANK_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    Workspace w;
+    if (!carve_ok(workspace, workspace_bytes, STU, N, &w)) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    RNNT_TRY(launch_prefix(s, xn, yn, N, prefix, prefix + N, totals ? totals : w.totals), RNNT_STATUS_GATHER_FAILED);
+    LossCall c = compact_call(xn, yn, prefix, prefix + N, N, STU, max_T, max_U, costs, fastemit_lambda, lse_mode);
+    RNNT_TRY(launch_lse_pairs_compact(s, logits, c.p, ys, STU, V, blank, w.pairs, lse, io_bf16), RNNT_STATUS_GATHER_FAILED);
+    c.pairs = w.pairs; c.pair_grads = reinterpret_cast<float2 *>(pair_grads);
+    return run_loss(s, workspace, workspace_bytes, c);
 }
 
 static int logits_compact_backward_any(void *stream, const void *logits, const float *lse, const float *pair_grads,
                                        const int *ys, const int *xn, const int *yn, const int64_t *prefix,
                                        const float *grad_out, void *out, int64_t STU, int N, int V, int blank,
                                        int io_bf16) {
-    if (N < 0 || STU < 0 || V < 1 || V >= (1 << 22) || blank < 0 || blank >= V || !lse || !prefix)
+    if (!compact_args_ok(N, STU, V, blank) || !lse || !prefix || !pairs_aligned(pair_grads))
         return RNNT_STATUS_INVALID_ARGUMENT;
-    if (reinterpret_cast<uintptr_t>(pair_grads) & 7u) return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0 || STU == 0) return RNNT_STATUS_SUCCESS;
     const Problem p = {xn, yn, prefix, prefix + N, N, 0, 0, 1};
     RNNT_TRY(launch_expand_logits_compact((cudaStream_t)stream, logits, lse, reinterpret_cast<const float2 *>(pair_grads),
@@ -481,60 +531,22 @@ int rnnt_b200_rescale(void *stream, void *grads, const float *grad_out, int grad
 int rnnt_b200_loss_pairs(void *stream, void *workspace, size_t workspace_bytes, const float *pairs, const int *xn,
                          const int *yn, float *costs, float *pair_grads, int N, int T, int U,
                          float fastemit_lambda, int lse_mode) {
-    if (!dense_args_ok(N, T, U, 2)) return RNNT_STATUS_INVALID_ARGUMENT;
-    if ((reinterpret_cast<uintptr_t>(pairs) & 7u) || (reinterpret_cast<uintptr_t>(pair_grads) & 7u))
+    if (!dense_args_ok(N, T, U, 2, 0) || !pairs_aligned(pairs) || !pairs_aligned(pair_grads))
         return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
-    cudaStream_t s = (cudaStream_t)stream;
-    const int64_t cells = (int64_t)N * T * U;
-    FusedPlan plan;
-    if (want_fused(N, T, U, &plan)) {
-        RNNT_TRY(launch_fused(s, resolve_kind(lse_mode, false), plan, pairs, nullptr, xn, yn, costs, nullptr,
-                              reinterpret_cast<float2 *>(pair_grads), nullptr, N, T, U, 2, 0, fastemit_lambda, 1, 1),
-                 RNNT_STATUS_WARP_FAILED);
-        return RNNT_STATUS_SUCCESS;
-    }
-    const Workspace w = carve(workspace, cells, N);
-    if (!workspace || workspace_bytes < w.bytes) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
-    Problem p = {xn, yn, nullptr, nullptr, N, T, U, 0};
-    const float2 *pr = reinterpret_cast<const float2 *>(pairs);
-    RNNT_TRY(launch_wavefront(s, resolve_kind(lse_mode, false), p, pr, w.alphas, w.betas, w.ll, w.bad, costs,
-                              pair_grads == nullptr, 1, T, U),
-             RNNT_STATUS_WARP_FAILED);
-    if (pair_grads)
-        RNNT_TRY(launch_grads_pairs(s, p, pr, w.alphas, w.betas, w.bad, fastemit_lambda,
-                                    reinterpret_cast<float2 *>(pair_grads), cells),
-                 RNNT_STATUS_GRADS_BLANK_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    LossCall c = dense_call(xn, yn, N, T, U, costs, fastemit_lambda, lse_mode);
+    c.pairs = reinterpret_cast<const float2 *>(pairs); c.pair_grads = reinterpret_cast<float2 *>(pair_grads);
+    return run_loss((cudaStream_t)stream, workspace, workspace_bytes, c);
 }
 
 int rnnt_b200_gather_forward(void *stream, void *workspace, size_t workspace_bytes, const float *log_probs,
                              const int *labels, const int *xn, const int *yn, float *costs, float *pair_grads,
                              int N, int T, int U, int V, int blank, float fastemit_lambda, int lse_mode) {
-    if (!dense_args_ok(N, T, U, V) || blank < 0 || blank >= V) return RNNT_STATUS_INVALID_ARGUMENT;
-    if (reinterpret_cast<uintptr_t>(pair_grads) & 7u) return RNNT_STATUS_INVALID_ARGUMENT;
+    if (!dense_args_ok(N, T, U, V, blank) || !pairs_aligned(pair_grads)) return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
-    cudaStream_t s = (cudaStream_t)stream;
-    const int64_t cells = (int64_t)N * T * U;
-    FusedPlan plan;
-    if (want_fused(N, T, U, &plan)) {
-        RNNT_TRY(launch_fused(s, resolve_kind(lse_mode, false), plan, log_probs, labels, xn, yn, costs, nullptr,
-                              reinterpret_cast<float2 *>(pair_grads), nullptr, N, T, U, V, blank, fastemit_lambda, 0, 1),
-                 RNNT_STATUS_WARP_FAILED);
-        return RNNT_STATUS_SUCCESS;
-    }
-    const Workspace w = carve(workspace, cells, N);
-    if (!workspace || workspace_bytes < w.bytes) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
-    Problem p = {xn, yn, nullptr, nullptr, N, T, U, 0};
-    RNNT_TRY(launch_gather(s, p, log_probs, labels, V, blank, w.pairs, nullptr, cells), RNNT_STATUS_GATHER_FAILED);
-    RNNT_TRY(launch_wavefront(s, resolve_kind(lse_mode, false), p, w.pairs, w.alphas, w.betas, w.ll, w.bad, costs,
-                              pair_grads == nullptr, 1, T, U),
-             RNNT_STATUS_WARP_FAILED);
-    if (pair_grads)
-        RNNT_TRY(launch_grads_pairs(s, p, w.pairs, w.alphas, w.betas, w.bad, fastemit_lambda,
-                                    reinterpret_cast<float2 *>(pair_grads), cells),
-                 RNNT_STATUS_GRADS_BLANK_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    LossCall c = dense_call(xn, yn, N, T, U, costs, fastemit_lambda, lse_mode);
+    c.lp = log_probs; c.labels = labels; c.V = V; c.blank = blank; c.pair_grads = reinterpret_cast<float2 *>(pair_grads);
+    return run_loss((cudaStream_t)stream, workspace, workspace_bytes, c);
 }
 
 int rnnt_b200_logits_forward(void *stream, void *workspace, size_t workspace_bytes, const float *logits,
@@ -570,8 +582,7 @@ int rnnt_b200_logits_backward_bf16(void *stream, const void *logits_bf16, const 
 
 int rnnt_b200_gather_backward(void *stream, const float *pair_grads, const int *labels, const float *grad_out,
                               float *out, int N, int T, int U, int V, int blank, int accumulate, const int *yn) {
-    if (!dense_args_ok(N, T, U, V) || blank < 0 || blank >= V) return RNNT_STATUS_INVALID_ARGUMENT;
-    if (reinterpret_cast<uintptr_t>(pair_grads) & 7u) return RNNT_STATUS_INVALID_ARGUMENT;
+    if (!dense_args_ok(N, T, U, V, blank) || !pairs_aligned(pair_grads)) return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
     Problem p = {nullptr, yn, nullptr, nullptr, N, T, U, 0};     // yn (optional): which labels are real
     ExpandSrc src = {};
@@ -579,7 +590,7 @@ int rnnt_b200_gather_backward(void *stream, const float *pair_grads, const int *
     src.scale = grad_out;
     src.labels = labels;
     src.label_adds = accumulate ? 1 : 0;
-    RNNT_TRY(launch_expand((cudaStream_t)stream, p, src, out, (int64_t)N * T * U, V, blank),
+    RNNT_TRY(launch_expand((cudaStream_t)stream, p, src, out, (int64_t)N * T * U, V, blank, false, 0),
              RNNT_STATUS_GRADS_BLANK_FAILED);
     return RNNT_STATUS_SUCCESS;
 }
@@ -588,34 +599,16 @@ int rnnt_b200_compact_forward(void *stream, void *workspace, size_t workspace_by
                               const int *xn, const int *yn, float *costs, float *pair_grads, int64_t *loc,
                               int *totals, int64_t STU, int N, int V, int blank, float fastemit_lambda,
                               int lse_mode, int max_T, int max_U) {
-    if (N < 0 || STU < 0 || V < 1 || V >= (1 << 22) || blank < 0 || blank >= V) return RNNT_STATUS_INVALID_ARGUMENT;
-    if (reinterpret_cast<uintptr_t>(pair_grads) & 7u) return RNNT_STATUS_INVALID_ARGUMENT;
+    if (!compact_args_ok(N, STU, V, blank) || !pairs_aligned(pair_grads)) return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
     cudaStream_t s = (cudaStream_t)stream;
-    const Workspace w = carve(workspace, STU, N);
-    if (!workspace || workspace_bytes < w.bytes) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    Workspace w;
+    if (!carve_ok(workspace, workspace_bytes, STU, N, &w)) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
     RNNT_TRY(launch_prefix(s, xn, yn, N, w.mem_pref, w.lab_pref, totals ? totals : w.totals), RNNT_STATUS_GATHER_FAILED);
-    Problem p = {xn, yn, w.mem_pref, w.lab_pref, N, 0, 0, 1};
-    FusedPlan fplan;
-    if (max_T > 0 && max_U > 0 && want_fused(N, max_T, max_U, &fplan)) {
-        // small lattices: gather + wavefront + (cells,2) gradients + loc in one launch (no mismatch guard in the
-        // compact reference, core_compact.cu:347-358)
-        RNNT_TRY(launch_fused(s, resolve_kind(lse_mode, true), fplan, xs, ys, xn, yn, costs, nullptr,
-                              reinterpret_cast<float2 *>(pair_grads), nullptr, N, max_T, max_U, V, blank,
-                              fastemit_lambda, 0, 0, w.mem_pref, w.lab_pref, loc),
-                 RNNT_STATUS_WARP_FAILED);
-        return RNNT_STATUS_SUCCESS;
-    }
-    RNNT_TRY(launch_gather(s, p, xs, ys, V, blank, w.pairs, loc, STU), RNNT_STATUS_GATHER_FAILED);
-    // no mismatch guard in the compact reference (core_compact.cu:347-358)
-    RNNT_TRY(launch_wavefront(s, resolve_kind(lse_mode, true), p, w.pairs, w.alphas, w.betas, w.ll, w.bad, costs,
-                              pair_grads == nullptr, 0, max_T, max_U),
-             RNNT_STATUS_WARP_FAILED);
-    if (pair_grads)
-        RNNT_TRY(launch_grads_pairs(s, p, w.pairs, w.alphas, w.betas, nullptr, fastemit_lambda,
-                                    reinterpret_cast<float2 *>(pair_grads), STU),
-                 RNNT_STATUS_GRADS_BLANK_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    LossCall c = compact_call(xn, yn, w.mem_pref, w.lab_pref, N, STU, max_T, max_U, costs, fastemit_lambda, lse_mode);
+    c.lp = xs; c.labels = ys; c.V = V; c.blank = blank; c.loc = loc;
+    c.pair_grads = reinterpret_cast<float2 *>(pair_grads);
+    return run_loss(s, workspace, workspace_bytes, c);
 }
 
 int rnnt_b200_logits_compact_forward(void *stream, void *workspace, size_t workspace_bytes, const float *logits,
@@ -682,8 +675,7 @@ int rnnt_b200_joint_pack_backward(void *stream, const float *dx, const int *lf, 
 
 int rnnt_b200_compact_backward(void *stream, const float *grad_cost, const float *pair_grads, const int64_t *loc,
                                const int *cum_lens, float *out, int64_t STU, int N, int V, int blank) {
-    if (N < 0 || STU < 0 || V < 1 || V >= (1 << 22) || blank < 0 || blank >= V) return RNNT_STATUS_INVALID_ARGUMENT;
-    if (reinterpret_cast<uintptr_t>(pair_grads) & 7u) return RNNT_STATUS_INVALID_ARGUMENT;
+    if (!compact_args_ok(N, STU, V, blank) || !pairs_aligned(pair_grads)) return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0 || STU == 0) return RNNT_STATUS_SUCCESS;
     Problem p = {nullptr, nullptr, nullptr, nullptr, N, 0, 0, 1};
     ExpandSrc src = {};
@@ -691,7 +683,7 @@ int rnnt_b200_compact_backward(void *stream, const float *grad_cost, const float
     src.scale = grad_cost;
     src.loc = loc;
     src.cum_lens = cum_lens;
-    RNNT_TRY(launch_expand((cudaStream_t)stream, p, src, out, STU, V, blank), RNNT_STATUS_GRADS_BLANK_FAILED);
+    RNNT_TRY(launch_expand((cudaStream_t)stream, p, src, out, STU, V, blank, false, 0), RNNT_STATUS_GRADS_BLANK_FAILED);
     return RNNT_STATUS_SUCCESS;
 }
 
@@ -709,7 +701,7 @@ int run_warp_rnnt(void *stream, unsigned int *counts, float *alphas, float *beta
                   const float *log_probs, float *grads, float *costs, const int *xn, const int *yn, int N, int T,
                   int U, int V, int blank, float fastemit_lambda) {
     (void)counts;
-    if (!dense_args_ok(N, T, U, V) || blank < 0 || blank >= V) return RNNT_STATUS_WARP_FAILED;
+    if (!dense_args_ok(N, T, U, V, blank)) return RNNT_STATUS_WARP_FAILED;
     if (N == 0) return RNNT_STATUS_SUCCESS;
     cudaStream_t s = (cudaStream_t)stream;
     const int64_t cells = (int64_t)N * T * U;
@@ -722,16 +714,17 @@ int run_warp_rnnt(void *stream, unsigned int *counts, float *alphas, float *beta
     int *bad = (int *)(tmp + pair_bytes + align_up(sizeof(float) * 2 * N, 256));
     Problem p = {xn, yn, nullptr, nullptr, N, T, U, 0};
     int status = RNNT_STATUS_SUCCESS;
-    if (launch_gather(s, p, log_probs, labels, V, blank, pairs, nullptr, cells) != cudaSuccess)
+    if (launch_gather(s, p, log_probs, labels, V, blank, pairs, nullptr, cells, 0) != cudaSuccess)
         status = RNNT_STATUS_WARP_FAILED;
-    if (!status && launch_wavefront(s, resolve_kind(RNNT_LSE_AUTO, false), p, pairs, alphas, betas, ll, bad, costs, 0,
-                                    1, T, U) != cudaSuccess)
+    if (!status && launch_wavefront(s, fast_lse(RNNT_LSE_AUTO), p, pairs, alphas, betas, ll, bad, costs, 0, T, U) !=
+                       cudaSuccess)
         status = RNNT_STATUS_WARP_FAILED;
     if (!status) {
         ExpandSrc src = {};
         src.pairs = pairs; src.alphas = alphas; src.betas = betas; src.bad = bad;
         src.labels = labels; src.fastemit_lambda = fastemit_lambda;
-        if (launch_expand(s, p, src, grads, cells, V, blank) != cudaSuccess) status = RNNT_STATUS_GRADS_BLANK_FAILED;
+        if (launch_expand(s, p, src, grads, cells, V, blank, false, 0) != cudaSuccess)
+            status = RNNT_STATUS_GRADS_BLANK_FAILED;
     }
     cudaFreeAsync(tmp, s);
     return status;
@@ -741,7 +734,7 @@ int run_warp_rnnt_gather(void *stream, unsigned int *counts, float *alphas, floa
                          float *grads, float *costs, const int *xn, const int *yn, int N, int T, int U,
                          float fastemit_lambda) {
     (void)counts;
-    if (!dense_args_ok(N, T, U, 2)) return RNNT_STATUS_WARP_FAILED;
+    if (!dense_args_ok(N, T, U, 2, 0)) return RNNT_STATUS_WARP_FAILED;
     if (N == 0) return RNNT_STATUS_SUCCESS;
     cudaStream_t s = (cudaStream_t)stream;
     const int64_t cells = (int64_t)N * T * U;
@@ -754,8 +747,7 @@ int run_warp_rnnt_gather(void *stream, unsigned int *counts, float *alphas, floa
     Problem p = {xn, yn, nullptr, nullptr, N, T, U, 0};
     const float2 *pr = reinterpret_cast<const float2 *>(log_probs);
     int status = RNNT_STATUS_SUCCESS;
-    if (launch_wavefront(s, resolve_kind(RNNT_LSE_AUTO, false), p, pr, alphas, betas, ll, bad, costs, 0, 1, T, U) !=
-        cudaSuccess)
+    if (launch_wavefront(s, fast_lse(RNNT_LSE_AUTO), p, pr, alphas, betas, ll, bad, costs, 0, T, U) != cudaSuccess)
         status = RNNT_STATUS_WARP_FAILED;
     if (!status && launch_grads_pairs(s, p, pr, alphas, betas, bad, fastemit_lambda, reinterpret_cast<float2 *>(grads),
                                       cells) != cudaSuccess)
@@ -780,7 +772,7 @@ void run_gather_for_compact(const float *xs, const int *ys, const unsigned int *
     bool ok = launch_prefix(s, xi, yi, (int)N, mp, lp, totals) == cudaSuccess;
     Problem p = {xi, yi, mp, lp, (int)N, 0, 0, 1};
     ok = ok && launch_gather(s, p, xs, ys, (int)V, (int)blank, reinterpret_cast<float2 *>(gather_xs),
-                             reinterpret_cast<int64_t *>(loc), (int64_t)N * T * U) == cudaSuccess;
+                             reinterpret_cast<int64_t *>(loc), (int64_t)N * T * U, 0) == cudaSuccess;
     cudaFreeAsync(tmp, s);
     if (!ok) compat_die("rnnt loss gather for compact", RNNT_STATUS_GATHER_FAILED);
 }
@@ -803,8 +795,8 @@ void run_warp_rnnt_compact(unsigned int *counts, float *alphas, float *betas, co
     bool ok = launch_prefix(s, xi, yi, (int)N, mp, lp, totals) == cudaSuccess;
     Problem p = {xi, yi, mp, lp, (int)N, 0, 0, 1};
     const float2 *pr = reinterpret_cast<const float2 *>(log_probs);
-    ok = ok && launch_wavefront(s, resolve_kind(RNNT_LSE_AUTO, true), p, pr, alphas, betas, ll, nullptr, costs,
-                                required_grad ? 0 : 1, 0, (int)T, (int)U) == cudaSuccess;
+    ok = ok && launch_wavefront(s, fast_lse(RNNT_LSE_AUTO), p, pr, alphas, betas, ll, nullptr, costs,
+                                required_grad ? 0 : 1, (int)T, (int)U) == cudaSuccess;
     if (ok && required_grad)
         ok = launch_grads_pairs(s, p, pr, alphas, betas, nullptr, fastemit_lambda, reinterpret_cast<float2 *>(grads),
                                 (int64_t)N * T * U) == cudaSuccess;

@@ -14,6 +14,7 @@
 #include <mutex>
 #include <string>
 #include <tuple>
+#include <utility>
 
 #include <c10/cuda/CUDAGuard.h>
 #include <c10/cuda/CUDAStream.h>
@@ -75,6 +76,28 @@ unsigned int *next_sync_counter(const at::Tensor &like) {
     std::lock_guard<std::mutex> lock(mu);
     if (!ring[dev].defined()) ring[dev] = at::zeros({kSlots}, like.options().dtype(at::kInt));
     return reinterpret_cast<unsigned int *>(ring[dev].data_ptr<int>()) + (next[dev]++ % kSlots);
+}
+
+// Upper bounds (max_T, max_U) of the lattices of a compact call: the caller's hints when both are positive (no host
+// sync, CUDA-graph capturable), else one 16-byte device->host copy of the device totals (the reference needs four
+// .item() syncs), which also checks ys and xs against xn and yn.  scratch: (2N) int64 for the prefix sums, or null.
+std::pair<int, int> compact_bounds(void *stream, const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn,
+                                   const at::Tensor &yn, int hint_T, int hint_U, int64_t *scratch) {
+    if (hint_T > 0 && hint_U > 0) return {hint_T, hint_U};
+    const int64_t N = xn.size(0);
+    at::Tensor own;
+    if (!scratch) {
+        own = at::empty({2 * N}, xs.options().dtype(at::kLong));
+        scratch = own.data_ptr<int64_t>();
+    }
+    at::Tensor totals = at::empty({4}, xs.options().dtype(at::kInt));
+    check_status(rnnt_b200_compact_totals(stream, xn.data_ptr<int>(), yn.data_ptr<int>(), (int)N, scratch,
+                                          totals.data_ptr<int>()));
+    at::Tensor h = totals.cpu();
+    const int *t = h.data_ptr<int>();
+    TORCH_CHECK(ys.numel() == t[1], "ys shape must be equal to (sum(yn), )");
+    TORCH_CHECK(xs.size(0) == t[0], "xs shape mismatch with (\\sum{xn*(yn+1)}, )");
+    return {t[2], t[3]};
 }
 
 // dense forward (+ gradients), optional per-sample scale, explicit LSE mode; loss_sum: (1) tensor or undefined
@@ -155,24 +178,7 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_loss_compact(const at::Tenso
     // placeholder the caller must not use
     at::Tensor grads = required_grad ? at::empty({STU, 2}, xs.options()) : at::empty({0}, xs.options());
     if (N == 0) return std::make_tuple(costs, grads, loc);
-    int max_T = 0, max_U = 0;
-    // shape validation: one 16-byte device->host copy (the reference needs four .item() syncs) -- or none at all
-    // when the caller vouches for upper bounds of xn and yn+1 (sync-free, CUDA-graph capturable)
-    if (hint_T > 0 && hint_U > 0) {
-        max_T = hint_T;
-        max_U = hint_U;
-    } else {
-        at::Tensor scratch = at::empty({2 * N}, xs.options().dtype(at::kLong));
-        at::Tensor totals = at::empty({4}, xs.options().dtype(at::kInt));
-        check_status(rnnt_b200_compact_totals(stream, xn.data_ptr<int>(), yn.data_ptr<int>(), (int)N,
-                                              scratch.data_ptr<int64_t>(), totals.data_ptr<int>()));
-        at::Tensor h = totals.cpu();
-        const int *t = h.data_ptr<int>();
-        TORCH_CHECK(ys.numel() == t[1], "ys shape must be equal to (sum(yn), )");
-        TORCH_CHECK(STU == t[0], "xs shape mismatch with (\\sum{xn*(yn+1)}, )");
-        max_T = t[2];
-        max_U = t[3];
-    }
+    const auto [max_T, max_U] = compact_bounds(stream, xs, ys, xn, yn, hint_T, hint_U, nullptr);
     at::Tensor ws = workspace_for(xs, STU, N);
     check_status(rnnt_b200_compact_forward(stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr<float>(),
                                            ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
@@ -367,17 +373,7 @@ rnnt_logits_compact_forward(const at::Tensor &xs, const at::Tensor &ys, const at
     at::Tensor pg = want_grads ? at::empty({STU, 2}, f32) : at::empty({0}, f32);
     at::Tensor prefix = at::empty({2 * N}, xs.options().dtype(at::kLong));
     if (N == 0) return std::make_tuple(costs, lse, pg, prefix);
-    if (!(max_T > 0 && max_U > 0)) {
-        at::Tensor totals = at::empty({4}, xs.options().dtype(at::kInt));
-        check_status(rnnt_b200_compact_totals(stream, xn.data_ptr<int>(), yn.data_ptr<int>(), (int)N,
-                                              prefix.data_ptr<int64_t>(), totals.data_ptr<int>()));
-        at::Tensor h = totals.cpu();
-        const int *t = h.data_ptr<int>();
-        TORCH_CHECK(ys.numel() == t[1], "ys shape must be equal to (sum(yn), )");
-        TORCH_CHECK(STU == t[0], "xs shape mismatch with (\\sum{xn*(yn+1)}, )");
-        max_T = t[2];
-        max_U = t[3];
-    }
+    std::tie(max_T, max_U) = compact_bounds(stream, xs, ys, xn, yn, max_T, max_U, prefix.data_ptr<int64_t>());
     at::Tensor ws = workspace_for(xs, STU, N);
     float *pgp = want_grads ? pg.data_ptr<float>() : nullptr;
     if (bf16)

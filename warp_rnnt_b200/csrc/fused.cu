@@ -1004,18 +1004,19 @@ static cudaError_t launch_fused_km(cudaStream_t s, const FusedArgs &a, size_t sm
     }
 }
 
-cudaError_t launch_fused(cudaStream_t s, int kind, const FusedPlan &plan, const void *lp, const int *labels,
-                         const int *xn, const int *yn, float *costs, void *grads, float2 *pair_grads,
-                         const float *scale, int N, int T, int U, int V, int blank, float lam, int pairs_in,
-                         int guard, const int64_t *mem_pref, const int64_t *lab_pref, int64_t *loc, float *loss_sum,
-                         unsigned *sync_counter, int io_bf16) {
+cudaError_t launch_fused(cudaStream_t s, const FusedPlan &plan, const FusedCall &c) {
+    const void *lp = c.lp;
+    void *grads = c.grads;
+    const int N = c.N, T = c.T, U = c.U, V = c.V, pairs_in = c.pairs_in, io_bf16 = c.io_bf16;
+    const int kind = lse_kind(c.fast_lse, c.mem_pref != nullptr);
     FusedArgs a;
-    if (io_bf16 && (!grads || pairs_in || mem_pref)) return cudaErrorInvalidValue;   // bf16 i/o: dense gradients only
-    a.loss_sum = sync_counter ? loss_sum : nullptr; a.sync_counter = sync_counter;
-    a.mem_pref = mem_pref; a.lab_pref = lab_pref; a.loc = loc;
-    a.lp = lp; a.labels = labels; a.xn = xn; a.yn = yn; a.costs = costs; a.grads = grads; a.pair_grads = pair_grads;
-    a.scale = scale; a.N = N; a.T = T; a.U = U; a.V = V; a.blank = blank; a.lam = lam; a.pairs_in = pairs_in;
-    a.guard = guard; a.slices = (grads || pair_grads) ? plan.slices : 1; a.Wd = plan.W; a.nd = plan.ring;
+    if (io_bf16 && (!grads || pairs_in || c.mem_pref)) return cudaErrorInvalidValue;   // bf16 i/o: dense gradients only
+    a.loss_sum = c.sync_counter ? c.loss_sum : nullptr; a.sync_counter = c.sync_counter;
+    a.mem_pref = c.mem_pref; a.lab_pref = c.lab_pref; a.loc = c.loc;
+    a.lp = lp; a.labels = c.labels; a.xn = c.xn; a.yn = c.yn; a.costs = c.costs; a.grads = grads;
+    a.pair_grads = c.pair_grads; a.scale = c.scale; a.N = N; a.T = T; a.U = U; a.V = V; a.blank = c.blank; a.lam = c.lam;
+    a.pairs_in = pairs_in; a.guard = c.mem_pref == nullptr;   // no mismatch guard in the compact reference
+    a.slices = (grads || c.pair_grads) ? plan.slices : 1; a.Wd = plan.W; a.nd = plan.ring;
     {
         static const int gw_raw = env_int("RNNT_B200_GATHER_WARPS", 0);   // tuning knob, in [1,14]
         const int gw_env = (gw_raw < 1 || gw_raw > kFusedThreads / 32 - 2) ? 0 : gw_raw;

@@ -12,11 +12,16 @@ GuardPoison guard_poison();
 
 cudaError_t launch_prefix(cudaStream_t s, const int *xn, const int *yn, int N, int64_t *mem_pref,
                           int64_t *lab_pref, int *totals);
+// The LSE flavour of a launch: the fast one, else the reference's exact formula of the layout (dense or compact).
+inline int lse_kind(bool fast_lse, bool compact) { return fast_lse ? kFast : compact ? kExactCompact : kExactDense; }
+
 cudaError_t launch_gather(cudaStream_t s, const Problem &p, const void *lp, const int *labels, int V, int blank,
-                          float2 *pairs, int64_t *loc, int64_t cells_hint, int io_bf16 = 0);
-cudaError_t launch_wavefront(cudaStream_t s, int kind, const Problem &p, const float2 *pairs, float *alphas,
-                             float *betas, float *ws_ll, int *bad, float *costs, int beta_only, int guard,
-                             int t_hint, int u_hint);
+                          float2 *pairs, int64_t *loc, int64_t cells_hint, int io_bf16);
+// the LSE kind follows p's layout; the forward/backward mismatch guard runs on the dense layout only (the compact
+// reference has none, core_compact.cu:347-358)
+cudaError_t launch_wavefront(cudaStream_t s, bool fast_lse, const Problem &p, const float2 *pairs, float *alphas,
+                             float *betas, float *ws_ll, int *bad, float *costs, int beta_only, int t_hint,
+                             int u_hint);
 cudaError_t launch_grads_pairs(cudaStream_t s, const Problem &p, const float2 *pairs, const float *alphas,
                                const float *betas, const int *bad, float fastemit_lambda, float2 *out,
                                int64_t cells_hint);
@@ -38,15 +43,15 @@ struct ExpandSrc {
     int label_adds;          // 1: label == blank accumulates (torch scatter_add semantics of gather=True)
 };
 cudaError_t launch_expand(cudaStream_t s, const Problem &p, const ExpandSrc &src, void *out, int64_t cells,
-                          int V, int blank, bool retire_early = false, int io_bf16 = 0);   // io_bf16: bf16 output (forward emit)
+                          int V, int blank, bool retire_early, int io_bf16);   // io_bf16: bf16 output (forward emit)
 
 // logits.cu -- loss from un-normalised logits (fused log_softmax forward / backward).  io_bf16: the logits (and the
 // gradient written by launch_expand_logits) are bf16, else float; lse, pairs, pg and grad_out are float either way.
 cudaError_t launch_lse_pairs(cudaStream_t s, const void *x, const int *labels, int N, int T, int U, int V, int blank,
-                             float2 *pairs, float *lse, int io_bf16 = 0);
+                             float2 *pairs, float *lse, int io_bf16);
 cudaError_t launch_expand_logits(cudaStream_t s, const void *x, const float *lse, const float2 *pg, const int *labels,
                                  const float *grad_out, void *out, int N, int T, int U, int V, int blank,
-                                 int io_bf16 = 0);
+                                 int io_bf16);
 // ... the same two passes over compact (STU,V) logits in joint_pack's row order: p is the compact Problem (prefix sums
 // on the device), labels (sum yn), grad_out (N) or nullptr
 cudaError_t launch_lse_pairs_compact(cudaStream_t s, const void *x, const Problem &p, const int *labels, int64_t STU,
@@ -65,17 +70,31 @@ cudaError_t launch_joint_grads(cudaStream_t s, const float *dx, const int *lf, c
 struct FusedPlan { int W, ring, nw, slices; size_t smem; };
 bool fused_plan(int N, int T, int U, FusedPlan *plan);
 void set_fused_trace(long long *buf);   // diagnostics: per-CTA phase stamps of k_fused (8 x clock64 per CTA)
-cudaError_t launch_fused(cudaStream_t s, int kind, const FusedPlan &plan, const void *lp, const int *labels,
-                         const int *xn, const int *yn, float *costs, void *grads, float2 *pair_grads,
-                         const float *scale, int N, int T, int U, int V, int blank, float lam, int pairs_in,
-                         int guard, const int64_t *mem_pref = nullptr, const int64_t *lab_pref = nullptr,
-                         int64_t *loc = nullptr,   // mem_pref != null: compact layout, T/U = max lengths
-                         float *loss_sum = nullptr, unsigned *sync_counter = nullptr,    // fused sum_n costs[n]*scale[n]
-                         int io_bf16 = 0);   // log_probs and the dense gradient are bf16 (dense MODE only)
+// One fused launch, filled by name; fields left zero are off.  The layout follows mem_pref: null = dense (N,T,U),
+// with the mismatch guard; set = compact (T, U = max lengths), without it.  The LSE kind follows fast_lse and the layout.
+struct FusedCall {
+    bool fast_lse;
+    const void *lp;                       // log-probs (N,T,U,V) or compact (STU,V); pairs_in: (cells,2) f32 pairs
+    const int *labels;                    // dense (N,U-1), compact (sum yn); null with pairs_in
+    const int *xn, *yn;
+    const int64_t *mem_pref, *lab_pref;   // compact: first cell / first label of lattice n
+    int64_t *loc;                         // compact: label id per cell, or null
+    float *costs;
+    void *grads;                          // dense gradient (N,T,U,V) of the element type, or null
+    float2 *pair_grads;                   // (cells,2) gradient, or null
+    const float *scale;                   // (N) or null
+    float *loss_sum;                      // sum_n costs[n]*scale[n] in the kernel; needs sync_counter
+    unsigned *sync_counter;
+    int N, T, U, V, blank;
+    float lam;
+    int pairs_in;
+    int io_bf16;                          // log_probs and the dense gradient are bf16 (dense gradient only)
+};
+cudaError_t launch_fused(cudaStream_t s, const FusedPlan &plan, const FusedCall &c);
 
 // expand.cu -- small helpers of the python-level API
 cudaError_t launch_loss_sum(cudaStream_t s, const float *costs, const float *scale, int N, float *loss_sum);
 cudaError_t launch_rescale(cudaStream_t s, void *grads, const float *grad_out, int grad_out_stride,
-                           const float *applied, int N, int64_t elems_per_sample, int io_bf16 = 0);
+                           const float *applied, int N, int64_t elems_per_sample, int io_bf16);
 
 }  // namespace rnnt

@@ -604,10 +604,11 @@ static cudaError_t launch_wavefront_kind(cudaStream_t s, const Problem &p, const
     return launch_wavefront_kp<KIND, PF>(s, p, pairs, alphas, betas, ws_ll, bad, costs, beta_only, guard, t_hint, u_hint);
 }
 
-cudaError_t launch_wavefront(cudaStream_t s, int kind, const Problem &p, const float2 *pairs, float *alphas,
-                             float *betas, float *ws_ll, int *bad, float *costs, int beta_only, int guard,
-                             int t_hint, int u_hint) {
-    switch (kind) {
+cudaError_t launch_wavefront(cudaStream_t s, bool fast_lse, const Problem &p, const float2 *pairs, float *alphas,
+                             float *betas, float *ws_ll, int *bad, float *costs, int beta_only, int t_hint,
+                             int u_hint) {
+    const int guard = !p.compact;
+    switch (lse_kind(fast_lse, p.compact)) {
         case kExactDense:
             return launch_wavefront_kind<kExactDense>(s, p, pairs, alphas, betas, ws_ll, bad, costs, beta_only, guard, t_hint, u_hint);
         case kExactCompact:
