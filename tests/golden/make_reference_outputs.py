@@ -22,7 +22,7 @@ import torch  # noqa: E402
 
 from oracle import build_ref  # noqa: E402
 from tests import test_gpu_fullsize as F, test_gpu_holes as H, test_gpu_logits as L, test_gpu_parity as P  # noqa: E402
-from tests import test_gpu_nonfinite as NF  # noqa: E402
+from tests import test_gpu_launch_configs as LC, test_gpu_nonfinite as NF  # noqa: E402
 from tests.common import REF_OUTPUTS, input_sample, make_inputs, record, to_compact  # noqa: E402
 
 
@@ -115,6 +115,14 @@ def main(out):
         dense(rec, "logits_%d" % k, ref, (lp.contiguous(), cu(ys), cu(xn), cu(yn)), blank=blank, fastemit_lambda=lam)
     # tests/test_gpu_nonfinite.py: masked and non-finite log-probs
     NF.record_reference(rec, ref)
+    # tests/test_gpu_launch_configs.py: one case on each side of each planner bound
+    for name in LC.REF_CASES:
+        lp, ys, xn, yn, blank = LC.case_inputs(name)
+        dense(rec, "launch_%s/dense" % name, ref, (cu(lp), cu(ys), cu(xn), cu(yn)), blank=blank, fastemit_lambda=LC.LAM)
+        g = P.gather_np(lp, ys, blank)
+        dense(rec, "launch_%s/gather" % name, ref, (cu(g), cu(ys), cu(xn), cu(yn)), blank=-1, fastemit_lambda=LC.LAM)
+        xs_c, ys_c = to_compact(lp, ys, xn, yn)
+        compact(rec, "launch_%s/compact" % name, ref, (cu(xs_c), cu(ys_c), cu(xn), cu(yn)), blank, LC.LAM)
     torch.cuda.synchronize()
     np.savez_compressed(out, **rec)
     print("wrote %s: %d arrays, %d bytes" % (out, len(rec), os.path.getsize(out)))

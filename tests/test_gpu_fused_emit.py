@@ -178,10 +178,11 @@ def _forced_compose_main(out_dir):
         np.save(os.path.join(out_dir, "grads_%d.npy" % i), g)
 
 
-def subprocess_outputs(env_name, env_value, main):
+def subprocess_outputs(env_name, env_value, main, module="tests.test_gpu_fused_emit"):
+    """Run module.main(out_dir) in a fresh process with env_name=env_value -> {file name: array} it saved."""
     with tempfile.TemporaryDirectory() as d:
         env = dict(os.environ, **{env_name: env_value})
-        code = "import sys; sys.path.insert(0, %r); from tests.test_gpu_fused_emit import %s; %s(%r)" % (ROOT, main, main, d)
+        code = "import sys; sys.path.insert(0, %r); from %s import %s; %s(%r)" % (ROOT, module, main, main, d)
         r = subprocess.run([sys.executable, "-c", code], env=env, cwd=ROOT, capture_output=True, text=True)
         assert r.returncode == 0, r.stdout + r.stderr
         return {k: np.load(os.path.join(d, k)) for k in os.listdir(d)}

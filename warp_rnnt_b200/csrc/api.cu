@@ -21,6 +21,17 @@ static std::atomic<int> g_poison_n{-1};
 static std::atomic<float> g_poison_delta{0.0f};
 GuardPoison guard_poison() { return {g_poison_n.load(std::memory_order_relaxed), g_poison_delta.load(std::memory_order_relaxed)}; }
 
+// per thread, so that calls from several host threads (one per device) neither race nor see each other's launches
+static thread_local int32_t t_record[RNNT_LAUNCH_RECORD_LEN];
+static thread_local int32_t t_record_seq;
+int32_t *launch_record() { return t_record; }
+void begin_launch_record(int path) {
+    memset(t_record, 0, sizeof(t_record));
+    t_record[RNNT_REC_SEQ] = ++t_record_seq;
+    t_record[RNNT_REC_PATH] = path;
+    t_record[RNNT_REC_GROUPS] = 1;
+}
+
 static int env_lse_mode() {
     const char *e = getenv("RNNT_B200_LSE");
     if (!e) return RNNT_LSE_AUTO;
@@ -350,7 +361,11 @@ static int run_loss(cudaStream_t s, void *workspace, size_t workspace_bytes, con
     const int groups = pipeline_groups(c);
     if (groups > 1) {
         std::lock_guard<std::mutex> lock(g_pipe_mu);    // the pipeline's events are shared by all calls on this device
-        if (Pipeline *pl = get_pipeline_locked()) return run_pipelined(s, pl, c, w, groups);
+        if (Pipeline *pl = get_pipeline_locked()) {
+            const int status = run_pipelined(s, pl, c, w, groups);
+            launch_record()[RNNT_REC_GROUPS] = groups;
+            return status;
+        }
     }
     const bool fast = fast_lse(c.lse_mode);
     const float2 *pairs = c.pairs;
@@ -488,6 +503,9 @@ int rnnt_b200_debug_lse_selfcheck(void *stream, unsigned long long *mismatches) 
     return cudaGetLastError() == cudaSuccess ? RNNT_STATUS_SUCCESS : RNNT_STATUS_WARP_FAILED;
 }
 void rnnt_b200_debug_fused_trace(void *buf) { rnnt::set_fused_trace(static_cast<long long *>(buf)); }
+void rnnt_b200_debug_last_launch(int32_t *out) {
+    if (out) memcpy(out, rnnt::launch_record(), sizeof(int32_t) * RNNT_LAUNCH_RECORD_LEN);
+}
 
 size_t rnnt_b200_workspace_bytes(int64_t cells, int N) { return carve(nullptr, cells, N).bytes; }
 

@@ -967,6 +967,7 @@ static cudaError_t launch_fused_kmc(cudaStream_t s, FusedArgs a, size_t smem) {
         const cudaError_t e = ensure_dyn_smem(k_fused<KIND, MODE, C, IO>, attr_done, kFusedMaxDynSmem);
         if (e != cudaSuccess) return e;
     }
+    int occ_queried = 0;
     if (a.slices > 1) {
         // CTAs per lattice: fill every SM with what is actually co-resident (registers can forbid the second
         // CTA that shared memory would allow; a second, partial wave costs more than it brings).  Cached per device.
@@ -987,10 +988,13 @@ static cudaError_t launch_fused_kmc(cudaStream_t s, FusedArgs a, size_t smem) {
             occ = o.occ;
         }
         a.slices = max(1, min(a.slices, (occ * sm_count(dev)) / a.N));
+        occ_queried = occ;
     }
     dim3 grid(a.slices, a.N);
     k_fused<KIND, MODE, C, IO><<<grid, kFusedThreads, smem, s>>>(a);
     count_launch();
+    int32_t *rec = launch_record();
+    rec[RNNT_REC_FUSED_SLICES] = a.slices; rec[RNNT_REC_FUSED_OCC] = occ_queried; rec[RNNT_REC_FUSED_SMEM] = (int32_t)smem;
     return cudaGetLastError();
 }
 
@@ -1077,6 +1081,10 @@ cudaError_t launch_fused(cudaStream_t s, const FusedPlan &plan, const FusedCall 
     { const GuardPoison gp = guard_poison(); a.poison_n = gp.n; a.poison_delta = gp.delta; }
     const bool dense = grads != nullptr;
     const int C = plan.nw;
+    begin_launch_record(1);
+    int32_t *rec = launch_record();
+    rec[RNNT_REC_FUSED_C] = C; rec[RNNT_REC_FUSED_GATHER_WARPS] = a.gwn; rec[RNNT_REC_FUSED_ROW_BUFS] = a.nbuf ? a.nb_per : 0;
+    rec[RNNT_REC_FUSED_COMPOSE] = a.compose; rec[RNNT_REC_FUSED_TMA_FILL] = dense ? a.tma_fill : 0;
     if (io_bf16)
         return kind == kFast ? launch_fused_km<kFast, 0, __nv_bfloat16>(s, a, smem, C)
                              : launch_fused_km<kExactDense, 0, __nv_bfloat16>(s, a, smem, C);

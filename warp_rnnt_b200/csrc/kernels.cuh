@@ -9,6 +9,10 @@ void count_launch();   // api.cu: bumps the library-wide launch counter
 // in front of the forward/backward mismatch guard; n < 0 = off
 struct GuardPoison { int n; float delta; };
 GuardPoison guard_poison();
+// api.cu: the calling thread's record of its last recurrence launch (rnnt_b200_debug_last_launch), indexed by
+// rnntLaunchRecord_t.  begin_launch_record(path) clears it, counts the launch and sets the path (1 fused, 2 general).
+int32_t *launch_record();
+void begin_launch_record(int path);
 
 cudaError_t launch_prefix(cudaStream_t s, const int *xn, const int *yn, int N, int64_t *mem_pref,
                           int64_t *lab_pref, int *totals);

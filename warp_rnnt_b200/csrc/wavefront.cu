@@ -588,6 +588,9 @@ static cudaError_t launch_wavefront_kp(cudaStream_t s, const Problem &p, const f
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     count_launch();
+    begin_launch_record(2);
+    int32_t *rec = launch_record();
+    rec[RNNT_REC_GEN_WARPS] = nwarps; rec[RNNT_REC_GEN_RING] = ring; rec[RNNT_REC_GEN_BETA_ONLY] = beta_only;
     return cudaLaunchKernelEx(&cfg, k_wavefront<KIND, PF>, p, pairs, alphas, betas, ws_ll, bad, costs, beta_only, guard,
                               ring, guard_poison());
 }
