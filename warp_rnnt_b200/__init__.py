@@ -366,6 +366,36 @@ def rnnt_loss(log_probs, labels, frames_lengths, labels_lengths, average_frames=
             f"Unknown reduction method: {reduction}, expected to be one of ['mean', 'sum', 'none']")
 
 
-__all__ = ["rnnt_loss", "rnnt_loss_from_logits", "joint_pack", "JointPack", "RNNTLossFromLogits",
+def rnnt_align(log_probs, labels, frames_lengths, labels_lengths, blank=0, compact=False):
+    """Viterbi forced alignment: the single best alignment of the labels to the frames on the RNN-T lattice, for token
+    timestamps, emission latency (what ``fastemit_lambda`` tunes), alignment-restricted targets or data debugging.
+
+    Inputs are those of ``rnnt_loss``: dense (N, T, U, V) log-probs, float32 or bfloat16, with labels (N, U-1); or
+    ``compact=True``: (STU, V) log-probs, float32 or bfloat16, with labels (sum(labels_lengths),), honouring
+    ``compact_hints``.  frames_lengths, labels_lengths (N,) int32.
+
+    Returns ``(scores, frames)``:
+      * ``scores`` (N,) float32: the largest path score.  A path starts at (0, 0), adds blank[t, u] for each step
+        (t, u) -> (t+1, u) and label[t, u] for each step (t, u) -> (t, u+1), and ends with blank[Tn-1, Un-1]; its
+        score is the float32 sum of those log-probs added left to right in path order.
+      * ``frames`` int32, dense (N, U-1), compact (sum(labels_lengths),) in the labels' order: frames[n, u] is the
+        frame t at which the best path emits label u (its edge (t, u) -> (t, u+1)); non-decreasing, in [0, Tn-1], and
+        -1 for u >= labels_lengths[n].
+
+    Choosing between the two predecessors of a cell, the label edge wins iff its candidate is larger or the blank
+    candidate is NaN: a NaN candidate loses to any number, and on an exact tie the blank edge wins, so each label is
+    emitted as early as the ties allow.  A lattice with no path above -inf gets score -inf, one whose every path is NaN
+    gets NaN; lengths outside (1..T, 1..U-1 labels; compact: outside ``compact_hints``) get score NaN.  All of these
+    get frames -1.  No autograd.  No host synchronisation in the dense layout and, inside ``compact_hints``, in the
+    compact one (CUDA-graph capturable); without hints the compact call makes one 16-byte device->host copy."""
+    assert isinstance(blank, int)
+    assert isinstance(compact, bool)
+    if compact:
+        hints = getattr(_tls, "hints", None) or (0, 0)
+        return _C.rnnt_align_compact(log_probs, labels, frames_lengths, labels_lengths, blank, hints[0], hints[1])
+    return _C.rnnt_align_dense(log_probs, labels, frames_lengths, labels_lengths, blank)
+
+
+__all__ = ["rnnt_loss", "rnnt_align", "rnnt_loss_from_logits", "joint_pack", "JointPack", "RNNTLossFromLogits",
            "RNNTLossFromLogitsCompact", "RNNTLoss", "RNNTLossGather", "RNNTLossEager", "RNNTLossCompact", "compact_hints", "set_lse_mode", "core", "_C",
            "__version__"]

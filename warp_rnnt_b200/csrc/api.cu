@@ -454,6 +454,62 @@ static int logits_compact_forward_any(void *stream, void *workspace, size_t work
     return run_loss(s, workspace, workspace_bytes, c);
 }
 
+// One alignment call (rnnt_b200_align_*): compact prefix sums, the gather into (cells,2) pairs, then k_align -- the
+// max-plus alpha sweep and the backtrace in one launch.
+struct AlignCall {
+    Problem p;                   // dense (N,T,U); compact: p.compact = 1, its prefix sums come from the workspace
+    int T, U;                    // lattice bounds: dense p.T, p.U; compact max_T, max_U (both > 0)
+    int64_t cells;               // N*T*U (dense) or STU (compact)
+    const void *lp;
+    const int *labels;
+    int V, blank, io_bf16;
+    float *scores;
+    int *frames;
+};
+
+struct AlignWorkspace {
+    float2 *pairs;
+    float *alphas;
+    uint32_t *dec;
+    int64_t *mem_pref, *lab_pref;
+    int *totals;
+    size_t bytes;
+};
+
+static AlignWorkspace carve_align(void *base, int64_t cells, int N, int T, int U) {
+    AlignWorkspace w;
+    size_t off = 0;
+    auto take = [&](size_t bytes) {
+        void *p = base ? (void *)((char *)base + off) : nullptr;
+        off += align_up(bytes, 256);
+        return p;
+    };
+    const size_t c = (size_t)(cells > 0 ? cells : 0), n = (size_t)(N > 0 ? N : 0);
+    const size_t words = n * (size_t)((max(U, 0) + 31) / 32) * (size_t)(max(T, 0) + 31);
+    w.pairs = (float2 *)take(c * sizeof(float2));
+    w.alphas = (float *)take(c * sizeof(float));
+    w.dec = (uint32_t *)take(words * sizeof(uint32_t));
+    w.mem_pref = (int64_t *)take(n * sizeof(int64_t));
+    w.lab_pref = (int64_t *)take(n * sizeof(int64_t));
+    w.totals = (int *)take(4 * sizeof(int));
+    w.bytes = off;
+    return w;
+}
+
+static int run_align(cudaStream_t s, void *workspace, size_t workspace_bytes, AlignCall c) {
+    const AlignWorkspace w = carve_align(workspace, c.cells, c.p.N, c.T, c.U);
+    if (!workspace || workspace_bytes < w.bytes) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    if (c.p.compact) {
+        RNNT_TRY(launch_prefix(s, c.p.xn, c.p.yn, c.p.N, w.mem_pref, w.lab_pref, w.totals), RNNT_STATUS_GATHER_FAILED);
+        c.p.mem_pref = w.mem_pref;
+        c.p.lab_pref = w.lab_pref;
+    }
+    RNNT_TRY(launch_gather(s, c.p, c.lp, c.labels, c.V, c.blank, w.pairs, nullptr, c.cells, c.io_bf16),
+             RNNT_STATUS_GATHER_FAILED);
+    RNNT_TRY(launch_align(s, c.p, w.pairs, w.alphas, w.dec, c.T, c.U, c.scores, c.frames), RNNT_STATUS_WARP_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
 static int logits_compact_backward_any(void *stream, const void *logits, const float *lse, const float *pair_grads,
                                        const int *ys, const int *xn, const int *yn, const int64_t *prefix,
                                        const float *grad_out, void *out, int64_t STU, int N, int V, int blank,
@@ -663,6 +719,40 @@ int rnnt_b200_logits_compact_backward_bf16(void *stream, const void *logits_bf16
         return RNNT_STATUS_INVALID_ARGUMENT;
     return logits_compact_backward_any(stream, logits_bf16, lse, pair_grads, ys, xn, yn, prefix, grad_out, out_bf16,
                                        STU, N, V, blank, 1);
+}
+
+size_t rnnt_b200_align_workspace_bytes(int64_t cells, int N, int T, int U) {
+    return carve_align(nullptr, cells, N, T, U).bytes;
+}
+
+int rnnt_b200_align_dense(void *stream, void *workspace, size_t workspace_bytes, const void *log_probs,
+                          const int *labels, const int *xn, const int *yn, float *scores, int *frames, int N, int T,
+                          int U, int V, int blank, int elem_bytes) {
+    if ((elem_bytes != 4 && elem_bytes != 2) || !dense_args_ok(N, T, U, V, blank) ||
+        (reinterpret_cast<uintptr_t>(log_probs) & (uintptr_t)(elem_bytes - 1)))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    AlignCall c = {};
+    c.p = {xn, yn, nullptr, nullptr, N, T, U, 0};
+    c.T = T; c.U = U; c.cells = (int64_t)N * T * U;
+    c.lp = log_probs; c.labels = labels; c.V = V; c.blank = blank; c.io_bf16 = elem_bytes == 2;
+    c.scores = scores; c.frames = frames;
+    return run_align((cudaStream_t)stream, workspace, workspace_bytes, c);
+}
+
+int rnnt_b200_align_compact(void *stream, void *workspace, size_t workspace_bytes, const void *log_probs,
+                            const int *labels, const int *xn, const int *yn, float *scores, int *frames, int64_t STU,
+                            int N, int V, int blank, int elem_bytes, int max_T, int max_U) {
+    if ((elem_bytes != 4 && elem_bytes != 2) || !compact_args_ok(N, STU, V, blank) || max_T <= 0 || max_U <= 0 ||
+        (reinterpret_cast<uintptr_t>(log_probs) & (uintptr_t)(elem_bytes - 1)))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    AlignCall c = {};
+    c.p = {xn, yn, nullptr, nullptr, N, 0, 0, 1};
+    c.T = max_T; c.U = max_U; c.cells = STU;
+    c.lp = log_probs; c.labels = labels; c.V = V; c.blank = blank; c.io_bf16 = elem_bytes == 2;
+    c.scores = scores; c.frames = frames;
+    return run_align((cudaStream_t)stream, workspace, workspace_bytes, c);
 }
 
 int rnnt_b200_compact_totals(void *stream, const int *xn, const int *yn, int N, int64_t *scratch, int *totals) {

@@ -516,6 +516,53 @@ at::Tensor rnnt_gather_backward(const at::Tensor &pair_grads, const at::Tensor &
     return out;
 }
 
+// Viterbi alignment, dense (N,T,U,V) f32 or bf16 log-probs: (scores (N) f32, frames (N,U-1) i32).  No host sync.
+std::tuple<at::Tensor, at::Tensor> rnnt_align_dense(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn,
+                                                    const at::Tensor &yn, int blank) {
+    check4(xs, ys, xn, yn, true);
+    check_dense_shapes(xs, ys, xn, yn);
+    const c10::cuda::CUDAGuard guard(xs.device());
+    const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), V = xs.size(3);
+    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    const bool bf16 = xs.scalar_type() == at::ScalarType::BFloat16;
+    at::Tensor scores = at::empty({N}, xs.options().dtype(at::kFloat));
+    at::Tensor frames = at::empty({N, U - 1}, xs.options().dtype(at::kInt));
+    if (N == 0) return std::make_tuple(scores, frames);
+    const size_t bytes = rnnt_b200_align_workspace_bytes(N * T * U, (int)N, (int)T, (int)U);
+    at::Tensor ws = at::empty({(int64_t)bytes}, xs.options().dtype(at::kByte));
+    check_status(rnnt_b200_align_dense(current_stream(xs), ws.data_ptr(), bytes, xs.data_ptr(), ys.data_ptr<int>(),
+                                       xn.data_ptr<int>(), yn.data_ptr<int>(), scores.data_ptr<float>(),
+                                       frames.data_ptr<int>(), (int)N, (int)T, (int)U, (int)V, blank, bf16 ? 2 : 4));
+    return std::make_tuple(scores, frames);
+}
+
+// Viterbi alignment, compact (STU,V) f32 or bf16 log-probs: (scores (N) f32, frames (sum yn) i32).  The bounds are
+// the hints when given (no host sync), else one 16-byte device->host copy, as in rnnt_loss_compact.
+std::tuple<at::Tensor, at::Tensor> rnnt_align_compact(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn,
+                                                      const at::Tensor &yn, int blank, int max_T, int max_U) {
+    check4(xs, ys, xn, yn, true);
+    TORCH_CHECK(xs.dim() == 2, "xs must have 2 dimensions");
+    TORCH_CHECK(xn.dim() == 1 && yn.dim() == 1 && xn.size(0) == yn.size(0), "xn and yn shape must be equal (N,)");
+    const c10::cuda::CUDAGuard guard(xs.device());
+    const int64_t N = xn.size(0), STU = xs.size(0), V = xs.size(1);
+    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    const bool bf16 = xs.scalar_type() == at::ScalarType::BFloat16;
+    void *stream = current_stream(xs);
+    at::Tensor scores = at::empty({N}, xs.options().dtype(at::kFloat));
+    at::Tensor frames = at::empty({ys.numel()}, xs.options().dtype(at::kInt));
+    if (N == 0) return std::make_tuple(scores, frames);
+    std::tie(max_T, max_U) = compact_bounds(stream, xs, ys, xn, yn, max_T, max_U, nullptr);
+    max_T = std::max(max_T, 1);              // lengths of 0 or less: the lattice is outside any bounds (score NaN)
+    max_U = std::max(max_U, 1);
+    const size_t bytes = rnnt_b200_align_workspace_bytes(STU, (int)N, max_T, max_U);
+    at::Tensor ws = at::empty({(int64_t)bytes}, xs.options().dtype(at::kByte));
+    check_status(rnnt_b200_align_compact(stream, ws.data_ptr(), bytes, xs.data_ptr(), ys.data_ptr<int>(),
+                                         xn.data_ptr<int>(), yn.data_ptr<int>(), scores.data_ptr<float>(),
+                                         frames.data_ptr<int>(), STU, (int)N, (int)V, blank, bf16 ? 2 : 4, max_T,
+                                         max_U));
+    return std::make_tuple(scores, frames);
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -553,6 +600,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("lse_mode") = 0);
     m.def("rnnt_gather_backward", &rnnt_gather_backward, py::arg("pair_grads"), py::arg("ys"), py::arg("grad_out"),
           py::arg("V"), py::arg("blank") = 0, py::arg("accumulate") = false, py::arg("yn") = py::none());
+    m.def("rnnt_align_dense", &rnnt_align_dense, "Viterbi forced alignment, dense layout.", py::arg("xs"), py::arg("ys"),
+          py::arg("xn"), py::arg("yn"), py::arg("blank") = 0);
+    m.def("rnnt_align_compact", &rnnt_align_compact, "Viterbi forced alignment, compact layout.", py::arg("xs"),
+          py::arg("ys"), py::arg("xn"), py::arg("yn"), py::arg("blank") = 0, py::arg("max_T") = 0,
+          py::arg("max_U") = 0);
     m.def("set_lse_mode", [](int mode) { rnnt_b200_set_lse_mode(mode); }, py::arg("mode"));
     m.def("get_lse_mode", []() { return rnnt_b200_get_lse_mode(); });
     m.def("launch_count", []() { return rnnt_b200_launch_count(); });

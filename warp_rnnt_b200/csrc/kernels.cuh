@@ -26,6 +26,10 @@ cudaError_t launch_gather(cudaStream_t s, const Problem &p, const void *lp, cons
 cudaError_t launch_wavefront(cudaStream_t s, bool fast_lse, const Problem &p, const float2 *pairs, float *alphas,
                              float *betas, float *ws_ll, int *bad, float *costs, int beta_only, int t_hint,
                              int u_hint);
+// Viterbi alignment (k_align): pairs -> alpha (workspace), decision words dec (N, ceil(U/32), T+31), scores (N) and
+// frames (dense (N,U-1), compact (sum yn)); T, U bound the lattices (compact: max_T, max_U > 0)
+cudaError_t launch_align(cudaStream_t s, const Problem &p, const float2 *pairs, float *alphas, uint32_t *dec, int T,
+                         int U, float *scores, int *frames);
 cudaError_t launch_grads_pairs(cudaStream_t s, const Problem &p, const float2 *pairs, const float *alphas,
                                const float *betas, const int *bad, float fastemit_lambda, float2 *out,
                                int64_t cells_hint);

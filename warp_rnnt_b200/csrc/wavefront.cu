@@ -1,5 +1,5 @@
 // wavefront.cu -- general (any-size) path: prefix sums, log-prob gather, the alpha/beta wavefront
-// and the (cells,2) gradient kernel.
+// and the (cells,2) gradient kernel; and the Viterbi alignment (k_align), the alpha wavefront in max-plus form.
 //
 // What it replaces in the reference (1ytic/warp-rnnt):
 //   k_prefix      : host-side cumsum + 4 .item() syncs        pytorch_binding/binding.cpp:132-158
@@ -224,6 +224,7 @@ struct Sweep {
     int j, lane;
     int nsteps, ring_mask;
     bool col_ok, publish, backpressure, override0;
+    uint32_t *dec;      // kMax: this warp's decision words, one per step (word s = the warp's bits at step s)
 };
 
 // "Minus infinity" that stays finite: cells outside the lattice carry kBig (common.cuh) so that the one
@@ -331,7 +332,19 @@ __device__ __forceinline__ float sweep_warp(const Sweep &S) {
             }
             const float skip = val + wb[k];
             const float emit = left + wl[k];
-            float v = lse<KIND>(skip, emit);
+            float v;
+            if constexpr (KIND == kMax) {
+                // max-plus step: the label predecessor iff it is larger or the blank one is NaN (a NaN candidate loses
+                // to any number, a tie goes to the blank edge); row 0 and column 0 take their one predecessor as is,
+                // so the kBig operands of the border never reach a real cell
+                bool bit = (emit > skip) || isnan(skip);
+                bit = (bit || s == lane) && !first_col;
+                v = bit ? emit : skip;
+                const unsigned word = __ballot_sync(0xffffffffu, bit);
+                if (lane == 0 && s < S.nsteps) S.dec[s] = word;
+            } else {
+                v = lse<KIND>(skip, emit);
+            }
             if (SRC == kLeftMem) {
                 if (S.override0 && lane == 0 && s >= 1) v = bnd[k];   // column 0 from the scan pre-pass
             }
@@ -348,9 +361,12 @@ __device__ __forceinline__ float sweep_warp(const Sweep &S) {
     return last;
 }
 
+// kMax (alpha only): dec = the lattice's decision words, column block w (lattice columns 32w .. 32w+31) at
+// dec + w * dec_stride; word s of a block holds bit u%32 of cell (t = s - u%32, u), 1 = the label predecessor.
 template <int KIND, bool BETA, int PF>
 __device__ void wavefront_dir(const Lattice &L, const float2 *__restrict__ pairs, float *__restrict__ out,
-                              Slot *ring, int ring_size, int *cons, float *ll_out) {
+                              Slot *ring, int ring_size, int *cons, float *ll_out, uint32_t *dec = nullptr,
+                              int dec_stride = 0) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
     const int Tn = L.Tn, Un = L.Un, st = L.stride;
     const int T1 = Tn - 1, U1 = Un - 1;
@@ -387,11 +403,12 @@ __device__ void wavefront_dir(const Lattice &L, const float2 *__restrict__ pairs
         S.ring_mask = ring_size - 1;
         S.backpressure = Tn > ring_size;
         S.override0 = false;
+        if constexpr (KIND == kMax) S.dec = dec + (size_t)(wcol / 32) * dec_stride;
 
         // Exact mode, column 0: the reference builds it with a 32-wide Kogge-Stone scan per tile
         // plus the tile's base value (core.cu:92-110 / :197-215); reproduce that summation order
         // so alpha/beta are bit-identical.  Done up front by warp 0; lane 0 then reads it back.
-        const bool col0_scan = (KIND != kFast) && (wcol == 0);
+        const bool col0_scan = (KIND == kExactDense || KIND == kExactCompact) && (wcol == 0);
         if (col0_scan) {
             float base = BETA ? pr[(int64_t)T1 * st + U1].x : 0.0f;
             if (lane == 0) o[BETA ? ((int64_t)T1 * st + U1) : 0] = base;
@@ -484,6 +501,77 @@ __global__ void __launch_bounds__(512, 1) k_wavefront(Problem p, const float2 *_
 }
 
 // ------------------------------------------------------------------------------------------
+// k_align: Viterbi forced alignment of one lattice per CTA, grid (1, N), no cluster.  The alpha wavefront in its
+// max-plus form (kMax) writes alpha and one decision word per warp and step; then warp 0 backtracks from
+// (Tn-1, Un-1) and writes the frame of every label edge and the best path's score alpha[Tn-1,Un-1] + blank[Tn-1,Un-1].
+// dec: (N, ceil(U/32), T+31) words laid out by the bounds T, U (dense: the padded sizes; compact: max_T, max_U); a
+// lattice outside them gets score NaN.  frames: dense (N, U-1), compact (sum yn) in the labels' order.
+// ------------------------------------------------------------------------------------------
+template <int PF>
+__global__ void __launch_bounds__(512, 1) k_align(Problem p, const float2 *__restrict__ pairs, float *__restrict__ alphas,
+                                                uint32_t *__restrict__ dec, int T, int U, int ring_size,
+                                                float *__restrict__ scores, int *__restrict__ frames) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    __shared__ float s_score;
+    const int nwarps = blockDim.x >> 5;
+    Slot *ring = reinterpret_cast<Slot *>(smem_raw);
+    int *cons = reinterpret_cast<int *>(smem_raw + sizeof(Slot) * (size_t)nwarps * ring_size);
+    const int n = blockIdx.y;
+    const Lattice L = get_lattice(p, n);
+    const bool ok = L.ok && L.Tn <= T && L.Un <= U;
+    const int stride = T + 31;
+    uint32_t *d = dec + (size_t)n * ((U + 31) / 32) * stride;
+    if (threadIdx.x == 0) s_score = NAN;     // ordered before the owner's write by the wavefront's first barrier
+    if (ok) wavefront_dir<kMax, false, PF>(L, pairs, alphas, ring, ring_size, cons, &s_score, d, stride);
+    __syncthreads();
+    if (threadIdx.x >= 32) return;
+    const int lane = threadIdx.x;
+    const float score = s_score;
+    // no path above -inf (or every path NaN): no alignment, every frame -1
+    const bool live = ok && score > -INFINITY;
+    int *fr = frames + (p.compact ? L.lab_base : (int64_t)n * (U - 1));
+    const int slots = p.compact ? max(L.Un - 1, 0) : U - 1;
+    for (int u = (live ? L.Un - 1 : 0) + lane; u < slots; u += 32) fr[u] = -1;
+    if (lane == 0) scores[n] = score;
+    if (!live) return;
+    // Backtrace.  The stored bits already follow the border rules (row 0: 1, column 0: 0), so inside column block w
+    // the walk is ul -= bit ul of word s, with s = t + ul falling by one per step (blank: t-1; label: ul-1): one
+    // coalesced load brings 32 steps' words (lane k: word s_hi - k) while the block's next 32 are prefetched, every lane
+    // walks the 32 steps on shuffled copies (no load on the chain), and lane k keeps its own step's column and bit to
+    // write that step's frame afterwards.  A label edge out of ul == 0 enters block w-1 at word t + 31, where the
+    // prefetch is dropped; block 0 ends at word 0, cell (0,0).  w, ul and s_hi are warp-uniform.
+    int w = (L.Un - 1) >> 5, ul = (L.Un - 1) & 31;
+    int s_hi = L.Tn - 1 + ul;
+    const uint32_t *blk = d + (size_t)w * stride;
+    uint32_t mine = (s_hi - lane >= 0) ? blk[s_hi - lane] : 0u;
+    while (true) {
+        const int s_next = s_hi - 32;
+        const uint32_t next = (s_next - lane >= 0) ? blk[s_next - lane] : 0u;
+        int my_ul = 0, my_b = 0;
+#pragma unroll
+        for (int k = 0; k < 32; ++k) {
+            const uint32_t word = __shfl_sync(0xffffffffu, mine, k);
+            const int b = ul >= 0 ? (int)((word >> ul) & 1u) : 0;    // ul == -1: left the block at an earlier step
+            if (lane == k) { my_ul = ul; my_b = b; }
+            ul -= b;
+        }
+        if (my_b) fr[32 * w + my_ul - 1] = s_hi - lane - my_ul;       // label edge into column 32w + my_ul at t
+        const unsigned out = __ballot_sync(0xffffffffu, my_b && my_ul == 0);
+        if (out) {
+            s_hi = s_hi - (__ffs(out) - 1) + 31;
+            --w;
+            ul = 31;
+            blk -= stride;
+            mine = (s_hi - lane >= 0) ? blk[s_hi - lane] : 0u;
+        } else {
+            if (s_next < 0) break;
+            s_hi = s_next;
+            mine = next;
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------
 // k_grads_pairs: out[cell] = (blank grad, label grad) for every cell of the layout (zeros on
 // padding and on the structural zeros).  Elementwise, all SMs.
 // ------------------------------------------------------------------------------------------
@@ -557,19 +645,32 @@ cudaError_t launch_gather(cudaStream_t s, const Problem &p, const void *lp, cons
     return cudaGetLastError();
 }
 
+// CTA shape of a general wavefront launch over lattices of at most t_hint rows and u_hint columns (0 = unknown)
+struct WaveShape {
+    int nwarps, ring;
+    size_t smem;
+};
+static WaveShape wave_shape(int t_hint, int u_hint) {
+    WaveShape w;
+    // warps per CTA: one per 32 lattice columns, at most 16 (more columns -> column passes)
+    w.nwarps = (u_hint > 0 ? u_hint + 31 : 512) / 32;
+    w.nwarps = max(1, min(w.nwarps, 16));
+    // boundary ring: one slot per row when it fits (no back-pressure), else a 128-slot ring
+    w.ring = 128;
+    if (w.nwarps > 1 && t_hint > 0) {
+        while (w.ring < t_hint && (size_t)w.ring * 2 * w.nwarps * sizeof(Slot) <= 160 * 1024) w.ring *= 2;
+    }
+    w.smem = sizeof(Slot) * (size_t)w.nwarps * w.ring + sizeof(int) * w.nwarps;
+    return w;
+}
+
 template <int KIND, int PF>
 static cudaError_t launch_wavefront_kp(cudaStream_t s, const Problem &p, const float2 *pairs, float *alphas,
                                        float *betas, float *ws_ll, int *bad, float *costs, int beta_only,
                                        int guard, int t_hint, int u_hint) {
-    // warps per CTA: one per 32 lattice columns, at most 16 (more columns -> column passes)
-    int nwarps = (u_hint > 0 ? u_hint + 31 : 512) / 32;
-    nwarps = max(1, min(nwarps, 16));
-    // boundary ring: one slot per row when it fits (no back-pressure), else a 128-slot ring
-    int ring = 128;
-    if (nwarps > 1 && t_hint > 0) {
-        while (ring < t_hint && (size_t)ring * 2 * nwarps * sizeof(Slot) <= 160 * 1024) ring *= 2;
-    }
-    const size_t smem = sizeof(Slot) * (size_t)nwarps * ring + sizeof(int) * nwarps;
+    const WaveShape shape = wave_shape(t_hint, u_hint);
+    const int nwarps = shape.nwarps, ring = shape.ring;
+    const size_t smem = shape.smem;
     static std::atomic<bool> attr_done[kMaxDevices];
     {
         const cudaError_t e = ensure_dyn_smem(k_wavefront<KIND, PF>, attr_done, 200 * 1024);
@@ -619,6 +720,25 @@ cudaError_t launch_wavefront(cudaStream_t s, bool fast_lse, const Problem &p, co
         default:
             return launch_wavefront_kind<kFast>(s, p, pairs, alphas, betas, ws_ll, bad, costs, beta_only, guard, t_hint, u_hint);
     }
+}
+
+cudaError_t launch_align(cudaStream_t s, const Problem &p, const float2 *pairs, float *alphas, uint32_t *dec, int T,
+                         int U, float *scores, int *frames) {
+    // the max-plus step is short like the fast LSE's: the fast flavour's unroll
+    constexpr int PF = 8;
+    const WaveShape shape = wave_shape(T, U);
+    static std::atomic<bool> attr_done[kMaxDevices];
+    {
+        const cudaError_t e = ensure_dyn_smem(k_align<PF>, attr_done, 200 * 1024);
+        if (e != cudaSuccess) return e;
+    }
+    count_launch();
+    begin_launch_record(2);
+    int32_t *rec = launch_record();
+    rec[RNNT_REC_GEN_WARPS] = shape.nwarps; rec[RNNT_REC_GEN_RING] = shape.ring;
+    k_align<PF><<<dim3(1, p.N, 1), 32 * shape.nwarps, shape.smem, s>>>(p, pairs, alphas, dec, T, U, shape.ring, scores,
+                                                                       frames);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_grads_pairs(cudaStream_t s, const Problem &p, const float2 *pairs, const float *alphas,
