@@ -18,7 +18,7 @@
 //                        the recurrence (replaces kernel_warp + the global-memory counts scheduler, core.cu:41-258)
 //            zero-fill   (MODE 0, patch order) when the gather is done, two warps' lane 0 issue TMA bulk stores of a
 //                        zeroed shared-memory buffer (evict_last) over this CTA's slice of the dense gradient (replaces
-//                        at::zeros_like, binding.cpp:58); fallback: 128-bit evict_last stores
+//                        at::zeros_like, binding.cpp:58)
 //            chase       the other free warps follow the two wavefronts from the middle anti-diagonal outwards and
 //                        replace each staged log-prob by (alpha + beta) + log-prob: all of the gradient that does not
 //                        need beta[0,0]
@@ -47,10 +47,10 @@ constexpr float kBigF = kBig;       // finite stand-in for -inf (see common.cuh,
 // L2 residency control (H100: 50 MB L2).  In the patch order the dense gradient slab is zero-filled while the
 // wavefront runs and patched afterwards; the patch is a partial-sector write, so it must still HIT
 // in L2 or ECC forces a DRAM read-modify-write per touched sector.  Filled lines are therefore
-// stored evict_last (TMA bulk stores with an evict_last policy, or 128-bit stores with the same policy), and the
-// one-pass log-prob gather is loaded evict_first so that it cannot displace them.  A gradient larger than L2 (cfg 2:
-// 86 MB) loses many zeroed lines before the patch reaches them, so the dense emit composes such gradients after
-// beta[0,0] instead and writes every line once, as whole sectors (launch_fused; DESIGN.md 3.1).
+// stored evict_last (TMA bulk stores with an evict_last policy), and the one-pass log-prob gather is loaded
+// evict_first so that it cannot displace them.  A gradient larger than L2 (cfg 2: 86 MB) loses many zeroed lines
+// before the patch reaches them, so the dense emit composes such gradients after beta[0,0] instead and writes every
+// line once, as whole sectors (launch_fused; DESIGN.md 3.1).
 __device__ __forceinline__ uint64_t policy_evict_first() {
     uint64_t p;
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
@@ -79,15 +79,11 @@ __device__ __forceinline__ float2 ldg_hint2(const float2 *ptr, uint64_t pol) {
 // queue slots -- with STG fills the queue stays full of back-pressured stores and the wavefront
 // warps' LDS/STS wait behind them (an exact-LSE step took about twice as long with an STG fill running).
 constexpr int kZeroBytes = 8192;
+constexpr int kFillWarps = 2;       // free warps that issue the zero-fill (see k_fused)
 __device__ __forceinline__ uint64_t policy_evict_last() {
     uint64_t p;
     asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
     return p;
-}
-// 32 zero bytes as two 128-bit stores (sm_90 has no 256-bit STG), evict_last in L2
-__device__ __forceinline__ void stg_zero32_evict_last(float *ptr, uint64_t pol) {
-    asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1,%1,%1,%1}, %2;" ::"l"(ptr), "r"(0), "l"(pol) : "memory");
-    asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1,%1,%1,%1}, %2;" ::"l"(ptr + 4), "r"(0), "l"(pol) : "memory");
 }
 __device__ __forceinline__ void bulk_store(void *gdst, uint32_t ssrc, uint32_t bytes, uint64_t pol) {
     asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;"
@@ -164,32 +160,28 @@ struct GatherWait {
     }
 };
 
-// C-wide shared-memory vector load / store (C in {1,2,4,8}); asm volatile keeps program order so
+// C-wide shared-memory vector load / store (C in {1,2,4}); asm volatile keeps program order so
 // the operand prefetch stays where it is written.
 template <int C>
 __device__ __forceinline__ void lds_vec(uint32_t a, float (&v)[C]) {
+    static_assert(C == 1 || C == 2 || C == 4, "fused_plan plans C = 1, 2 or 4");
     if constexpr (C == 1) {
         asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v[0]) : "r"(a) : "memory");
     } else if constexpr (C == 2) {
         asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(v[0]), "=f"(v[1]) : "r"(a) : "memory");
-    } else if constexpr (C == 4) {
-        asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]) : "r"(a) : "memory");
     } else {
         asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]) : "r"(a) : "memory");
-        asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]) : "r"(a + 16u) : "memory");
     }
 }
 template <int C>
 __device__ __forceinline__ void sts_vec(uint32_t a, const float (&v)[C]) {
+    static_assert(C == 1 || C == 2 || C == 4, "fused_plan plans C = 1, 2 or 4");
     if constexpr (C == 1) {
         asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(v[0]) : "memory");
     } else if constexpr (C == 2) {
         asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(a), "f"(v[0]), "f"(v[1]) : "memory");
-    } else if constexpr (C == 4) {
-        asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(a), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]) : "memory");
     } else {
         asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(a), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]) : "memory");
-        asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(a + 16u), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7]) : "memory");
     }
 }
 
@@ -236,10 +228,7 @@ struct FusedArgs {
     int gwn, nb_per;        // TMA row gather: gather warps and row buffers per warp (nbuf = gwn * nb_per)
     int Wd;                 // staged row stride (floats) = C * ceil(U / C), even
     int nd;                 // staged rows (diagonals) allocated = T + Wd + 16
-    int gw;                 // warps that gather (of the 14 non-wavefront warps); MODE 0: the rest start the zero-fill at once
     int compose;            // MODE 0: emit order -- 1: composed rows after beta[0,0]; 0: zero-fill + patch
-    int tma_fill;           // MODE 0, zero-fill: bulk shared->global copies (else 128-bit STG)
-    int fill_warps;         // MODE 0, bulk fill: how many of the 14 free warps issue it (the others chase at once)
     FastDiv divV, divU;     // MODE 0, composed emit: element -> cell, cell -> (row, column)
     long long *trace;       // optional per-CTA phase stamps (clock64), 8 per CTA; null = off
     float *loss_sum;        // optional: sum_n costs[n] * (scale ? scale[n] : 1), written by the last CTA to finish
@@ -422,7 +411,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
     int *s_lab = reinterpret_cast<int *>(preB + T);     // [U]
     // zero buffer for the bulk fill: the last kZeroBytes of the dynamic allocation (128-byte aligned)
     float *zbuf = reinterpret_cast<float *>(smem_raw + A.zoff);
-    __shared__ __align__(16) float s_scratch[2][256];   // wavefront lanes past the staged row store here
+    __shared__ __align__(16) float s_scratch[2][32 * 4];   // wavefront lanes past the staged row store here (C <= 4)
     __shared__ int s_next;                              // fill work counter
     __shared__ int s_bad;
     __shared__ int s_flag[kMaxChunks];                  // gather chunk q staged / rows finished by gather warp g
@@ -455,7 +444,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
-    if (MODE == 0 && !A.compose && A.tma_fill) {
+    if (MODE == 0 && !A.compose) {
         for (int k = tid; k < kZeroBytes / 4; k += kFusedThreads) zbuf[k] = 0.0f;
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy zeros -> async-proxy reads
     }
@@ -477,10 +466,11 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
     // ids, so the latency-critical recurrence is never starved by the fill / gather warps sharing its
     // scheduler (with the sweep on warps 0/1 the exact flavour's time varied several-fold from run to run).
     //   logical warp 0 / 1      alpha / beta wavefront, chasing the gather chunk by chunk
-    //   logical warps [2,2+GW)  gather, then (MODE 0) zero-fill
-    //   the rest (MODE 0)       zero-fill from the start: HBM reads (gather) and writes (fill) overlap
+    //   logical warps 2..15     gather, then (MODE 0) zero-fill and chase
     const int lw = (warp + 2) & (kFusedThreads / 32 - 1);
-    const int GW = A.gw;
+    // LDG gather: every non-wavefront warp gathers before it fills (on an H100, faster in both LSE modes than
+    // starting part of the fill during the gather)
+    constexpr int GW = kFusedThreads / 32 - 2;
     const int cells_n = ok ? Tn * Un : 0;
     const int nchunks = (cells_n + kChunkCells - 1) >> kChunkLog;
     if (use_tma) {
@@ -531,7 +521,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
         }
         // the zero-fill starts when the whole gather is done (HBM serves the critical reads first)
         if (MODE == 0 && !A.compose && lw >= 2) asm volatile("bar.sync 1, %0;" ::"r"(kFusedThreads - 64) : "memory");
-    } else if (ok && lw >= 2 && lw < 2 + GW) {
+    } else if (ok && lw >= 2) {
         const float inv = 1.0f / (float)Un;
         const uint64_t pol_first = policy_evict_first();
         constexpr int G = kChunkCells / 32;             // cells per lane per chunk: all loads first
@@ -630,7 +620,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
     }
     if (MODE == 0 && !A.compose) {
         // zero-fill rows [t0,t1) of this lattice's slab: elements [f0,f1); 32 KB chunks handed out by
-        // s_next; 2 x 128-bit evict_last stores per 32 bytes (or bulk copies) on the 32-byte aligned interior
+        // s_next; bulk copies on the 32-byte aligned interior
         const int64_t f0 = (slab + (int64_t)t0 * U) * V, f1 = (slab + (int64_t)t1 * U) * V;
         IO *g = static_cast<IO *>(A.grads);
         constexpr int EPV = 32 / ESZ;                   // elements per 32 bytes
@@ -639,37 +629,24 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
         const int64_t a1 = vec ? max(a0, f1 & ~(int64_t)(EPV - 1)) : f1;
         constexpr int kChunk = 32768 / ESZ;             // elements per chunk
         const int64_t nfill = (a1 - a0 + kChunk - 1) / kChunk;
-        if (A.tma_fill) {
-            // the bulk-copy issue blocks when the SM's copy queue is full (the zeros drain at HBM speed), so only
-            // `fill_warps` warps issue -- one instruction per 8 KB keeps the queue full -- and the others chase at once
-            if (lane == 0 && (lw < 2 || lw >= 2 + (kFusedThreads / 32 - 2) - A.fill_warps)) {
-                const uint64_t pol = policy_evict_last();
-                const uint32_t zs = (uint32_t)__cvta_generic_to_shared(zbuf);
-                constexpr int piece = kZeroBytes / ESZ; // elements per bulk copy
-                for (;;) {
-                    const int c = atomicAdd(&s_next, 1);
-                    if (c >= nfill) break;
-                    const int64_t b = a0 + (int64_t)c * kChunk;
-                    const int64_t e = min(a1, b + kChunk);
-                    for (int64_t f = b; f < e; f += piece)
-                        bulk_store(g + f, zs, (uint32_t)(min(e - f, (int64_t)piece) * ESZ), pol);
-                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                }
-            }
-            __syncwarp();
-        } else {
+        // the bulk-copy issue blocks when the SM's copy queue is full (the zeros drain at HBM speed), so only
+        // kFillWarps free warps issue -- one instruction per 8 KB keeps the queue full -- and the others chase at once
+        // (the wavefront warps join the issuers when their sweep ends)
+        if (lane == 0 && (lw < 2 || lw >= kFusedThreads / 32 - kFillWarps)) {
             const uint64_t pol = policy_evict_last();
+            const uint32_t zs = (uint32_t)__cvta_generic_to_shared(zbuf);
+            constexpr int piece = kZeroBytes / ESZ;     // elements per bulk copy
             for (;;) {
-                int c = 0;
-                if (lane == 0) c = atomicAdd(&s_next, 1);
-                c = __shfl_sync(0xffffffffu, c, 0);
+                const int c = atomicAdd(&s_next, 1);
                 if (c >= nfill) break;
                 const int64_t b = a0 + (int64_t)c * kChunk;
                 const int64_t e = min(a1, b + kChunk);
-#pragma unroll 4
-                for (int64_t f = b + EPV * lane; f < e; f += 32 * EPV) stg_zero32_evict_last(reinterpret_cast<float *>(g + f), pol);
+                for (int64_t f = b; f < e; f += piece)
+                    bulk_store(g + f, zs, (uint32_t)(min(e - f, (int64_t)piece) * ESZ), pol);
+                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
             }
         }
+        __syncwarp();
         if (lw == kFusedThreads / 32 - 1) {             // unaligned head / tail (< 32 bytes each, or everything if !vec)
             for (int64_t f = f0 + lane; f < a0; f += 32) g[f] = io_from_float<IO>(0.0f);
             for (int64_t f = a1 + lane; f < f1; f += 32) g[f] = io_from_float<IO>(0.0f);
@@ -714,7 +691,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
             }
             stamp(8);
         }
-        if (!A.compose && A.tma_fill && lane == 0) {
+        if (!A.compose && lane == 0) {
             asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // the zeros have landed ...
             asm volatile("fence.proxy.async;" ::: "memory");            // ... before anyone patches them
         }
@@ -943,8 +920,8 @@ static size_t fused_smem_bytes(int T, int U, int Wd, int nd) {
 
 // Can the fused kernel take this shape?  Fills `plan` with the derived launch parameters.
 bool fused_plan(int N, int T, int U, FusedPlan *plan) {
-    if (N < 1 || T < 1 || U < 1 || U > 256) return false;
-    const int C = U <= 32 ? 1 : (U <= 64 ? 2 : (U <= 128 ? 4 : 8));
+    if (N < 1 || T < 1 || U < 1 || U > 128) return false;    // (the shared-memory bound below already rejects U >= 105)
+    const int C = U <= 32 ? 1 : (U <= 64 ? 2 : 4);
     int Wd = (U + C - 1) / C * C;
     if (Wd & 1) ++Wd;                                   // C == 1: keep the diagonal stride even
     const int nd = (T + Wd + 16 + 1) & ~1;              // diagonals + prefetch overshoot; even, so a plane is whole float4s
@@ -956,7 +933,7 @@ bool fused_plan(int N, int T, int U, FusedPlan *plan) {
     const int per_sm = (smem <= 110 * 1024) ? 2 : 1;
     int slices = (per_sm * sms) / N;
     slices = max(1, min(slices, T));
-    plan->W = Wd; plan->ring = nd; plan->nw = C; plan->slices = slices; plan->smem = smem;
+    plan->Wd = Wd; plan->nd = nd; plan->C = C; plan->slices = slices; plan->smem = smem;
     return true;
 }
 
@@ -1004,7 +981,7 @@ static cudaError_t launch_fused_km(cudaStream_t s, const FusedArgs &a, size_t sm
         case 1: return launch_fused_kmc<KIND, MODE, 1, IO>(s, a, smem);
         case 2: return launch_fused_kmc<KIND, MODE, 2, IO>(s, a, smem);
         case 4: return launch_fused_kmc<KIND, MODE, 4, IO>(s, a, smem);
-        default: return launch_fused_kmc<KIND, MODE, 8, IO>(s, a, smem);
+        default: return cudaErrorInvalidValue;
     }
 }
 
@@ -1020,16 +997,7 @@ cudaError_t launch_fused(cudaStream_t s, const FusedPlan &plan, const FusedCall 
     a.lp = lp; a.labels = c.labels; a.xn = c.xn; a.yn = c.yn; a.costs = c.costs; a.grads = grads;
     a.pair_grads = c.pair_grads; a.scale = c.scale; a.N = N; a.T = T; a.U = U; a.V = V; a.blank = c.blank; a.lam = c.lam;
     a.pairs_in = pairs_in; a.guard = c.mem_pref == nullptr;   // no mismatch guard in the compact reference
-    a.slices = (grads || c.pair_grads) ? plan.slices : 1; a.Wd = plan.W; a.nd = plan.ring;
-    {
-        static const int gw_raw = env_int("RNNT_B200_GATHER_WARPS", 0);   // tuning knob, in [1,14]
-        const int gw_env = (gw_raw < 1 || gw_raw > kFusedThreads / 32 - 2) ? 0 : gw_raw;
-        // fast LSE: the fill (HBM-write bound) outlasts the wavefront, so start it during the gather;
-        // exact LSE: the wavefront outlasts the fill, so let every free warp gather and feed it sooner
-        // (measured with the TMA fill: starting the fill only when the gather is done is best in both modes)
-        a.gw = gw_env ? gw_env : kFusedThreads / 32 - 2;
-        if (!grads) a.gw = kFusedThreads / 32 - 2;      // nothing to fill: everyone gathers
-    }
+    a.slices = (grads || c.pair_grads) ? plan.slices : 1; a.Wd = plan.Wd; a.nd = plan.nd;
     {
         // dense emit order (DESIGN.md 3.1): a gradient of small rows of whole 16-byte vectors that does not fit in L2
         // is composed and written once after beta[0,0]; otherwise it is zero-filled under the recurrence and patched --
@@ -1045,25 +1013,22 @@ cudaError_t launch_fused(cudaStream_t s, const FusedPlan &plan, const FusedCall 
     }
     a.zoff = (int)(plan.smem - kZeroBytes);
     // TMA row gather when a lattice row (U*V floats) is a 16-byte multiple at a 16-byte aligned address and
-    // at least four row buffers fit behind the planes (RNNT_B200_GATHER=ldg forces the LDG gather); the composed
-    // emit needs no zero buffer, so they start where it would be
+    // at least four row buffers fit behind the planes; the composed emit needs no zero buffer, so they start where it
+    // would be
     const size_t base = a.compose ? plan.smem - kZeroBytes : plan.smem;
     size_t smem = base;
     a.nbuf = 0; a.row_off = 0; a.row_stride = 0; a.gwn = 0; a.nb_per = 1;
     {
-        static const bool want_tma = !env_is("RNNT_B200_GATHER", 'l');
-        static const int nb_env = env_int("RNNT_B200_ROW_BUFS", 0);     // tuning knob: row buffers per gather warp (1 or 2)
         const size_t row = (size_t)U * V * (io_bf16 ? 2 : sizeof(float));
         const size_t stride = (row + 127) / 128 * 128;
         // keep two CTAs per SM where the plan counted on them
         const size_t cap = (plan.smem <= 110 * 1024) ? (size_t)113 * 1024 : (size_t)kFusedMaxDynSmem;
-        if (want_tma && !pairs_in && (row % 16) == 0 && (reinterpret_cast<uintptr_t>(lp) % 16) == 0 && row <= 32 * 1024 &&
+        if (!pairs_in && (row % 16) == 0 && (reinterpret_cast<uintptr_t>(lp) % 16) == 0 && row <= 32 * 1024 &&
             base + 4 * stride <= cap) {
             const int fit = (int)((cap - base) / stride);
             // two buffers per gather warp once at least 8 fit (the copy of the next row overlaps the picking of this one
             // and more bytes stay in flight per SM: the gather is bound by that, not by HBM, up to ~20 rows); else one
-            a.nb_per = (nb_env == 1 || nb_env == 2) ? nb_env : (fit >= 8 ? 2 : 1);
-            if (a.nb_per == 2 && fit < 2) a.nb_per = 1;
+            a.nb_per = fit >= 8 ? 2 : 1;
             a.gwn = min(kMaxRowBufs, fit / a.nb_per);
             a.nbuf = a.gwn * a.nb_per;
             a.row_off = (int)base;
@@ -1071,20 +1036,14 @@ cudaError_t launch_fused(cudaStream_t s, const FusedPlan &plan, const FusedCall 
             smem = base + (size_t)a.nbuf * stride;
         }
     }
-    {
-        static const bool tma = !env_is("RNNT_B200_FILL", 's');   // RNNT_B200_FILL=stg selects the 128-bit store fill
-        a.tma_fill = tma ? 1 : 0;
-        static const int fw = env_int("RNNT_B200_FILL_WARPS", 2);
-        a.fill_warps = max(1, min(fw, kFusedThreads / 32 - 2));
-    }
     a.trace = g_fused_trace;
     { const GuardPoison gp = guard_poison(); a.poison_n = gp.n; a.poison_delta = gp.delta; }
     const bool dense = grads != nullptr;
-    const int C = plan.nw;
+    const int C = plan.C;
     begin_launch_record(1);
     int32_t *rec = launch_record();
     rec[RNNT_REC_FUSED_C] = C; rec[RNNT_REC_FUSED_GATHER_WARPS] = a.gwn; rec[RNNT_REC_FUSED_ROW_BUFS] = a.nbuf ? a.nb_per : 0;
-    rec[RNNT_REC_FUSED_COMPOSE] = a.compose; rec[RNNT_REC_FUSED_TMA_FILL] = dense ? a.tma_fill : 0;
+    rec[RNNT_REC_FUSED_COMPOSE] = a.compose; rec[RNNT_REC_FUSED_TMA_FILL] = dense ? 1 : 0;   // the zero-fill is always TMA
     if (io_bf16)
         return kind == kFast ? launch_fused_km<kFast, 0, __nv_bfloat16>(s, a, smem, C)
                              : launch_fused_km<kExactDense, 0, __nv_bfloat16>(s, a, smem, C);

@@ -75,7 +75,10 @@ cudaError_t launch_joint_grads(cudaStream_t s, const float *dx, const int *lf, c
                                float *df, float *dg, int N, int T, int U1, int H);
 
 // fused.cu -- single-kernel path for lattices that fit shared memory
-struct FusedPlan { int W, ring, nw, slices; size_t smem; };
+// Wd: staged row stride (floats); nd: staged diagonals; C: lattice columns per lane (1, 2 or 4); slices: CTAs per
+// lattice; smem: dynamic shared memory of the staged lattice and the zero buffer (bytes; launch_fused adds the TMA
+// row buffers)
+struct FusedPlan { int Wd, nd, C, slices; size_t smem; };
 bool fused_plan(int N, int T, int U, FusedPlan *plan);
 void set_fused_trace(long long *buf);   // diagnostics: per-CTA phase stamps of k_fused (8 x clock64 per CTA)
 // One fused launch, filled by name; fields left zero are off.  The layout follows mem_pref: null = dense (N,T,U),
