@@ -216,6 +216,69 @@ def rnnt_loss_from_logits(logits, labels, frames_lengths, labels_lengths, averag
     return costs
 
 
+class RNNTLossPruned(torch.autograd.Function):
+    """``RNNTLossFromLogits`` on the (N,T,S,V) logits of a joint evaluated in a window of S labels per frame.  Forward
+    reads the window rows once and runs the recurrence on the full (N,T,U) lattice, with the edges out of the cells
+    outside the windows removed; it keeps lse (N,T,S) and the (N,T,U,2) pair gradients.  Backward writes d loss /
+    d logits (N,T,S,V), of the logits' dtype."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, frames_lengths, labels_lengths, ranges, blank=0, fastemit_lambda=0.0):
+        need = ctx.needs_input_grad[0]
+        costs, lse, pg = _C.rnnt_logits_pruned_forward(logits, labels, frames_lengths, labels_lengths, ranges, blank,
+                                                       fastemit_lambda, need, 0)
+        if need:
+            ctx.save_for_backward(logits, lse, pg, labels, ranges)
+            ctx.blank = blank
+        return costs
+
+    @staticmethod
+    def backward(ctx, grads_output):
+        logits, lse, pg, labels, ranges = ctx.saved_tensors
+        go = grads_output.contiguous().to(torch.float32)
+        g = _C.rnnt_logits_pruned_backward(logits, lse, pg, labels, ranges, go, ctx.blank)
+        return g, None, None, None, None, None, None
+
+
+def rnnt_loss_pruned(logits, labels, frames_lengths, labels_lengths, ranges, average_frames=False, reduction="none",
+                     blank=0, fastemit_lambda=0.0):
+    """Pruned RNN-T loss: the transducer loss from a joint network evaluated only in a window of S label columns per
+    frame, which takes about U/S times less memory and traffic than the full (N,T,U,V) joint output.
+
+    Args:
+        logits: (N, T, S, V) float32 or bfloat16, not normalised.
+        labels: (N, U-1) int32, as for ``rnnt_loss``; U = labels.size(1) + 1 is the full lattice's width.
+        frames_lengths, labels_lengths: (N,) int32.
+        ranges: (N, T) int32; ranges[n, t] is the first label column of frame t's window.
+        average_frames, reduction, blank, fastemit_lambda: as in ``rnnt_loss_from_logits``.
+
+    Row (n, t, s) of ``logits`` is lattice cell (t, u = ranges[n, t] + s) when t < frames_lengths[n] and
+    0 <= u <= labels_lengths[n]; any other row is padding.  Frame t's window is {u : r <= u < r + S} clipped to the
+    lattice; windows need not be monotone or connected, and r < 0 or r + S > labels_lengths[n] + 1 simply clip.  The
+    loss is the RNN-T loss of lattice n in which the blank edge (t,u)->(t+1,u) and the label edge (t,u)->(t,u+1) of an
+    in-window cell carry log_softmax(logits[n,t,s]) at ``blank`` and at labels[n,u], and every edge out of a cell outside
+    its frame's window is removed.  This is k2's ``rnnt_loss_pruned(..., rnnt_type="regular")`` with k2's
+    ``ranges[:, :, 0]`` as ``ranges``.
+
+    Costs are float32; the gradient is w.r.t. ``logits``, of their dtype (bfloat16: the float32 gradient of the
+    widened logits rounded once).  Padding rows get exact zeros, or NaN where the row's normaliser is NaN.  A lattice
+    with no path left gets the dense classes of ``rnnt_loss_from_logits``: cost NaN, +inf when it has one frame or no
+    labels.  No host synchronisation: the step can be captured in a CUDA graph."""
+    assert average_frames is None or isinstance(average_frames, bool)
+    assert reduction is None or reduction in ("none", "mean", "sum")
+    assert isinstance(blank, int)
+    assert not labels.requires_grad and not frames_lengths.requires_grad and not labels_lengths.requires_grad
+    assert not ranges.requires_grad
+    costs = RNNTLossPruned.apply(logits, labels, frames_lengths, labels_lengths, ranges, blank, fastemit_lambda)
+    if average_frames:
+        costs = costs / frames_lengths.to(costs.dtype)
+    if reduction == "sum":
+        return costs.sum()
+    if reduction == "mean":
+        return costs.mean()
+    return costs
+
+
 class JointPack(torch.autograd.Function):
     """x[(n,t,u), :] = f[n,t,:] + g[n,u,:] in the compact (ragged) row order that ``rnnt_loss(compact=True)`` takes --
     the joint network's input without padding (the reference's benchmark2.py:37-50 builds it with a python loop over
@@ -396,6 +459,6 @@ def rnnt_align(log_probs, labels, frames_lengths, labels_lengths, blank=0, compa
     return _C.rnnt_align_dense(log_probs, labels, frames_lengths, labels_lengths, blank)
 
 
-__all__ = ["rnnt_loss", "rnnt_align", "rnnt_loss_from_logits", "joint_pack", "JointPack", "RNNTLossFromLogits",
-           "RNNTLossFromLogitsCompact", "RNNTLoss", "RNNTLossGather", "RNNTLossEager", "RNNTLossCompact", "compact_hints", "set_lse_mode", "core", "_C",
-           "__version__"]
+__all__ = ["rnnt_loss", "rnnt_align", "rnnt_loss_from_logits", "rnnt_loss_pruned", "RNNTLossPruned", "joint_pack",
+           "JointPack", "RNNTLossFromLogits", "RNNTLossFromLogitsCompact", "RNNTLoss", "RNNTLossGather", "RNNTLossEager",
+           "RNNTLossCompact", "compact_hints", "set_lse_mode", "core", "_C", "__version__"]

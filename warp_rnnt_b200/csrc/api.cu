@@ -117,6 +117,11 @@ static bool dense_args_ok(int N, int T, int U, int V, int blank) {
 static bool compact_args_ok(int N, int64_t STU, int V, int blank) {
     return N >= 0 && STU >= 0 && V >= 1 && V < (1 << 22) && blank >= 0 && blank < V;
 }
+// pruned (N,T,S,V) window rows over a full (N,T,U) lattice: the full lattice as dense_args_ok takes it, and row ids
+// that fit 32 bits as cell ids do
+static bool pruned_args_ok(int N, int T, int S, int U, int V, int blank) {
+    return S >= 1 && dense_args_ok(N, T, U, V, blank) && (int64_t)N * T * S < (int64_t)1 << 31;
+}
 // (cells,2) pairs and their gradients are read and written as float2
 static bool pairs_aligned(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 7u) == 0; }
 
@@ -719,6 +724,39 @@ int rnnt_b200_logits_compact_backward_bf16(void *stream, const void *logits_bf16
         return RNNT_STATUS_INVALID_ARGUMENT;
     return logits_compact_backward_any(stream, logits_bf16, lse, pair_grads, ys, xn, yn, prefix, grad_out, out_bf16,
                                        STU, N, V, blank, 1);
+}
+
+int rnnt_b200_logits_pruned_forward(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                    const int *labels, const int *xn, const int *yn, const int *ranges, float *costs,
+                                    float *lse, float *pair_grads, int N, int T, int S, int U, int V, int blank,
+                                    float fastemit_lambda, int lse_mode, int elem_bytes) {
+    if ((elem_bytes != 4 && elem_bytes != 2) || (reinterpret_cast<uintptr_t>(logits) & (uintptr_t)(elem_bytes - 1)) ||
+        !pruned_args_ok(N, T, S, U, V, blank) || !lse || !pairs_aligned(pair_grads))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    cudaStream_t s = (cudaStream_t)stream;
+    LossCall c = dense_call(xn, yn, N, T, U, costs, fastemit_lambda, lse_mode);
+    Workspace w;
+    if (!carve_ok(workspace, workspace_bytes, c.cells, N, &w)) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    // one pass over the window rows: their normalisers, and the full lattice's pairs ((kBig, kBig) off the windows)
+    RNNT_TRY(launch_lse_pairs_pruned(s, logits, labels, ranges, N, T, S, U, V, blank, w.pairs, lse, elem_bytes == 2),
+             RNNT_STATUS_GATHER_FAILED);
+    c.pairs = w.pairs; c.pair_grads = reinterpret_cast<float2 *>(pair_grads);
+    return run_loss(s, workspace, workspace_bytes, c);
+}
+
+int rnnt_b200_logits_pruned_backward(void *stream, const void *logits, const float *lse, const float *pair_grads,
+                                     const int *labels, const int *ranges, const float *grad_out, void *out, int N,
+                                     int T, int S, int U, int V, int blank, int elem_bytes) {
+    if ((elem_bytes != 4 && elem_bytes != 2) ||
+        ((reinterpret_cast<uintptr_t>(logits) | reinterpret_cast<uintptr_t>(out)) & (uintptr_t)(elem_bytes - 1)) ||
+        !pruned_args_ok(N, T, S, U, V, blank) || !pairs_aligned(pair_grads))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    RNNT_TRY(launch_expand_logits_pruned((cudaStream_t)stream, logits, lse, reinterpret_cast<const float2 *>(pair_grads),
+                                         labels, ranges, grad_out, out, N, T, S, U, V, blank, elem_bytes == 2),
+             RNNT_STATUS_GRADS_BLANK_FAILED);
+    return RNNT_STATUS_SUCCESS;
 }
 
 size_t rnnt_b200_align_workspace_bytes(int64_t cells, int N, int T, int U) {

@@ -433,6 +433,75 @@ at::Tensor rnnt_logits_compact_backward(const at::Tensor &xs, const at::Tensor &
     return out;
 }
 
+// pruned loss from (N,T,S,V) window logits, float32 or bfloat16, ranges (N,T): (costs (N), lse (N,T,S), pair_grads
+// (N,T,U,2) of the full lattice or empty), all float32; U = ys.size(1) + 1.  No host sync.
+std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_logits_pruned_forward(const at::Tensor &xs, const at::Tensor &ys,
+                                                                          const at::Tensor &xn, const at::Tensor &yn,
+                                                                          const at::Tensor &ranges, int blank,
+                                                                          float fastemit_lambda, bool want_grads,
+                                                                          int lse_mode) {
+    check4(xs, ys, xn, yn, true);
+    TORCH_CHECK(xs.dim() == 4, "xs must have 4 dimensions");
+    TORCH_CHECK(xn.numel() == xs.size(0), "xn shape must be equal (N,)");
+    TORCH_CHECK(yn.numel() == xs.size(0), "yn shape must be equal (N,)");
+    TORCH_CHECK(ys.dim() == 2 && ys.size(0) == xs.size(0), "ys shape must be (N, U-1)");
+    const int64_t N = xs.size(0), T = xs.size(1), S = xs.size(2), V = xs.size(3), U = ys.size(1) + 1;
+    TORCH_CHECK(ranges.is_contiguous() && ranges.scalar_type() == at::ScalarType::Int && ranges.device() == xs.device() &&
+                    ranges.dim() == 2 && ranges.size(0) == N && ranges.size(1) == T,
+                "ranges must be a contiguous Int tensor of shape (N, T) on the device of xs");
+    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    const c10::cuda::CUDAGuard guard(xs.device());
+    const bool bf16 = xs.scalar_type() == at::ScalarType::BFloat16;
+    const auto f32 = xs.options().dtype(at::kFloat);
+    at::Tensor costs = at::empty({N}, f32);
+    at::Tensor lse = at::empty({N, T, S}, f32);
+    at::Tensor pg = want_grads ? at::empty({N, T, U, 2}, f32) : at::empty({0}, f32);
+    if (N == 0) return std::make_tuple(costs, lse, pg);
+    at::Tensor ws = workspace_for(xs, N * T * U, N);
+    check_status(rnnt_b200_logits_pruned_forward(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
+                                                 ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
+                                                 ranges.data_ptr<int>(), costs.data_ptr<float>(), lse.data_ptr<float>(),
+                                                 want_grads ? pg.data_ptr<float>() : nullptr, (int)N, (int)T, (int)S,
+                                                 (int)U, (int)V, blank, fastemit_lambda, lse_mode, bf16 ? 2 : 4));
+    return std::make_tuple(costs, lse, pg);
+}
+
+// d loss / d pruned logits (N,T,S,V), of the dtype of xs
+at::Tensor rnnt_logits_pruned_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &pair_grads,
+                                       const at::Tensor &ys, const at::Tensor &ranges, const at::Tensor &grad_out,
+                                       int blank) {
+    const bool bf16 = xs.scalar_type() == at::ScalarType::BFloat16;
+    TORCH_CHECK(xs.is_contiguous() && (xs.scalar_type() == at::ScalarType::Float || bf16) && xs.device().is_cuda() &&
+                    xs.dim() == 4,
+                "xs must be a contiguous CUDA Float tensor of shape (N, T, S, V)");
+    const int64_t N = xs.size(0), T = xs.size(1), S = xs.size(2), V = xs.size(3);
+    TORCH_CHECK(ys.is_contiguous() && ys.scalar_type() == at::ScalarType::Int && ys.device() == xs.device() &&
+                    ys.dim() == 2 && ys.size(0) == N,
+                "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
+    const int64_t U = ys.size(1) + 1;
+    TORCH_CHECK(lse.is_contiguous() && lse.scalar_type() == at::ScalarType::Float && lse.device() == xs.device() &&
+                    lse.numel() == N * T * S,
+                "lse must be a contiguous Float tensor of shape (N, T, S) on the device of xs");
+    TORCH_CHECK(pair_grads.is_contiguous() && pair_grads.scalar_type() == at::ScalarType::Float &&
+                    pair_grads.device() == xs.device() && pair_grads.numel() == N * T * U * 2,
+                "pair_grads must be a contiguous Float tensor of shape (N, T, U, 2) on the device of xs");
+    TORCH_CHECK(ranges.is_contiguous() && ranges.scalar_type() == at::ScalarType::Int && ranges.device() == xs.device() &&
+                    ranges.dim() == 2 && ranges.size(0) == N && ranges.size(1) == T,
+                "ranges must be a contiguous Int tensor of shape (N, T) on the device of xs");
+    TORCH_CHECK(grad_out.is_contiguous() && grad_out.scalar_type() == at::ScalarType::Float &&
+                    grad_out.device() == xs.device() && grad_out.numel() == N,
+                "grad_out must be a contiguous Float tensor of shape (N,)");
+    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    const c10::cuda::CUDAGuard guard(xs.device());
+    at::Tensor out = at::empty_like(xs);
+    if (N == 0) return out;
+    check_status(rnnt_b200_logits_pruned_backward(current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(),
+                                                  pair_grads.data_ptr<float>(), ys.data_ptr<int>(),
+                                                  ranges.data_ptr<int>(), grad_out.data_ptr<float>(), out.data_ptr(),
+                                                  (int)N, (int)T, (int)S, (int)U, (int)V, blank, bf16 ? 2 : 4));
+    return out;
+}
+
 // compact packing of the joint input: (x (STU,H), mem_pref (N) int64).  stu < 0: STU is read back from the device
 // (one 16-byte copy); stu >= 0: trusted, no host sync.
 std::tuple<at::Tensor, at::Tensor> rnnt_joint_pack(const at::Tensor &f, const at::Tensor &g, const at::Tensor &lf,
@@ -592,6 +661,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("rnnt_logits_compact_backward", &rnnt_logits_compact_backward, py::arg("xs"), py::arg("lse"),
           py::arg("pair_grads"), py::arg("ys"), py::arg("xn"), py::arg("yn"), py::arg("prefix"), py::arg("grad_out"),
           py::arg("blank") = 0);
+    m.def("rnnt_logits_pruned_forward", &rnnt_logits_pruned_forward, py::arg("xs"), py::arg("ys"), py::arg("xn"),
+          py::arg("yn"), py::arg("ranges"), py::arg("blank") = 0, py::arg("fastemit_lambda") = 0.0,
+          py::arg("want_grads") = true, py::arg("lse_mode") = 0);
+    m.def("rnnt_logits_pruned_backward", &rnnt_logits_pruned_backward, py::arg("xs"), py::arg("lse"),
+          py::arg("pair_grads"), py::arg("ys"), py::arg("ranges"), py::arg("grad_out"), py::arg("blank") = 0);
     m.def("rnnt_joint_pack", &rnnt_joint_pack, py::arg("f"), py::arg("g"), py::arg("lf"), py::arg("lg"), py::arg("stu") = -1);
     m.def("rnnt_joint_pack_backward", &rnnt_joint_pack_backward, py::arg("dx"), py::arg("lf"), py::arg("lg"),
           py::arg("mem_pref"), py::arg("T"), py::arg("U1"));

@@ -67,6 +67,14 @@ cudaError_t launch_lse_pairs_compact(cudaStream_t s, const void *x, const Proble
 cudaError_t launch_expand_logits_compact(cudaStream_t s, const void *x, const float *lse, const float2 *pg,
                                          const Problem &p, const int *labels, const float *grad_out, void *out,
                                          int64_t STU, int V, int blank, int io_bf16);
+// ... and over rnnt_loss_pruned's (N,T,S,V) window rows: row (n,t,s) is cell (t, ranges[n,t] + s) of the full (N,T,U)
+// lattice.  The forward writes lse (N,T,S) and the full (N,T,U,2) pairs: every cell (kBig, kBig), then each window
+// row's pair at its cell (u in [0, U)); the backward writes (N,T,S,V) from the full (N,T,U,2) pair gradients.
+cudaError_t launch_lse_pairs_pruned(cudaStream_t s, const void *x, const int *labels, const int *ranges, int N, int T,
+                                    int S, int U, int V, int blank, float2 *pairs, float *lse, int io_bf16);
+cudaError_t launch_expand_logits_pruned(cudaStream_t s, const void *x, const float *lse, const float2 *pg,
+                                        const int *labels, const int *ranges, const float *grad_out, void *out, int N,
+                                        int T, int S, int U, int V, int blank, int io_bf16);
 
 // joint.cu -- compact packing of the joint network's input (caller side of compact=True)
 cudaError_t launch_joint_pack(cudaStream_t s, const float *f, const float *g, const int *lf, const int *lg,

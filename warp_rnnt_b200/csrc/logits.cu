@@ -44,10 +44,19 @@ __device__ __forceinline__ float4 ld_group4(const __nv_bfloat16 *row, int q) {
 // COMPACT: the rows are joint_pack's ragged (STU, V) order and the grid is (gx, N): CTA row blockIdx.y streams over the
 // Tn*Un rows of lattice n (Problem `lay`, compact prefix sums), the pointers rebased to its first row.  Only the
 // (lattice, u, label) of a row differs from the dense kernel; a row is summed exactly as the dense row of its values.
-template <typename IN, int SUB, bool VEC4, bool COMPACT = false>
-__global__ void __launch_bounds__(kLogitThreads)
-k_lse_pairs(const IN *__restrict__ x, const int *__restrict__ labels, int64_t cells, int V, int blank, int U,
-            FastDiv divU, FastDiv divTU, float2 *__restrict__ pairs, float *__restrict__ lse_out, Problem lay) {
+//
+// PRUNED (ROWS == kRowsPruned): the rows are rnnt_loss_pruned's (N,T,S,V) windows; row (n,t,s) is cell (t, u) of the
+// full (N,T,U) lattice with u = ranges[n,t] + s (divU divides by S, divTU by T).  lse is written for every row, the
+// pair only for 0 <= u < U, at that cell of the full (N,T,U,2) pairs; k_fill_pairs gave every other cell
+// (kBig, kBig) before.  Again only the mapping differs: a row is summed exactly as the dense row of its values.
+enum { kRowsDense = 0, kRowsCompact = 1, kRowsPruned = 2 };
+
+template <typename IN, int SUB, bool VEC4, int ROWS>
+__device__ __forceinline__ void
+lse_pairs_rows(const IN *__restrict__ x, const int *__restrict__ labels, int64_t cells, int V, int blank, int U,
+               FastDiv divU, FastDiv divTU, float2 *__restrict__ pairs, float *__restrict__ lse_out, Problem lay,
+               const int *__restrict__ ranges) {
+    constexpr bool COMPACT = ROWS == kRowsCompact;
     Lattice L;
     if constexpr (COMPACT) {
         // `cells` = STU on entry: a lattice never reaches past the rows of the tensor (lengths the hints vouched for)
@@ -109,7 +118,18 @@ k_lse_pairs(const IN *__restrict__ x, const int *__restrict__ labels, int64_t ce
             // every logit -inf: NaN, as torch.log_softmax gives (and as the max-first paths above compute it)
             const float l = (m == -INFINITY) ? NAN : m + logf(s);
             int lab;
-            if constexpr (COMPACT) {
+            if constexpr (ROWS == kRowsPruned) {
+                uint32_t nt, srow;                               // row = nt * S + srow, nt = n * T + t
+                divU.divmod((uint32_t)cell, nt, srow);
+                const uint32_t n = divTU.div(nt);
+                const int64_t u = (int64_t)ranges[nt] + srow;
+                lse_out[cell] = l;
+                if (u >= 0 && u < U) {
+                    lab = (u < U - 1) ? labels[(int64_t)n * (U - 1) + u] : blank;
+                    pairs[(int64_t)nt * U + u] = make_float2(io_load(row + blank) - l, io_load(row + lab) - l);
+                }
+                continue;
+            } else if constexpr (COMPACT) {
                 const int u = (int)cell % L.Un;
                 lab = (u < L.Un - 1) ? labels[L.lab_base + u] : blank;
             } else {
@@ -122,6 +142,34 @@ k_lse_pairs(const IN *__restrict__ x, const int *__restrict__ labels, int64_t ce
             lse_out[cell] = l;
         }
     }
+}
+
+template <typename IN, int SUB, bool VEC4, bool COMPACT = false>
+__global__ void __launch_bounds__(kLogitThreads)
+k_lse_pairs(const IN *__restrict__ x, const int *__restrict__ labels, int64_t cells, int V, int blank, int U,
+            FastDiv divU, FastDiv divTU, float2 *__restrict__ pairs, float *__restrict__ lse_out, Problem lay) {
+    lse_pairs_rows<IN, SUB, VEC4, COMPACT ? kRowsCompact : kRowsDense>(x, labels, cells, V, blank, U, divU, divTU,
+                                                                       pairs, lse_out, lay, nullptr);
+}
+
+// rows = N*T*S pruned rows; divS, divT: FastDiv(S), FastDiv(T)
+template <typename IN, int SUB, bool VEC4>
+__global__ void __launch_bounds__(kLogitThreads)
+k_lse_pairs_pruned(const IN *__restrict__ x, const int *__restrict__ labels, const int *__restrict__ ranges,
+                   int64_t rows, int V, int blank, int U, FastDiv divS, FastDiv divT, float2 *__restrict__ pairs,
+                   float *__restrict__ lse_out) {
+    lse_pairs_rows<IN, SUB, VEC4, kRowsPruned>(x, labels, rows, V, blank, U, divS, divT, pairs, lse_out, Problem{},
+                                               ranges);
+}
+
+// every cell of the full (cells,2) pairs (kBig, kBig): an edge out of a cell that no window row covers is removed
+__global__ void __launch_bounds__(kLogitThreads) k_fill_pairs(float4 *__restrict__ pairs2, int64_t cells) {
+    const float4 big = make_float4(kBig, kBig, kBig, kBig);
+    const int64_t quads = cells >> 1;
+    for (int64_t i = (int64_t)blockIdx.x * kLogitThreads + threadIdx.x; i < quads; i += (int64_t)gridDim.x * kLogitThreads)
+        pairs2[i] = big;
+    if ((cells & 1) && blockIdx.x == 0 && threadIdx.x == 0)
+        reinterpret_cast<float2 *>(pairs2)[cells - 1] = make_float2(kBig, kBig);
 }
 
 // VEC consecutive elements at p (VEC * sizeof(T) bytes, aligned to that) <-> fp32
@@ -191,12 +239,16 @@ __device__ __forceinline__ void st_logit_grads(__nv_bfloat16 *p, const float (&e
 // 1; bf16 also 8): a vector never straddles a row, so one (gb, gl, lse, label) fetch serves it.  IO is the element
 // type of the logits and of the gradient.  COMPACT: as in k_lse_pairs, CTA row blockIdx.y streams over the Tn*Un*V
 // elements of lattice n.
-template <typename IO, int VEC, bool COMPACT = false>
-__global__ void __launch_bounds__(kLogitThreads)
-k_expand_logits(const IO *__restrict__ x, const float *__restrict__ lse, const float2 *__restrict__ pg,
-                const int *__restrict__ labels, const float *__restrict__ grad_out, IO *__restrict__ out,
-                int64_t cells, int V, int blank, int U, FastDiv divU, FastDiv divTU, int64_t stride_rows,
-                int stride_v, Problem lay) {
+// PRUNED: the rows are the (N,T,S,V) windows, divU divides by S and divTU by T as in k_lse_pairs; row (n,t,s) takes
+// (gb, gl) from the full (N,T,U,2) pair gradients at cell (t, u = ranges[n,t] + s), and a row with u outside [0, U) is
+// a padding row (pair gradients (0, 0)).
+template <typename IO, int VEC, int ROWS>
+__device__ __forceinline__ void
+expand_logits_rows(const IO *__restrict__ x, const float *__restrict__ lse, const float2 *__restrict__ pg,
+                   const int *__restrict__ labels, const float *__restrict__ grad_out, IO *__restrict__ out,
+                   int64_t cells, int V, int blank, int U, FastDiv divU, FastDiv divTU, int64_t stride_rows,
+                   int stride_v, const Problem &lay, const int *__restrict__ ranges) {
+    constexpr bool COMPACT = ROWS == kRowsCompact;
     Lattice L;
     if constexpr (COMPACT) {
         L = get_lattice(lay, blockIdx.y);
@@ -213,7 +265,17 @@ k_expand_logits(const IO *__restrict__ x, const float *__restrict__ lse, const f
     const int64_t stride = stride_rows * V + stride_v;
     for (; f < total; f += stride, row += stride_rows, v0 += stride_v) {
         if (v0 >= V) { v0 -= V; ++row; }
-        const float2 q = pg[row];
+        float2 q;
+        int64_t u;                                           // PRUNED: the row's lattice column
+        uint32_t nt;                                         // PRUNED: n*T + t
+        if constexpr (ROWS == kRowsPruned) {
+            uint32_t s;
+            divU.divmod((uint32_t)row, nt, s);
+            u = (int64_t)ranges[nt] + s;
+            q = (u >= 0 && u < U) ? pg[(int64_t)nt * U + u] : make_float2(0.0f, 0.0f);
+        } else {
+            q = pg[row];
+        }
         float e[VEC];
         if (q.x == 0.0f && q.y == 0.0f) {
             // padding (or a cell without gradient): exact zeros -- (0 - softmax * 0), as log_softmax's backward gives,
@@ -224,7 +286,11 @@ k_expand_logits(const IO *__restrict__ x, const float *__restrict__ lse, const f
         } else {
             int lab;
             float sc;
-            if constexpr (COMPACT) {
+            if constexpr (ROWS == kRowsPruned) {
+                const uint32_t n = divTU.div(nt);
+                lab = (u < U - 1) ? labels[(int64_t)n * (U - 1) + u] : -1;
+                sc = grad_out ? grad_out[n] : 1.0f;
+            } else if constexpr (COMPACT) {
                 const int u = (int)row % L.Un;
                 lab = (u < L.Un - 1) ? labels[L.lab_base + u] : -1;
                 sc = grad_out ? grad_out[blockIdx.y] : 1.0f;
@@ -249,6 +315,28 @@ k_expand_logits(const IO *__restrict__ x, const float *__restrict__ lse, const f
     }
 }
 
+template <typename IO, int VEC, bool COMPACT = false>
+__global__ void __launch_bounds__(kLogitThreads)
+k_expand_logits(const IO *__restrict__ x, const float *__restrict__ lse, const float2 *__restrict__ pg,
+                const int *__restrict__ labels, const float *__restrict__ grad_out, IO *__restrict__ out,
+                int64_t cells, int V, int blank, int U, FastDiv divU, FastDiv divTU, int64_t stride_rows,
+                int stride_v, Problem lay) {
+    expand_logits_rows<IO, VEC, COMPACT ? kRowsCompact : kRowsDense>(x, lse, pg, labels, grad_out, out, cells, V, blank,
+                                                                     U, divU, divTU, stride_rows, stride_v, lay,
+                                                                     nullptr);
+}
+
+// rows = N*T*S pruned rows, written (N,T,S,V); pg: the full (N,T,U,2) pair gradients; divS, divT: FastDiv(S), FastDiv(T)
+template <typename IO, int VEC>
+__global__ void __launch_bounds__(kLogitThreads)
+k_expand_logits_pruned(const IO *__restrict__ x, const float *__restrict__ lse, const float2 *__restrict__ pg,
+                       const int *__restrict__ labels, const int *__restrict__ ranges, const float *__restrict__ grad_out,
+                       IO *__restrict__ out, int64_t rows, int V, int blank, int U, FastDiv divS, FastDiv divT,
+                       int64_t stride_rows, int stride_v) {
+    expand_logits_rows<IO, VEC, kRowsPruned>(x, lse, pg, labels, grad_out, out, rows, V, blank, U, divS, divT,
+                                             stride_rows, stride_v, Problem{}, ranges);
+}
+
 // Compact grids are (gx, N): lattice lengths are on the device only, so gx covers twice the average lattice
 // (STU / N rows, as launch_gather sizes its grid) in CTAs of kCompactIters grid-stride iterations each; a larger lattice
 // is finished by the grid stride, the surplus CTAs of a smaller one return at once.
@@ -259,13 +347,22 @@ static int compact_gx(int64_t STU, int N, int64_t per_cta_rows) {
 }
 
 // lay == nullptr: dense (N,T,U,V) logits; else the compact (STU,V) rows of lattices lay->N, lay->T = lay->U = 0.
+// ranges != nullptr: the pruned (N,T,S,V) rows of windows ranges (N,T) on the full (N,T,U) lattice.
 template <typename IN>
 static cudaError_t lse_pairs_as(cudaStream_t s, const IN *x, const int *labels, int N, int T, int U, int V, int blank,
-                                float2 *pairs, float *lse, const Problem *lay, int64_t STU) {
-    const int64_t cells = lay ? STU : (int64_t)N * T * U;
+                                float2 *pairs, float *lse, const Problem *lay, int64_t STU, const int *ranges = nullptr,
+                                int S = 0) {
+    const int64_t cells = lay ? STU : (int64_t)N * T * (ranges ? S : U);
     if (cells <= 0 || N <= 0) return cudaSuccess;
-    const FastDiv divU((uint32_t)max(U, 1)), divTU((uint32_t)max(T * U, 1));
+    // pruned: the row -> (n*T + t, s) -> (n, t) divisions
+    const FastDiv divU((uint32_t)max(ranges ? S : U, 1)), divTU((uint32_t)max(ranges ? T : T * U, 1));
     const int sms = sm_count(current_device());
+    if (ranges) {
+        const int64_t quads = (int64_t)N * T * U / 2 + 1;
+        k_fill_pairs<<<(unsigned)min((quads + kLogitThreads - 1) / kLogitThreads, (int64_t)sms * 16), kLogitThreads, 0,
+                       s>>>(reinterpret_cast<float4 *>(pairs), (int64_t)N * T * U);
+        count_launch();
+    }
     // groups of 4 elements: float4 (16 bytes) or 4 bf16 (8 bytes) per load
     const bool vec4 = (V % 4 == 0) && ((reinterpret_cast<uintptr_t>(x) & (4 * sizeof(IN) - 1)) == 0);
     const int sub = vec4 ? (V <= 32 ? 8 : 32) : (V <= 12 ? 1 : (V <= 512 ? 8 : 32));
@@ -275,6 +372,7 @@ static cudaError_t lse_pairs_as(cudaStream_t s, const IN *x, const int *labels, 
                           : dim3((unsigned)min((cells + per_block - 1) / per_block, (int64_t)sms * 16));
 #define RNNT_LSE_LAUNCH(SUB, VEC)                                                                                          \
     (lay ? k_lse_pairs<IN, SUB, VEC, true><<<grid, kLogitThreads, 0, s>>>(x, labels, cells, V, blank, U, divU, divTU, pairs, lse, p) \
+     : ranges ? k_lse_pairs_pruned<IN, SUB, VEC><<<grid, kLogitThreads, 0, s>>>(x, labels, ranges, cells, V, blank, U, divU, divTU, pairs, lse) \
          : k_lse_pairs<IN, SUB, VEC><<<grid, kLogitThreads, 0, s>>>(x, labels, cells, V, blank, U, divU, divTU, pairs, lse, p))
     if (vec4) { if (sub == 8) RNNT_LSE_LAUNCH(8, true); else RNNT_LSE_LAUNCH(32, true); }
     else if (sub == 1) RNNT_LSE_LAUNCH(1, false);
@@ -299,13 +397,14 @@ cudaError_t launch_lse_pairs_compact(cudaStream_t s, const void *x, const Proble
     return lse_pairs_as(s, static_cast<const float *>(x), labels, p.N, 0, 0, V, blank, pairs, lse, &p, STU);
 }
 
+// lay, ranges: as for lse_pairs_as
 template <typename IO>
 static cudaError_t expand_logits_as(cudaStream_t s, const IO *x, const float *lse, const float2 *pg, const int *labels,
                                     const float *grad_out, IO *out, int N, int T, int U, int V, int blank,
-                                    const Problem *lay, int64_t STU) {
-    const int64_t cells = lay ? STU : (int64_t)N * T * U;
+                                    const Problem *lay, int64_t STU, const int *ranges = nullptr, int S = 0) {
+    const int64_t cells = lay ? STU : (int64_t)N * T * (ranges ? S : U);
     if (cells <= 0 || N <= 0) return cudaSuccess;
-    const FastDiv divU((uint32_t)max(U, 1)), divTU((uint32_t)max(T * U, 1));
+    const FastDiv divU((uint32_t)max(ranges ? S : U, 1)), divTU((uint32_t)max(ranges ? T : T * U, 1));
     const int sms = sm_count(current_device());
     // the widest vector (at most 16 bytes) that V and the alignment of both tensors allow
     const uintptr_t al = reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out);
@@ -323,6 +422,7 @@ static cudaError_t expand_logits_as(cudaStream_t s, const IO *x, const float *ls
     const int sv = (int)(stride - srows * V);
 #define RNNT_EXPAND_LAUNCH(VEC)                                                                                            \
     (lay ? k_expand_logits<IO, VEC, true><<<grid, kLogitThreads, 0, s>>>(x, lse, pg, labels, grad_out, out, cells, V, blank, U, divU, divTU, srows, sv, p) \
+     : ranges ? k_expand_logits_pruned<IO, VEC><<<grid, kLogitThreads, 0, s>>>(x, lse, pg, labels, ranges, grad_out, out, cells, V, blank, U, divU, divTU, srows, sv) \
          : k_expand_logits<IO, VEC><<<grid, kLogitThreads, 0, s>>>(x, lse, pg, labels, grad_out, out, cells, V, blank, U, divU, divTU, srows, sv, p))
     if constexpr (sizeof(IO) == 2) {
         if (vec == 8) RNNT_EXPAND_LAUNCH(8);
@@ -356,6 +456,24 @@ cudaError_t launch_expand_logits_compact(cudaStream_t s, const void *x, const fl
                                 static_cast<__nv_bfloat16 *>(out), p.N, 0, 0, V, blank, &p, STU);
     return expand_logits_as(s, static_cast<const float *>(x), lse, pg, labels, grad_out, static_cast<float *>(out), p.N,
                             0, 0, V, blank, &p, STU);
+}
+
+cudaError_t launch_lse_pairs_pruned(cudaStream_t s, const void *x, const int *labels, const int *ranges, int N, int T,
+                                    int S, int U, int V, int blank, float2 *pairs, float *lse, int io_bf16) {
+    if (io_bf16)
+        return lse_pairs_as(s, static_cast<const __nv_bfloat16 *>(x), labels, N, T, U, V, blank, pairs, lse, nullptr, 0,
+                            ranges, S);
+    return lse_pairs_as(s, static_cast<const float *>(x), labels, N, T, U, V, blank, pairs, lse, nullptr, 0, ranges, S);
+}
+
+cudaError_t launch_expand_logits_pruned(cudaStream_t s, const void *x, const float *lse, const float2 *pg,
+                                        const int *labels, const int *ranges, const float *grad_out, void *out, int N,
+                                        int T, int S, int U, int V, int blank, int io_bf16) {
+    if (io_bf16)
+        return expand_logits_as(s, static_cast<const __nv_bfloat16 *>(x), lse, pg, labels, grad_out,
+                                static_cast<__nv_bfloat16 *>(out), N, T, U, V, blank, nullptr, 0, ranges, S);
+    return expand_logits_as(s, static_cast<const float *>(x), lse, pg, labels, grad_out, static_cast<float *>(out), N, T,
+                            U, V, blank, nullptr, 0, ranges, S);
 }
 
 }  // namespace rnnt
