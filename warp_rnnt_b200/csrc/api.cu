@@ -124,6 +124,8 @@ static bool pruned_args_ok(int N, int T, int S, int U, int V, int blank) {
 }
 // (cells,2) pairs and their gradients are read and written as float2
 static bool pairs_aligned(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 7u) == 0; }
+// k_fill_pairs writes the workspace's pairs, carved at its base, two cells per float4
+static bool workspace_aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 // Internal streams for the pipelined general path: one for gathers, one for emits, four
 // high-priority ones for wavefronts (their CTAs are few and long-lived; priority lets them take the
@@ -731,7 +733,8 @@ int rnnt_b200_logits_pruned_forward(void *stream, void *workspace, size_t worksp
                                     float *lse, float *pair_grads, int N, int T, int S, int U, int V, int blank,
                                     float fastemit_lambda, int lse_mode, int elem_bytes) {
     if ((elem_bytes != 4 && elem_bytes != 2) || (reinterpret_cast<uintptr_t>(logits) & (uintptr_t)(elem_bytes - 1)) ||
-        !pruned_args_ok(N, T, S, U, V, blank) || !lse || !pairs_aligned(pair_grads))
+        !pruned_args_ok(N, T, S, U, V, blank) || !lse || !pairs_aligned(pair_grads) ||
+        !workspace_aligned16(workspace))
         return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
     cudaStream_t s = (cudaStream_t)stream;
