@@ -258,7 +258,8 @@ def rnnt_loss_pruned(logits, labels, frames_lengths, labels_lengths, ranges, ave
     loss is the RNN-T loss of lattice n in which the blank edge (t,u)->(t+1,u) and the label edge (t,u)->(t,u+1) of an
     in-window cell carry log_softmax(logits[n,t,s]) at ``blank`` and at labels[n,u], and every edge out of a cell outside
     its frame's window is removed.  This is k2's ``rnnt_loss_pruned(..., rnnt_type="regular")`` with k2's
-    ``ranges[:, :, 0]`` as ``ranges``.
+    ``ranges[:, :, 0]`` as ``ranges``.  ``rnnt_loss_simple(..., prune_range=S)`` returns such ranges, chosen from the
+    occupation probabilities of the simple (factorised) joint, as k2's ``get_rnnt_prune_ranges`` does.
 
     Costs are float32; the gradient is w.r.t. ``logits``, of their dtype (bfloat16: the float32 gradient of the
     widened logits rounded once).  Padding rows get exact zeros, or NaN where the row's normaliser is NaN.  A lattice
@@ -277,6 +278,86 @@ def rnnt_loss_pruned(logits, labels, frames_lengths, labels_lengths, ranges, ave
     if reduction == "mean":
         return costs.mean()
     return costs
+
+
+class RNNTLossSimple(torch.autograd.Function):
+    """The simple loss of the pruned recipe: the transducer loss of the joint ``am[n,t] + lm[n,u]``, whose normaliser is
+    a (T,V) x (V,U) product per lattice, so no (N,T,U,V) tensor is formed.  Forward keeps the normaliser (N,T,U), the
+    row offsets of ``am`` and ``lm`` and the (N,T,U,2) pair gradients; backward writes d loss / d ``am`` and d ``lm``.
+    With ``prune_range`` > 0 the forward also returns the (N,T) prune ranges (else an empty int tensor)."""
+
+    @staticmethod
+    def forward(ctx, am, lm, labels, frames_lengths, labels_lengths, blank=0, prune_range=0):
+        need = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
+        costs, saved, pg, ranges = _C.rnnt_simple_forward(am, lm, labels, frames_lengths, labels_lengths, blank, need,
+                                                          prune_range, 0)
+        if need:
+            ctx.save_for_backward(am, lm, labels, frames_lengths, labels_lengths, saved, pg)
+            ctx.blank = blank
+        ctx.mark_non_differentiable(ranges)
+        return costs, ranges
+
+    @staticmethod
+    def backward(ctx, grads_output, _grad_ranges):
+        am, lm, labels, xn, yn, saved, pg = ctx.saved_tensors
+        go = grads_output.contiguous().to(torch.float32)
+        dam, dlm = _C.rnnt_simple_backward(am, lm, labels, xn, yn, saved, pg, go, ctx.blank)
+        return (dam if ctx.needs_input_grad[0] else None), (dlm if ctx.needs_input_grad[1] else None), \
+            None, None, None, None, None
+
+
+def rnnt_loss_simple(am, lm, labels, frames_lengths, labels_lengths, average_frames=False, reduction="none", blank=0,
+                     prune_range=None):
+    """Simple transducer loss of the pruned recipe, and the windows ``rnnt_loss_pruned`` takes.  Follows k2's
+    ``rnnt_loss_simple`` + ``get_rnnt_prune_ranges`` (regular lattice); not tested against k2.
+
+    Args:
+        am: (N, T, V) float32, the encoder output projected to the vocabulary.
+        lm: (N, U, V) float32, the predictor output projected to the vocabulary; U = labels.size(1) + 1.
+        labels: (N, U-1) int32; frames_lengths, labels_lengths: (N,) int32, as for ``rnnt_loss``.
+        average_frames, reduction, blank: as in ``rnnt_loss_from_logits``.
+        prune_range: None, or an int S >= 2: also return the (N, T) int32 ``ranges`` for
+            ``rnnt_loss_pruned(..., ranges)`` with windows of S labels.
+
+    The loss is the RNN-T loss of lattice n in which cell (t, u) has the log-probs log_softmax(am[n,t] + lm[n,u]) at
+    ``blank`` and at labels[n,u].  Its normaliser is log(sum_v exp(am[n,t,v]) exp(lm[n,u,v])), a fp32 contraction over
+    V (include/rnnt_b200.h gives the exact operation order); a cell whose products all underflow is clamped to
+    log(FLT_MIN) plus the row maxima instead of going to -inf.  The gradient flows to ``am`` and ``lm``, deterministic.
+
+    The ranges come from the occupation probabilities of this loss's lattice: each frame takes the window of S columns
+    with the most occupation, then the windows are made to start at 0, never move back, move by at most S-1 columns a
+    frame and end on the last label.  The call returns ``(loss, ranges)`` then.  The ranges carry no gradient.
+
+    bfloat16 ``am`` / ``lm`` are refused: these tensors are small beside the joint, and the loss is run in float32.
+    Lengths outside (1..T, 0..U-1) give cost NaN, zero gradient rows and ranges 0.  No host synchronisation: the step
+    can be captured in a CUDA graph.
+
+    Typical use, with no (N, T, U, V) tensor anywhere::
+
+        simple, ranges = rnnt_loss_simple(am, lm, labels, xn, yn, reduction="sum", prune_range=5)
+        idx = (ranges[:, :, None] + torch.arange(5, device=ranges.device)).clamp(max=lm_in.size(1) - 1)
+        lm_win = lm_in[torch.arange(N, device=lm_in.device)[:, None, None], idx]     # (N, T, 5, H)
+        logits = joint(enc_in[:, :, None] + lm_win)                                  # (N, T, 5, V)
+        loss = simple_scale * simple + rnnt_loss_pruned(logits, labels, xn, yn, ranges, reduction="sum")
+    """
+    assert average_frames is None or isinstance(average_frames, bool)
+    assert reduction is None or reduction in ("none", "mean", "sum")
+    assert isinstance(blank, int)
+    assert not labels.requires_grad and not frames_lengths.requires_grad and not labels_lengths.requires_grad
+    if am.dtype != torch.float32 or lm.dtype != torch.float32:
+        raise TypeError("rnnt_loss_simple: am and lm must be float32, got %s and %s (bfloat16 is not supported; "
+                        "run this loss outside autocast or cast with .float())" % (am.dtype, lm.dtype))
+    if prune_range is not None and (isinstance(prune_range, bool) or not isinstance(prune_range, int)
+                                    or prune_range < 2):
+        raise ValueError("rnnt_loss_simple: prune_range must be None or an int >= 2, got %r" % (prune_range,))
+    costs, ranges = RNNTLossSimple.apply(am, lm, labels, frames_lengths, labels_lengths, blank, prune_range or 0)
+    if average_frames:
+        costs = costs / frames_lengths.to(costs.dtype)
+    if reduction == "sum":
+        costs = costs.sum()
+    elif reduction == "mean":
+        costs = costs.mean()
+    return costs if prune_range is None else (costs, ranges)
 
 
 class JointPack(torch.autograd.Function):
@@ -459,6 +540,7 @@ def rnnt_align(log_probs, labels, frames_lengths, labels_lengths, blank=0, compa
     return _C.rnnt_align_dense(log_probs, labels, frames_lengths, labels_lengths, blank)
 
 
-__all__ = ["rnnt_loss", "rnnt_align", "rnnt_loss_from_logits", "rnnt_loss_pruned", "RNNTLossPruned", "joint_pack",
+__all__ = ["rnnt_loss", "rnnt_align", "rnnt_loss_from_logits", "rnnt_loss_pruned", "RNNTLossPruned",
+           "rnnt_loss_simple", "RNNTLossSimple", "joint_pack",
            "JointPack", "RNNTLossFromLogits", "RNNTLossFromLogitsCompact", "RNNTLoss", "RNNTLossGather", "RNNTLossEager",
            "RNNTLossCompact", "compact_hints", "set_lse_mode", "core", "_C", "__version__"]

@@ -122,6 +122,21 @@ static bool compact_args_ok(int N, int64_t STU, int V, int blank) {
 static bool pruned_args_ok(int N, int T, int S, int U, int V, int blank) {
     return S >= 1 && dense_args_ok(N, T, U, V, blank) && (int64_t)N * T * S < (int64_t)1 << 31;
 }
+// the simple loss: the (N,T,U) lattice as dense_args_ok takes it; its contractions put N on the grid's z axis
+static bool simple_args_ok(int N, int T, int U, int V, int blank) {
+    return dense_args_ok(N, T, U, V, blank) && N <= 65535;
+}
+// the simple loss's saved buffer: norm (N,T,U), then the row offsets of am (N,T) and of lm (N,U)
+static SimpleArgs simple_call(const float *am, const float *lm, const int *labels, const int *xn, const int *yn,
+                              float *saved, int N, int T, int U, int V, int blank) {
+    SimpleArgs a = {};
+    a.am = am; a.lm = lm; a.labels = labels; a.xn = xn; a.yn = yn;
+    a.norm = saved;
+    a.off_a = saved + (int64_t)N * T * U;
+    a.off_l = a.off_a + (int64_t)N * T;
+    a.T = T; a.U = U; a.V = V; a.blank = blank;
+    return a;
+}
 // (cells,2) pairs and their gradients are read and written as float2
 static bool pairs_aligned(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 7u) == 0; }
 // k_fill_pairs writes the workspace's pairs, carved at its base, two cells per float4
@@ -759,6 +774,51 @@ int rnnt_b200_logits_pruned_backward(void *stream, const void *logits, const flo
     RNNT_TRY(launch_expand_logits_pruned((cudaStream_t)stream, logits, lse, reinterpret_cast<const float2 *>(pair_grads),
                                          labels, ranges, grad_out, out, N, T, S, U, V, blank, elem_bytes == 2),
              RNNT_STATUS_GRADS_BLANK_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+size_t rnnt_b200_simple_workspace_bytes(int N, int T, int U) {
+    return carve(nullptr, (int64_t)max(N, 0) * max(T, 0) * max(U, 0), N).bytes;
+}
+
+int rnnt_b200_simple_forward(void *stream, void *workspace, size_t workspace_bytes, const float *am, const float *lm,
+                             const int *labels, const int *xn, const int *yn, float *costs, float *saved,
+                             float *pair_grads, int N, int T, int U, int V, int blank, int lse_mode) {
+    if (!simple_args_ok(N, T, U, V, blank) || !saved || !pairs_aligned(pair_grads) || !pairs_aligned(workspace))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    cudaStream_t s = (cudaStream_t)stream;
+    LossCall c = dense_call(xn, yn, N, T, U, costs, 0.0f, lse_mode);
+    Workspace w;
+    if (!carve_ok(workspace, workspace_bytes, c.cells, N, &w)) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    SimpleArgs a = simple_call(am, lm, labels, xn, yn, saved, N, T, U, V, blank);
+    a.pairs = w.pairs;
+    RNNT_TRY(launch_simple_forward(s, a, N), RNNT_STATUS_GATHER_FAILED);
+    c.pairs = w.pairs; c.pair_grads = reinterpret_cast<float2 *>(pair_grads);
+    return run_loss(s, workspace, workspace_bytes, c);
+}
+
+int rnnt_b200_simple_backward(void *stream, const float *am, const float *lm, const int *labels, const int *xn,
+                              const int *yn, const float *saved, const float *pair_grads, const float *grad_out,
+                              float *dam, float *dlm, int N, int T, int U, int V, int blank) {
+    if (!simple_args_ok(N, T, U, V, blank) || !saved || !pair_grads || !pairs_aligned(pair_grads) || !dam || !dlm)
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    SimpleArgs a = simple_call(am, lm, labels, xn, yn, const_cast<float *>(saved), N, T, U, V, blank);
+    a.pg = reinterpret_cast<const float2 *>(pair_grads);
+    a.grad_out = grad_out;
+    RNNT_TRY(launch_simple_backward((cudaStream_t)stream, a, dam, dlm, N), RNNT_STATUS_GRADS_BLANK_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+int rnnt_b200_prune_ranges(void *stream, const float *pair_grads, const int *xn, const int *yn, int N, int T, int U,
+                           int S, int *ranges) {
+    if (!simple_args_ok(N, T, U, 1, 0) || S < 2 || !pair_grads || !pairs_aligned(pair_grads) || !ranges)
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    RNNT_TRY(launch_prune_ranges((cudaStream_t)stream, reinterpret_cast<const float2 *>(pair_grads), xn, yn, N, T, U, S,
+                                 ranges),
+             RNNT_STATUS_GATHER_FAILED);
     return RNNT_STATUS_SUCCESS;
 }
 

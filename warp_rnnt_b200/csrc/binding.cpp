@@ -502,6 +502,103 @@ at::Tensor rnnt_logits_pruned_backward(const at::Tensor &xs, const at::Tensor &l
     return out;
 }
 
+void check_simple_inputs(const at::Tensor &am, const at::Tensor &lm, const at::Tensor &ys, const at::Tensor &xn,
+                         const at::Tensor &yn) {
+    TORCH_CHECK(am.scalar_type() == at::ScalarType::Float && lm.scalar_type() == at::ScalarType::Float,
+                "am and lm must be float32 tensors (the simple loss does not take bfloat16)");
+    TORCH_CHECK(am.is_contiguous() && lm.is_contiguous() && am.device().is_cuda() && lm.device() == am.device(),
+                "am and lm must be contiguous CUDA tensors on one device");
+    TORCH_CHECK(am.dim() == 3 && lm.dim() == 3 && lm.size(0) == am.size(0) && lm.size(2) == am.size(2),
+                "am must be (N, T, V) and lm (N, U, V)");
+    const int64_t N = am.size(0);
+    TORCH_CHECK(ys.is_contiguous() && ys.scalar_type() == at::ScalarType::Int && ys.device() == am.device() &&
+                    ys.dim() == 2 && ys.size(0) == N && ys.size(1) + 1 == lm.size(1),
+                "ys must be a contiguous Int tensor of shape (N, U-1) on the device of am");
+    TORCH_CHECK(xn.is_contiguous() && yn.is_contiguous() && xn.scalar_type() == at::ScalarType::Int &&
+                    yn.scalar_type() == at::ScalarType::Int && xn.device() == am.device() &&
+                    yn.device() == am.device() && xn.numel() == N && yn.numel() == N,
+                "xn and yn must be contiguous Int tensors of shape (N,) on the device of am");
+}
+
+// simple loss from am (N,T,V) and lm (N,U,V), float32: (costs (N), saved (N*T*U + N*T + N*U), pair_grads (N,T,U,2) or
+// empty, ranges (N,T) int32 or empty).  The pair gradients are computed when want_grads or prune_range > 0; the ranges
+// when prune_range > 0.  No host sync.
+std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor>
+rnnt_simple_forward(const at::Tensor &am, const at::Tensor &lm, const at::Tensor &ys, const at::Tensor &xn,
+                    const at::Tensor &yn, int blank, bool want_grads, int prune_range, int lse_mode) {
+    check_simple_inputs(am, lm, ys, xn, yn);
+    const int64_t N = am.size(0), T = am.size(1), U = lm.size(1), V = am.size(2);
+    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    TORCH_CHECK(prune_range == 0 || prune_range >= 2, "prune_range must be an int >= 2");
+    const c10::cuda::CUDAGuard guard(am.device());
+    const auto f32 = am.options().dtype(at::kFloat);
+    const bool pairs = want_grads || prune_range > 0;
+    at::Tensor costs = at::empty({N}, f32);
+    at::Tensor saved = at::empty({N * T * U + N * T + N * U}, f32);
+    at::Tensor pg = pairs ? at::empty({N, T, U, 2}, f32) : at::empty({0}, f32);
+    at::Tensor ranges = at::empty({prune_range > 0 ? N : 0, prune_range > 0 ? T : 0}, am.options().dtype(at::kInt));
+    if (N == 0) return std::make_tuple(costs, saved, pg, ranges);
+    void *stream = current_stream(am);
+    const size_t bytes = rnnt_b200_simple_workspace_bytes((int)N, (int)T, (int)U);
+    at::Tensor ws = at::empty({(int64_t)bytes}, am.options().dtype(at::kByte));
+    check_status(rnnt_b200_simple_forward(stream, ws.data_ptr(), bytes, am.data_ptr<float>(), lm.data_ptr<float>(),
+                                          ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
+                                          costs.data_ptr<float>(), saved.data_ptr<float>(),
+                                          pairs ? pg.data_ptr<float>() : nullptr, (int)N, (int)T, (int)U, (int)V, blank,
+                                          lse_mode));
+    if (prune_range > 0)
+        check_status(rnnt_b200_prune_ranges(stream, pg.data_ptr<float>(), xn.data_ptr<int>(), yn.data_ptr<int>(), (int)N,
+                                            (int)T, (int)U, prune_range, ranges.data_ptr<int>()));
+    return std::make_tuple(costs, saved, pg, ranges);
+}
+
+// d sum_n grad_out[n] cost[n] / d (am, lm)
+std::tuple<at::Tensor, at::Tensor> rnnt_simple_backward(const at::Tensor &am, const at::Tensor &lm, const at::Tensor &ys,
+                                                        const at::Tensor &xn, const at::Tensor &yn,
+                                                        const at::Tensor &saved, const at::Tensor &pair_grads,
+                                                        const at::Tensor &grad_out, int blank) {
+    check_simple_inputs(am, lm, ys, xn, yn);
+    const int64_t N = am.size(0), T = am.size(1), U = lm.size(1), V = am.size(2);
+    TORCH_CHECK(saved.is_contiguous() && saved.scalar_type() == at::ScalarType::Float && saved.device() == am.device() &&
+                    saved.numel() == N * T * U + N * T + N * U,
+                "saved must be the simple forward's contiguous Float tensor on the device of am");
+    TORCH_CHECK(pair_grads.is_contiguous() && pair_grads.scalar_type() == at::ScalarType::Float &&
+                    pair_grads.device() == am.device() && pair_grads.numel() == N * T * U * 2,
+                "pair_grads must be a contiguous Float tensor of shape (N, T, U, 2) on the device of am");
+    TORCH_CHECK(grad_out.is_contiguous() && grad_out.scalar_type() == at::ScalarType::Float &&
+                    grad_out.device() == am.device() && grad_out.numel() == N,
+                "grad_out must be a contiguous Float tensor of shape (N,)");
+    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    const c10::cuda::CUDAGuard guard(am.device());
+    at::Tensor dam = at::empty_like(am), dlm = at::empty_like(lm);
+    if (N == 0) return std::make_tuple(dam, dlm);
+    check_status(rnnt_b200_simple_backward(current_stream(am), am.data_ptr<float>(), lm.data_ptr<float>(),
+                                           ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
+                                           saved.data_ptr<float>(), pair_grads.data_ptr<float>(),
+                                           grad_out.data_ptr<float>(), dam.data_ptr<float>(), dlm.data_ptr<float>(),
+                                           (int)N, (int)T, (int)U, (int)V, blank));
+    return std::make_tuple(dam, dlm);
+}
+
+// prune ranges (N,T) int32 from pair gradients (N,T,U,2) of a loss call
+at::Tensor rnnt_prune_ranges(const at::Tensor &pair_grads, const at::Tensor &xn, const at::Tensor &yn, int S) {
+    TORCH_CHECK(pair_grads.is_contiguous() && pair_grads.scalar_type() == at::ScalarType::Float &&
+                    pair_grads.device().is_cuda() && pair_grads.dim() == 4 && pair_grads.size(3) == 2,
+                "pair_grads must be a contiguous CUDA Float tensor of shape (N, T, U, 2)");
+    const int64_t N = pair_grads.size(0), T = pair_grads.size(1), U = pair_grads.size(2);
+    TORCH_CHECK(xn.is_contiguous() && yn.is_contiguous() && xn.scalar_type() == at::ScalarType::Int &&
+                    yn.scalar_type() == at::ScalarType::Int && xn.device() == pair_grads.device() &&
+                    yn.device() == pair_grads.device() && xn.numel() == N && yn.numel() == N,
+                "xn and yn must be contiguous Int tensors of shape (N,) on the device of pair_grads");
+    TORCH_CHECK(S >= 2, "prune_range must be an int >= 2");
+    const c10::cuda::CUDAGuard guard(pair_grads.device());
+    at::Tensor ranges = at::empty({N, T}, pair_grads.options().dtype(at::kInt));
+    if (N == 0) return ranges;
+    check_status(rnnt_b200_prune_ranges(current_stream(pair_grads), pair_grads.data_ptr<float>(), xn.data_ptr<int>(),
+                                        yn.data_ptr<int>(), (int)N, (int)T, (int)U, S, ranges.data_ptr<int>()));
+    return ranges;
+}
+
 // compact packing of the joint input: (x (STU,H), mem_pref (N) int64).  stu < 0: STU is read back from the device
 // (one 16-byte copy); stu >= 0: trusted, no host sync.
 std::tuple<at::Tensor, at::Tensor> rnnt_joint_pack(const at::Tensor &f, const at::Tensor &g, const at::Tensor &lf,
@@ -666,6 +763,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("want_grads") = true, py::arg("lse_mode") = 0);
     m.def("rnnt_logits_pruned_backward", &rnnt_logits_pruned_backward, py::arg("xs"), py::arg("lse"),
           py::arg("pair_grads"), py::arg("ys"), py::arg("ranges"), py::arg("grad_out"), py::arg("blank") = 0);
+    m.def("rnnt_simple_forward", &rnnt_simple_forward, py::arg("am"), py::arg("lm"), py::arg("ys"), py::arg("xn"),
+          py::arg("yn"), py::arg("blank") = 0, py::arg("want_grads") = true, py::arg("prune_range") = 0,
+          py::arg("lse_mode") = 0);
+    m.def("rnnt_simple_backward", &rnnt_simple_backward, py::arg("am"), py::arg("lm"), py::arg("ys"), py::arg("xn"),
+          py::arg("yn"), py::arg("saved"), py::arg("pair_grads"), py::arg("grad_out"), py::arg("blank") = 0);
+    m.def("rnnt_prune_ranges", &rnnt_prune_ranges, py::arg("pair_grads"), py::arg("xn"), py::arg("yn"), py::arg("S"));
     m.def("rnnt_joint_pack", &rnnt_joint_pack, py::arg("f"), py::arg("g"), py::arg("lf"), py::arg("lg"), py::arg("stu") = -1);
     m.def("rnnt_joint_pack_backward", &rnnt_joint_pack_backward, py::arg("dx"), py::arg("lf"), py::arg("lg"),
           py::arg("mem_pref"), py::arg("T"), py::arg("U1"));

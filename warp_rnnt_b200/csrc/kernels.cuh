@@ -76,6 +76,25 @@ cudaError_t launch_expand_logits_pruned(cudaStream_t s, const void *x, const flo
                                         const int *labels, const int *ranges, const float *grad_out, void *out, int N,
                                         int T, int S, int U, int V, int blank, int io_bf16);
 
+// simple.cu -- the simple (factorised-joint) loss: am (N,T,V) + lm (N,U,V), and the prune ranges of its lattice
+struct SimpleArgs {
+    const float *am, *lm;              // (N,T,V), (N,U,V)
+    const int *labels, *xn, *yn;       // (N,U-1), (N), (N)
+    float *norm, *off_a, *off_l;       // (N,T,U), (N,T), (N,U): written by the forward, read by the backward
+    float2 *pairs;                     // forward: (N,T,U) (blank, label) log-probs out
+    const float2 *pg;                  // backward: (N,T,U) pair gradients
+    const float *grad_out;             // backward: (N), or null (ones)
+    float *out;                        // the contraction's output (set by launch_simple_backward)
+    int T, U, V, blank;
+};
+// row offsets, Z and the epilogue: norm and the pairs of every cell (0 outside the lattice)
+cudaError_t launch_simple_forward(cudaStream_t s, const SimpleArgs &a, int N);
+// dam (N,T,V) and dlm (N,U,V), every element written
+cudaError_t launch_simple_backward(cudaStream_t s, const SimpleArgs &a, float *dam, float *dlm, int N);
+// ranges (N,T) from the pair gradients (N,T,U,2) of a loss call; S >= 2
+cudaError_t launch_prune_ranges(cudaStream_t s, const float2 *pg, const int *xn, const int *yn, int N, int T, int U,
+                                int S, int *ranges);
+
 // joint.cu -- compact packing of the joint network's input (caller side of compact=True)
 cudaError_t launch_joint_pack(cudaStream_t s, const float *f, const float *g, const int *lf, const int *lg,
                               const int64_t *mem_pref, float *x, int N, int T, int U1, int H, int64_t stu_hint);
