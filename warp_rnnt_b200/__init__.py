@@ -169,7 +169,7 @@ class RNNTLossFromLogitsCompact(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logits, labels, frames_lengths, labels_lengths, blank=0, fastemit_lambda=0.0):
         need = ctx.needs_input_grad[0]
-        hints = getattr(_tls, "hints", None) or (0, 0)
+        hints = _hints()
         costs, lse, pg, prefix = _C.rnnt_logits_compact_forward(logits, labels, frames_lengths, labels_lengths, blank,
                                                                 fastemit_lambda, need, 0, hints[0], hints[1])
         if need:
@@ -183,6 +183,18 @@ class RNNTLossFromLogitsCompact(torch.autograd.Function):
         go = grads_output.contiguous().to(torch.float32)
         g = _C.rnnt_logits_compact_backward(logits, lse, pg, labels, xn, yn, prefix, go, ctx.blank)
         return g, None, None, None, None, None
+
+
+def _reduce(costs, frames_lengths, average_frames, reduction):
+    """The float32 costs of a loss call divided by the frame counts when ``average_frames``, then summed or averaged
+    for ``reduction`` 'sum' or 'mean' ('none' and None keep them)."""
+    if average_frames:
+        costs = costs / frames_lengths.to(costs.dtype)      # float32: bf16 would round frame counts (601 -> 600)
+    if reduction == "sum":
+        return costs.sum()
+    if reduction == "mean":
+        return costs.mean()
+    return costs
 
 
 def rnnt_loss_from_logits(logits, labels, frames_lengths, labels_lengths, average_frames=False, reduction="none",
@@ -207,13 +219,7 @@ def rnnt_loss_from_logits(logits, labels, frames_lengths, labels_lengths, averag
     assert not labels.requires_grad and not frames_lengths.requires_grad and not labels_lengths.requires_grad
     fn = RNNTLossFromLogitsCompact if compact else RNNTLossFromLogits
     costs = fn.apply(logits, labels, frames_lengths, labels_lengths, blank, fastemit_lambda)
-    if average_frames:
-        costs = costs / frames_lengths.to(costs.dtype)      # float32: bf16 would round frame counts (601 -> 600)
-    if reduction == "sum":
-        return costs.sum()
-    if reduction == "mean":
-        return costs.mean()
-    return costs
+    return _reduce(costs, frames_lengths, average_frames, reduction)
 
 
 class RNNTLossPruned(torch.autograd.Function):
@@ -271,13 +277,7 @@ def rnnt_loss_pruned(logits, labels, frames_lengths, labels_lengths, ranges, ave
     assert not labels.requires_grad and not frames_lengths.requires_grad and not labels_lengths.requires_grad
     assert not ranges.requires_grad
     costs = RNNTLossPruned.apply(logits, labels, frames_lengths, labels_lengths, ranges, blank, fastemit_lambda)
-    if average_frames:
-        costs = costs / frames_lengths.to(costs.dtype)
-    if reduction == "sum":
-        return costs.sum()
-    if reduction == "mean":
-        return costs.mean()
-    return costs
+    return _reduce(costs, frames_lengths, average_frames, reduction)
 
 
 class RNNTLossSimple(torch.autograd.Function):
@@ -351,12 +351,7 @@ def rnnt_loss_simple(am, lm, labels, frames_lengths, labels_lengths, average_fra
                                     or prune_range < 2):
         raise ValueError("rnnt_loss_simple: prune_range must be None or an int >= 2, got %r" % (prune_range,))
     costs, ranges = RNNTLossSimple.apply(am, lm, labels, frames_lengths, labels_lengths, blank, prune_range or 0)
-    if average_frames:
-        costs = costs / frames_lengths.to(costs.dtype)
-    if reduction == "sum":
-        costs = costs.sum()
-    elif reduction == "mean":
-        costs = costs.mean()
+    costs = _reduce(costs, frames_lengths, average_frames, reduction)
     return costs if prune_range is None else (costs, ranges)
 
 
@@ -405,6 +400,11 @@ class RNNTLossEager(torch.autograd.Function):
 _tls = threading.local()
 
 
+def _hints():
+    """(max_T, max_U) of the enclosing ``compact_hints``, or (0, 0): none."""
+    return getattr(_tls, "hints", None) or (0, 0)
+
+
 @contextlib.contextmanager
 def compact_hints(max_T, max_U):
     """Inside this context ``rnnt_loss(compact=True)`` trusts the caller's upper bounds of ``frames_lengths`` and
@@ -425,7 +425,7 @@ class RNNTLossCompact(torch.autograd.Function):
     @staticmethod
     def forward(ctx, log_probs, labels, frames_lengths, labels_lengths, blank=0, fastemit_lambda=0.0,
                 enable_grad: bool = True):
-        hints = getattr(_tls, "hints", None) or (0, 0)
+        hints = _hints()
         costs, grads, loc = _C.rnnt_loss_compact(
             xs=log_probs, ys=labels, xn=frames_lengths, yn=labels_lengths, blank=blank,
             fastemit_lambda=fastemit_lambda, required_grad=enable_grad, max_T=hints[0], max_U=hints[1])
@@ -535,7 +535,7 @@ def rnnt_align(log_probs, labels, frames_lengths, labels_lengths, blank=0, compa
     assert isinstance(blank, int)
     assert isinstance(compact, bool)
     if compact:
-        hints = getattr(_tls, "hints", None) or (0, 0)
+        hints = _hints()
         return _C.rnnt_align_compact(log_probs, labels, frames_lengths, labels_lengths, blank, hints[0], hints[1])
     return _C.rnnt_align_dense(log_probs, labels, frames_lengths, labels_lengths, blank)
 

@@ -11,6 +11,7 @@
 // Extra entry points (rnnt_loss_dense, rnnt_gather_forward/backward) serve the fused python-level
 // paths of warp_rnnt_b200/__init__.py.
 #include <algorithm>
+#include <limits>
 #include <mutex>
 #include <string>
 #include <tuple>
@@ -24,9 +25,65 @@
 
 namespace {
 
+// ---- argument checks ------------------------------------------------------------------------------------------
+// Every tensor argument must be on the device of the call's primary tensor (xs, am, grad_cost, grads, pair_grads, f
+// or dx), which must be a CUDA device: the kernels run there, under its device guard.  Messages are the callers',
+// passed through unformatted, so a call that passes its checks builds no string.
+
+enum class Dt { F32, F32orBF16, I32, I64 };
+
+bool has_dtype(const at::Tensor &t, Dt dt) {
+    const at::ScalarType s = t.scalar_type();
+    switch (dt) {
+    case Dt::F32: return s == at::ScalarType::Float;
+    case Dt::F32orBF16: return s == at::ScalarType::Float || s == at::ScalarType::BFloat16;
+    case Dt::I32: return s == at::ScalarType::Int;
+    case Dt::I64: return s == at::ScalarType::Long;
+    }
+    return false;
+}
+
+// on the device of `on`, a CUDA device (`on` may be `t` itself: then t is on any CUDA device)
+bool on_device(const at::Tensor &t, const at::Tensor &on) { return t.device() == on.device() && on.device().is_cuda(); }
+
+// contiguous, of dtype `dt`, on the device of `on`
+bool is_arg(const at::Tensor &t, Dt dt, const at::Tensor &on) {
+    return t.is_contiguous() && has_dtype(t, dt) && on_device(t, on);
+}
+
+constexpr int64_t kAny = std::numeric_limits<int64_t>::min();   // a size that matches any extent
+
+bool has_sizes(const at::Tensor &t, at::IntArrayRef sizes) {
+    if (t.dim() != (int64_t)sizes.size()) return false;
+    for (size_t d = 0; d < sizes.size(); ++d)
+        if (sizes[d] != kAny && t.size(d) != sizes[d]) return false;
+    return true;
+}
+
+// is_arg, and `numel` elements
+void check_arg(const at::Tensor &t, Dt dt, const at::Tensor &on, int64_t numel, const char *msg) {
+    TORCH_CHECK(is_arg(t, dt, on) && t.numel() == numel, msg);
+}
+
+// is_arg, and of shape `sizes` (kAny: any extent)
+void check_arg(const at::Tensor &t, Dt dt, const at::Tensor &on, at::IntArrayRef sizes, const char *msg) {
+    TORCH_CHECK(is_arg(t, dt, on) && has_sizes(t, sizes), msg);
+}
+
+// an optional tensor argument: null when absent, else checked as check_arg does and its data
+template <typename T>
+const T *optional_arg(const c10::optional<at::Tensor> &t, Dt dt, const at::Tensor &on, int64_t numel,
+                      const char *msg) {
+    if (!t.has_value() || !t->defined()) return nullptr;
+    check_arg(*t, dt, on, numel, msg);
+    return t->data_ptr<T>();
+}
+
+void check_blank(int blank, int64_t V) { TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)"); }
+
 void check4(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
             bool allow_bf16 = false) {
-    // order as in the reference (binding.cpp:31-46): contiguity, then dtypes, then device
+    // order as in the reference (binding.cpp:31-46): contiguity, then dtypes, then device; then the device of xs
     TORCH_CHECK(xs.is_contiguous(), "xs must be contiguous");
     TORCH_CHECK(ys.is_contiguous(), "ys must be contiguous");
     TORCH_CHECK(xn.is_contiguous(), "xn must be contiguous");
@@ -40,23 +97,64 @@ void check4(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn, co
     TORCH_CHECK(ys.device().is_cuda(), "ys must be located in the CUDA");
     TORCH_CHECK(xn.device().is_cuda(), "xn must be located in the CUDA");
     TORCH_CHECK(yn.device().is_cuda(), "yn must be located in the CUDA");
+    TORCH_CHECK(ys.device() == xs.device(), "ys must be on the device of xs");
+    TORCH_CHECK(xn.device() == xs.device(), "xn must be on the device of xs");
+    TORCH_CHECK(yn.device() == xs.device(), "yn must be on the device of xs");
 }
 
-void check_dense_shapes(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn) {
+// xs (N, ...) with 4 dimensions, xn and yn (N,)
+void check_batch4(const at::Tensor &xs, const at::Tensor &xn, const at::Tensor &yn) {
     TORCH_CHECK(xs.dim() == 4, "xs must have 4 dimensions");
     TORCH_CHECK(xn.numel() == xs.size(0), "xn shape must be equal (N,)");
     TORCH_CHECK(yn.numel() == xs.size(0), "yn shape must be equal (N,)");
-    TORCH_CHECK(ys.dim() == 2 && xs.size(2) == ys.size(1) + 1, "ys shape (N, U-1) mismatched with xs (N, T, U, V)");
 }
 
-at::Tensor workspace_for(const at::Tensor &like, int64_t cells, int64_t N) {
-    const size_t bytes = rnnt_b200_workspace_bytes(cells, (int)N);
+// The front of a dense (N,T,U,V) call: check4, the shapes, then the device guard of xs, held by the caller.
+struct DenseFront {
+    int64_t N, T, U, V;
+    bool bf16;
+    c10::cuda::CUDAGuard guard;
+};
+
+DenseFront dense_front(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
+                       bool allow_bf16) {
+    check4(xs, ys, xn, yn, allow_bf16);
+    check_batch4(xs, xn, yn);
+    TORCH_CHECK(ys.dim() == 2 && xs.size(2) == ys.size(1) + 1, "ys shape (N, U-1) mismatched with xs (N, T, U, V)");
+    return {xs.size(0), xs.size(1), xs.size(2), xs.size(3), xs.scalar_type() == at::ScalarType::BFloat16,
+            c10::cuda::CUDAGuard(xs.device())};
+}
+
+// The front of a compact (STU,V) call: check4, the shapes and blank, then the device guard of xs, held by the caller.
+struct CompactFront {
+    int64_t N, STU, V;
+    bool bf16;
+    c10::cuda::CUDAGuard guard;
+};
+
+CompactFront compact_front(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
+                           int blank, bool allow_bf16) {
+    check4(xs, ys, xn, yn, allow_bf16);
+    TORCH_CHECK(xs.dim() == 2, "xs must have 2 dimensions");
+    TORCH_CHECK(xn.dim() == 1 && yn.dim() == 1 && xn.size(0) == yn.size(0), "xn and yn shape must be equal (N,)");
+    check_blank(blank, xs.size(1));
+    return {xn.size(0), xs.size(0), xs.size(1), xs.scalar_type() == at::ScalarType::BFloat16,
+            c10::cuda::CUDAGuard(xs.device())};
+}
+
+// ---- outputs, workspaces, launches ----------------------------------------------------------------------------
+
+// an output the caller asked for, or the empty placeholder returned in its place
+at::Tensor output(bool want, at::IntArrayRef sizes, const at::TensorOptions &options) {
+    return want ? at::empty(sizes, options) : at::empty({0}, options);
+}
+
+at::Tensor workspace(const at::Tensor &like, size_t bytes) {
     return at::empty({(int64_t)bytes}, like.options().dtype(at::kByte));
 }
 
 void check_status(int status) {
-    TORCH_CHECK(status == RNNT_STATUS_SUCCESS, "rnnt_loss status " + std::to_string(status) + " (" +
-                                                   rnnt_b200_status_string(status) + ")");
+    TORCH_CHECK(status == RNNT_STATUS_SUCCESS, "rnnt_loss status ", status, " (", rnnt_b200_status_string(status), ")");
 }
 
 void *current_stream(const at::Tensor &t) {
@@ -106,50 +204,38 @@ std::tuple<at::Tensor, at::Tensor> loss_dense_impl(const at::Tensor &xs, const a
                                                    const c10::optional<at::Tensor> &scale, bool want_grads,
                                                    int lse_mode, at::Tensor loss_sum = at::Tensor(),
                                                    bool allow_bf16 = false) {
-    check4(xs, ys, xn, yn, allow_bf16);
-    check_dense_shapes(xs, ys, xn, yn);
-    const c10::cuda::CUDAGuard guard(xs.device());
-    const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), V = xs.size(3);
-    const bool bf16 = xs.scalar_type() == at::ScalarType::BFloat16;
+    const auto [N, T, U, V, bf16, guard] = dense_front(xs, ys, xn, yn, allow_bf16);
     at::Tensor costs = at::empty({N}, xs.options().dtype(at::kFloat));
-    at::Tensor grads = want_grads ? at::empty_like(xs) : at::empty({0}, xs.options());
+    at::Tensor grads = output(want_grads, xs.sizes(), xs.options());
     if (N == 0) return std::make_tuple(costs, grads);
     TORCH_CHECK(!bf16 || (want_grads && blank != -1), "bfloat16 xs: dense (N,T,U,V) layout with gradients only");
-    const float *sc = nullptr;
-    if (scale.has_value() && scale->defined()) {
-        TORCH_CHECK(scale->is_contiguous() && scale->scalar_type() == at::ScalarType::Float &&
-                        scale->device() == xs.device() && scale->numel() == N,
-                    "grad_scale must be a contiguous Float tensor of shape (N,) on the device of xs");
-        sc = scale->data_ptr<float>();
-    }
-    int status;
+    const float *sc = optional_arg<float>(scale, Dt::F32, xs, N,
+                                          "grad_scale must be a contiguous Float tensor of shape (N,) on the device of xs");
     if (blank == -1) {
-        // gathered (N,T,U,2) form, binding.cpp:81-90
-        TORCH_CHECK(V == 2, "xs must have values only for blank and label");
-        at::Tensor ws = workspace_for(xs, N * T * U, N);
-        status = rnnt_b200_loss_pairs(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr<float>(),
-                                      xn.data_ptr<int>(), yn.data_ptr<int>(), costs.data_ptr<float>(),
-                                      want_grads ? grads.data_ptr<float>() : nullptr, (int)N, (int)T, (int)U,
-                                      fastemit_lambda, lse_mode);
-        check_status(status);
-        if (want_grads && sc) grads.mul_(scale->view({-1, 1, 1, 1}));
+        TORCH_CHECK(V == 2, "xs must have values only for blank and label");    // gathered (N,T,U,2) form, binding.cpp:81-90
     } else {
         TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V) (or -1 for the gathered layout)");
-        at::Tensor ws = workspace_for(xs, N * T * U, N);
-        float *ls = loss_sum.defined() ? loss_sum.data_ptr<float>() : nullptr;
-        if (bf16)
-            status = rnnt_b200_loss_dense_bf16(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
+    }
+    at::Tensor ws = workspace(xs, rnnt_b200_workspace_bytes(N * T * U, (int)N));
+    float *ls = loss_sum.defined() ? loss_sum.data_ptr<float>() : nullptr;
+    unsigned int *counter = ls ? next_sync_counter(xs) : nullptr;
+    if (blank == -1) {
+        check_status(rnnt_b200_loss_pairs(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr<float>(),
+                                          xn.data_ptr<int>(), yn.data_ptr<int>(), costs.data_ptr<float>(),
+                                          want_grads ? grads.data_ptr<float>() : nullptr, (int)N, (int)T, (int)U,
+                                          fastemit_lambda, lse_mode));
+        if (want_grads && sc) grads.mul_(scale->view({-1, 1, 1, 1}));
+    } else if (bf16) {
+        check_status(rnnt_b200_loss_dense_bf16(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
                                                ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
-                                               costs.data_ptr<float>(), grads.data_ptr(), sc, ls,
-                                               ls ? next_sync_counter(xs) : nullptr, (int)N, (int)T, (int)U, (int)V,
-                                               blank, fastemit_lambda, lse_mode);
-        else
-        status = rnnt_b200_loss_dense_reduced(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr<float>(),
-                                              ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
-                                              costs.data_ptr<float>(), want_grads ? grads.data_ptr<float>() : nullptr,
-                                              sc, ls, ls ? next_sync_counter(xs) : nullptr, (int)N, (int)T, (int)U,
-                                              (int)V, blank, fastemit_lambda, lse_mode);
-        check_status(status);
+                                               costs.data_ptr<float>(), grads.data_ptr(), sc, ls, counter, (int)N,
+                                               (int)T, (int)U, (int)V, blank, fastemit_lambda, lse_mode));
+    } else {
+        check_status(rnnt_b200_loss_dense_reduced(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(),
+                                                  xs.data_ptr<float>(), ys.data_ptr<int>(), xn.data_ptr<int>(),
+                                                  yn.data_ptr<int>(), costs.data_ptr<float>(),
+                                                  want_grads ? grads.data_ptr<float>() : nullptr, sc, ls, counter,
+                                                  (int)N, (int)T, (int)U, (int)V, blank, fastemit_lambda, lse_mode));
     }
     return std::make_tuple(costs, grads);
 }
@@ -165,21 +251,16 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_loss_compact(const at::Tenso
                                                                  const at::Tensor &xn, const at::Tensor &yn,
                                                                  const int blank, const float fastemit_lambda,
                                                                  const bool required_grad, int hint_T, int hint_U) {
-    check4(xs, ys, xn, yn);
-    TORCH_CHECK(xs.dim() == 2, "xs must have 2 dimensions");
-    TORCH_CHECK(xn.dim() == 1 && yn.dim() == 1 && xn.size(0) == yn.size(0), "xn and yn shape must be equal (N,)");
-    const c10::cuda::CUDAGuard guard(xs.device());
-    const int64_t N = xn.size(0), STU = xs.size(0), V = xs.size(1);
-    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    const auto [N, STU, V, bf16, guard] = compact_front(xs, ys, xn, yn, blank, false);
     void *stream = current_stream(xs);
     at::Tensor costs = at::empty({N}, xs.options());
     at::Tensor loc = at::empty({STU}, xs.options().dtype(at::kLong));
     // like the reference (binding.cpp:196-201): without required_grad the returned "grads" is a
     // placeholder the caller must not use
-    at::Tensor grads = required_grad ? at::empty({STU, 2}, xs.options()) : at::empty({0}, xs.options());
+    at::Tensor grads = output(required_grad, {STU, 2}, xs.options());
     if (N == 0) return std::make_tuple(costs, grads, loc);
     const auto [max_T, max_U] = compact_bounds(stream, xs, ys, xn, yn, hint_T, hint_U, nullptr);
-    at::Tensor ws = workspace_for(xs, STU, N);
+    at::Tensor ws = workspace(xs, rnnt_b200_workspace_bytes(STU, (int)N));
     check_status(rnnt_b200_compact_forward(stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr<float>(),
                                            ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
                                            costs.data_ptr<float>(), required_grad ? grads.data_ptr<float>() : nullptr,
@@ -190,6 +271,8 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_loss_compact(const at::Tenso
 
 at::Tensor rnnt_loss_compact_backward(const at::Tensor &grad_cost, const at::Tensor &grad_xs,
                                       const at::Tensor &cum_lens, const at::Tensor &loc, int64_t V, int blank) {
+    // order as in the reference (binding.cpp:212-221): contiguity, then dtypes, then device; then the device of
+    // grad_cost
     TORCH_CHECK(grad_cost.is_contiguous(), "grad_cost must be contiguous");
     TORCH_CHECK(grad_xs.is_contiguous(), "grad_xs must be contiguous");
     TORCH_CHECK(loc.is_contiguous(), "loc must be contiguous");
@@ -200,6 +283,9 @@ at::Tensor rnnt_loss_compact_backward(const at::Tensor &grad_cost, const at::Ten
     TORCH_CHECK(grad_xs.device().is_cuda(), "grad_xs must be located in the CUDA");
     TORCH_CHECK(cum_lens.device().is_cuda(), "cum_lens must be located in the CUDA");
     TORCH_CHECK(loc.device().is_cuda(), "loc must be located in the CUDA");
+    TORCH_CHECK(grad_xs.device() == grad_cost.device(), "grad_xs must be on the device of grad_cost");
+    TORCH_CHECK(cum_lens.device() == grad_cost.device(), "cum_lens must be on the device of grad_cost");
+    TORCH_CHECK(loc.device() == grad_cost.device(), "loc must be on the device of grad_cost");
     TORCH_CHECK(grad_cost.dim() == 1, "grad_cost must have 1 dimensions");
     TORCH_CHECK(grad_xs.dim() == 2, "grad must have 2 dimensions");
     TORCH_CHECK(grad_xs.size(0) == loc.size(0), "grad and loc must be equal in dim=0");
@@ -207,7 +293,7 @@ at::Tensor rnnt_loss_compact_backward(const at::Tensor &grad_cost, const at::Ten
                     cum_lens.numel() == grad_cost.size(0),
                 "cum_lens must be a contiguous Int tensor of shape (N,)");
     TORCH_CHECK(grad_xs.size(1) == 2, "grad must have shape (STU, 2)");
-    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    check_blank(blank, V);
     const c10::cuda::CUDAGuard guard(grad_cost.device());
     const int64_t N = grad_cost.size(0), STU = grad_xs.size(0);
     at::Tensor out = at::empty({STU, V}, grad_cost.options());
@@ -244,40 +330,29 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_loss_fused(const at::Tensor 
 
 // in place: grads[n] *= grad_out[n] / applied[n] where they differ (grad_out with one element: one scalar for all)
 void rnnt_rescale_(at::Tensor grads, const at::Tensor &grad_out, const c10::optional<at::Tensor> &applied) {
-    const bool bf16 = grads.scalar_type() == at::ScalarType::BFloat16;
-    TORCH_CHECK(grads.is_contiguous() && (grads.scalar_type() == at::ScalarType::Float || bf16) &&
-                    grads.device().is_cuda() && grads.dim() >= 1,
+    TORCH_CHECK(is_arg(grads, Dt::F32orBF16, grads) && grads.dim() >= 1,
                 "grads must be a contiguous CUDA Float (or BFloat16) tensor");
     const int64_t N = grads.size(0);
-    TORCH_CHECK(grad_out.is_contiguous() && grad_out.scalar_type() == at::ScalarType::Float &&
-                    grad_out.device() == grads.device() && (grad_out.numel() == N || grad_out.numel() == 1),
+    TORCH_CHECK(is_arg(grad_out, Dt::F32, grads) && (grad_out.numel() == N || grad_out.numel() == 1),
                 "grad_out must be a contiguous Float tensor with N elements (or one) on the device of grads");
-    const float *ap = nullptr;
-    if (applied.has_value() && applied->defined()) {
-        TORCH_CHECK(applied->is_contiguous() && applied->scalar_type() == at::ScalarType::Float &&
-                        applied->device() == grads.device() && applied->numel() == N,
-                    "applied must be a contiguous Float tensor of shape (N,) on the device of grads");
-        ap = applied->data_ptr<float>();
-    }
+    const float *ap = optional_arg<float>(applied, Dt::F32, grads, N,
+                                          "applied must be a contiguous Float tensor of shape (N,) on the device of grads");
     if (N == 0) return;
     const c10::cuda::CUDAGuard guard(grads.device());
     check_status(rnnt_b200_rescale(current_stream(grads), grads.data_ptr(), grad_out.data_ptr<float>(),
                                    (grad_out.numel() == 1 && N != 1) ? 0 : 1, ap, (int)N, grads.numel() / N,
-                                   bf16 ? 2 : 4));
+                                   grads.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
 }
 
 std::tuple<at::Tensor, at::Tensor> rnnt_gather_forward(const at::Tensor &xs, const at::Tensor &ys,
                                                        const at::Tensor &xn, const at::Tensor &yn, int blank,
                                                        float fastemit_lambda, bool want_grads, int lse_mode) {
-    check4(xs, ys, xn, yn);
-    check_dense_shapes(xs, ys, xn, yn);
-    const c10::cuda::CUDAGuard guard(xs.device());
-    const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), V = xs.size(3);
-    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    const auto [N, T, U, V, bf16, guard] = dense_front(xs, ys, xn, yn, false);
+    check_blank(blank, V);
     at::Tensor costs = at::empty({N}, xs.options());
-    at::Tensor pg = want_grads ? at::empty({N, T, U, 2}, xs.options()) : at::empty({0}, xs.options());
+    at::Tensor pg = output(want_grads, {N, T, U, 2}, xs.options());
     if (N == 0) return std::make_tuple(costs, pg);
-    at::Tensor ws = workspace_for(xs, N * T * U, N);
+    at::Tensor ws = workspace(xs, rnnt_b200_workspace_bytes(N * T * U, (int)N));
     check_status(rnnt_b200_gather_forward(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(),
                                           xs.data_ptr<float>(), ys.data_ptr<int>(), xn.data_ptr<int>(),
                                           yn.data_ptr<int>(), costs.data_ptr<float>(),
@@ -292,18 +367,14 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_logits_forward(const at::Ten
                                                                    const at::Tensor &xn, const at::Tensor &yn,
                                                                    int blank, float fastemit_lambda, bool want_grads,
                                                                    int lse_mode) {
-    check4(xs, ys, xn, yn, true);
-    check_dense_shapes(xs, ys, xn, yn);
-    const c10::cuda::CUDAGuard guard(xs.device());
-    const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), V = xs.size(3);
-    const bool bf16 = xs.scalar_type() == at::ScalarType::BFloat16;
-    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    const auto [N, T, U, V, bf16, guard] = dense_front(xs, ys, xn, yn, true);
+    check_blank(blank, V);
     const auto f32 = xs.options().dtype(at::kFloat);
     at::Tensor costs = at::empty({N}, f32);
     at::Tensor lse = at::empty({N, T, U}, f32);
-    at::Tensor pg = want_grads ? at::empty({N, T, U, 2}, f32) : at::empty({0}, f32);
+    at::Tensor pg = output(want_grads, {N, T, U, 2}, f32);
     if (N == 0) return std::make_tuple(costs, lse, pg);
-    at::Tensor ws = workspace_for(xs, N * T * U, N);
+    at::Tensor ws = workspace(xs, rnnt_b200_workspace_bytes(N * T * U, (int)N));
     float *pgp = want_grads ? pg.data_ptr<float>() : nullptr;
     if (bf16)
         check_status(rnnt_b200_logits_forward_bf16(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
@@ -321,27 +392,18 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_logits_forward(const at::Ten
 // d loss / d logits, of the dtype of xs (float32 or bfloat16)
 at::Tensor rnnt_logits_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &pair_grads,
                                 const at::Tensor &ys, const at::Tensor &grad_out, int blank) {
-    const bool bf16 = xs.scalar_type() == at::ScalarType::BFloat16;
-    TORCH_CHECK(xs.is_contiguous() && (xs.scalar_type() == at::ScalarType::Float || bf16) && xs.device().is_cuda() &&
-                    xs.dim() == 4,
-                "xs must be a contiguous CUDA Float tensor of shape (N, T, U, V)");
+    check_arg(xs, Dt::F32orBF16, xs, {kAny, kAny, kAny, kAny},
+              "xs must be a contiguous CUDA Float tensor of shape (N, T, U, V)");
     const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), V = xs.size(3);
-    TORCH_CHECK(lse.is_contiguous() && lse.scalar_type() == at::ScalarType::Float && lse.device() == xs.device() &&
-                    lse.numel() == N * T * U,
-                "lse must be a contiguous Float tensor of shape (N, T, U) on the device of xs");
-    TORCH_CHECK(pair_grads.is_contiguous() && pair_grads.scalar_type() == at::ScalarType::Float &&
-                    pair_grads.device() == xs.device() && pair_grads.numel() == N * T * U * 2,
-                "pair_grads must be a contiguous Float tensor of shape (N, T, U, 2) on the device of xs");
-    TORCH_CHECK(ys.is_contiguous() && ys.scalar_type() == at::ScalarType::Int && ys.device() == xs.device() &&
-                    ys.dim() == 2 && ys.size(0) == N && ys.size(1) + 1 == U,
-                "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
-    TORCH_CHECK(grad_out.is_contiguous() && grad_out.scalar_type() == at::ScalarType::Float &&
-                    grad_out.device() == xs.device() && grad_out.numel() == N,
-                "grad_out must be a contiguous Float tensor of shape (N,)");
-    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    check_arg(lse, Dt::F32, xs, N * T * U, "lse must be a contiguous Float tensor of shape (N, T, U) on the device of xs");
+    check_arg(pair_grads, Dt::F32, xs, N * T * U * 2,
+              "pair_grads must be a contiguous Float tensor of shape (N, T, U, 2) on the device of xs");
+    check_arg(ys, Dt::I32, xs, {N, U - 1}, "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
+    check_arg(grad_out, Dt::F32, xs, N, "grad_out must be a contiguous Float tensor of shape (N,)");
+    check_blank(blank, V);
     const c10::cuda::CUDAGuard guard(xs.device());
     at::Tensor out = at::empty_like(xs);
-    if (bf16)
+    if (xs.scalar_type() == at::ScalarType::BFloat16)
         check_status(rnnt_b200_logits_backward_bf16(current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(),
                                                     pair_grads.data_ptr<float>(), ys.data_ptr<int>(),
                                                     grad_out.data_ptr<float>(), out.data_ptr(), (int)N, (int)T, (int)U,
@@ -359,22 +421,16 @@ at::Tensor rnnt_logits_backward(const at::Tensor &xs, const at::Tensor &lse, con
 std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor>
 rnnt_logits_compact_forward(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
                             int blank, float fastemit_lambda, bool want_grads, int lse_mode, int max_T, int max_U) {
-    check4(xs, ys, xn, yn, true);
-    TORCH_CHECK(xs.dim() == 2, "xs must have 2 dimensions");
-    TORCH_CHECK(xn.dim() == 1 && yn.dim() == 1 && xn.size(0) == yn.size(0), "xn and yn shape must be equal (N,)");
-    const c10::cuda::CUDAGuard guard(xs.device());
-    const int64_t N = xn.size(0), STU = xs.size(0), V = xs.size(1);
-    const bool bf16 = xs.scalar_type() == at::ScalarType::BFloat16;
-    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    const auto [N, STU, V, bf16, guard] = compact_front(xs, ys, xn, yn, blank, true);
     void *stream = current_stream(xs);
     const auto f32 = xs.options().dtype(at::kFloat);
     at::Tensor costs = at::empty({N}, f32);
     at::Tensor lse = at::empty({STU}, f32);
-    at::Tensor pg = want_grads ? at::empty({STU, 2}, f32) : at::empty({0}, f32);
+    at::Tensor pg = output(want_grads, {STU, 2}, f32);
     at::Tensor prefix = at::empty({2 * N}, xs.options().dtype(at::kLong));
     if (N == 0) return std::make_tuple(costs, lse, pg, prefix);
     std::tie(max_T, max_U) = compact_bounds(stream, xs, ys, xn, yn, max_T, max_U, prefix.data_ptr<int64_t>());
-    at::Tensor ws = workspace_for(xs, STU, N);
+    at::Tensor ws = workspace(xs, rnnt_b200_workspace_bytes(STU, (int)N));
     float *pgp = want_grads ? pg.data_ptr<float>() : nullptr;
     if (bf16)
         check_status(rnnt_b200_logits_compact_forward_bf16(
@@ -393,34 +449,22 @@ rnnt_logits_compact_forward(const at::Tensor &xs, const at::Tensor &ys, const at
 at::Tensor rnnt_logits_compact_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &pair_grads,
                                         const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
                                         const at::Tensor &prefix, const at::Tensor &grad_out, int blank) {
-    const bool bf16 = xs.scalar_type() == at::ScalarType::BFloat16;
-    TORCH_CHECK(xs.is_contiguous() && (xs.scalar_type() == at::ScalarType::Float || bf16) && xs.device().is_cuda() &&
-                    xs.dim() == 2,
-                "xs must be a contiguous CUDA Float tensor of shape (STU, V)");
+    check_arg(xs, Dt::F32orBF16, xs, {kAny, kAny}, "xs must be a contiguous CUDA Float tensor of shape (STU, V)");
     const int64_t STU = xs.size(0), V = xs.size(1), N = xn.numel();
-    TORCH_CHECK(lse.is_contiguous() && lse.scalar_type() == at::ScalarType::Float && lse.device() == xs.device() &&
-                    lse.numel() == STU,
-                "lse must be a contiguous Float tensor of shape (STU,) on the device of xs");
-    TORCH_CHECK(pair_grads.is_contiguous() && pair_grads.scalar_type() == at::ScalarType::Float &&
-                    pair_grads.device() == xs.device() && pair_grads.numel() == STU * 2,
-                "pair_grads must be a contiguous Float tensor of shape (STU, 2) on the device of xs");
-    TORCH_CHECK(ys.is_contiguous() && ys.scalar_type() == at::ScalarType::Int && ys.device() == xs.device(),
-                "ys must be a contiguous Int tensor on the device of xs");
-    TORCH_CHECK(xn.is_contiguous() && yn.is_contiguous() && xn.scalar_type() == at::ScalarType::Int &&
-                    yn.scalar_type() == at::ScalarType::Int && xn.device() == xs.device() &&
-                    yn.device() == xs.device() && yn.numel() == N,
-                "xn and yn must be contiguous Int tensors of shape (N,) on the device of xs");
-    TORCH_CHECK(prefix.is_contiguous() && prefix.scalar_type() == at::ScalarType::Long && prefix.device() == xs.device() &&
-                    prefix.numel() == 2 * N,
-                "prefix must be a contiguous Long tensor of shape (2N,) on the device of xs");
-    TORCH_CHECK(grad_out.is_contiguous() && grad_out.scalar_type() == at::ScalarType::Float &&
-                    grad_out.device() == xs.device() && grad_out.numel() == N,
-                "grad_out must be a contiguous Float tensor of shape (N,)");
-    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    check_arg(lse, Dt::F32, xs, STU, "lse must be a contiguous Float tensor of shape (STU,) on the device of xs");
+    check_arg(pair_grads, Dt::F32, xs, STU * 2,
+              "pair_grads must be a contiguous Float tensor of shape (STU, 2) on the device of xs");
+    TORCH_CHECK(is_arg(ys, Dt::I32, xs), "ys must be a contiguous Int tensor on the device of xs");
+    const char *lengths = "xn and yn must be contiguous Int tensors of shape (N,) on the device of xs";
+    check_arg(xn, Dt::I32, xs, N, lengths);
+    check_arg(yn, Dt::I32, xs, N, lengths);
+    check_arg(prefix, Dt::I64, xs, 2 * N, "prefix must be a contiguous Long tensor of shape (2N,) on the device of xs");
+    check_arg(grad_out, Dt::F32, xs, N, "grad_out must be a contiguous Float tensor of shape (N,)");
+    check_blank(blank, V);
     const c10::cuda::CUDAGuard guard(xs.device());
     at::Tensor out = at::empty_like(xs);
     if (N == 0 || STU == 0) return out;                 // empty tensors: nothing to write (and no data pointers)
-    if (bf16)
+    if (xs.scalar_type() == at::ScalarType::BFloat16)
         check_status(rnnt_b200_logits_compact_backward_bf16(
             current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(), pair_grads.data_ptr<float>(), ys.data_ptr<int>(),
             xn.data_ptr<int>(), yn.data_ptr<int>(), prefix.data_ptr<int64_t>(), grad_out.data_ptr<float>(),
@@ -441,28 +485,24 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_logits_pruned_forward(const 
                                                                           float fastemit_lambda, bool want_grads,
                                                                           int lse_mode) {
     check4(xs, ys, xn, yn, true);
-    TORCH_CHECK(xs.dim() == 4, "xs must have 4 dimensions");
-    TORCH_CHECK(xn.numel() == xs.size(0), "xn shape must be equal (N,)");
-    TORCH_CHECK(yn.numel() == xs.size(0), "yn shape must be equal (N,)");
+    check_batch4(xs, xn, yn);
     TORCH_CHECK(ys.dim() == 2 && ys.size(0) == xs.size(0), "ys shape must be (N, U-1)");
     const int64_t N = xs.size(0), T = xs.size(1), S = xs.size(2), V = xs.size(3), U = ys.size(1) + 1;
-    TORCH_CHECK(ranges.is_contiguous() && ranges.scalar_type() == at::ScalarType::Int && ranges.device() == xs.device() &&
-                    ranges.dim() == 2 && ranges.size(0) == N && ranges.size(1) == T,
-                "ranges must be a contiguous Int tensor of shape (N, T) on the device of xs");
-    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    check_arg(ranges, Dt::I32, xs, {N, T}, "ranges must be a contiguous Int tensor of shape (N, T) on the device of xs");
+    check_blank(blank, V);
     const c10::cuda::CUDAGuard guard(xs.device());
-    const bool bf16 = xs.scalar_type() == at::ScalarType::BFloat16;
     const auto f32 = xs.options().dtype(at::kFloat);
     at::Tensor costs = at::empty({N}, f32);
     at::Tensor lse = at::empty({N, T, S}, f32);
-    at::Tensor pg = want_grads ? at::empty({N, T, U, 2}, f32) : at::empty({0}, f32);
+    at::Tensor pg = output(want_grads, {N, T, U, 2}, f32);
     if (N == 0) return std::make_tuple(costs, lse, pg);
-    at::Tensor ws = workspace_for(xs, N * T * U, N);
+    at::Tensor ws = workspace(xs, rnnt_b200_workspace_bytes(N * T * U, (int)N));
     check_status(rnnt_b200_logits_pruned_forward(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
                                                  ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
                                                  ranges.data_ptr<int>(), costs.data_ptr<float>(), lse.data_ptr<float>(),
                                                  want_grads ? pg.data_ptr<float>() : nullptr, (int)N, (int)T, (int)S,
-                                                 (int)U, (int)V, blank, fastemit_lambda, lse_mode, bf16 ? 2 : 4));
+                                                 (int)U, (int)V, blank, fastemit_lambda, lse_mode,
+                                                 xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
     return std::make_tuple(costs, lse, pg);
 }
 
@@ -470,54 +510,42 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_logits_pruned_forward(const 
 at::Tensor rnnt_logits_pruned_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &pair_grads,
                                        const at::Tensor &ys, const at::Tensor &ranges, const at::Tensor &grad_out,
                                        int blank) {
-    const bool bf16 = xs.scalar_type() == at::ScalarType::BFloat16;
-    TORCH_CHECK(xs.is_contiguous() && (xs.scalar_type() == at::ScalarType::Float || bf16) && xs.device().is_cuda() &&
-                    xs.dim() == 4,
-                "xs must be a contiguous CUDA Float tensor of shape (N, T, S, V)");
+    check_arg(xs, Dt::F32orBF16, xs, {kAny, kAny, kAny, kAny},
+              "xs must be a contiguous CUDA Float tensor of shape (N, T, S, V)");
     const int64_t N = xs.size(0), T = xs.size(1), S = xs.size(2), V = xs.size(3);
-    TORCH_CHECK(ys.is_contiguous() && ys.scalar_type() == at::ScalarType::Int && ys.device() == xs.device() &&
-                    ys.dim() == 2 && ys.size(0) == N,
-                "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
+    check_arg(ys, Dt::I32, xs, {N, kAny}, "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
     const int64_t U = ys.size(1) + 1;
-    TORCH_CHECK(lse.is_contiguous() && lse.scalar_type() == at::ScalarType::Float && lse.device() == xs.device() &&
-                    lse.numel() == N * T * S,
-                "lse must be a contiguous Float tensor of shape (N, T, S) on the device of xs");
-    TORCH_CHECK(pair_grads.is_contiguous() && pair_grads.scalar_type() == at::ScalarType::Float &&
-                    pair_grads.device() == xs.device() && pair_grads.numel() == N * T * U * 2,
-                "pair_grads must be a contiguous Float tensor of shape (N, T, U, 2) on the device of xs");
-    TORCH_CHECK(ranges.is_contiguous() && ranges.scalar_type() == at::ScalarType::Int && ranges.device() == xs.device() &&
-                    ranges.dim() == 2 && ranges.size(0) == N && ranges.size(1) == T,
-                "ranges must be a contiguous Int tensor of shape (N, T) on the device of xs");
-    TORCH_CHECK(grad_out.is_contiguous() && grad_out.scalar_type() == at::ScalarType::Float &&
-                    grad_out.device() == xs.device() && grad_out.numel() == N,
-                "grad_out must be a contiguous Float tensor of shape (N,)");
-    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    check_arg(lse, Dt::F32, xs, N * T * S, "lse must be a contiguous Float tensor of shape (N, T, S) on the device of xs");
+    check_arg(pair_grads, Dt::F32, xs, N * T * U * 2,
+              "pair_grads must be a contiguous Float tensor of shape (N, T, U, 2) on the device of xs");
+    check_arg(ranges, Dt::I32, xs, {N, T}, "ranges must be a contiguous Int tensor of shape (N, T) on the device of xs");
+    check_arg(grad_out, Dt::F32, xs, N, "grad_out must be a contiguous Float tensor of shape (N,)");
+    check_blank(blank, V);
     const c10::cuda::CUDAGuard guard(xs.device());
     at::Tensor out = at::empty_like(xs);
     if (N == 0) return out;
     check_status(rnnt_b200_logits_pruned_backward(current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(),
                                                   pair_grads.data_ptr<float>(), ys.data_ptr<int>(),
                                                   ranges.data_ptr<int>(), grad_out.data_ptr<float>(), out.data_ptr(),
-                                                  (int)N, (int)T, (int)S, (int)U, (int)V, blank, bf16 ? 2 : 4));
+                                                  (int)N, (int)T, (int)S, (int)U, (int)V, blank,
+                                                  xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
     return out;
 }
 
+// am (N,T,V) and lm (N,U,V): dtypes, then contiguity and device, then shapes; then ys, xn and yn
 void check_simple_inputs(const at::Tensor &am, const at::Tensor &lm, const at::Tensor &ys, const at::Tensor &xn,
                          const at::Tensor &yn) {
-    TORCH_CHECK(am.scalar_type() == at::ScalarType::Float && lm.scalar_type() == at::ScalarType::Float,
+    TORCH_CHECK(has_dtype(am, Dt::F32) && has_dtype(lm, Dt::F32),
                 "am and lm must be float32 tensors (the simple loss does not take bfloat16)");
-    TORCH_CHECK(am.is_contiguous() && lm.is_contiguous() && am.device().is_cuda() && lm.device() == am.device(),
+    TORCH_CHECK(am.is_contiguous() && lm.is_contiguous() && on_device(am, am) && on_device(lm, am),
                 "am and lm must be contiguous CUDA tensors on one device");
     TORCH_CHECK(am.dim() == 3 && lm.dim() == 3 && lm.size(0) == am.size(0) && lm.size(2) == am.size(2),
                 "am must be (N, T, V) and lm (N, U, V)");
     const int64_t N = am.size(0);
-    TORCH_CHECK(ys.is_contiguous() && ys.scalar_type() == at::ScalarType::Int && ys.device() == am.device() &&
-                    ys.dim() == 2 && ys.size(0) == N && ys.size(1) + 1 == lm.size(1),
-                "ys must be a contiguous Int tensor of shape (N, U-1) on the device of am");
-    TORCH_CHECK(xn.is_contiguous() && yn.is_contiguous() && xn.scalar_type() == at::ScalarType::Int &&
-                    yn.scalar_type() == at::ScalarType::Int && xn.device() == am.device() &&
-                    yn.device() == am.device() && xn.numel() == N && yn.numel() == N,
-                "xn and yn must be contiguous Int tensors of shape (N,) on the device of am");
+    check_arg(ys, Dt::I32, am, {N, lm.size(1) - 1}, "ys must be a contiguous Int tensor of shape (N, U-1) on the device of am");
+    const char *lengths = "xn and yn must be contiguous Int tensors of shape (N,) on the device of am";
+    check_arg(xn, Dt::I32, am, N, lengths);
+    check_arg(yn, Dt::I32, am, N, lengths);
 }
 
 // simple loss from am (N,T,V) and lm (N,U,V), float32: (costs (N), saved (N*T*U + N*T + N*U), pair_grads (N,T,U,2) or
@@ -528,22 +556,21 @@ rnnt_simple_forward(const at::Tensor &am, const at::Tensor &lm, const at::Tensor
                     const at::Tensor &yn, int blank, bool want_grads, int prune_range, int lse_mode) {
     check_simple_inputs(am, lm, ys, xn, yn);
     const int64_t N = am.size(0), T = am.size(1), U = lm.size(1), V = am.size(2);
-    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    check_blank(blank, V);
     TORCH_CHECK(prune_range == 0 || prune_range >= 2, "prune_range must be an int >= 2");
     const c10::cuda::CUDAGuard guard(am.device());
     const auto f32 = am.options().dtype(at::kFloat);
     const bool pairs = want_grads || prune_range > 0;
     at::Tensor costs = at::empty({N}, f32);
     at::Tensor saved = at::empty({N * T * U + N * T + N * U}, f32);
-    at::Tensor pg = pairs ? at::empty({N, T, U, 2}, f32) : at::empty({0}, f32);
+    at::Tensor pg = output(pairs, {N, T, U, 2}, f32);
     at::Tensor ranges = at::empty({prune_range > 0 ? N : 0, prune_range > 0 ? T : 0}, am.options().dtype(at::kInt));
     if (N == 0) return std::make_tuple(costs, saved, pg, ranges);
     void *stream = current_stream(am);
-    const size_t bytes = rnnt_b200_simple_workspace_bytes((int)N, (int)T, (int)U);
-    at::Tensor ws = at::empty({(int64_t)bytes}, am.options().dtype(at::kByte));
-    check_status(rnnt_b200_simple_forward(stream, ws.data_ptr(), bytes, am.data_ptr<float>(), lm.data_ptr<float>(),
-                                          ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
-                                          costs.data_ptr<float>(), saved.data_ptr<float>(),
+    at::Tensor ws = workspace(am, rnnt_b200_simple_workspace_bytes((int)N, (int)T, (int)U));
+    check_status(rnnt_b200_simple_forward(stream, ws.data_ptr(), (size_t)ws.numel(), am.data_ptr<float>(),
+                                          lm.data_ptr<float>(), ys.data_ptr<int>(), xn.data_ptr<int>(),
+                                          yn.data_ptr<int>(), costs.data_ptr<float>(), saved.data_ptr<float>(),
                                           pairs ? pg.data_ptr<float>() : nullptr, (int)N, (int)T, (int)U, (int)V, blank,
                                           lse_mode));
     if (prune_range > 0)
@@ -559,16 +586,12 @@ std::tuple<at::Tensor, at::Tensor> rnnt_simple_backward(const at::Tensor &am, co
                                                         const at::Tensor &grad_out, int blank) {
     check_simple_inputs(am, lm, ys, xn, yn);
     const int64_t N = am.size(0), T = am.size(1), U = lm.size(1), V = am.size(2);
-    TORCH_CHECK(saved.is_contiguous() && saved.scalar_type() == at::ScalarType::Float && saved.device() == am.device() &&
-                    saved.numel() == N * T * U + N * T + N * U,
-                "saved must be the simple forward's contiguous Float tensor on the device of am");
-    TORCH_CHECK(pair_grads.is_contiguous() && pair_grads.scalar_type() == at::ScalarType::Float &&
-                    pair_grads.device() == am.device() && pair_grads.numel() == N * T * U * 2,
-                "pair_grads must be a contiguous Float tensor of shape (N, T, U, 2) on the device of am");
-    TORCH_CHECK(grad_out.is_contiguous() && grad_out.scalar_type() == at::ScalarType::Float &&
-                    grad_out.device() == am.device() && grad_out.numel() == N,
-                "grad_out must be a contiguous Float tensor of shape (N,)");
-    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
+    check_arg(saved, Dt::F32, am, N * T * U + N * T + N * U,
+              "saved must be the simple forward's contiguous Float tensor on the device of am");
+    check_arg(pair_grads, Dt::F32, am, N * T * U * 2,
+              "pair_grads must be a contiguous Float tensor of shape (N, T, U, 2) on the device of am");
+    check_arg(grad_out, Dt::F32, am, N, "grad_out must be a contiguous Float tensor of shape (N,)");
+    check_blank(blank, V);
     const c10::cuda::CUDAGuard guard(am.device());
     at::Tensor dam = at::empty_like(am), dlm = at::empty_like(lm);
     if (N == 0) return std::make_tuple(dam, dlm);
@@ -582,14 +605,12 @@ std::tuple<at::Tensor, at::Tensor> rnnt_simple_backward(const at::Tensor &am, co
 
 // prune ranges (N,T) int32 from pair gradients (N,T,U,2) of a loss call
 at::Tensor rnnt_prune_ranges(const at::Tensor &pair_grads, const at::Tensor &xn, const at::Tensor &yn, int S) {
-    TORCH_CHECK(pair_grads.is_contiguous() && pair_grads.scalar_type() == at::ScalarType::Float &&
-                    pair_grads.device().is_cuda() && pair_grads.dim() == 4 && pair_grads.size(3) == 2,
-                "pair_grads must be a contiguous CUDA Float tensor of shape (N, T, U, 2)");
+    check_arg(pair_grads, Dt::F32, pair_grads, {kAny, kAny, kAny, 2},
+              "pair_grads must be a contiguous CUDA Float tensor of shape (N, T, U, 2)");
     const int64_t N = pair_grads.size(0), T = pair_grads.size(1), U = pair_grads.size(2);
-    TORCH_CHECK(xn.is_contiguous() && yn.is_contiguous() && xn.scalar_type() == at::ScalarType::Int &&
-                    yn.scalar_type() == at::ScalarType::Int && xn.device() == pair_grads.device() &&
-                    yn.device() == pair_grads.device() && xn.numel() == N && yn.numel() == N,
-                "xn and yn must be contiguous Int tensors of shape (N,) on the device of pair_grads");
+    const char *lengths = "xn and yn must be contiguous Int tensors of shape (N,) on the device of pair_grads";
+    check_arg(xn, Dt::I32, pair_grads, N, lengths);
+    check_arg(yn, Dt::I32, pair_grads, N, lengths);
     TORCH_CHECK(S >= 2, "prune_range must be an int >= 2");
     const c10::cuda::CUDAGuard guard(pair_grads.device());
     at::Tensor ranges = at::empty({N, T}, pair_grads.options().dtype(at::kInt));
@@ -603,12 +624,11 @@ at::Tensor rnnt_prune_ranges(const at::Tensor &pair_grads, const at::Tensor &xn,
 // (one 16-byte copy); stu >= 0: trusted, no host sync.
 std::tuple<at::Tensor, at::Tensor> rnnt_joint_pack(const at::Tensor &f, const at::Tensor &g, const at::Tensor &lf,
                                                    const at::Tensor &lg, int64_t stu) {
+    // contiguity, then dtypes, then device, each for all four
     TORCH_CHECK(f.is_contiguous() && g.is_contiguous() && lf.is_contiguous() && lg.is_contiguous(), "inputs must be contiguous");
-    TORCH_CHECK(f.scalar_type() == at::ScalarType::Float && g.scalar_type() == at::ScalarType::Float,
-                "f and g must be Float tensors");
-    TORCH_CHECK(lf.scalar_type() == at::ScalarType::Int && lg.scalar_type() == at::ScalarType::Int,
-                "lf and lg must be Int tensors");
-    TORCH_CHECK(f.device().is_cuda() && g.device() == f.device() && lf.device() == f.device() && lg.device() == f.device(),
+    TORCH_CHECK(has_dtype(f, Dt::F32) && has_dtype(g, Dt::F32), "f and g must be Float tensors");
+    TORCH_CHECK(has_dtype(lf, Dt::I32) && has_dtype(lg, Dt::I32), "lf and lg must be Int tensors");
+    TORCH_CHECK(on_device(f, f) && on_device(g, f) && on_device(lf, f) && on_device(lg, f),
                 "f, g, lf, lg must be on the same CUDA device");
     TORCH_CHECK(f.dim() == 3 && g.dim() == 3 && f.size(0) == g.size(0) && f.size(2) == g.size(2),
                 "f must be (N, T, H) and g (N, U+1, H)");
@@ -638,14 +658,13 @@ std::tuple<at::Tensor, at::Tensor> rnnt_joint_pack(const at::Tensor &f, const at
 std::tuple<at::Tensor, at::Tensor> rnnt_joint_pack_backward(const at::Tensor &dx, const at::Tensor &lf,
                                                             const at::Tensor &lg, const at::Tensor &mem_pref,
                                                             int64_t T, int64_t U1) {
-    TORCH_CHECK(dx.is_contiguous() && dx.scalar_type() == at::ScalarType::Float && dx.device().is_cuda() && dx.dim() == 2,
-                "dx must be a contiguous CUDA Float tensor of shape (STU, H)");
-    TORCH_CHECK(mem_pref.is_contiguous() && mem_pref.scalar_type() == at::ScalarType::Long && mem_pref.device() == dx.device(),
-                "mem_pref must be a contiguous Long tensor on the device of dx");
+    check_arg(dx, Dt::F32, dx, {kAny, kAny}, "dx must be a contiguous CUDA Float tensor of shape (STU, H)");
+    TORCH_CHECK(is_arg(mem_pref, Dt::I64, dx), "mem_pref must be a contiguous Long tensor on the device of dx");
     const int64_t N = mem_pref.numel(), H = dx.size(1);
     TORCH_CHECK(lf.numel() == N && lg.numel() == N && lf.is_contiguous() && lg.is_contiguous() &&
-                    lf.scalar_type() == at::ScalarType::Int && lg.scalar_type() == at::ScalarType::Int,
+                    has_dtype(lf, Dt::I32) && has_dtype(lg, Dt::I32),
                 "lf and lg must be contiguous Int tensors with N elements");
+    TORCH_CHECK(on_device(lf, dx) && on_device(lg, dx), "lf and lg must be on the device of dx");
     const c10::cuda::CUDAGuard guard(dx.device());
     at::Tensor df = at::empty({N, T, H}, dx.options()), dg = at::empty({N, U1, H}, dx.options());
     check_status(rnnt_b200_joint_pack_backward(current_stream(dx), dx.data_ptr<float>(), lf.data_ptr<int>(),
@@ -656,24 +675,15 @@ std::tuple<at::Tensor, at::Tensor> rnnt_joint_pack_backward(const at::Tensor &dx
 
 at::Tensor rnnt_gather_backward(const at::Tensor &pair_grads, const at::Tensor &ys, const at::Tensor &grad_out,
                                 int64_t V, int blank, bool accumulate, const c10::optional<at::Tensor> &yn) {
-    TORCH_CHECK(pair_grads.is_contiguous() && pair_grads.scalar_type() == at::ScalarType::Float &&
-                    pair_grads.device().is_cuda() && pair_grads.dim() == 4 && pair_grads.size(3) == 2,
-                "pair_grads must be a contiguous CUDA Float tensor of shape (N, T, U, 2)");
-    TORCH_CHECK(ys.is_contiguous() && ys.scalar_type() == at::ScalarType::Int && ys.device() == pair_grads.device(),
-                "ys must be a contiguous Int tensor on the device of pair_grads");
-    TORCH_CHECK(grad_out.is_contiguous() && grad_out.scalar_type() == at::ScalarType::Float &&
-                    grad_out.device() == pair_grads.device() && grad_out.numel() == pair_grads.size(0),
-                "grad_out must be a contiguous Float tensor of shape (N,)");
+    check_arg(pair_grads, Dt::F32, pair_grads, {kAny, kAny, kAny, 2},
+              "pair_grads must be a contiguous CUDA Float tensor of shape (N, T, U, 2)");
+    TORCH_CHECK(is_arg(ys, Dt::I32, pair_grads), "ys must be a contiguous Int tensor on the device of pair_grads");
     const int64_t N = pair_grads.size(0), T = pair_grads.size(1), U = pair_grads.size(2);
-    TORCH_CHECK(ys.dim() == 2 && ys.size(0) == N && ys.size(1) + 1 == U, "ys shape (N, U-1) mismatched");
-    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
-    const int *ynp = nullptr;
-    if (yn.has_value() && yn->defined()) {
-        TORCH_CHECK(yn->is_contiguous() && yn->scalar_type() == at::ScalarType::Int && yn->device() == pair_grads.device() &&
-                        yn->numel() == N,
-                    "yn must be a contiguous Int tensor of shape (N,) on the device of pair_grads");
-        ynp = yn->data_ptr<int>();
-    }
+    check_arg(grad_out, Dt::F32, pair_grads, N, "grad_out must be a contiguous Float tensor of shape (N,)");
+    TORCH_CHECK(has_sizes(ys, {N, U - 1}), "ys shape (N, U-1) mismatched");
+    check_blank(blank, V);
+    const int *ynp = optional_arg<int>(yn, Dt::I32, pair_grads, N,
+                                       "yn must be a contiguous Int tensor of shape (N,) on the device of pair_grads");
     const c10::cuda::CUDAGuard guard(pair_grads.device());
     at::Tensor out = at::empty({N, T, U, V}, pair_grads.options());
     check_status(rnnt_b200_gather_backward(current_stream(pair_grads), pair_grads.data_ptr<float>(),
@@ -685,20 +695,16 @@ at::Tensor rnnt_gather_backward(const at::Tensor &pair_grads, const at::Tensor &
 // Viterbi alignment, dense (N,T,U,V) f32 or bf16 log-probs: (scores (N) f32, frames (N,U-1) i32).  No host sync.
 std::tuple<at::Tensor, at::Tensor> rnnt_align_dense(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn,
                                                     const at::Tensor &yn, int blank) {
-    check4(xs, ys, xn, yn, true);
-    check_dense_shapes(xs, ys, xn, yn);
-    const c10::cuda::CUDAGuard guard(xs.device());
-    const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), V = xs.size(3);
-    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
-    const bool bf16 = xs.scalar_type() == at::ScalarType::BFloat16;
+    const auto [N, T, U, V, bf16, guard] = dense_front(xs, ys, xn, yn, true);
+    check_blank(blank, V);
     at::Tensor scores = at::empty({N}, xs.options().dtype(at::kFloat));
     at::Tensor frames = at::empty({N, U - 1}, xs.options().dtype(at::kInt));
     if (N == 0) return std::make_tuple(scores, frames);
-    const size_t bytes = rnnt_b200_align_workspace_bytes(N * T * U, (int)N, (int)T, (int)U);
-    at::Tensor ws = at::empty({(int64_t)bytes}, xs.options().dtype(at::kByte));
-    check_status(rnnt_b200_align_dense(current_stream(xs), ws.data_ptr(), bytes, xs.data_ptr(), ys.data_ptr<int>(),
-                                       xn.data_ptr<int>(), yn.data_ptr<int>(), scores.data_ptr<float>(),
-                                       frames.data_ptr<int>(), (int)N, (int)T, (int)U, (int)V, blank, bf16 ? 2 : 4));
+    at::Tensor ws = workspace(xs, rnnt_b200_align_workspace_bytes(N * T * U, (int)N, (int)T, (int)U));
+    check_status(rnnt_b200_align_dense(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
+                                       ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
+                                       scores.data_ptr<float>(), frames.data_ptr<int>(), (int)N, (int)T, (int)U, (int)V,
+                                       blank, bf16 ? 2 : 4));
     return std::make_tuple(scores, frames);
 }
 
@@ -706,13 +712,7 @@ std::tuple<at::Tensor, at::Tensor> rnnt_align_dense(const at::Tensor &xs, const 
 // the hints when given (no host sync), else one 16-byte device->host copy, as in rnnt_loss_compact.
 std::tuple<at::Tensor, at::Tensor> rnnt_align_compact(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn,
                                                       const at::Tensor &yn, int blank, int max_T, int max_U) {
-    check4(xs, ys, xn, yn, true);
-    TORCH_CHECK(xs.dim() == 2, "xs must have 2 dimensions");
-    TORCH_CHECK(xn.dim() == 1 && yn.dim() == 1 && xn.size(0) == yn.size(0), "xn and yn shape must be equal (N,)");
-    const c10::cuda::CUDAGuard guard(xs.device());
-    const int64_t N = xn.size(0), STU = xs.size(0), V = xs.size(1);
-    TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)");
-    const bool bf16 = xs.scalar_type() == at::ScalarType::BFloat16;
+    const auto [N, STU, V, bf16, guard] = compact_front(xs, ys, xn, yn, blank, true);
     void *stream = current_stream(xs);
     at::Tensor scores = at::empty({N}, xs.options().dtype(at::kFloat));
     at::Tensor frames = at::empty({ys.numel()}, xs.options().dtype(at::kInt));
@@ -720,9 +720,8 @@ std::tuple<at::Tensor, at::Tensor> rnnt_align_compact(const at::Tensor &xs, cons
     std::tie(max_T, max_U) = compact_bounds(stream, xs, ys, xn, yn, max_T, max_U, nullptr);
     max_T = std::max(max_T, 1);              // lengths of 0 or less: the lattice is outside any bounds (score NaN)
     max_U = std::max(max_U, 1);
-    const size_t bytes = rnnt_b200_align_workspace_bytes(STU, (int)N, max_T, max_U);
-    at::Tensor ws = at::empty({(int64_t)bytes}, xs.options().dtype(at::kByte));
-    check_status(rnnt_b200_align_compact(stream, ws.data_ptr(), bytes, xs.data_ptr(), ys.data_ptr<int>(),
+    at::Tensor ws = workspace(xs, rnnt_b200_align_workspace_bytes(STU, (int)N, max_T, max_U));
+    check_status(rnnt_b200_align_compact(stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(), ys.data_ptr<int>(),
                                          xn.data_ptr<int>(), yn.data_ptr<int>(), scores.data_ptr<float>(),
                                          frames.data_ptr<int>(), STU, (int)N, (int)V, blank, bf16 ? 2 : 4, max_T,
                                          max_U));
