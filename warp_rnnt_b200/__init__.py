@@ -15,6 +15,7 @@ eager-PyTorch fallback: importing this package without the built extension raise
 import contextlib
 import importlib.machinery
 import importlib.util
+import math
 import os
 import sys
 import threading
@@ -284,16 +285,20 @@ class RNNTLossSimple(torch.autograd.Function):
     """The simple loss of the pruned recipe: the transducer loss of the joint ``am[n,t] + lm[n,u]``, whose normaliser is
     a (T,V) x (V,U) product per lattice, so no (N,T,U,V) tensor is formed.  Forward keeps the normaliser (N,T,U), the
     row offsets of ``am`` and ``lm`` and the (N,T,U,2) pair gradients; backward writes d loss / d ``am`` and d ``lm``.
-    With ``prune_range`` > 0 the forward also returns the (N,T) prune ranges (else an empty int tensor)."""
+    With ``prune_range`` > 0 the forward also returns the (N,T) prune ranges (else an empty int tensor).
+    ``lm_only_scale`` / ``am_only_scale``: k2's smoothing (``rnnt_loss_simple``); with either > 0 the forward also keeps
+    the LM-only and AM-only normalisers and the log of the batch unigram."""
 
     @staticmethod
-    def forward(ctx, am, lm, labels, frames_lengths, labels_lengths, blank=0, prune_range=0):
+    def forward(ctx, am, lm, labels, frames_lengths, labels_lengths, blank=0, prune_range=0, lm_only_scale=0.0,
+                am_only_scale=0.0):
         need = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
         costs, saved, pg, ranges = _C.rnnt_simple_forward(am, lm, labels, frames_lengths, labels_lengths, blank, need,
-                                                          prune_range, 0)
+                                                          prune_range, 0, lm_only_scale, am_only_scale)
         if need:
             ctx.save_for_backward(am, lm, labels, frames_lengths, labels_lengths, saved, pg)
             ctx.blank = blank
+            ctx.scales = (lm_only_scale, am_only_scale)
         ctx.mark_non_differentiable(ranges)
         return costs, ranges
 
@@ -301,15 +306,22 @@ class RNNTLossSimple(torch.autograd.Function):
     def backward(ctx, grads_output, _grad_ranges):
         am, lm, labels, xn, yn, saved, pg = ctx.saved_tensors
         go = grads_output.contiguous().to(torch.float32)
-        dam, dlm = _C.rnnt_simple_backward(am, lm, labels, xn, yn, saved, pg, go, ctx.blank)
+        dam, dlm = _C.rnnt_simple_backward(am, lm, labels, xn, yn, saved, pg, go, ctx.blank, *ctx.scales)
         return (dam if ctx.needs_input_grad[0] else None), (dlm if ctx.needs_input_grad[1] else None), \
-            None, None, None, None, None
+            None, None, None, None, None, None, None
+
+
+def _smoothing_scale(name, x):
+    if isinstance(x, bool) or not isinstance(x, (int, float)) or not math.isfinite(x) or x < 0:
+        raise ValueError("rnnt_loss_simple: %s must be a finite number >= 0, got %r" % (name, x))
+    return float(x)
 
 
 def rnnt_loss_simple(am, lm, labels, frames_lengths, labels_lengths, average_frames=False, reduction="none", blank=0,
-                     prune_range=None):
+                     prune_range=None, lm_only_scale=0.0, am_only_scale=0.0):
     """Simple transducer loss of the pruned recipe, and the windows ``rnnt_loss_pruned`` takes.  Follows k2's
-    ``rnnt_loss_simple`` + ``get_rnnt_prune_ranges`` (regular lattice); not tested against k2.
+    ``rnnt_loss_simple`` + ``get_rnnt_prune_ranges`` (regular lattice), and with ``lm_only_scale`` /
+    ``am_only_scale`` k2's ``rnnt_loss_smoothed``; not tested against k2.
 
     Args:
         am: (N, T, V) float32, the encoder output projected to the vocabulary.
@@ -318,23 +330,37 @@ def rnnt_loss_simple(am, lm, labels, frames_lengths, labels_lengths, average_fra
         average_frames, reduction, blank: as in ``rnnt_loss_from_logits``.
         prune_range: None, or an int S >= 2: also return the (N, T) int32 ``ranges`` for
             ``rnnt_loss_pruned(..., ranges)`` with windows of S labels.
+        lm_only_scale, am_only_scale: k2's smoothing scales sl, sa: finite, >= 0, sl + sa < 1 (else ValueError).
+            Both 0 (the default) is the plain simple loss, with the same kernels and the same bits.
 
     The loss is the RNN-T loss of lattice n in which cell (t, u) has the log-probs log_softmax(am[n,t] + lm[n,u]) at
     ``blank`` and at labels[n,u].  Its normaliser is log(sum_v exp(am[n,t,v]) exp(lm[n,u,v])), a fp32 contraction over
     V (include/rnnt_b200.h gives the exact operation order); a cell whose products all underflow is clamped to
     log(FLT_MIN) plus the row maxima instead of going to -inf.  The gradient flows to ``am`` and ``lm``, deterministic.
 
+    Smoothing (k2's ``rnnt_loss_smoothed(..., lm_only_scale=sl, am_only_scale=sa)``): with c = 1 - sl - sa, each of the
+    two log-probs of cell (t, u), for k = blank or labels[n,u], becomes
+    ``c * simple_k + sl * log_softmax(lm[n,u])[k] + sa * log(exp(am[n,t,k]) uni[k] / sum_v exp(am[n,t,v]) uni[v])``,
+    where ``uni`` is the unigram of the batch: the mean over every row of ``lm`` (padding rows included, as in k2) of
+    softmax(lm[n,u]), plus FLT_MIN.  A term whose scale is 0 is left out; k2 multiplies it by 1e-20 instead, which
+    differs only where that term is +-inf or NaN.  With ``am_only_scale`` > 0 the unigram couples the batch: a NaN
+    anywhere in ``lm`` makes every cost NaN, every row of ``lm`` gets a gradient, and a call on a micro-batch or a shard
+    uses that part's own unigram, as k2 does with a smaller batch.  The ranges come from the smoothed lattice, as k2's
+    recipes take them.  k2's own defaults are ``lm_only_scale=0.1, am_only_scale=0.1``, and icefall's recipes pass
+    ``lm_only_scale=0.25, am_only_scale=0.0``: a port passes the scales explicitly.
+
     The ranges come from the occupation probabilities of this loss's lattice: each frame takes the window of S columns
     with the most occupation, then the windows are made to start at 0, never move back, move by at most S-1 columns a
     frame and end on the last label.  The call returns ``(loss, ranges)`` then.  The ranges carry no gradient.
 
     bfloat16 ``am`` / ``lm`` are refused: these tensors are small beside the joint, and the loss is run in float32.
-    Lengths outside (1..T, 0..U-1) give cost NaN, zero gradient rows and ranges 0.  No host synchronisation: the step
-    can be captured in a CUDA graph.
+    Lengths outside (1..T, 0..U-1) give cost NaN, zero gradient rows and ranges 0 (with ``am_only_scale`` > 0 their
+    ``lm`` rows still get the unigram's gradient).  No host synchronisation: the step can be captured in a CUDA graph.
 
     Typical use, with no (N, T, U, V) tensor anywhere::
 
-        simple, ranges = rnnt_loss_simple(am, lm, labels, xn, yn, reduction="sum", prune_range=5)
+        simple, ranges = rnnt_loss_simple(am, lm, labels, xn, yn, reduction="sum", prune_range=5,
+                                          lm_only_scale=0.25, am_only_scale=0.0)
         idx = (ranges[:, :, None] + torch.arange(5, device=ranges.device)).clamp(max=lm_in.size(1) - 1)
         lm_win = lm_in[torch.arange(N, device=lm_in.device)[:, None, None], idx]     # (N, T, 5, H)
         logits = joint(enc_in[:, :, None] + lm_win)                                  # (N, T, 5, V)
@@ -350,7 +376,12 @@ def rnnt_loss_simple(am, lm, labels, frames_lengths, labels_lengths, average_fra
     if prune_range is not None and (isinstance(prune_range, bool) or not isinstance(prune_range, int)
                                     or prune_range < 2):
         raise ValueError("rnnt_loss_simple: prune_range must be None or an int >= 2, got %r" % (prune_range,))
-    costs, ranges = RNNTLossSimple.apply(am, lm, labels, frames_lengths, labels_lengths, blank, prune_range or 0)
+    sl = _smoothing_scale("lm_only_scale", lm_only_scale)
+    sa = _smoothing_scale("am_only_scale", am_only_scale)
+    # the kernels take the scales as float32: the check is on the values they see
+    if torch.tensor(sl, dtype=torch.float32).item() + torch.tensor(sa, dtype=torch.float32).item() >= 1.0:
+        raise ValueError("rnnt_loss_simple: lm_only_scale + am_only_scale must be < 1, got %r + %r" % (sl, sa))
+    costs, ranges = RNNTLossSimple.apply(am, lm, labels, frames_lengths, labels_lengths, blank, prune_range or 0, sl, sa)
     costs = _reduce(costs, frames_lengths, average_frames, reduction)
     return costs if prune_range is None else (costs, ranges)
 

@@ -4,6 +4,7 @@
 // (B) run_warp_rnnt & co: the reference's C ABI (the reference's core.h:29-60) implemented on top
 //     of (A)'s kernels so the reference's own bindings link against this library unchanged.
 #include <atomic>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -136,6 +137,57 @@ static SimpleArgs simple_call(const float *am, const float *lm, const int *label
     a.off_l = a.off_a + (int64_t)N * T;
     a.T = T; a.U = U; a.V = V; a.blank = blank;
     return a;
+}
+// k2's smoothing scales: finite, >= 0, sl + sa < 1 (so c = 1 - sl - sa > 0)
+static bool smooth_scales_ok(float sl, float sa) {
+    return std::isfinite(sl) && std::isfinite(sa) && sl >= 0.0f && sa >= 0.0f && (double)sl + (double)sa < 1.0;
+}
+static bool smoothed(float sl, float sa) { return sl > 0.0f || sa > 0.0f; }
+// the smoothed loss's saved buffer: the simple loss's, then Ll (N,U), Am (N,T), log uni (V)
+static int64_t simple_saved_len(int N, int T, int U, int V, bool smooth) {
+    const int64_t n = N, base = n * T * U + n * T + n * U;
+    return smooth ? base + n * U + n * T + V : base;
+}
+// the smoothed workspace: forward = the loss's, then uni (V) and the unigram partials; backward = c*grad_out (N),
+// Cb, Cl (N,U), the G partials and G (V); one size covers both
+struct SmoothWorkspace {
+    float *uni, *upart, *cgo, *cb, *cl, *gpart, *G;
+    size_t fwd_bytes, bwd_bytes;
+};
+static SmoothWorkspace carve_smooth(void *base, int N, int T, int U, int V) {
+    SmoothWorkspace w;
+    const size_t n = (size_t)max(N, 0), t = (size_t)max(T, 0), u = (size_t)max(U, 0), v = (size_t)max(V, 0);
+    size_t off = carve(nullptr, (int64_t)(n * t * u), N).bytes;
+    auto take = [&](size_t bytes) {
+        void *p = base ? (void *)((char *)base + off) : nullptr;
+        off += align_up(bytes, 256);
+        return (float *)p;
+    };
+    w.uni = take(v * sizeof(float));
+    w.upart = take((n * u + kSmoothRows - 1) / kSmoothRows * v * sizeof(float));
+    w.fwd_bytes = off;
+    off = 0;
+    w.cgo = take(n * sizeof(float));
+    w.cb = take(n * u * sizeof(float));
+    w.cl = take(n * u * sizeof(float));
+    w.gpart = take((n * t + kSmoothRows - 1) / kSmoothRows * v * sizeof(float));
+    w.G = take(v * sizeof(float));
+    w.bwd_bytes = off;
+    return w;
+}
+static SmoothArgs smooth_call(const SimpleArgs &a, const SmoothWorkspace &w, float *saved, int N, float sl, float sa) {
+    SmoothArgs m = {};
+    m.am = a.am; m.lm = a.lm; m.labels = a.labels; m.xn = a.xn; m.yn = a.yn;
+    m.off_a = a.off_a; m.off_l = a.off_l;
+    m.Ll = saved + simple_saved_len(N, a.T, a.U, a.V, false);
+    m.Am = m.Ll + (int64_t)N * a.U;
+    m.loguni = m.Am + (int64_t)N * a.T;
+    m.uni = w.uni; m.upart = w.upart;
+    m.cgo = w.cgo; m.cb = w.cb; m.cl = w.cl; m.gpart = w.gpart; m.G = w.G;
+    m.c = (float)(1.0 - (double)sl - (double)sa);
+    m.sl = sl; m.sa = sa;
+    m.N = N; m.T = a.T; m.U = a.U; m.V = a.V; m.blank = a.blank;
+    return m;
 }
 // (cells,2) pairs and their gradients are read and written as float2
 static bool pairs_aligned(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 7u) == 0; }
@@ -781,33 +833,78 @@ size_t rnnt_b200_simple_workspace_bytes(int N, int T, int U) {
     return carve(nullptr, (int64_t)max(N, 0) * max(T, 0) * max(U, 0), N).bytes;
 }
 
+size_t rnnt_b200_simple_smoothed_workspace_bytes(int N, int T, int U, int V) {
+    const SmoothWorkspace w = carve_smooth(nullptr, N, T, U, V);
+    return max(w.fwd_bytes, w.bwd_bytes);
+}
+
 int rnnt_b200_simple_forward(void *stream, void *workspace, size_t workspace_bytes, const float *am, const float *lm,
                              const int *labels, const int *xn, const int *yn, float *costs, float *saved,
                              float *pair_grads, int N, int T, int U, int V, int blank, int lse_mode) {
-    if (!simple_args_ok(N, T, U, V, blank) || !saved || !pairs_aligned(pair_grads) || !pairs_aligned(workspace))
-        return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0) return RNNT_STATUS_SUCCESS;
-    cudaStream_t s = (cudaStream_t)stream;
-    LossCall c = dense_call(xn, yn, N, T, U, costs, 0.0f, lse_mode);
-    Workspace w;
-    if (!carve_ok(workspace, workspace_bytes, c.cells, N, &w)) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
-    SimpleArgs a = simple_call(am, lm, labels, xn, yn, saved, N, T, U, V, blank);
-    a.pairs = w.pairs;
-    RNNT_TRY(launch_simple_forward(s, a, N), RNNT_STATUS_GATHER_FAILED);
-    c.pairs = w.pairs; c.pair_grads = reinterpret_cast<float2 *>(pair_grads);
-    return run_loss(s, workspace, workspace_bytes, c);
+    return rnnt_b200_simple_smoothed_forward(stream, workspace, workspace_bytes, am, lm, labels, xn, yn, costs, saved,
+                                             pair_grads, N, T, U, V, blank, lse_mode, 0.0f, 0.0f);
 }
 
 int rnnt_b200_simple_backward(void *stream, const float *am, const float *lm, const int *labels, const int *xn,
                               const int *yn, const float *saved, const float *pair_grads, const float *grad_out,
                               float *dam, float *dlm, int N, int T, int U, int V, int blank) {
-    if (!simple_args_ok(N, T, U, V, blank) || !saved || !pair_grads || !pairs_aligned(pair_grads) || !dam || !dlm)
+    return rnnt_b200_simple_smoothed_backward(stream, nullptr, 0, am, lm, labels, xn, yn, saved, pair_grads, grad_out,
+                                              dam, dlm, N, T, U, V, blank, 0.0f, 0.0f);
+}
+
+int rnnt_b200_simple_smoothed_forward(void *stream, void *workspace, size_t workspace_bytes, const float *am,
+                                      const float *lm, const int *labels, const int *xn, const int *yn, float *costs,
+                                      float *saved, float *pair_grads, int N, int T, int U, int V, int blank,
+                                      int lse_mode, float lm_only_scale, float am_only_scale) {
+    if (!simple_args_ok(N, T, U, V, blank) || !smooth_scales_ok(lm_only_scale, am_only_scale) || !saved ||
+        !pairs_aligned(pair_grads) || !pairs_aligned(workspace))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    const bool smooth = smoothed(lm_only_scale, am_only_scale);
+    cudaStream_t s = (cudaStream_t)stream;
+    LossCall c = dense_call(xn, yn, N, T, U, costs, 0.0f, lse_mode);
+    Workspace w;
+    if (!carve_ok(workspace, workspace_bytes, c.cells, N, &w)) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    if (smooth && workspace_bytes < rnnt_b200_simple_smoothed_workspace_bytes(N, T, U, V))
+        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    SimpleArgs a = simple_call(am, lm, labels, xn, yn, saved, N, T, U, V, blank);
+    a.pairs = w.pairs;
+    RNNT_TRY(launch_simple_forward(s, a, N), RNNT_STATUS_GATHER_FAILED);
+    if (smooth) {
+        SmoothArgs m = smooth_call(a, carve_smooth(workspace, N, T, U, V), saved, N, lm_only_scale, am_only_scale);
+        m.pairs = w.pairs;
+        // with sa = 0 nothing computes Am and log uni: they are saved as 0
+        if (!(am_only_scale > 0.0f))
+            RNNT_TRY(cudaMemsetAsync(m.Am, 0, ((int64_t)N * T + V) * sizeof(float), s), RNNT_STATUS_GATHER_FAILED);
+        RNNT_TRY(launch_simple_smoothed_forward(s, m), RNNT_STATUS_GATHER_FAILED);
+    }
+    c.pairs = w.pairs; c.pair_grads = reinterpret_cast<float2 *>(pair_grads);
+    return run_loss(s, workspace, workspace_bytes, c);
+}
+
+int rnnt_b200_simple_smoothed_backward(void *stream, void *workspace, size_t workspace_bytes, const float *am,
+                                       const float *lm, const int *labels, const int *xn, const int *yn,
+                                       const float *saved, const float *pair_grads, const float *grad_out, float *dam,
+                                       float *dlm, int N, int T, int U, int V, int blank, float lm_only_scale,
+                                       float am_only_scale) {
+    if (!simple_args_ok(N, T, U, V, blank) || !smooth_scales_ok(lm_only_scale, am_only_scale) || !saved ||
+        !pair_grads || !pairs_aligned(pair_grads) || !dam || !dlm || !pairs_aligned(workspace))
         return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
     SimpleArgs a = simple_call(am, lm, labels, xn, yn, const_cast<float *>(saved), N, T, U, V, blank);
     a.pg = reinterpret_cast<const float2 *>(pair_grads);
     a.grad_out = grad_out;
-    RNNT_TRY(launch_simple_backward((cudaStream_t)stream, a, dam, dlm, N), RNNT_STATUS_GRADS_BLANK_FAILED);
+    if (!smoothed(lm_only_scale, am_only_scale)) {
+        RNNT_TRY(launch_simple_backward((cudaStream_t)stream, a, dam, dlm, N), RNNT_STATUS_GRADS_BLANK_FAILED);
+        return RNNT_STATUS_SUCCESS;
+    }
+    if (!workspace || workspace_bytes < rnnt_b200_simple_smoothed_workspace_bytes(N, T, U, V))
+        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    SmoothArgs m = smooth_call(a, carve_smooth(workspace, N, T, U, V), const_cast<float *>(saved), N, lm_only_scale,
+                               am_only_scale);
+    m.pg = a.pg;
+    m.grad_out = grad_out;
+    RNNT_TRY(launch_simple_smoothed_backward((cudaStream_t)stream, a, m, dam, dlm), RNNT_STATUS_GRADS_BLANK_FAILED);
     return RNNT_STATUS_SUCCESS;
 }
 

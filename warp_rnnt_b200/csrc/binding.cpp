@@ -548,46 +548,60 @@ void check_simple_inputs(const at::Tensor &am, const at::Tensor &lm, const at::T
     check_arg(yn, Dt::I32, am, N, lengths);
 }
 
-// simple loss from am (N,T,V) and lm (N,U,V), float32: (costs (N), saved (N*T*U + N*T + N*U), pair_grads (N,T,U,2) or
+// the saved buffer of the simple loss: norm, oa, ol; with a smoothing scale also Ll, Am and log uni
+int64_t simple_saved_len(int64_t N, int64_t T, int64_t U, int64_t V, bool smooth) {
+    const int64_t base = N * T * U + N * T + N * U;
+    return smooth ? base + N * U + N * T + V : base;
+}
+
+// simple loss from am (N,T,V) and lm (N,U,V), float32: (costs (N), saved (simple_saved_len), pair_grads (N,T,U,2) or
 // empty, ranges (N,T) int32 or empty).  The pair gradients are computed when want_grads or prune_range > 0; the ranges
-// when prune_range > 0.  No host sync.
+// when prune_range > 0.  lm_only_scale / am_only_scale: k2's smoothing (both 0: the plain simple loss).  No host sync.
 std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor>
 rnnt_simple_forward(const at::Tensor &am, const at::Tensor &lm, const at::Tensor &ys, const at::Tensor &xn,
-                    const at::Tensor &yn, int blank, bool want_grads, int prune_range, int lse_mode) {
+                    const at::Tensor &yn, int blank, bool want_grads, int prune_range, int lse_mode,
+                    double lm_only_scale, double am_only_scale) {
     check_simple_inputs(am, lm, ys, xn, yn);
     const int64_t N = am.size(0), T = am.size(1), U = lm.size(1), V = am.size(2);
     check_blank(blank, V);
     TORCH_CHECK(prune_range == 0 || prune_range >= 2, "prune_range must be an int >= 2");
+    const float sl = (float)lm_only_scale, sa = (float)am_only_scale;
+    const bool smooth = sl != 0.0f || sa != 0.0f;
     const c10::cuda::CUDAGuard guard(am.device());
     const auto f32 = am.options().dtype(at::kFloat);
     const bool pairs = want_grads || prune_range > 0;
     at::Tensor costs = at::empty({N}, f32);
-    at::Tensor saved = at::empty({N * T * U + N * T + N * U}, f32);
+    at::Tensor saved = at::empty({simple_saved_len(N, T, U, V, smooth)}, f32);
     at::Tensor pg = output(pairs, {N, T, U, 2}, f32);
     at::Tensor ranges = at::empty({prune_range > 0 ? N : 0, prune_range > 0 ? T : 0}, am.options().dtype(at::kInt));
     if (N == 0) return std::make_tuple(costs, saved, pg, ranges);
     void *stream = current_stream(am);
-    at::Tensor ws = workspace(am, rnnt_b200_simple_workspace_bytes((int)N, (int)T, (int)U));
-    check_status(rnnt_b200_simple_forward(stream, ws.data_ptr(), (size_t)ws.numel(), am.data_ptr<float>(),
-                                          lm.data_ptr<float>(), ys.data_ptr<int>(), xn.data_ptr<int>(),
-                                          yn.data_ptr<int>(), costs.data_ptr<float>(), saved.data_ptr<float>(),
-                                          pairs ? pg.data_ptr<float>() : nullptr, (int)N, (int)T, (int)U, (int)V, blank,
-                                          lse_mode));
+    at::Tensor ws = workspace(am, smooth ? rnnt_b200_simple_smoothed_workspace_bytes((int)N, (int)T, (int)U, (int)V)
+                                         : rnnt_b200_simple_workspace_bytes((int)N, (int)T, (int)U));
+    check_status(rnnt_b200_simple_smoothed_forward(stream, ws.data_ptr(), (size_t)ws.numel(), am.data_ptr<float>(),
+                                                   lm.data_ptr<float>(), ys.data_ptr<int>(), xn.data_ptr<int>(),
+                                                   yn.data_ptr<int>(), costs.data_ptr<float>(), saved.data_ptr<float>(),
+                                                   pairs ? pg.data_ptr<float>() : nullptr, (int)N, (int)T, (int)U,
+                                                   (int)V, blank, lse_mode, sl, sa));
     if (prune_range > 0)
         check_status(rnnt_b200_prune_ranges(stream, pg.data_ptr<float>(), xn.data_ptr<int>(), yn.data_ptr<int>(), (int)N,
                                             (int)T, (int)U, prune_range, ranges.data_ptr<int>()));
     return std::make_tuple(costs, saved, pg, ranges);
 }
 
-// d sum_n grad_out[n] cost[n] / d (am, lm)
+// d sum_n grad_out[n] cost[n] / d (am, lm); the scales must be the forward's
 std::tuple<at::Tensor, at::Tensor> rnnt_simple_backward(const at::Tensor &am, const at::Tensor &lm, const at::Tensor &ys,
                                                         const at::Tensor &xn, const at::Tensor &yn,
                                                         const at::Tensor &saved, const at::Tensor &pair_grads,
-                                                        const at::Tensor &grad_out, int blank) {
+                                                        const at::Tensor &grad_out, int blank, double lm_only_scale,
+                                                        double am_only_scale) {
     check_simple_inputs(am, lm, ys, xn, yn);
     const int64_t N = am.size(0), T = am.size(1), U = lm.size(1), V = am.size(2);
-    check_arg(saved, Dt::F32, am, N * T * U + N * T + N * U,
-              "saved must be the simple forward's contiguous Float tensor on the device of am");
+    const float sl = (float)lm_only_scale, sa = (float)am_only_scale;
+    const bool smooth = sl != 0.0f || sa != 0.0f;
+    check_arg(saved, Dt::F32, am, simple_saved_len(N, T, U, V, smooth),
+              smooth ? "saved must be the smoothed simple forward's contiguous Float tensor on the device of am"
+                     : "saved must be the simple forward's contiguous Float tensor on the device of am");
     check_arg(pair_grads, Dt::F32, am, N * T * U * 2,
               "pair_grads must be a contiguous Float tensor of shape (N, T, U, 2) on the device of am");
     check_arg(grad_out, Dt::F32, am, N, "grad_out must be a contiguous Float tensor of shape (N,)");
@@ -595,11 +609,14 @@ std::tuple<at::Tensor, at::Tensor> rnnt_simple_backward(const at::Tensor &am, co
     const c10::cuda::CUDAGuard guard(am.device());
     at::Tensor dam = at::empty_like(am), dlm = at::empty_like(lm);
     if (N == 0) return std::make_tuple(dam, dlm);
-    check_status(rnnt_b200_simple_backward(current_stream(am), am.data_ptr<float>(), lm.data_ptr<float>(),
-                                           ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
-                                           saved.data_ptr<float>(), pair_grads.data_ptr<float>(),
-                                           grad_out.data_ptr<float>(), dam.data_ptr<float>(), dlm.data_ptr<float>(),
-                                           (int)N, (int)T, (int)U, (int)V, blank));
+    at::Tensor ws = workspace(am, smooth ? rnnt_b200_simple_smoothed_workspace_bytes((int)N, (int)T, (int)U, (int)V) : 0);
+    check_status(rnnt_b200_simple_smoothed_backward(current_stream(am), smooth ? ws.data_ptr() : nullptr,
+                                                    (size_t)ws.numel(), am.data_ptr<float>(), lm.data_ptr<float>(),
+                                                    ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
+                                                    saved.data_ptr<float>(), pair_grads.data_ptr<float>(),
+                                                    grad_out.data_ptr<float>(), dam.data_ptr<float>(),
+                                                    dlm.data_ptr<float>(), (int)N, (int)T, (int)U, (int)V, blank, sl,
+                                                    sa));
     return std::make_tuple(dam, dlm);
 }
 
@@ -764,9 +781,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("pair_grads"), py::arg("ys"), py::arg("ranges"), py::arg("grad_out"), py::arg("blank") = 0);
     m.def("rnnt_simple_forward", &rnnt_simple_forward, py::arg("am"), py::arg("lm"), py::arg("ys"), py::arg("xn"),
           py::arg("yn"), py::arg("blank") = 0, py::arg("want_grads") = true, py::arg("prune_range") = 0,
-          py::arg("lse_mode") = 0);
+          py::arg("lse_mode") = 0, py::arg("lm_only_scale") = 0.0, py::arg("am_only_scale") = 0.0);
     m.def("rnnt_simple_backward", &rnnt_simple_backward, py::arg("am"), py::arg("lm"), py::arg("ys"), py::arg("xn"),
-          py::arg("yn"), py::arg("saved"), py::arg("pair_grads"), py::arg("grad_out"), py::arg("blank") = 0);
+          py::arg("yn"), py::arg("saved"), py::arg("pair_grads"), py::arg("grad_out"), py::arg("blank") = 0,
+          py::arg("lm_only_scale") = 0.0, py::arg("am_only_scale") = 0.0);
     m.def("rnnt_prune_ranges", &rnnt_prune_ranges, py::arg("pair_grads"), py::arg("xn"), py::arg("yn"), py::arg("S"));
     m.def("rnnt_joint_pack", &rnnt_joint_pack, py::arg("f"), py::arg("g"), py::arg("lf"), py::arg("lg"), py::arg("stu") = -1);
     m.def("rnnt_joint_pack_backward", &rnnt_joint_pack_backward, py::arg("dx"), py::arg("lf"), py::arg("lg"),

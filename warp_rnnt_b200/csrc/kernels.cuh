@@ -91,6 +91,29 @@ struct SimpleArgs {
 cudaError_t launch_simple_forward(cudaStream_t s, const SimpleArgs &a, int N);
 // dam (N,T,V) and dlm (N,U,V), every element written
 cudaError_t launch_simple_backward(cudaStream_t s, const SimpleArgs &a, float *dam, float *dlm, int N);
+// k2's smoothed simple loss (lm_only_scale sl, am_only_scale sa, c = 1 - sl - sa): the extra row passes, the batch
+// unigram and the mixed pairs (forward), and the sl / sa / unigram gradient terms (backward)
+constexpr int kSmoothRows = 32;        // rows per CTA of the unigram and G partials: the partition depends on shapes only
+struct SmoothArgs {
+    const float *am, *lm;              // (N,T,V), (N,U,V)
+    const int *labels, *xn, *yn;       // (N,U-1), (N), (N)
+    const float *off_a, *off_l;        // oa (N,T), ol (N,U) of the simple forward
+    float *Ll, *Am, *loguni;           // saved: (N,U), (N,T), (V)
+    float *uni, *upart;                // forward workspace: uni (V), unigram partials (ceil(N*U / kSmoothRows), V)
+    float2 *pairs;                     // forward: the simple pairs in, the mixed pairs out
+    const float2 *pg;                  // backward: (N,T,U) pair gradients
+    const float *grad_out;             // backward: (N), or null (ones)
+    float *cgo, *cb, *cl, *gpart, *G;  // backward workspace: c*grad_out (N), column sums of gb, gl (N,U), G partials
+                                       // (ceil(N*T / kSmoothRows), V), G (V)
+    float c, sl, sa;
+    int N, T, U, V, blank;
+};
+// after launch_simple_forward: Ll (and, with sa > 0, uni, log uni, Am), then the mixed pairs in place
+cudaError_t launch_simple_smoothed_forward(cudaStream_t s, const SmoothArgs &m);
+// column sums and c*grad_out; launch_simple_backward on c*grad_out; then the sa (am rows, G) and sl / unigram (lm rows)
+// terms added to dam, dlm
+cudaError_t launch_simple_smoothed_backward(cudaStream_t s, const SimpleArgs &a, const SmoothArgs &m, float *dam,
+                                            float *dlm);
 // ranges (N,T) from the pair gradients (N,T,U,2) of a loss call; S >= 2
 cudaError_t launch_prune_ranges(cudaStream_t s, const float2 *pg, const int *xn, const int *yn, int N, int T, int U,
                                 int S, int *ranges);

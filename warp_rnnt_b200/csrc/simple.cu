@@ -306,6 +306,338 @@ cudaError_t launch_simple_backward(cudaStream_t s, const SimpleArgs &a, float *d
     return cudaGetLastError();
 }
 
+// ---- k2's smoothed simple loss (rnnt_loss_smoothed: lm_only_scale sl, am_only_scale sa, c = 1 - sl - sa) ----------
+//
+//   Ll[n,u] = log(sum_v exp(lm[u,v] - ol[u])) + ol[u]          p[n,u,v] = exp(lm[u,v] - Ll[u])
+//   uni[v]  = (sum over every lm row of p[.,v]) / (N U) + FLT_MIN
+//   Am[n,t] = log(sum_v exp(am[t,v] - oa[t]) uni[v]) + oa[t]
+//   pair_k  = (c simple_k + sl (lm[u,k] - Ll[u])) + sa ((am[t,k] + log uni[k]) - Am[t]),   a zero-scale term absent
+//
+//   k_smooth_lm_rows     Ll, one warp per row; with sa > 0 also the unigram partial of its CTA's kSmoothRows rows
+//   k_smooth_uni         uni and log uni: one thread per v sums the partials in CTA order
+//   k_smooth_am_norm     Am, one warp per row
+//   k_smooth_mix         the mixed pairs, one thread per cell, in place
+//   k_smooth_cols        backward: Cb[n,u] = sum_t gb, Cl[n,u] = sum_t gl (one thread per column), and c*grad_out
+//   k_smooth_am_rows     the sa terms of dam, and the partials of G's dense part, kSmoothRows am rows per CTA
+//   k_smooth_G           G[v] = sa (Gs[v] / uni[v] - Gd[v]); Gs is the blank / label scatter, found by a scan
+//   k_smooth_lm_rows_bwd the sl and unigram terms of dlm, one warp per row
+//
+// Every reduction is partitioned by the shapes alone (fixed rows per CTA, warp-strided rows, fixed loop orders), so
+// the bits do not depend on the grid size or the SM count; there are no atomics.
+
+__device__ __forceinline__ float warp_sum(float x) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+    return x;
+}
+
+// CTA b owns lm rows [b kSmoothRows, (b+1) kSmoothRows) of the flattened (N*U); 8 warps, 4 rows each.  With sa = 0 only
+// live rows (u < Un) are read, and the others get Ll = 0.
+__global__ void __launch_bounds__(kRowThreads) k_smooth_lm_rows(SmoothArgs m) {
+    __shared__ float Ls[kSmoothRows];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t rows = (int64_t)m.N * m.U, r0 = (int64_t)blockIdx.x * kSmoothRows;
+    const int V = m.V;
+    for (int i = warp; i < kSmoothRows; i += kRowThreads / 32) {
+        const int64_t r = r0 + i;
+        if (r >= rows) break;
+        const int n = (int)(r / m.U), u = (int)(r % m.U);
+        int Tn, Un;
+        simple_lengths(m.xn, m.yn, n, m.T, m.U, Tn, Un);
+        float L = 0.0f;
+        if (m.sa > 0.0f || u < Un) {
+            const float *x = m.lm + r * V, o = m.off_l[r];
+            float s = 0.0f;
+            for (int v = lane; v < V; v += 32) s += expf(__ldg(x + v) - o);
+            L = logf(warp_sum(s)) + o;
+        }
+        if (lane == 0) { m.Ll[r] = L; Ls[i] = L; }
+    }
+    if (!(m.sa > 0.0f)) return;
+    __syncthreads();
+    const int nr = (int)min((int64_t)kSmoothRows, rows - r0);
+    for (int v = threadIdx.x; v < V; v += kRowThreads) {
+        float acc = 0.0f;
+        for (int i = 0; i < nr; ++i) acc += expf(__ldg(m.lm + (r0 + i) * V + v) - Ls[i]);
+        m.upart[(int64_t)blockIdx.x * V + v] = acc;
+    }
+}
+
+__global__ void __launch_bounds__(kRowThreads) k_smooth_uni(SmoothArgs m, int parts) {
+    const int v = blockIdx.x * kRowThreads + threadIdx.x;
+    if (v >= m.V) return;
+    float s = 0.0f;
+    for (int b = 0; b < parts; ++b) s += m.upart[(int64_t)b * m.V + v];
+    const float u = __fadd_rn(__fdiv_rn(s, (float)((int64_t)m.N * m.U)), FLT_MIN);
+    m.uni[v] = u;
+    m.loguni[v] = logf(u);
+}
+
+// one warp per am row; rows past Tn (and every row of a lattice with invalid lengths) get Am = 0 and are not read
+__global__ void __launch_bounds__(kRowThreads) k_smooth_am_norm(SmoothArgs m) {
+    const int lane = threadIdx.x & 31;
+    const int64_t rows = (int64_t)m.N * m.T;
+    for (int64_t r = ((int64_t)blockIdx.x * kRowThreads + threadIdx.x) >> 5; r < rows;
+         r += (int64_t)gridDim.x * (kRowThreads / 32)) {
+        const int n = (int)(r / m.T), t = (int)(r % m.T);
+        int Tn, Un;
+        simple_lengths(m.xn, m.yn, n, m.T, m.U, Tn, Un);
+        float A = 0.0f;
+        if (t < Tn) {
+            const float *x = m.am + r * m.V, o = m.off_a[r];
+            float s = 0.0f;
+            for (int v = lane; v < m.V; v += 32) s = fmaf(expf(__ldg(x + v) - o), m.uni[v], s);
+            A = logf(warp_sum(s)) + o;
+        }
+        if (lane == 0) m.Am[r] = A;
+    }
+}
+
+// pair_k = (c simple_k + sl lmonly_k) + sa amonly_k in round-to-nearest steps (no contraction), each term only when its
+// scale is not 0; cells outside the lattice keep (0, 0)
+__device__ __forceinline__ float smooth_pair(const SmoothArgs &m, float simple, const float *ra, const float *rl,
+                                             float Ll, float Am, int k) {
+    float p = __fmul_rn(m.c, simple);
+    if (m.sl > 0.0f) p = __fadd_rn(p, __fmul_rn(m.sl, __fsub_rn(__ldg(rl + k), Ll)));
+    if (m.sa > 0.0f) p = __fadd_rn(p, __fmul_rn(m.sa, __fsub_rn(__fadd_rn(__ldg(ra + k), m.loguni[k]), Am)));
+    return p;
+}
+
+__global__ void __launch_bounds__(kRowThreads) k_smooth_mix(SmoothArgs m) {
+    const int T = m.T, U = m.U, V = m.V;
+    const int64_t cells = (int64_t)m.N * T * U;
+    for (int64_t i = (int64_t)blockIdx.x * kRowThreads + threadIdx.x; i < cells; i += (int64_t)gridDim.x * kRowThreads) {
+        const int u = (int)(i % U);
+        const int64_t nt = i / U;
+        const int t = (int)(nt % T), n = (int)(nt / T);
+        int Tn, Un;
+        simple_lengths(m.xn, m.yn, n, T, U, Tn, Un);
+        if (t >= Tn || u >= Un) continue;
+        const int y = (u < Un - 1) ? m.labels[(int64_t)n * (U - 1) + u] : m.blank;
+        const float *ra = m.am + nt * V, *rl = m.lm + ((int64_t)n * U + u) * V;
+        const float Ll = m.sl > 0.0f ? m.Ll[(int64_t)n * U + u] : 0.0f, Am = m.sa > 0.0f ? m.Am[nt] : 0.0f;
+        const float2 q = m.pairs[i];
+        m.pairs[i] = make_float2(smooth_pair(m, q.x, ra, rl, Ll, Am, m.blank), smooth_pair(m, q.y, ra, rl, Ll, Am, y));
+    }
+}
+
+// thread r < N*U owns column (n,u): Cb, Cl summed over t < Tn in increasing t (0 outside the lattice); thread r < N
+// also writes cgo[r] = c * grad_out[r]
+__global__ void __launch_bounds__(kRowThreads) k_smooth_cols(SmoothArgs m) {
+    const int T = m.T, U = m.U;
+    const int64_t rows = (int64_t)m.N * U;
+    for (int64_t r = (int64_t)blockIdx.x * kRowThreads + threadIdx.x; r < rows; r += (int64_t)gridDim.x * kRowThreads) {
+        const int n = (int)(r / U), u = (int)(r % U);
+        if (r < m.N) m.cgo[r] = __fmul_rn(m.c, m.grad_out ? m.grad_out[r] : 1.0f);
+        int Tn, Un;
+        simple_lengths(m.xn, m.yn, n, T, U, Tn, Un);
+        float sb = 0.0f, sl = 0.0f;
+        if (u < Un) {
+            const float2 *q = m.pg + (int64_t)n * T * U + u;
+            for (int t = 0; t < Tn; ++t) {
+                const float2 p = q[(int64_t)t * U];
+                sb += p.x;
+                sl += p.y;
+            }
+        }
+        m.cb[r] = sb;
+        m.cl[r] = sl;
+    }
+}
+
+// CTA b owns am rows [b kSmoothRows, (b+1) kSmoothRows) of the flattened (N*T).  Per live row (t < Tn), with
+// go = grad_out[n], Ra = sum_u (gb + gl), Sb = sum_u gb (one warp, lane-strided u, then a butterfly):
+//   dam[t,v] += -(sa go Ra) (exp(am[t,v] - Am[t]) uni[v])                     (thread per v, rows in order)
+//   gpart[b,v] = sum over the CTA's live rows of (go Ra) exp(am[t,v] - Am[t])  (the same loop)
+//   then dam[t,y_u] += sa go gl[t,u] for u < Un-1 in turn, dam[t,blank] += sa go Sb   (thread per row)
+// uni[v] is taken as expf(log uni[v]).
+__global__ void __launch_bounds__(kRowThreads) k_smooth_am_rows(SmoothArgs m, float *__restrict__ dam) {
+    __shared__ float As[kSmoothRows], Ws[kSmoothRows], Qs[kSmoothRows], Bs[kSmoothRows];
+    __shared__ bool Live[kSmoothRows];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int T = m.T, U = m.U, V = m.V;
+    const int64_t rows = (int64_t)m.N * T, r0 = (int64_t)blockIdx.x * kSmoothRows;
+    const int nr = (int)min((int64_t)kSmoothRows, rows - r0);
+    for (int i = warp; i < nr; i += kRowThreads / 32) {
+        const int64_t r = r0 + i;
+        const int n = (int)(r / T), t = (int)(r % T);
+        int Tn, Un;
+        simple_lengths(m.xn, m.yn, n, T, U, Tn, Un);
+        float ra = 0.0f, sb = 0.0f, go = 0.0f;
+        const bool live = t < Tn;
+        if (live) {
+            go = m.grad_out ? m.grad_out[n] : 1.0f;
+            const float2 *q = m.pg + r * U;
+            for (int u = lane; u < Un; u += 32) {
+                const float2 p = q[u];
+                ra += p.x + p.y;
+                sb += p.x;
+            }
+            ra = warp_sum(ra);
+            sb = warp_sum(sb);
+        }
+        if (lane == 0) {
+            Live[i] = live;
+            As[i] = m.Am[r];
+            Ws[i] = -(m.sa * go * ra);
+            Qs[i] = go * ra;
+            Bs[i] = __fmul_rn(m.sa, go) * sb;
+        }
+    }
+    __syncthreads();
+    for (int v = threadIdx.x; v < V; v += kRowThreads) {
+        const float un = expf(m.loguni[v]);
+        float acc = 0.0f;
+        for (int i = 0; i < nr; ++i) {
+            if (!Live[i]) continue;
+            const int64_t r = r0 + i;
+            const float e = expf(__ldg(m.am + r * V + v) - As[i]);
+            dam[r * V + v] = __fadd_rn(dam[r * V + v], __fmul_rn(Ws[i], __fmul_rn(e, un)));
+            acc = __fadd_rn(acc, __fmul_rn(Qs[i], e));
+        }
+        m.gpart[(int64_t)blockIdx.x * V + v] = acc;
+    }
+    __syncthreads();
+    if (threadIdx.x < nr) {
+        const int i = threadIdx.x;
+        const int64_t r = r0 + i;
+        const int n = (int)(r / T);
+        if (Live[i]) {
+            const int Un = m.yn[n] + 1;                // live rows belong to lattices with valid lengths
+            const float w = __fmul_rn(m.sa, m.grad_out ? m.grad_out[n] : 1.0f);
+            const float2 *q = m.pg + r * U;
+            const int *lab = m.labels + (int64_t)n * (U - 1);
+            float *o = dam + r * V;
+            for (int u = 0; u < Un - 1; ++u) o[lab[u]] += w * q[u].y;
+            o[m.blank] += Bs[i];
+        }
+    }
+}
+
+// One thread per v (CTAs of kRowThreads over V).  Gd[v] = the gpart column summed in CTA order.  Gs[v] = sum over the
+// flattened (n,u) in order of go_n Cb[n,u] when v = blank (u < Un) and go_n Cl[n,u] when v = labels[n,u] (u < Un-1),
+// the blank term of an entry before its label term: every CTA stages kRowThreads entries in shared memory at a time
+// and each thread scans them for its v.
+__global__ void __launch_bounds__(kRowThreads) k_smooth_G(SmoothArgs m, int parts) {
+    __shared__ int Yb[kRowThreads], Yl[kRowThreads];
+    __shared__ float Fb[kRowThreads], Fl[kRowThreads];
+    const int v = blockIdx.x * kRowThreads + threadIdx.x, U = m.U;
+    const int64_t ents = (int64_t)m.N * U;
+    float gs = 0.0f;
+    for (int64_t j0 = 0; j0 < ents; j0 += kRowThreads) {
+        const int64_t j = j0 + threadIdx.x;
+        int yb = -1, yl = -1;
+        float fb = 0.0f, fl = 0.0f;
+        if (j < ents) {
+            const int n = (int)(j / U), u = (int)(j % U);
+            int Tn, Un;
+            simple_lengths(m.xn, m.yn, n, m.T, U, Tn, Un);
+            if (u < Un) {
+                const float go = m.grad_out ? m.grad_out[n] : 1.0f;
+                yb = m.blank;
+                fb = go * m.cb[j];
+                if (u < Un - 1) { yl = m.labels[(int64_t)n * (U - 1) + u]; fl = go * m.cl[j]; }
+            }
+        }
+        Yb[threadIdx.x] = yb; Yl[threadIdx.x] = yl; Fb[threadIdx.x] = fb; Fl[threadIdx.x] = fl;
+        __syncthreads();
+        const int k1 = (int)min((int64_t)kRowThreads, ents - j0);
+        for (int k = 0; k < k1; ++k) {
+            if (Yb[k] == v) gs += Fb[k];
+            if (Yl[k] == v) gs += Fl[k];
+        }
+        __syncthreads();
+    }
+    if (v >= m.V) return;
+    float gd = 0.0f;
+    for (int b = 0; b < parts; ++b) gd += m.gpart[(int64_t)b * m.V + v];
+    m.G[v] = __fmul_rn(m.sa, __fsub_rn(__fdiv_rn(gs, expf(m.loguni[v])), gd));
+}
+
+// One warp per lm row (n,u).  With p[v] = exp(lm[u,v] - Ll[u]) and, when sa > 0, pG = sum_v p[v] G[v] (lane-strided,
+// then a butterfly):
+//   dlm[u,v] += -(sl go (Cb + Cl)[u]) p[v]           (sl > 0, live rows u < Un)
+//   dlm[u,v] += (p[v] (G[v] - pG)) / (N U)           (sa > 0, every row)
+//   then dlm[u,blank] += sl go Cb[u], dlm[u,y_u] += sl go Cl[u] for u < Un-1   (sl > 0, live rows; lane 0)
+// With sa = 0 rows past Un are not read.
+__global__ void __launch_bounds__(kRowThreads) k_smooth_lm_rows_bwd(SmoothArgs m, float *__restrict__ dlm) {
+    const int lane = threadIdx.x & 31;
+    const int U = m.U, V = m.V;
+    const int64_t rows = (int64_t)m.N * U;
+    const bool sa = m.sa > 0.0f, sl = m.sl > 0.0f;
+    const float nu = (float)rows;
+    for (int64_t r = ((int64_t)blockIdx.x * kRowThreads + threadIdx.x) >> 5; r < rows;
+         r += (int64_t)gridDim.x * (kRowThreads / 32)) {
+        const int n = (int)(r / U), u = (int)(r % U);
+        int Tn, Un;
+        simple_lengths(m.xn, m.yn, n, m.T, U, Tn, Un);
+        const bool live = sl && u < Un;
+        if (!sa && !live) continue;
+        const float *x = m.lm + r * V, L = m.Ll[r];
+        float *o = dlm + r * V;
+        float pG = 0.0f;
+        if (sa) {
+            for (int v = lane; v < V; v += 32) pG = fmaf(expf(__ldg(x + v) - L), m.G[v], pG);
+            pG = warp_sum(pG);
+        }
+        const float go = m.grad_out ? m.grad_out[n] : 1.0f;
+        const float wl = live ? -(m.sl * go * (m.cb[r] + m.cl[r])) : 0.0f;
+        for (int v = lane; v < V; v += 32) {
+            const float p = expf(__ldg(x + v) - L);
+            float d = o[v];
+            if (live) d = __fadd_rn(d, __fmul_rn(wl, p));
+            if (sa) d = __fadd_rn(d, __fdiv_rn(__fmul_rn(p, __fsub_rn(m.G[v], pG)), nu));
+            o[v] = d;
+        }
+        if (live) {
+            __syncwarp();
+            if (lane == 0) {
+                const float w = __fmul_rn(m.sl, go);
+                o[m.blank] += w * m.cb[r];
+                if (u < Un - 1) o[m.labels[(int64_t)n * (U - 1) + u]] += w * m.cl[r];
+            }
+            __syncwarp();
+        }
+    }
+}
+
+cudaError_t launch_simple_smoothed_forward(cudaStream_t s, const SmoothArgs &m) {
+    const int64_t lrows = (int64_t)m.N * m.U, arows = (int64_t)m.N * m.T;
+    const int lparts = (int)((lrows + kSmoothRows - 1) / kSmoothRows);
+    k_smooth_lm_rows<<<lparts, kRowThreads, 0, s>>>(m);
+    count_launch();
+    if (m.sa > 0.0f) {
+        k_smooth_uni<<<(m.V + kRowThreads - 1) / kRowThreads, kRowThreads, 0, s>>>(m, lparts);
+        count_launch();
+        k_smooth_am_norm<<<row_grid(arows, kRowThreads / 32), kRowThreads, 0, s>>>(m);
+        count_launch();
+    }
+    k_smooth_mix<<<row_grid((int64_t)m.N * m.T * m.U, kRowThreads), kRowThreads, 0, s>>>(m);
+    count_launch();
+    return cudaGetLastError();
+}
+
+cudaError_t launch_simple_smoothed_backward(cudaStream_t s, const SimpleArgs &a, const SmoothArgs &m, float *dam,
+                                            float *dlm) {
+    const int64_t lrows = (int64_t)m.N * m.U, arows = (int64_t)m.N * m.T;
+    k_smooth_cols<<<row_grid(lrows, kRowThreads), kRowThreads, 0, s>>>(m);
+    count_launch();
+    SimpleArgs b = a;
+    b.grad_out = m.cgo;
+    cudaError_t e = launch_simple_backward(s, b, dam, dlm, m.N);
+    if (e != cudaSuccess) return e;
+    if (m.sa > 0.0f) {
+        const int aparts = (int)((arows + kSmoothRows - 1) / kSmoothRows);
+        k_smooth_am_rows<<<aparts, kRowThreads, 0, s>>>(m, dam);
+        count_launch();
+        k_smooth_G<<<(m.V + kRowThreads - 1) / kRowThreads, kRowThreads, 0, s>>>(m, aparts);
+        count_launch();
+    }
+    k_smooth_lm_rows_bwd<<<row_grid(lrows, kRowThreads / 32), kRowThreads, 0, s>>>(m, dlm);
+    count_launch();
+    return cudaGetLastError();
+}
+
 cudaError_t launch_prune_ranges(cudaStream_t s, const float2 *pg, const int *xn, const int *yn, int N, int T, int U,
                                 int S, int *ranges) {
     k_prune_ranges<<<N, kRangeThreads, 0, s>>>(pg, xn, yn, T, U, S, ranges);
