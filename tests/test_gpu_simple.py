@@ -82,26 +82,50 @@ def make(N, T, U, V, seed, blank=0, scale=1.5):
     return am, lm, ys, xn, yn
 
 
-def check(c, dam, dlm, am, lm, ys, xn, yn, blank, go):
-    """costs to 1e-5 relative; each gradient element to the per-cell bound of tests/test_gpu_pruned_paths.py,
-    1e-4 + max(2 gtol(T,U), 2^-23 max|cost| sqrt(T+U)), times the occupation it sums: a d am row sums the cells of
-    its frame, a d lm row those of its column (up to Tn / Un frames' worth), and the recurrence's fp32 error of each
-    cell's occupation adds up along them."""
-    N, T, V = am.shape
-    U = lm.shape[1]
+def simple_ref(am, lm, ys, xn, yn, blank, go):
+    """The full-joint fp64 restatement -> (costs, d am, d lm, pair gradients) as check() takes them."""
     c0, dam0, dlm0 = so.simple(am, lm, ys, xn, yn, blank, grad_output=go)
-    np.testing.assert_allclose(c, c0, rtol=1e-5)
     x = np.asarray(am, np.float64)[:, :, None] + np.asarray(lm, np.float64)[:, None]
     m = x.max(axis=-1, keepdims=True)
     lp = x - (m + np.log(np.exp(x - m).sum(axis=-1, keepdims=True)))
-    occ = np.abs(so.pair_grads_of(lp, ys, xn, yn, blank)).sum(axis=3)          # (N,T,U)
+    return c0, dam0, dlm0, so.pair_grads_of(lp, ys, xn, yn, blank)
+
+
+def bounds(c0, pg0, go):
+    """-> (cell, occ, ta, tl): the per-cell bound of tests/test_gpu_pruned_paths.py,
+    cell = 1e-4 + max(2 gtol(T,U), 2^-23 max|cost| sqrt(T+U)), the occupation occ (N,T,U) = |gb| + |gl| of the
+    reference's pair gradients pg0, and the bounds of d am and d lm: cell times the occupation each element sums.  A
+    d am row sums the cells of its frame, a d lm row those of its column (up to Tn / Un frames' worth), and the
+    recurrence's fp32 error of each cell's occupation adds up along them."""
+    N, T, U, _ = pg0.shape
+    occ = np.abs(pg0).sum(axis=3)
     cell = 1e-4 + max(2 * gtol(T, U), 2.0 ** -23 * np.nanmax(np.abs(c0)) * np.sqrt(T + U))
     g = np.abs(np.asarray(go, np.float64)).reshape(N, 1, 1)
     ta = cell * g * np.maximum(1.0, occ.sum(axis=2))[:, :, None]
     tl = cell * g * np.maximum(1.0, occ.sum(axis=1))[:, :, None]
+    return cell, occ, ta, tl
+
+
+def compare(c, dam, dlm, ref, ta, tl):
+    """costs to 1e-5 relative, d am and d lm elementwise within ta, tl -> (largest relative cost error, the gradient
+    error and bound at the element nearest its bound, their ratio)."""
+    c0, dam0, dlm0 = ref[:3]
+    np.testing.assert_allclose(c, c0, rtol=1e-5)
+    cost_rel = np.nanmax(np.abs(c - c0)) / np.nanmax(np.abs(c0))
+    worst = (0.0, 0.0, 1.0)
     for name, got, want, tol in (("d am", dam, dam0, ta), ("d lm", dlm, dlm0, tl)):
-        err = np.abs(got - want)
+        err, tol = np.abs(got - want), np.broadcast_to(tol, got.shape)
         assert (err <= tol).all(), (name, err.max(), np.unravel_index(np.argmax(err - tol), err.shape))
+        i = np.unravel_index(np.argmax(err / tol), err.shape)
+        if err[i] / tol[i] > worst[0]:
+            worst = (err[i] / tol[i], err[i], tol[i])
+    return cost_rel, worst[1], worst[2], worst[0]
+
+
+def check(c, dam, dlm, ref, go):
+    """c, dam, dlm against the reference's (costs, d am, d lm, pair gradients) ref: compare() within bounds()."""
+    _, _, ta, tl = bounds(ref[0], ref[3], go)
+    return compare(c, dam, dlm, ref, ta, tl)
 
 
 SHAPES = [  # N, T, U, V, blank, path
@@ -132,7 +156,8 @@ def test_vs_oracle(w, shape, mode):
         (c * cu(go.astype(np.float32))).sum().backward()
     finally:
         w.set_lse_mode("auto")
-    check(c.detach().cpu().numpy(), a.grad.cpu().numpy(), l.grad.cpu().numpy(), am, lm, ys, xn, yn, blank, go)
+    ref = simple_ref(am, lm, ys, xn, yn, blank, go)
+    check(c.detach().cpu().numpy(), a.grad.cpu().numpy(), l.grad.cpu().numpy(), ref, go)
 
 
 @pytest.mark.parametrize("average_frames", [False, True])
@@ -152,9 +177,9 @@ def test_reductions(w, shape, reduction, average_frames):
         wts = wts * np.linspace(1.0, 2.0, N)
         out = (out * cu(np.linspace(1.0, 2.0, N).astype(np.float32))).sum()
     out.backward()
-    c0 = so.simple(am, lm, ys, xn, yn, blank)[0]
-    np.testing.assert_allclose(out.item(), (c0 * wts).sum(), rtol=1e-5)
-    check(c0, a.grad.cpu().numpy(), l.grad.cpu().numpy(), am, lm, ys, xn, yn, blank, wts)
+    ref = simple_ref(am, lm, ys, xn, yn, blank, wts)
+    np.testing.assert_allclose(out.item(), (ref[0] * wts).sum(), rtol=1e-5)
+    check(ref[0], a.grad.cpu().numpy(), l.grad.cpu().numpy(), ref, wts)
 
 
 def rebuilt_pairs(am, lm, ys, xn, yn, norm, blank):
@@ -251,7 +276,8 @@ def test_masked_vocabulary(w):
     a, l = cu(am).requires_grad_(True), cu(lm).requires_grad_(True)
     c = w.rnnt_loss_simple(a, l, cu(ys), cu(xn), cu(yn))
     c.sum().backward()
-    check(c.detach().cpu().numpy(), a.grad.cpu().numpy(), l.grad.cpu().numpy(), am, lm, ys, xn, yn, 0, np.ones(N))
+    check(c.detach().cpu().numpy(), a.grad.cpu().numpy(), l.grad.cpu().numpy(),
+          simple_ref(am, lm, ys, xn, yn, 0, np.ones(N)), np.ones(N))
 
 
 @pytest.mark.parametrize("shape", [(4, 30, 20, 28), (4, 150, 140, 16)])

@@ -19,8 +19,8 @@ import torch
 
 from tests import simple_oracle as so
 from tests import smoothed_oracle as sm
-from tests.test_gpu_logits import gtol
-from tests.test_gpu_simple import EXACT, FAST, INVALID, SHAPES, TOO_SMALL, _abi, cu, last_path, make, rebuilt_pairs
+from tests.test_gpu_simple import (EXACT, FAST, INVALID, SHAPES, TOO_SMALL, _abi, bounds, compare, cu, last_path, make,
+                                   rebuilt_pairs)
 
 pytestmark = pytest.mark.gpu
 
@@ -74,34 +74,29 @@ def oracle(am, lm, ys, xn, yn, blank, sl, sa, go):
     return _oracle_cache[key]
 
 
-def check(c, dam, dlm, am, lm, ys, xn, yn, blank, go, sl, sa):
-    """costs to 1e-5 relative.  d am and the c and sl parts of d lm: test_gpu_simple.check's per-cell bound times the
-    occupation each element sums (now the smoothed lattice's).  The unigram term of d lm, (1/(N U)) p (G - p.G), adds
-    the error of G: G[v] sums go_n times occupations over the whole batch, each divided by uni[v] or weighted by
-    exp(am - Am) <= 1/uni[v], so |dG[v]| <= 2 sa cell sum_n |go_n| (sum_{t,u} occ_n) / uni[v]."""
-    N, T, V = am.shape
-    U = lm.shape[1]
-    c0, dam0, dlm0, pg0, du = oracle(am, lm, ys, xn, yn, blank, sl, sa, go)
-    np.testing.assert_allclose(c, c0, rtol=1e-5)
-    occ = np.abs(pg0).sum(axis=3)
-    cell = 1e-4 + max(2 * gtol(T, U), 2.0 ** -23 * np.nanmax(np.abs(c0)) * np.sqrt(T + U))
-    g = np.abs(np.asarray(go, np.float64)).reshape(N, 1, 1)
-    ta = cell * g * np.maximum(1.0, occ.sum(axis=2))[:, :, None]
-    tl = cell * g * np.maximum(1.0, occ.sum(axis=1))[:, :, None]
+def check(c, dam, dlm, ref, lm, go, sa):
+    """c, dam, dlm against the reference's (costs, d am, d lm, pair gradients, unigram term of d lm or None) ref.
+    costs to 1e-5 relative.  d am and the c and sl parts of d lm: test_gpu_simple.bounds, the per-cell bound times
+    the occupation each element sums (now the smoothed lattice's).  The unigram term of d lm, (1/(N U)) p (G - p.G),
+    adds the error of G: G[v] sums go_n times occupations over the whole batch, each divided by uni[v] or weighted by
+    exp(am - Am) <= 1/uni[v], so |dG[v]| <= 2 sa cell sum_n |go_n| (sum_{t,u} occ_n) / uni[v].  -> compare()'s
+    (cost_rel, grad_err, bound, ratio)."""
+    N, U, V = lm.shape
+    du = ref[4]
+    cell, occ, ta, tl = bounds(ref[0], ref[3], go)
     if sa > 0:
+        g = np.abs(np.asarray(go, np.float64))
         l64 = np.asarray(lm, np.float64)
         p = np.exp(l64 - l64.max(-1, keepdims=True))
         p /= p.sum(-1, keepdims=True)
         uni = p.mean(axis=(0, 1)) + sm.FLT_MIN
-        dG = 2 * sa * cell * (g[:, 0, 0] * occ.sum(axis=(1, 2))).sum() / uni
+        dG = 2 * sa * cell * (g * occ.sum(axis=(1, 2))).sum() / uni
         tu = p * (dG + (p * dG).sum(-1, keepdims=True)) / (N * U)
         tl = tl + tu
         # the unigram term is larger than the whole bound somewhere: a backward without it would fail (with V = 1 the
         # term is identically 0)
         assert V == 1 or (np.abs(du) > tl).any(), (np.abs(du).max(), tl.max())
-    for name, got, want, tol in (("d am", dam, dam0, ta), ("d lm", dlm, dlm0, tl)):
-        err = np.abs(got - want)
-        assert (err <= tol).all(), (name, err.max(), np.unravel_index(np.argmax(err - tol), err.shape))
+    return compare(c, dam, dlm, ref, ta, tl)
 
 
 def test_zero_scales_are_the_simple_loss(w):
@@ -142,7 +137,8 @@ def test_vs_oracle(w, shape, mode, scales):
         (c * cu(go.astype(np.float32))).sum().backward()
     finally:
         w.set_lse_mode("auto")
-    check(c.detach().cpu().numpy(), a.grad.cpu().numpy(), l.grad.cpu().numpy(), am, lm, ys, xn, yn, blank, go, sl, sa)
+    check(c.detach().cpu().numpy(), a.grad.cpu().numpy(), l.grad.cpu().numpy(),
+          oracle(am, lm, ys, xn, yn, blank, sl, sa, go), lm, go, sa)
 
 
 @pytest.mark.parametrize("average_frames", [False, True])
@@ -163,9 +159,9 @@ def test_reductions(w, shape, reduction, average_frames):
         wts = wts * np.linspace(1.0, 2.0, N)
         out = (out * cu(np.linspace(1.0, 2.0, N).astype(np.float32))).sum()
     out.backward()
-    c0 = sm.smoothed(am, lm, ys, xn, yn, blank, sl, sa)[0]
-    np.testing.assert_allclose(out.item(), (c0 * wts).sum(), rtol=1e-5)
-    check(c0, a.grad.cpu().numpy(), l.grad.cpu().numpy(), am, lm, ys, xn, yn, blank, wts, sl, sa)
+    ref = oracle(am, lm, ys, xn, yn, blank, sl, sa, wts)
+    np.testing.assert_allclose(out.item(), (ref[0] * wts).sum(), rtol=1e-5)
+    check(ref[0], a.grad.cpu().numpy(), l.grad.cpu().numpy(), ref, lm, wts, sa)
 
 
 def rebuilt_smoothed_pairs(at, lt, yt, xt, nt, saved, blank, sl, sa):
@@ -296,8 +292,8 @@ def test_masked_vocabulary(w):
         a, l = cu(am).requires_grad_(True), cu(lm).requires_grad_(True)
         c = w.rnnt_loss_simple(a, l, cu(ys), cu(xn), cu(yn), lm_only_scale=sl, am_only_scale=sa)
         c.sum().backward()
-        check(c.detach().cpu().numpy(), a.grad.cpu().numpy(), l.grad.cpu().numpy(), am, lm, ys, xn, yn, 0,
-              np.ones(N), sl, sa)
+        check(c.detach().cpu().numpy(), a.grad.cpu().numpy(), l.grad.cpu().numpy(),
+              oracle(am, lm, ys, xn, yn, 0, sl, sa, np.ones(N)), lm, np.ones(N), sa)
 
 
 def test_forward_only_and_empty(w):

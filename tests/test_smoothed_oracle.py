@@ -5,6 +5,7 @@ constant, and a padding row of lm reaches another lattice's cost exactly when am
 import numpy as np
 import pytest
 
+from tests import pruned_oracle as po
 from tests import simple_oracle as so
 from tests import smoothed_oracle as sm
 
@@ -87,3 +88,84 @@ def test_padding_row_couples_the_batch_iff_am_only_scale(scales):
     c1 = sm.smoothed(am, l, ys, xn, yn, 0, sl, sa)[0]
     assert (abs(c1[0] - c0[0]) > 1e-6) == (sa > 0)
     assert (abs(c1[1] - c0[1]) > 1e-6) == (sa > 0)
+
+
+# ------------------------------------------------------------------------------------------ factorised
+SCALES = [(0.25, 0.0), (0.0, 0.3), (0.1, 0.1), (0.5, 0.45)]
+FACTORISED = [  # N, T, U, V, blank
+    (3, 6, 4, 7, 0),
+    (4, 9, 6, 5, 2),
+    (2, 70, 66, 4, 1),                # more than one 64-row / 64-column tile of the kernels' contractions
+]
+
+
+def edge_inputs(N, T, U, V, blank, seed):
+    """make()'s inputs with padding rows in lattice 1, invalid lengths in lattice 2 (N >= 3) and about a quarter of
+    the labels equal to blank."""
+    am, lm, ys, xn, yn = make(N, T, U, V, seed=seed, blank=blank)
+    rng = np.random.RandomState(seed + 1)
+    ys[rng.rand(*ys.shape) < 0.25] = blank
+    yn[1] = min(int(yn[1]), U - 2)
+    if N >= 3:
+        xn[2] = T + 1
+    return am, lm, ys, xn, yn
+
+
+@pytest.mark.parametrize("scales", [(0.0, 0.0)] + SCALES)
+@pytest.mark.parametrize("shape", FACTORISED)
+def test_factorised_is_smoothed(shape, scales):
+    """The factorised restatement gives smoothed()'s costs, d am, d lm and pair gradients, labels equal to blank,
+    padding rows and an invalid lattice included; with detach_unigram the same d lm as smoothed()'s."""
+    N, T, U, V, blank = shape
+    sl, sa = scales
+    am, lm, ys, xn, yn = edge_inputs(N, T, U, V, blank, seed=T + U)
+    assert (ys[:, :int(yn[0])] == blank).any()
+    go = np.linspace(0.5, 1.5, N)
+    want = sm.smoothed(am, lm, ys, xn, yn, blank, sl, sa, grad_output=go, want_pairs=True)
+    got = sm.factorised(am, lm, ys, xn, yn, blank, sl, sa, grad_output=go)
+    if N >= 3:
+        assert np.isnan(got[0][2]) and not got[1][2].any() and not got[3][2].any()
+        assert np.isfinite(np.delete(got[0], 2)).all()
+    for name, x, y in zip(("costs", "d am", "d lm", "pair grads"), got, want):
+        np.testing.assert_allclose(x, y, rtol=0, atol=1e-10, err_msg=name)
+    if sa > 0:
+        d0 = sm.smoothed(am, lm, ys, xn, yn, blank, sl, sa, grad_output=go, detach_unigram=True)[2]
+        d1 = sm.factorised(am, lm, ys, xn, yn, blank, sl, sa, grad_output=go, detach_unigram=True)[2]
+        np.testing.assert_allclose(d1, d0, rtol=0, atol=1e-10)
+        assert np.abs(d1 - got[2]).max() > 1e-4
+
+
+def test_factorised_zero_scales_is_the_simple_oracle():
+    """At zero scales, with its pairs rounded to float32 as simple_oracle's log-probs are, the factorised restatement
+    is simple_oracle.simple (the full joint through oracle.from_logits), over several tiles."""
+    N, T, U, V, blank = 3, 70, 66, 6, 2
+    am, lm, ys, xn, yn = make(N, T, U, V, seed=5, blank=blank)
+    go = np.array([0.5, 1.0, 1.5])
+    c0, da0, dl0 = so.simple(am, lm, ys, xn, yn, blank=blank, grad_output=go)
+    c1, da1, dl1, _ = sm.factorised(am, lm, ys, xn, yn, blank, grad_output=go, round_pairs=True)
+    np.testing.assert_allclose(c1, c0, rtol=1e-12)
+    np.testing.assert_allclose(da1, da0, rtol=0, atol=1e-10)
+    np.testing.assert_allclose(dl1, dl0, rtol=0, atol=1e-10)
+
+
+def test_vectorised_recurrences_are_the_per_lattice_ones():
+    """alphas() / betas() over a ragged batch equal pruned_oracle._alphas / _betas lattice by lattice, and are -inf
+    outside every lattice; lattice_grads' costs are -beta[0,0]."""
+    rng = np.random.RandomState(3)
+    N, T, U = 5, 13, 9
+    B, L = np.log(rng.rand(N, T, U)), np.log(rng.rand(N, T, U))
+    Tn = np.array([13, 1, 7, 13, 0])
+    Un = np.array([9, 4, 1, 5, 0])
+    a, b = sm.alphas(B, L, Tn, Un), sm.betas(B, L, Tn, Un)
+    costs, gb, gl = sm.lattice_grads(B, L, Tn, Un)
+    for n in range(N - 1):
+        t, u = Tn[n], Un[n]
+        np.testing.assert_allclose(a[n, :t, :u], po._alphas(B[n, :t, :u], L[n, :t, :u]), rtol=1e-14, atol=0)
+        np.testing.assert_allclose(b[n, :t, :u], po._betas(B[n, :t, :u], L[n, :t, :u]), rtol=1e-14, atol=0)
+        outside = np.ones((T, U), bool)
+        outside[:t, :u] = False
+        assert (a[n][outside] == -np.inf).all() and (b[n][outside] == -np.inf).all()
+        assert not gb[n][outside].any() and not gl[n][outside].any()
+        assert costs[n] == -b[n, 0, 0]
+        assert gb[n, t - 1, u - 1] == pytest.approx(-1.0, abs=1e-12)
+    assert (a[N - 1] == -np.inf).all() and np.isnan(costs[N - 1]) and not gb[N - 1].any()
