@@ -1,8 +1,10 @@
 """Phase timeline of the fused small-lattice kernel (k_fused) from its optional clock64 stamps
 (rnnt_b200_debug_fused_trace, include/rnnt_b200.h).  Prints, per LSE mode, the median over CTAs of each
 phase's end time relative to the CTA's start, in microseconds.  Phases the launch's dense-gradient emit order does
-not have are left out: fill_issued / zeros_landed belong to zero-fill + patch, store_start (composed rows staged,
-the stores begin) to the composed emit; emit_start is where beta[0,0] is known and either emit begins.
+not have are left out: fill_issued / chase_done / zeros_landed belong to zero-fill + patch, first_store / last_store
+(the composed emit's first and last piece stored) to the composed emit; emit_start is where
+beta[0,0] is known and either emit begins.  In the composed order the gather runs bottom row up and alpha starts when
+it is done, so alpha's step time while the pieces are written is (alpha_done - gather_done) / (T + U - 1).
 
     python tools/fused_timeline.py [c2|c3] [out.json]
 """
@@ -18,7 +20,7 @@ import warp_rnnt_b200 as w  # noqa: E402
 
 SHAPES = {"c2": (128, 150, 40, 28), "c2n32": (32, 150, 40, 28), "c2n132": (132, 150, 40, 28), "c3": (32, 150, 20, 5000), "c1": (1, 150, 40, 28)}
 NAMES = ["start", "sentinels", "gather_done", "sweep_start", "alpha_done", "beta_done", "fill_issued", "end", "chase_done",
-         "zeros_landed", "emit_start", "store_start"]
+         "zeros_landed", "emit_start", "first_store", "last_store"]
 
 
 def sm_mhz():
@@ -70,6 +72,9 @@ def main():
         out[mode] = {"ctas": int(tr.shape[0]), "sm_mhz": mhz, "event_us": e0.elapsed_time(e1) * 1e3,
                      "median_us": {k: round(x, 2) for k, x, s in zip(NAMES, med, seen) if s},
                      "max_us": {k: round(x, 2) for k, x, s in zip(NAMES, mx, seen) if s}}
+        if seen[NAMES.index("first_store")]:
+            m = dict(zip(NAMES, med))
+            out[mode]["alpha_step_us"] = round((m["alpha_done"] - m["gather_done"]) / (T + U - 1), 4)
         print(mode, json.dumps(out[mode]))
     if len(sys.argv) > 2:
         json.dump(out, open(sys.argv[2], "w"), indent=1)

@@ -8,9 +8,10 @@
 //                        bulk copy per lattice row (U*V contiguous elements, f32 or bf16) into a row buffer -- two
 //                        buffers per gather warp, so the next row is in flight while this one is picked apart -- then
 //                        two LDS per cell pick blank and label (fallback: LDG picks in 128-cell chunks).  Rows are
-//                        staged from both ends towards the middle and each warp publishes its progress (st.release),
-//                        so the two wavefronts START WHILE THE GATHER IS STILL RUNNING and chase it (alpha needs the
-//                        top rows first, beta the bottom rows)
+//                        staged from both ends towards the middle (composed emit: bottom row up) and each warp
+//                        publishes its progress (st.release), so the wavefronts START WHILE THE GATHER IS STILL RUNNING
+//                        and chase it (alpha needs the top rows first, beta the bottom rows; composed emit: beta chases
+//                        the gather, alpha starts when it is done)
 //   phase 1  wavefront   ONE warp runs alpha and one runs beta: lane l owns C adjacent lattice columns, every
 //                        anti-diagonal is one step = one shuffle + C independent LSE chains, operands and results
 //                        move as C-wide vector LDS/STS (a diagonal's cells are contiguous in the staged layout; alpha
@@ -19,13 +20,16 @@
 //            zero-fill   (MODE 0, patch order) when the gather is done, two warps' lane 0 issue TMA bulk stores of a
 //                        zeroed shared-memory buffer (evict_last) over this CTA's slice of the dense gradient (replaces
 //                        at::zeros_like, binding.cpp:58)
-//            chase       the other free warps follow the two wavefronts from the middle anti-diagonal outwards and
-//                        replace each staged log-prob by (alpha + beta) + log-prob: all of the gradient that does not
-//                        need beta[0,0]
+//            chase       (MODE 0, patch order) the other free warps follow the two wavefronts from the middle
+//                        anti-diagonal outwards and replace each staged log-prob by (alpha + beta) + log-prob: all of
+//                        the gradient that does not need beta[0,0]
+//            emit        (MODE 0, composed order) once beta[0,0] is known, the free warps write the CTA's rows behind
+//                        alpha, one row at a time, composed in shared memory and stored as 16-byte streaming stores
+//                        (replaces zeros_like + kernel_grads_*)
 //   phase 2  cost/guard  kernel_fill_costs (core.cu:334-370) + the reduced loss sum_n costs[n]*scale[n] by the last CTA
 //            emit        MODE 0, two orders (chosen per launch, see launch_fused):
-//                          compose: expf(x - beta00) of every cell in place, then every element of the CTA's rows is
-//                                   written once as 16-byte streaming stores (replaces zeros_like + kernel_grads_*)
+//                          compose: already written in phase 1; the unaligned head / tail, or zeros over everything if
+//                                   the mismatch guard fired
 //                          patch:   expf(x - beta00) and <= 2 four-byte stores per cell into the zeroed lines
 //                                   (kernel_grads_blank/label, core.cu:260-332)
 //                        MODE 1: the gradients are emitted in (N,T,U,2) form for the deferred dense backward (+ loc for
@@ -124,9 +128,11 @@ __device__ __forceinline__ int flag_acquire(const int *f) {
 constexpr int kChunkLog = 7, kChunkCells = 1 << kChunkLog;   // gather granule: 4 cells per lane
 constexpr int kMaxChunks = 96;                                 // >= ceil(max staged cells / kChunkCells)
 
-// Consumer side of the gather.  Order-row k: even k = top row k/2, odd k = bottom row Tn-1-(k-1)/2.
-// A wavefront that is about to read lattice rows within m of its starting edge needs order-rows
-// <= 2m+1 staged.
+// Consumer side of the gather.  Two orders of the lattice rows:
+//   seq = 0 : order-row k: even k = top row k/2, odd k = bottom row Tn-1-(k-1)/2.  A wavefront that is about to read
+//             lattice rows within m of its starting edge needs order-rows <= 2m+1 staged.
+//   seq = 1 : order-row k = bottom row Tn-1-k (beta first, the composed emit).  Beta needs order-rows <= m; alpha
+//             waits once for the whole gather (all()).
 //   chunked LDG gather : chunk q holds order-space cells [128q, 128q+128); flag[q] set when staged
 //   TMA row gather     : gather warp g stages order-rows g, g+gwn, ...; flag[g] counts its finished rows
 struct GatherWait {
@@ -134,16 +140,36 @@ struct GatherWait {
     int Un, Tn, lane, gwn;  // gwn > 0: TMA row gather with gwn warps
     int ready;              // chunks [0, ready) / order-rows [0, ready) are known complete
     int m_ok;               // rows(m) is known to hold for every m <= m_ok (one compare on the per-step path)
+    bool seq;               // row order (above)
     __device__ __forceinline__ void ensure(int m) {
         if (m > m_ok) {
             rows(m);
-            // order-rows known complete -> largest m with min(2m+1, Tn-1) < rows_done
+            // order-rows known complete -> largest m with min(2m+1, Tn-1) (seq: min(m, Tn-1)) < rows_done
             const int rows_done = gwn > 0 ? ready : min(Tn, (ready << kChunkLog) / Un);
-            m_ok = (rows_done >= Tn) ? 0x7fffffff : ((rows_done - 2) >> 1);
+            m_ok = (rows_done >= Tn) ? 0x7fffffff : (seq ? rows_done - 1 : ((rows_done - 2) >> 1));
         }
     }
+    // every order-row staged.  Polled with a back-off: the caller is a wavefront warp, which the issue arbiter favours,
+    // and it must not take issue slots from the gather it waits for.
+    __device__ __forceinline__ void all() {
+        if (gwn > 0) {
+            while (ready < Tn) {
+                int first_open = 0x7fffffff;
+                if (lane < gwn) first_open = flag_acquire(flag + lane) * gwn + lane;
+                ready = __reduce_min_sync(0xffffffffu, first_open);
+                if (ready < Tn) __nanosleep(256);
+            }
+        } else {
+            const int q = (Tn * Un - 1) >> kChunkLog;
+            while (ready <= q) {
+                if (flag_acquire(flag + ready) != 0) ++ready;
+                else __nanosleep(256);
+            }
+        }
+        m_ok = 0x7fffffff;
+    }
     __device__ __forceinline__ void rows(int m) {
-        const int k = min(2 * m + 1, Tn - 1);
+        const int k = seq ? min(m, Tn - 1) : min(2 * m + 1, Tn - 1);
         if (gwn > 0) {
             while (ready <= k) {
                 int first_open = 0x7fffffff;          // this gather warp's first unfinished order-row
@@ -435,6 +461,9 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
     // TMA rows need 16-byte aligned, 16-byte multiple rows: always true when chosen for the dense layout,
     // per lattice in the compact layout
     const bool use_tma = A.nbuf > 0 && (!compact || ((((slab * V) | ((int64_t)Un * V)) & (16 / ESZ - 1)) == 0));
+    // gather order: beta first (bottom row up) under the composed emit, so that beta[0,0] -- which every gradient value
+    // needs -- is known soon after the last row arrives; from both ends towards the middle otherwise
+    const bool seq = MODE == 0 && A.compose;
 
     // ---- phase 0: sentinels, labels, gather
     if (tid == 0) { s_next = 0; s_bad = ok ? 0 : 1; s_prog[0] = 0; s_prog[1] = 0; }
@@ -481,7 +510,10 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
             const uint64_t pol_first = policy_evict_first();
             const uint32_t bytes = ((uint32_t)(Un * V) * (uint32_t)ESZ + 15u) & ~15u;   // <= U*V*ESZ, which is a multiple of 16
             auto buf_of = [&](int slot) { return reinterpret_cast<const IO *>(smem_raw + A.row_off + (size_t)(g * NB + slot) * A.row_stride); };
-            auto row_of = [&](int k) { return (k & 1) ? T1 - (k >> 1) : (k >> 1); };   // rows alternate: top, bottom, top, ...
+            auto row_of = [&](int k) {
+                if constexpr (MODE == 0) { if (seq) return T1 - k; }
+                return (k & 1) ? T1 - (k >> 1) : (k >> 1);   // rows alternate: top, bottom, top, ...
+            };
             auto issue = [&](int k, int slot) {
                 if (lane == 0) {
                     const uint32_t bar = (uint32_t)__cvta_generic_to_shared(&s_bar[g * NB + slot]);
@@ -536,6 +568,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
                 int u = c - k * Un;
                 if (u < 0) { --k; u += Un; } else if (u >= Un) { ++k; u -= Un; }
                 int t = (k & 1) ? T1 - (k >> 1) : (k >> 1);        // rows alternate: top, bottom, top, ...
+                if constexpr (MODE == 0) { if (seq) t = T1 - k; }
                 if (!in) { t = 0; u = 0; }
                 tt[g] = in ? t : -1;
                 uu[g] = u;
@@ -612,7 +645,9 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
         const uint32_t out_a = (uint32_t)__cvta_generic_to_shared(beta ? BE : AL);
         GatherWait gwait;
         gwait.flag = s_flag; gwait.Un = Un; gwait.Tn = Tn; gwait.ready = 0; gwait.lane = lane; gwait.gwn = use_tma ? A.gwn : 0; gwait.m_ok = -1;
+        gwait.seq = seq;
         stamp(3);
+        if (seq && !beta) gwait.all();                  // the top rows, which alpha starts from, arrive last
         const uint32_t scr = (uint32_t)__cvta_generic_to_shared(&s_scratch[lw][0]);
         if (beta) sweep_diag<KIND, C, false>(wb_a, wl_a, out_a, Wd, ndiag, lane, first_col, pre, Tn, gwait, scr, &s_prog[1], 0);
         else sweep_diag<KIND, C, true>(wb_a, wl_a, out_a, Wd, ndiag, lane, first_col, pre, Tn, gwait, scr, &s_prog[0], T1 + Wd);
@@ -653,7 +688,115 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
         }
         stamp(6);
     }
-    if (MODE == 0) {
+    // one cell's (blank, label) gradient: the same operation order as core.cu:284-294 and :319-331
+    auto grad_of = [&](int t, int u, const float &b00, const float &sc, const bool &has_lam) -> float2 {
+        const int ib = idxB(t, u);
+        const float a0v = AL[idxA(t, u)];
+        float gb = 0.0f, gl = 0.0f;
+        const bool last_t = (t == T1), last_u = (u == U1);
+        if (!(last_t && !last_u)) {
+            float a = a0v;
+            if (!last_t) a += BE[ib - Wd];              // beta[t+1,u]: one diagonal earlier, same column
+            a = expf(a + WBb[ib] - b00);
+            gb = -a;
+        }
+        if (!last_u) {
+            float a = a0v + BE[ib - Wd - 1];            // beta[t,u+1]: previous diagonal, previous primed column
+            a = expf(a + WLb[ib] - b00);
+            // (1. + lambda) * a is a double multiply in the reference (core.cu:327-329); with lambda == 0
+            // it returns a unchanged, so the fp64 round trip is skipped without changing a bit
+            if (has_lam) a = (float)((1.0 + (double)A.lam) * (double)a);
+            gl = -a;
+        }
+        if (A.scale) { gb *= sc; gl *= sc; }
+        return make_float2(gb, gl);
+    };
+    if (MODE == 0 && A.compose) {
+        if constexpr (MODE == 0) if (lw >= 2) {   // (constexpr: MODE 1 does not carry this even as dead code)
+            // ---- composed emit.  The gather ran bottom row up, so beta[0,0] is known a few dozen steps after the last
+            // (top) row arrived, while alpha, which starts from that row, still has most of its diagonals to go.  The
+            // free warps write the CTA's slab [f0,f1) behind alpha in pieces -- one lattice row when rows are whole
+            // 16-byte vectors, else slot-sized ranges of the aligned interior [a0,a1).  A warp composes its piece in
+            // its own shared-memory slot (a TMA row buffer, free once the gather is done -- and it is, once beta is --
+            // or else a slice of the zero buffer's region) and copies it out with 16-byte streaming stores.  The staged
+            // planes are only read here: alpha's operand prefetch still reads them.  The values are stored before the
+            // mismatch guard is known (it needs alpha[T1,U1]); a guard that fires zeroes the slab in phase 2.
+            // (TMA bulk stores of the slots instead kept the LSU free for alpha, but on an H100 the SM's copy engine
+            // wrote the 4.5 KB pieces of cfg 2 at only ~2.5 TB/s over all SMs: the emit ended no earlier than the one
+            // it replaces.  The streaming stores slow alpha's step by ~40 %, which it has the slack for.)
+            constexpr int VEC = 16 / ESZ;
+            const int i = lw - 2;
+            const int nslot = use_tma ? A.nbuf : GW;
+            if (i < nslot) {
+                IO *const g = static_cast<IO *>(A.grads);
+                const int64_t f0 = (slab + (int64_t)t0 * U) * V, f1 = (slab + (int64_t)t1 * U) * V;
+                const bool vec = ((reinterpret_cast<uintptr_t>(g) & 15u) == 0);
+                const int64_t a0 = vec ? min(f1, (f0 + VEC - 1) & ~(int64_t)(VEC - 1)) : f1;
+                const int64_t a1 = vec ? max(a0, f1 & ~(int64_t)(VEC - 1)) : f1;
+                const int sbytes = use_tma ? A.row_stride : (kZeroBytes / GW) & ~15;
+                IO *const buf = reinterpret_cast<IO *>(smem_raw + (use_tma ? A.row_off : A.zoff) + (size_t)i * sbytes);
+                const int rowE = U * V;
+                // whole rows: every piece has its non-zeros at the same offsets, so the slot is zeroed only once
+                const bool whole = vec && rowE % VEC == 0 && rowE * ESZ <= sbytes;
+                const int PE = whole ? rowE : sbytes / 16 * VEC;
+                const int npieces = (int)((a1 - a0 + PE - 1) / PE);
+                const float sc = A.scale ? A.scale[n] : 1.0f;
+                const bool has_lam = (A.lam != 0.0f);
+                float b00 = 0.0f;
+                if (ok) {
+                    while (flag_acquire(&s_prog[1]) != 0x3fffffff) __nanosleep(128);   // beta done
+                    b00 = dead_b00(BE[idxB(0, 0)]);     // dead lattice: NaN
+                    stamp(10);
+                }
+                int pa = 0, k = 0;
+                for (;; ++k) {
+                    int p = 0;
+                    if (lane == 0) p = atomicAdd(&s_next, 1);
+                    p = __shfl_sync(0xffffffffu, p, 0);
+                    if (p >= npieces) break;
+                    const int64_t pb = a0 + (int64_t)p * PE, pe = min(a1, pb + PE);
+                    const int ne = (int)(pe - pb);
+                    uint32_t c_lo, c_hi, r;
+                    A.divV.divmod((uint32_t)(pb - f0), c_lo, r);
+                    A.divV.divmod((uint32_t)(pe - 1 - f0), c_hi, r);
+                    if (ok) {
+                        // alpha has passed the piece's last row, with the chase's margin (patch order below)
+                        uint32_t tq;
+                        A.divU.divmod(c_hi, tq, r);
+                        const int e = min(t0 + (int)tq, T1) + U1 + 2;
+                        while (pa < e) { pa = flag_acquire(&s_prog[0]); if (pa < e) __nanosleep(100); }
+                    }
+                    if (!whole || k == 0) {
+                        for (int j = lane; j < ne / VEC; j += 32) reinterpret_cast<float4 *>(buf)[j] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+                        __syncwarp();
+                    }
+                    if (ok) {
+                        // the blank's and the label's element of every cell the piece touches; padding rows write zeros
+                        // there (whole rows: over the previous piece's values), padding columns have none
+                        for (uint32_t c = c_lo + lane; c <= c_hi; c += 32) {
+                            uint32_t tq, u;
+                            A.divU.divmod(c, tq, u);
+                            const int t = t0 + (int)tq;
+                            if ((int)u >= Un) continue;
+                            const int lab = ((int)u < U1) ? s_lab[u] : -1;
+                            const float2 gq = (t < Tn) ? grad_of(t, (int)u, b00, sc, has_lam) : make_float2(0.0f, 0.0f);
+                            const int at = (int)(f0 + (int64_t)c * V - pb);   // the cell's column 0, relative to the piece
+                            // label == blank: the label gradient wins (core.cu:383-390)
+                            if (lab != A.blank && at + A.blank >= 0 && at + A.blank < ne) buf[at + A.blank] = io_from_float<IO>(gq.x);
+                            if (lab >= 0 && at + lab >= 0 && at + lab < ne) buf[at + lab] = io_from_float<IO>(gq.y);
+                        }
+                    }
+                    __syncwarp();
+                    for (int j = lane; j < ne / VEC; j += 32)
+                        st_cs_v4(reinterpret_cast<float *>(g + pb) + 4 * j, reinterpret_cast<const float4 *>(buf)[j]);
+                    __syncwarp();                       // the slot is read out before the next piece is composed in it
+                    if (p == 0) stamp(11);
+                }
+                if (k > 0) stamp(12);
+                if (npieces == 0 && i == 0) stamp(11);
+            }
+        }
+    } else if (MODE == 0) {
         // ---- chase: while the zeros drain and the two wavefronts run their last diagonals, the 14 free warps follow
         // them from the MIDDLE anti-diagonal outwards (alpha has passed it from above, beta from below: the cells of
         // diagonal e are final once alpha is past e+1 and beta past e+1 from the other side) and replace each staged
@@ -691,11 +834,11 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
             }
             stamp(8);
         }
-        if (!A.compose && lane == 0) {
+        if (lane == 0) {
             asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // the zeros have landed ...
             asm volatile("fence.proxy.async;" ::: "memory");            // ... before anyone patches them
         }
-        if (!A.compose) stamp(9);
+        stamp(9);
     }
     __syncthreads();
 
@@ -709,8 +852,9 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
                 // (The layout is re-read from the argument: a flag kept live since phase 0 costs the recurrence a register.)
                 b = -dead_cost(Tn, Un, MODE == 1 && A.mem_pref != nullptr);
             } else if (A.guard) {
-                // alpha-side ll = alpha[T-1,U-1] + blank[T-1,U-1] (core.cu:346); MODE 0: the chase has left exactly this sum
-                float a = (MODE == 0 && t0 <= T1 && T1 < t1) ? WBb[idxB(T1, U1)] : AL[idxA(T1, U1)] + WBb[idxB(T1, U1)];
+                // alpha-side ll = alpha[T-1,U-1] + blank[T-1,U-1] (core.cu:346); patch order: the chase has left exactly
+                // this sum
+                float a = (MODE == 0 && !A.compose && t0 <= T1 && T1 < t1) ? WBb[idxB(T1, U1)] : AL[idxA(T1, U1)] + WBb[idxB(T1, U1)];
                 if (n == A.poison_n) a += A.poison_delta;              // test hook, see rnnt_b200_debug_guard_poison
                 const float ratio = fabsf(a - b) / fabsf(fmaxf(a, b));
                 if (ratio > 0.001f) {
@@ -726,117 +870,44 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(FusedArgs A) {
     }
     if (A.loss_sum && slice == 0 && warp == 0) loss_reduce_last(A.costs, A.scale, A.N, A.loss_sum, A.sync_counter);
     __syncthreads();
-    stamp(10);
+    if (!(MODE == 0 && A.compose)) stamp(10);       // (the composed emit stamps beta[0,0] known)
     const bool live = ok && !s_bad;
     const float b00 = live ? dead_b00(BE[idxB(0, 0)]) : 0.0f;   // dead lattice: NaN, in every emit order and MODE 1
     const float sc = A.scale ? A.scale[n] : 1.0f;
     const bool has_lam = (A.lam != 0.0f);
-    auto cell_grad = [&](int t, int u) -> float2 {
-        // same operation order as core.cu:284-294 and :319-331
-        const int ib = idxB(t, u);
-        const float a0v = AL[idxA(t, u)];
-        float gb = 0.0f, gl = 0.0f;
-        const bool last_t = (t == T1), last_u = (u == U1);
-        if (!(last_t && !last_u)) {
-            float a = a0v;
-            if (!last_t) a += BE[ib - Wd];              // beta[t+1,u]: one diagonal earlier, same column
-            a = expf(a + WBb[ib] - b00);
-            gb = -a;
-        }
-        if (!last_u) {
-            float a = a0v + BE[ib - Wd - 1];            // beta[t,u+1]: previous diagonal, previous primed column
-            a = expf(a + WLb[ib] - b00);
-            // (1. + lambda) * a is a double multiply in the reference (core.cu:327-329); with lambda == 0
-            // it returns a unchanged, so the fp64 round trip is skipped without changing a bit
-            if (has_lam) a = (float)((1.0 + (double)A.lam) * (double)a);
-            gl = -a;
-        }
-        if (A.scale) { gb *= sc; gl *= sc; }
-        return make_float2(gb, gl);
-    };
+    auto cell_grad = [&](int t, int u) -> float2 { return grad_of(t, u, b00, sc, has_lam); };
     if (MODE == 0 && A.compose) {
-        // Composed emit: every element of rows [t0,t1) is written once, as whole 16-byte vectors.
-        // Pass 1 turns the chase's x = alpha + beta + lp of the rows this CTA emits into the final values in place, with
-        // the patch's arithmetic (expf(x - beta00), FastEmit, scale): WBb = gradient at the blank's column, +0 where the
-        // reference writes none (the last row's inner cells, or label == blank: there the label gradient wins);
-        // WLb = gradient at the label's column.
-        const int r0 = t0, r1 = min(t1, Tn);
-        if (live) {
-            // thread i takes cells i, i + 512, ... of the rows (row-major), K at a time: all loads first, so that one
-            // thread's K cells overlap their shared-memory and MUFU latencies (one CTA per SM leaves few warps to hide them)
-            constexpr int K = 4;
-            const double lam1 = 1.0 + (double)A.lam;
-            const int dq = kFusedThreads / Un, dr = kFusedThreads - dq * Un;   // one step: dq rows down, dr columns right
-            int t = r0 + tid / Un, u = tid % Un;
-            while (t < r1) {
-                int ib[K];
-                bool in[K], go_b[K], go_l[K];
-                float xb[K], xl[K];
-#pragma unroll
-                for (int k = 0; k < K; ++k) {
-                    in[k] = t < r1;
-                    const bool last_t = (t == T1), last_u = (u == U1);
-                    ib[k] = idxB(t, u);
-                    go_b[k] = in[k] && !(last_t && !last_u) && (last_u || s_lab[u] != A.blank);
-                    go_l[k] = in[k] && !last_u;
-                    if (in[k]) { xb[k] = WBb[ib[k]]; xl[k] = WLb[ib[k]]; }
-                    u += dr; t += dq;
-                    if (u >= Un) { u -= Un; ++t; }
-                }
-#pragma unroll
-                for (int k = 0; k < K; ++k) {
-                    float gb = 0.0f, gl = 0.0f;
-                    if (go_b[k]) {
-                        gb = -expf(xb[k] - b00);
-                        if (A.scale) gb *= sc;
-                    }
-                    if (go_l[k]) {
-                        float a = expf(xl[k] - b00);
-                        if (has_lam) a = (float)(lam1 * (double)a);   // see the patch below
-                        gl = -a;
-                        if (A.scale) gl *= sc;
-                    }
-                    if (in[k]) { WBb[ib[k]] = gb; WLb[ib[k]] = gl; }
-                }
-            }
-        }
-        __syncthreads();
-        stamp(11);
-        // Pass 2: all 16 warps sweep the slab's elements [f0,f1) with streaming stores, each vector composed from the
-        // staged values of the cells it covers; padding rows / columns and a dead lattice (invalid lengths, guard
-        // fired) are zeros.  Unaligned head and tail: scalar stores.
+        // Composed emit, the rest: the aligned interior [a0,a1) of the slab is stored (above); the unaligned head and
+        // tail (< 16 bytes each, or everything if the gradient is not 16-byte aligned) are scalar stores.  A fired
+        // mismatch guard replaces everything by zeros (the barriers since order them after the speculative values).
         constexpr int VEC = 16 / ESZ;
         IO *const g = static_cast<IO *>(A.grads);
         const int64_t f0 = (slab + (int64_t)t0 * U) * V, f1 = (slab + (int64_t)t1 * U) * V;
         const bool vec = ((reinterpret_cast<uintptr_t>(g) & 15u) == 0);
         const int64_t a0 = vec ? min(f1, (f0 + VEC - 1) & ~(int64_t)(VEC - 1)) : f1;
         const int64_t a1 = vec ? max(a0, f1 & ~(int64_t)(VEC - 1)) : f1;
-        auto row_at = [&](int c) -> GradRow {          // c: cell of rows [t0,t1), row-major
-            uint32_t tt, u;
-            A.divU.divmod((uint32_t)c, tt, u);
-            const int t = t0 + (int)tt;
-            GradRow r{make_float2(0.0f, 0.0f), -1};
-            if (live && t < Tn && (int)u < Un) {
-                const int ib = idxB(t, (int)u);
-                r.g = make_float2(WBb[ib], WLb[ib]);
-                if ((int)u < U1) r.lab = s_lab[u];
-            }
-            return r;
-        };
-        auto scalar = [&](int64_t f) {
-            uint32_t c, v;
-            A.divV.divmod((uint32_t)(f - f0), c, v);
-            st_one(g + f, grad_row_elem(row_at((int)c), A.blank, (int)v, false));
-        };
-        for (int64_t f = f0 + tid; f < a0; f += kFusedThreads) scalar(f);
-        for (int64_t f = a1 + tid; f < f1; f += kFusedThreads) scalar(f);
-        const bool rows_whole = (V & (VEC - 1)) == 0;
-        for (int64_t f = a0 + VEC * tid; f < a1; f += VEC * kFusedThreads) {
-            uint32_t c, v;
-            A.divV.divmod((uint32_t)(f - f0), c, v);
-            float e[VEC];
-            compose_vec<VEC>(e, (int)c, (int)v, V, A.blank, false, rows_whole, row_at);
-            st_vec(g + f, e);
+        if (ok && !live) {
+            for (int64_t f = f0 + tid; f < a0; f += kFusedThreads) st_one(g + f, 0.0f);
+            for (int64_t f = a1 + tid; f < f1; f += kFusedThreads) st_one(g + f, 0.0f);
+            float z[VEC];
+#pragma unroll
+            for (int k = 0; k < VEC; ++k) z[k] = 0.0f;
+            for (int64_t f = a0 + VEC * tid; f < a1; f += VEC * kFusedThreads) st_vec(g + f, z);
+        } else {
+            auto scalar = [&](int64_t f) {
+                uint32_t c, v, tt, u;
+                A.divV.divmod((uint32_t)(f - f0), c, v);
+                A.divU.divmod(c, tt, u);
+                const int t = t0 + (int)tt;
+                GradRow r{make_float2(0.0f, 0.0f), -1};
+                if (live && t < Tn && (int)u < Un) {
+                    r.g = cell_grad(t, (int)u);
+                    if ((int)u < U1) r.lab = s_lab[u];
+                }
+                st_one(g + f, grad_row_elem(r, A.blank, (int)v, false));
+            };
+            for (int64_t f = f0 + tid; f < a0; f += kFusedThreads) scalar(f);
+            for (int64_t f = a1 + tid; f < f1; f += kFusedThreads) scalar(f);
         }
     } else if (MODE == 0) {
         if (live) {
@@ -1036,6 +1107,7 @@ cudaError_t launch_fused(cudaStream_t s, const FusedPlan &plan, const FusedCall 
             smem = base + (size_t)a.nbuf * stride;
         }
     }
+    if (a.nbuf == 0) smem = plan.smem;                  // without row buffers the composed emit stages in the zero buffer
     a.trace = g_fused_trace;
     { const GuardPoison gp = guard_poison(); a.poison_n = gp.n; a.poison_delta = gp.delta; }
     const bool dense = grads != nullptr;
