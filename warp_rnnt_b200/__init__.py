@@ -281,6 +281,105 @@ def rnnt_loss_pruned(logits, labels, frames_lengths, labels_lengths, ranges, ave
     return _reduce(costs, frames_lengths, average_frames, reduction)
 
 
+class RNNTLossTDT(torch.autograd.Function):
+    """The Token-and-Duration Transducer loss from (N,T,U,V+D) joint logits.  Forward reads the logits once (two
+    normalisers per cell, the 2 + D log-probs the recurrence needs), runs alpha and beta on the lattice and keeps lse
+    (N,T,U,2) and the per-cell posteriors (N,T,U,2+D); backward reads the logits again and writes d loss / d logits, of
+    their dtype."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, frames_lengths, labels_lengths, durations, sigma=0.0, blank=0):
+        need = ctx.needs_input_grad[0]
+        costs, lse, pg = _C.rnnt_tdt_forward(logits, labels, frames_lengths, labels_lengths, list(durations), sigma,
+                                             blank, need)
+        if need:
+            ctx.save_for_backward(logits, lse, pg, labels)
+            ctx.durations = list(durations)
+            ctx.blank = blank
+        return costs
+
+    @staticmethod
+    def backward(ctx, grads_output):
+        logits, lse, pg, labels = ctx.saved_tensors
+        go = grads_output.contiguous().to(torch.float32)
+        g = _C.rnnt_tdt_backward(logits, lse, pg, labels, ctx.durations, go, ctx.blank)
+        return g, None, None, None, None, None, None
+
+
+def _tdt_durations(durations):
+    if not isinstance(durations, (list, tuple)) or not durations or \
+            any(isinstance(d, bool) or not isinstance(d, int) for d in durations):
+        raise ValueError("rnnt_loss_tdt: durations must be a non-empty list or tuple of ints, got %r" % (durations,))
+    if any(d < 0 or d > 16 for d in durations) or any(b <= a for a, b in zip(durations, durations[1:])) \
+            or max(durations) == 0:
+        raise ValueError("rnnt_loss_tdt: durations must be strictly increasing, in [0, 16], with at least one > 0, "
+                         "got %r" % (durations,))
+    return tuple(durations)
+
+
+def rnnt_loss_tdt(logits, labels, frames_lengths, labels_lengths, durations, sigma=0.0, average_frames=False,
+                  reduction="none", blank=0):
+    """Token-and-Duration Transducer loss (TDT, Xu et al. 2023, arXiv:2304.06795), the loss of NeMo's Parakeet-TDT
+    models, from the joint network's logits.  Follows NeMo's definition (``TDTLossPytorch``: the same alpha recursion
+    and terminal sum); not tested against NeMo.
+
+    Args:
+        logits: (N, T, U, V + D) float32 or bfloat16, NeMo's layout: V token logits (blank included), then D duration
+            logits, D = len(durations).  U = labels.size(1) + 1.  Compact (ragged) input is not offered.
+        labels: (N, U-1) int32; frames_lengths, labels_lengths: (N,) int32, as for ``rnnt_loss_from_logits``.
+        durations: list or tuple of ints, strictly increasing, in [0, 16], at least one > 0 (else ValueError), e.g.
+            [0, 1, 2, 3, 4].  Host values: they reach the kernels as launch parameters.
+        sigma: NeMo's logit under-normalisation, a finite float >= 0 (else ValueError).
+        average_frames, reduction: as in ``rnnt_loss_from_logits``.
+        blank: in [0, V).
+
+    Lattice n has Tn = frames_lengths[n] frames and Un = labels_lengths[n] + 1 columns.  Cell (t, u) has
+    lt = log_softmax(logits[n,t,u,:V]) - sigma, the token log-probs, and ld = log_softmax(logits[n,t,u,V:]), the
+    duration log-probs.  Edges out of cell (t, u), with t < Tn and u < Un:
+
+    * blank edge, for each j with d = durations[j] > 0, weight lt[blank] + ld[j]: to (t + d, u) if t + d < Tn; terminal
+      if u = Un - 1 and t + d = Tn; otherwise no edge.
+    * label edge, for u < Un - 1 and each j (d = 0 included), weight lt[labels[n,u]] + ld[j]: to (t + d, u + 1) if
+      t + d < Tn; otherwise no edge.  A path therefore always ends with a blank.
+
+    P is the sum, over paths from (0, 0) to a terminal edge, of exp(sum of edge weights); cost[n] = -log P.  Edge
+    posterior gamma_e = exp(alpha(src) + w_e + beta(dst) - log P), with beta = 0 after a terminal edge.  Per cell, Pb is
+    the sum of gamma over its blank edges, Pl over its label edges, Pd[j] over its edges of duration durations[j], and
+    occ = Pb + Pl = sum Pd.  The gradient of the cost w.r.t. the logits, times grad_output[n] (and the reduction's
+    weights), is occ * softmax_tok[v] - Pb [v = blank] - Pl [v = label] on the tokens and occ * softmax_dur[j] - Pd[j]
+    on the durations; a label equal to blank gets both terms, as autograd gives.
+
+    Degenerate input, without host synchronisation:
+
+    * padding rows (t >= Tn or u >= Un) are never read, so a NaN there changes nothing; their gradient is exactly 0;
+    * invalid lengths (Tn outside [1, T] or labels_lengths[n] outside [0, U-1]) or a live label outside [0, V): cost
+      NaN, all-zero gradient rows;
+    * no path of finite log-probability, structurally (e.g. Tn < min(d > 0)) or through -inf token or duration logits:
+      cost +inf, all-zero gradient rows;
+    * a NaN or +inf in a live row, or a live row whose token or duration logits are all -inf: cost NaN and NaN gradients
+      on that lattice's live rows; every other lattice of the batch is bit-identical to a batch without it.
+
+    Costs are float32; ``logits.grad`` has the logits' dtype.  bfloat16: costs equal those of the float32 logits with
+    the same values bit for bit, and the gradient is their float32 gradient rounded once.  Deterministic (no atomics),
+    no host synchronisation: a step can be captured in a CUDA graph.  ``set_lse_mode`` does not apply.
+
+    Not offered: ``fastemit_lambda``, NeMo's ``omega`` mixing with the regular transducer loss, multi-blank, and a TDT
+    variant of ``rnnt_align``."""
+    assert average_frames is None or isinstance(average_frames, bool)
+    assert reduction is None or reduction in ("none", "mean", "sum")
+    assert not labels.requires_grad and not frames_lengths.requires_grad and not labels_lengths.requires_grad
+    durations = _tdt_durations(durations)
+    if isinstance(sigma, bool) or not isinstance(sigma, (int, float)) or not math.isfinite(sigma) or sigma < 0:
+        raise ValueError("rnnt_loss_tdt: sigma must be a finite number >= 0, got %r" % (sigma,))
+    if logits.dim() != 4 or logits.size(-1) <= len(durations):
+        raise ValueError("rnnt_loss_tdt: logits must be (N, T, U, V + D) with V >= 1, D = len(durations) = %d, got "
+                         "shape %s" % (len(durations), tuple(logits.shape)))
+    if isinstance(blank, bool) or not isinstance(blank, int) or not 0 <= blank < logits.size(-1) - len(durations):
+        raise ValueError("rnnt_loss_tdt: blank must be an int in [0, V), got %r" % (blank,))
+    costs = RNNTLossTDT.apply(logits, labels, frames_lengths, labels_lengths, durations, float(sigma), blank)
+    return _reduce(costs, frames_lengths, average_frames, reduction)
+
+
 class RNNTLossSimple(torch.autograd.Function):
     """The simple loss of the pruned recipe: the transducer loss of the joint ``am[n,t] + lm[n,u]``, whose normaliser is
     a (T,V) x (V,U) product per lattice, so no (N,T,U,V) tensor is formed.  Forward keeps the normaliser (N,T,U), the
@@ -572,6 +671,6 @@ def rnnt_align(log_probs, labels, frames_lengths, labels_lengths, blank=0, compa
 
 
 __all__ = ["rnnt_loss", "rnnt_align", "rnnt_loss_from_logits", "rnnt_loss_pruned", "RNNTLossPruned",
-           "rnnt_loss_simple", "RNNTLossSimple", "joint_pack",
+           "rnnt_loss_simple", "RNNTLossSimple", "rnnt_loss_tdt", "RNNTLossTDT", "joint_pack",
            "JointPack", "RNNTLossFromLogits", "RNNTLossFromLogitsCompact", "RNNTLoss", "RNNTLossGather", "RNNTLossEager",
            "RNNTLossCompact", "compact_hints", "set_lse_mode", "core", "_C", "__version__"]

@@ -598,6 +598,44 @@ static int logits_compact_backward_any(void *stream, const void *logits, const f
     return RNNT_STATUS_SUCCESS;
 }
 
+// TDT: its own entry points (a cell carries 2 + D values, not the pair run_loss drives).  durations: strictly
+// increasing, in [0, 16], at least one > 0.
+static bool tdt_durations(const int *durations, int D, TdtDurations *out) {
+    if (!durations || D < 1 || D > kTdtMaxD) return false;
+    *out = {};
+    out->D = D;
+    for (int j = 0; j < D; ++j) {
+        const int d = durations[j];
+        if (d < 0 || d > 16 || (j > 0 && d <= durations[j - 1])) return false;
+        out->d[j] = d;
+    }
+    out->dmax = durations[D - 1];
+    return out->dmax > 0;
+}
+static bool tdt_args_ok(int N, int T, int U, int V, int D, int blank, int elem_bytes, const void *logits) {
+    return (elem_bytes == 4 || elem_bytes == 2) && !(reinterpret_cast<uintptr_t>(logits) & (uintptr_t)(elem_bytes - 1)) &&
+           N >= 0 && T >= 1 && U >= 1 && V >= 1 && (int64_t)V + D < ((int64_t)1 << 22) &&
+           (int64_t)N * T * U < ((int64_t)1 << 31) && blank >= 0 && blank < V;
+}
+struct TdtWorkspace { float *lp, *alpha, *beta, *ll; int *status; size_t bytes; };
+static TdtWorkspace carve_tdt(void *base, int N, int T, int U, int D) {
+    TdtWorkspace w;
+    size_t off = 0;
+    auto take = [&](size_t bytes) {
+        void *p = base ? (void *)((char *)base + off) : nullptr;
+        off += align_up(bytes, 256);
+        return p;
+    };
+    const size_t c = (size_t)max(N, 0) * (size_t)max(T, 0) * (size_t)max(U, 0), n = (size_t)max(N, 0);
+    w.lp = (float *)take(c * (size_t)(2 + max(D, 0)) * sizeof(float));
+    w.alpha = (float *)take(c * sizeof(float));
+    w.beta = (float *)take(c * sizeof(float));
+    w.ll = (float *)take(n * sizeof(float));
+    w.status = (int *)take(n * sizeof(int));
+    w.bytes = off;
+    return w;
+}
+
 extern "C" {
 
 const char *rnnt_b200_version(void) { return "0.1.0 (sm_90a)"; }
@@ -827,6 +865,52 @@ int rnnt_b200_logits_pruned_backward(void *stream, const void *logits, const flo
                                          labels, ranges, grad_out, out, N, T, S, U, V, blank, elem_bytes == 2),
              RNNT_STATUS_GRADS_BLANK_FAILED);
     return RNNT_STATUS_SUCCESS;
+}
+
+size_t rnnt_b200_tdt_workspace_bytes(int N, int T, int U, int num_durations) {
+    return carve_tdt(nullptr, N, T, U, num_durations).bytes;
+}
+
+int rnnt_b200_tdt_forward(void *stream, void *workspace, size_t workspace_bytes, const void *logits, const int *labels,
+                          const int *xn, const int *yn, const int *durations, int num_durations, float sigma,
+                          float *costs, float *lse, float *grads, int N, int T, int U, int V, int blank,
+                          int elem_bytes) {
+    TdtDurations dur;
+    if (!tdt_durations(durations, num_durations, &dur) || !tdt_args_ok(N, T, U, V, num_durations, blank, elem_bytes, logits) ||
+        !std::isfinite(sigma) || sigma < 0.0f || !costs || !lse || !pairs_aligned(lse) ||
+        !workspace_aligned16(workspace))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    if (!workspace || workspace_bytes < rnnt_b200_tdt_workspace_bytes(N, T, U, num_durations))
+        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    const TdtWorkspace w = carve_tdt(workspace, N, T, U, num_durations);
+    TdtFwd c = {};
+    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = costs;
+    c.lse = reinterpret_cast<float2 *>(lse); c.pg = grads;
+    c.lp = w.lp; c.alpha = w.alpha; c.beta = w.beta; c.ll = w.ll; c.status = w.status;
+    c.N = N; c.T = T; c.U = U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur; c.io_bf16 = elem_bytes == 2;
+    RNNT_TRY(launch_tdt_forward((cudaStream_t)stream, c), RNNT_STATUS_WARP_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+int rnnt_b200_tdt_backward(void *stream, const void *logits, const float *lse, const float *grads, const int *labels,
+                           const int *durations, int num_durations, const float *grad_out, void *out, int N, int T,
+                           int U, int V, int blank, int elem_bytes) {
+    TdtDurations dur;
+    if (!tdt_durations(durations, num_durations, &dur) || !tdt_args_ok(N, T, U, V, num_durations, blank, elem_bytes, logits) ||
+        (reinterpret_cast<uintptr_t>(out) & (uintptr_t)(elem_bytes - 1)) || !lse || !pairs_aligned(lse) || !grads ||
+        !out)
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    TdtBwd c = {};
+    c.x = logits; c.lse = reinterpret_cast<const float2 *>(lse); c.pg = grads; c.labels = labels; c.grad_out = grad_out;
+    c.out = out; c.N = N; c.T = T; c.U = U; c.V = V; c.D = num_durations; c.blank = blank; c.io_bf16 = elem_bytes == 2;
+    RNNT_TRY(launch_tdt_backward((cudaStream_t)stream, c), RNNT_STATUS_GRADS_BLANK_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+void rnnt_b200_debug_last_tdt_launch(int32_t *out) {
+    if (out) rnnt::tdt_launch_record(out);
 }
 
 size_t rnnt_b200_simple_workspace_bytes(int N, int T, int U) {

@@ -532,6 +532,58 @@ at::Tensor rnnt_logits_pruned_backward(const at::Tensor &xs, const at::Tensor &l
     return out;
 }
 
+// TDT loss from (N,T,U,V+D) logits, float32 or bfloat16, D = durations.size(): (costs (N), lse (N,T,U,2),
+// grads (N,T,U,2+D) or empty), all float32.  No host sync.
+std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_tdt_forward(const at::Tensor &xs, const at::Tensor &ys,
+                                                                const at::Tensor &xn, const at::Tensor &yn,
+                                                                const std::vector<int> &durations, double sigma,
+                                                                int blank, bool want_grads) {
+    check4(xs, ys, xn, yn, true);
+    check_batch4(xs, xn, yn);
+    const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), D = (int64_t)durations.size();
+    check_arg(ys, Dt::I32, xs, {N, U - 1}, "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
+    TORCH_CHECK(D >= 1 && xs.size(3) > D, "xs must have more than len(durations) logits per cell (V + D)");
+    const int64_t V = xs.size(3) - D;
+    check_blank(blank, V);
+    const c10::cuda::CUDAGuard guard(xs.device());
+    const auto f32 = xs.options().dtype(at::kFloat);
+    at::Tensor costs = at::empty({N}, f32);
+    at::Tensor lse = at::empty({N, T, U, 2}, f32);
+    at::Tensor pg = output(want_grads, {N, T, U, 2 + D}, f32);
+    if (N == 0) return std::make_tuple(costs, lse, pg);
+    at::Tensor ws = workspace(xs, rnnt_b200_tdt_workspace_bytes((int)N, (int)T, (int)U, (int)D));
+    check_status(rnnt_b200_tdt_forward(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
+                                       ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(), durations.data(),
+                                       (int)D, (float)sigma, costs.data_ptr<float>(), lse.data_ptr<float>(),
+                                       want_grads ? pg.data_ptr<float>() : nullptr, (int)N, (int)T, (int)U, (int)V,
+                                       blank, xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
+    return std::make_tuple(costs, lse, pg);
+}
+
+// d loss / d TDT logits (N,T,U,V+D), of the dtype of xs
+at::Tensor rnnt_tdt_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &grads, const at::Tensor &ys,
+                             const std::vector<int> &durations, const at::Tensor &grad_out, int blank) {
+    check_arg(xs, Dt::F32orBF16, xs, {kAny, kAny, kAny, kAny},
+              "xs must be a contiguous CUDA Float tensor of shape (N, T, U, V+D)");
+    const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), D = (int64_t)durations.size();
+    TORCH_CHECK(D >= 1 && xs.size(3) > D, "xs must have more than len(durations) logits per cell (V + D)");
+    const int64_t V = xs.size(3) - D;
+    check_arg(lse, Dt::F32, xs, {N, T, U, 2}, "lse must be a contiguous Float tensor of shape (N, T, U, 2) on the device of xs");
+    check_arg(grads, Dt::F32, xs, {N, T, U, 2 + D},
+              "grads must be a contiguous Float tensor of shape (N, T, U, 2+D) on the device of xs");
+    check_arg(ys, Dt::I32, xs, {N, U - 1}, "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
+    check_arg(grad_out, Dt::F32, xs, N, "grad_out must be a contiguous Float tensor of shape (N,)");
+    check_blank(blank, V);
+    const c10::cuda::CUDAGuard guard(xs.device());
+    at::Tensor out = at::empty_like(xs);
+    if (N == 0) return out;
+    check_status(rnnt_b200_tdt_backward(current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(), grads.data_ptr<float>(),
+                                        ys.data_ptr<int>(), durations.data(), (int)D, grad_out.data_ptr<float>(),
+                                        out.data_ptr(), (int)N, (int)T, (int)U, (int)V, blank,
+                                        xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
+    return out;
+}
+
 // am (N,T,V) and lm (N,U,V): dtypes, then contiguity and device, then shapes; then ys, xn and yn
 void check_simple_inputs(const at::Tensor &am, const at::Tensor &lm, const at::Tensor &ys, const at::Tensor &xn,
                          const at::Tensor &yn) {
@@ -779,6 +831,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("want_grads") = true, py::arg("lse_mode") = 0);
     m.def("rnnt_logits_pruned_backward", &rnnt_logits_pruned_backward, py::arg("xs"), py::arg("lse"),
           py::arg("pair_grads"), py::arg("ys"), py::arg("ranges"), py::arg("grad_out"), py::arg("blank") = 0);
+    m.def("rnnt_tdt_forward", &rnnt_tdt_forward, py::arg("xs"), py::arg("ys"), py::arg("xn"), py::arg("yn"),
+          py::arg("durations"), py::arg("sigma") = 0.0, py::arg("blank") = 0, py::arg("want_grads") = true);
+    m.def("rnnt_tdt_backward", &rnnt_tdt_backward, py::arg("xs"), py::arg("lse"), py::arg("grads"), py::arg("ys"),
+          py::arg("durations"), py::arg("grad_out"), py::arg("blank") = 0);
     m.def("rnnt_simple_forward", &rnnt_simple_forward, py::arg("am"), py::arg("lm"), py::arg("ys"), py::arg("xn"),
           py::arg("yn"), py::arg("blank") = 0, py::arg("want_grads") = true, py::arg("prune_range") = 0,
           py::arg("lse_mode") = 0, py::arg("lm_only_scale") = 0.0, py::arg("am_only_scale") = 0.0);

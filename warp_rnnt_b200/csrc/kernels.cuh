@@ -153,6 +153,44 @@ struct FusedCall {
 };
 cudaError_t launch_fused(cudaStream_t s, const FusedPlan &plan, const FusedCall &c);
 
+// tdt.cu -- the Token-and-Duration Transducer loss from (N,T,U,V+D) joint logits (include/rnnt_b200.h)
+constexpr int kTdtMaxD = 17;              // durations are distinct values in [0, 16]
+struct TdtDurations { int d[kTdtMaxD]; int D, dmax; };
+// the launch shape the planner picks (recorded by rnnt_b200_debug_last_tdt_launch)
+struct TdtPlan {
+    int norm_group, norm_lanes;           // normaliser: elements per load (4, 2, 1), lanes per row (8, 32)
+    int kd;                               // recurrence / posterior instantiation: candidate slots (5 or kTdtMaxD)
+    int warps, passes;                    // recurrence: warps per CTA, column passes per diagonal
+    int ring, smem;                       // ring slots in shared memory (0: read back from global), its bytes
+};
+TdtPlan tdt_plan(int U, const TdtDurations &dur, const void *x, int elem_bytes, int V);
+struct TdtFwd {
+    const void *x;                        // logits (N,T,U,V+D), f32 or bf16
+    const int *labels, *xn, *yn;
+    float *costs;
+    float2 *lse;                          // (N,T,U) (lse_tok, lse_dur) out
+    float *pg;                            // (N,T,U,2+D) posteriors out, or null (costs only)
+    float *lp, *alpha, *beta, *ll;        // workspace: (N,T,U,2+D), (N,T,U), (N,T,U), (N)
+    int *status;                          // workspace: (N) lattice class
+    int N, T, U, V, blank;
+    float sigma;
+    TdtDurations dur;
+    int io_bf16;
+};
+cudaError_t launch_tdt_forward(cudaStream_t s, const TdtFwd &c);
+struct TdtBwd {
+    const void *x;                        // logits (N,T,U,V+D)
+    const float2 *lse;
+    const float *pg;                      // (N,T,U,2+D) posteriors of the forward
+    const int *labels;
+    const float *grad_out;                // (N), or null (ones)
+    void *out;                            // (N,T,U,V+D), of the logits' type
+    int N, T, U, V, D, blank;
+    int io_bf16;
+};
+cudaError_t launch_tdt_backward(cudaStream_t s, const TdtBwd &c);
+void tdt_launch_record(int32_t *out);     // copy of the last TDT launch's record (rnntTdtLaunchRecord_t)
+
 // expand.cu -- small helpers of the python-level API
 cudaError_t launch_loss_sum(cudaStream_t s, const float *costs, const float *scale, int N, float *loss_sum);
 cudaError_t launch_rescale(cudaStream_t s, void *grads, const float *grad_out, int grad_out_stride,

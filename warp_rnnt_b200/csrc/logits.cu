@@ -172,41 +172,6 @@ __global__ void __launch_bounds__(kLogitThreads) k_fill_pairs(float4 *__restrict
         reinterpret_cast<float2 *>(pairs2)[cells - 1] = make_float2(kBig, kBig);
 }
 
-// VEC consecutive elements at p (VEC * sizeof(T) bytes, aligned to that) <-> fp32
-template <int VEC>
-__device__ __forceinline__ void ld_logits(const float *p, float (&v)[VEC]) {
-    if constexpr (VEC == 4) {
-        const float4 t4 = __ldg(reinterpret_cast<const float4 *>(p));
-        v[0] = t4.x; v[1] = t4.y; v[2] = t4.z; v[3] = t4.w;
-    } else if constexpr (VEC == 2) {
-        const float2 t2 = __ldg(reinterpret_cast<const float2 *>(p));
-        v[0] = t2.x; v[1] = t2.y;
-    } else {
-        v[0] = __ldg(p);
-    }
-}
-template <int VEC>
-__device__ __forceinline__ void ld_logits(const __nv_bfloat16 *p, float (&v)[VEC]) {
-    if constexpr (VEC == 1) {
-        v[0] = io_load(p);
-    } else {
-        uint32_t w[VEC / 2];                                 // element 2k in the low half of word k
-        if constexpr (VEC == 8) {
-            const uint4 t = __ldg(reinterpret_cast<const uint4 *>(p));
-            w[0] = t.x; w[1] = t.y; w[2] = t.z; w[3] = t.w;
-        } else if constexpr (VEC == 4) {
-            const uint2 t = __ldg(reinterpret_cast<const uint2 *>(p));
-            w[0] = t.x; w[1] = t.y;
-        } else {
-            w[0] = __ldg(reinterpret_cast<const unsigned int *>(p));
-        }
-#pragma unroll
-        for (int k = 0; k < VEC / 2; ++k) {
-            v[2 * k] = __uint_as_float(w[k] << 16);
-            v[2 * k + 1] = __uint_as_float(w[k] & 0xffff0000u);
-        }
-    }
-}
 template <int VEC>
 __device__ __forceinline__ void st_logit_grads(float *p, const float (&e)[VEC]) {
     if constexpr (VEC == 4) st_cs_v4(p, make_float4(e[0], e[1], e[2], e[3]));

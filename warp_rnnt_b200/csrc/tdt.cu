@@ -1,0 +1,506 @@
+// tdt.cu -- the Token-and-Duration Transducer loss (TDT, Xu et al. 2023, arXiv:2304.06795) from joint logits.
+//
+// A TDT joint gives, per lattice cell, V token logits and D duration logits (NeMo's layout: row width W = V + D).  A
+// token emitted with duration d moves the path d frames ahead, so the recurrence looks back up to max(d) frames.  The
+// semantics (edges, classes of degenerate input) are stated in include/rnnt_b200.h.  Three stages, as the from-logits
+// path of logits.cu:
+//
+//   k_tdt_norm   one read of every live row: two online max / sum reductions (tokens, durations) -> lse (N,T,U,2) and
+//                the 2 + D f32 log-probs the recurrence needs, lp (N,T,U,2+D) = (blank - sigma, label - sigma, ld[0..D)),
+//                each clamped below at kBig (a masked -inf becomes the finite sentinel)
+//   k_tdt_recur  one CTA per lattice and direction (grid (N, 2)): alpha (blockIdx.y = 0) and beta (1) along
+//                anti-diagonals s = t + u, threads over columns; the last max(d) + 2 diagonals in a shared-memory ring
+//                (or, when the ring does not fit, read back from the alpha / beta arrays in global memory).  The beta
+//                CTA also classifies the lattice and writes its cost.
+//   k_tdt_post   per cell, the edge posteriors -> (Pb, Pl, Pd[0..D)) (N,T,U,2+D), unscaled
+//   k_tdt_emit   (backward) one read of the logits and one write of d loss / d logits (N,T,U,V+D), every element once
+//
+// Every LSE is one max-then-sum over all candidate terms of a cell.  All candidates are finite (kBig sentinels) or NaN,
+// absent ones are -inf and only ever subtracted from a finite maximum: -inf - -inf is never formed.  No atomics: every
+// value has one writer and a fixed operation order, so results are deterministic.  A bf16 row is read in exactly the
+// f32 row's order (branch and lanes depend on the row width and the element alignment only), so lse, lp, costs and the
+// posteriors are bit for bit those of the widened logits, and the bf16 gradient is the f32 gradient rounded once.
+#include "common.cuh"
+#include "kernels.cuh"
+
+namespace rnnt {
+
+constexpr int kTdtRowThreads = 256;   // k_tdt_norm, k_tdt_post, k_tdt_emit
+constexpr int kTdtMaxThreads = 512;   // k_tdt_recur: at most 16 warps over the columns, then column passes
+
+// lattice classes, written by the beta CTA (status (N) in the workspace)
+enum { kTdtOk = 0, kTdtInvalid = 1, kTdtNan = 2, kTdtDead = 3 };
+
+__device__ __forceinline__ float clamp_big(float v) { return v < kBig ? kBig : v; }   // NaN stays NaN
+
+// online max / sum: the running max m stays -inf while every element seen is -inf; until a finite one arrives the
+// sum subtracts 0 instead (exp(-inf) = 0), so -inf - -inf is never formed.  A NaN makes the sum NaN, +inf too.
+__device__ __forceinline__ void online_add(float &m, float &s, float a) {
+    if (a > m) { s = s * expf(m - a); m = a; }
+    s += expf(a - (m == -INFINITY ? 0.0f : m));
+}
+__device__ __forceinline__ void online_merge(float &m, float &s, float m2, float s2) {
+    const float mm = fmaxf(m, m2);
+    s = (m == mm ? s : s * expf(m - mm)) + (m2 == mm ? s2 : s2 * expf(m2 - mm));
+    m = mm;
+}
+// every element -inf: NaN, as torch.log_softmax gives
+__device__ __forceinline__ float online_lse(float m, float s) { return m == -INFINITY ? NAN : m + logf(s); }
+
+// Normaliser pass.  SUB lanes per row (8 or 32), groups of G elements per load (4: rows of whole groups at group-aligned
+// addresses, 2: the same for pairs, 1: any row); lanes stride over the groups, each lane keeps a token and a duration
+// accumulator (an element goes to the one of its column), then a butterfly merges the lanes.  Lane 0 writes lse and lp.
+// Rows outside the live lattice (padding, or a lattice with invalid lengths) are not read: lse (0, 0), lp untouched.
+template <typename IN, int SUB, int G>
+__global__ void __launch_bounds__(kTdtRowThreads)
+k_tdt_norm(const IN *__restrict__ x, const int *__restrict__ labels, const int *__restrict__ xn,
+           const int *__restrict__ yn, int64_t cells, int T, int U, int V, int D, int blank, float sigma, FastDiv divU,
+           FastDiv divTU, float2 *__restrict__ lse, float *__restrict__ lp) {
+    const int W = V + D, W2 = 2 + D;
+    const int sub = threadIdx.x % SUB;
+    const int64_t per_block = kTdtRowThreads / SUB;
+    for (int64_t base = (int64_t)blockIdx.x * per_block; base < cells; base += (int64_t)gridDim.x * per_block) {
+        const int64_t cell = min(base + threadIdx.x / SUB, cells - 1);   // surplus groups redo the last row
+        uint32_t n, rem, t, u;
+        divTU.divmod((uint32_t)cell, n, rem);
+        divU.divmod(rem, t, u);
+        const int Tn = xn[n], Un = yn[n] + 1;
+        const bool live = Tn >= 1 && Tn <= T && Un >= 1 && Un <= U && (int)t < Tn && (int)u < Un;
+        const IN *row = x + cell * W;
+        float mt = -INFINITY, st = 0.0f, md = -INFINITY, sd = 0.0f;
+        if (live) {
+            for (int q = sub; q < W / G; q += SUB) {
+                float v[G];
+                ld_logits<G>(row + q * G, v);
+#pragma unroll
+                for (int k = 0; k < G; ++k) {
+                    if (q * G + k < V) online_add(mt, st, v[k]);
+                    else online_add(md, sd, v[k]);
+                }
+            }
+        }
+#pragma unroll
+        for (int o = SUB / 2; o > 0; o >>= 1) {
+            const float mt2 = __shfl_xor_sync(0xffffffffu, mt, o), st2 = __shfl_xor_sync(0xffffffffu, st, o);
+            const float md2 = __shfl_xor_sync(0xffffffffu, md, o), sd2 = __shfl_xor_sync(0xffffffffu, sd, o);
+            online_merge(mt, st, mt2, st2);
+            online_merge(md, sd, md2, sd2);
+        }
+        if (sub != 0) continue;
+        if (!live) {
+            lse[cell] = make_float2(0.0f, 0.0f);
+            continue;
+        }
+        const float lt = online_lse(mt, st), ld = online_lse(md, sd);
+        lse[cell] = make_float2(lt, ld);
+        float *o = lp + cell * W2;
+        o[0] = clamp_big((io_load(row + blank) - lt) - sigma);
+        float l = kBig;                                         // the last column has no label edge
+        if ((int)u < Un - 1) {
+            const int lab = labels[(int64_t)n * (U - 1) + u];
+            l = (lab >= 0 && lab < V) ? clamp_big((io_load(row + lab) - lt) - sigma) : NAN;   // bad label: k_tdt_recur
+        }
+        o[1] = l;
+        for (int j = 0; j < D; ++j) o[2 + j] = clamp_big(io_load(row + V + j) - ld);
+    }
+}
+
+struct TdtRec {
+    const float *lp;
+    const int *labels, *xn, *yn;
+    float *alpha, *beta, *ll, *costs;
+    int *status;
+    int T, U, V, D;
+    int ring;                 // ring slots in shared memory (max(d) + 2), or 0: read back from alpha / beta
+    TdtDurations dur;
+};
+
+// max-then-sum LSE over C candidates; absent ones are -inf.  No candidate: kBig (the cell has no edge).
+template <int C>
+__device__ __forceinline__ float lse_cands(const float (&c)[C]) {
+    float m = -INFINITY;
+#pragma unroll
+    for (int k = 0; k < C; ++k) m = fmaxf(m, c[k]);
+    if (m == -INFINITY) return kBig;
+    float s = 0.0f;
+#pragma unroll
+    for (int k = 0; k < C; ++k) s += expf(c[k] - m);          // a NaN candidate makes s NaN (fmaxf skipped it)
+    return m + logf(s);
+}
+
+// alpha (blockIdx.y == 0) or beta (1) of lattice blockIdx.x.  KD >= D: the candidate arrays' compile-time size.
+template <int KD>
+__global__ void __launch_bounds__(kTdtMaxThreads) k_tdt_recur(TdtRec a) {
+    extern __shared__ float ring[];
+    const int n = blockIdx.x;
+    const bool beta_side = blockIdx.y == 1;
+    const int Tn = a.xn[n], Un = a.yn[n] + 1;
+    if (!(Tn >= 1 && Tn <= a.T && Un >= 1 && Un <= a.U)) {
+        if (beta_side && threadIdx.x == 0) {
+            a.status[n] = kTdtInvalid;
+            a.costs[n] = NAN;
+            a.ll[n] = NAN;
+        }
+        return;
+    }
+    const int U = a.U, W2 = 2 + a.D, D = a.D, R = a.ring;
+    const int64_t base = (int64_t)n * a.T * U;
+    float *out = (beta_side ? a.beta : a.alpha) + base;
+    const float *lp = a.lp + base * W2;
+    // the value of cell (t, u) on the diagonal whose ring slot is sl (computed on an earlier step)
+    auto rd = [&](int t, int u, int sl) -> float { return R ? ring[sl * U + u] : out[(int64_t)t * U + u]; };
+    const int S = Tn + Un - 1;
+    bool saw_nan = false;
+    for (int step = 0; step < S; ++step) {
+        const int s = beta_side ? S - 1 - step : step;
+        const int slot = R ? s % R : 0;
+        auto back = [&](int k) { const int q = slot - k; return q < 0 ? q + R : q; };
+        auto fwd = [&](int k) { const int q = slot + k; return q >= R ? q - R : q; };
+        for (int u = max(0, s - Tn + 1) + (int)threadIdx.x; u <= min(s, Un - 1); u += blockDim.x) {
+            const int t = s - u;
+            float c[2 * KD];
+            float v;
+            if (!beta_side) {
+                // pull: blank from (t-d, u) for d > 0, label from (t-d, u-1) for every d; weights at the source cell
+#pragma unroll
+                for (int j = 0; j < KD; ++j) {
+                    c[2 * j] = c[2 * j + 1] = -INFINITY;
+                    if (j < D) {
+                        const int d = a.dur.d[j], tp = t - d;
+                        if (tp >= 0) {
+                            if (d > 0) {
+                                const float *r = lp + ((int64_t)tp * U + u) * W2;
+                                c[2 * j] = (rd(tp, u, back(d)) + r[0]) + r[2 + j];
+                            }
+                            if (u > 0) {
+                                const float *r = lp + ((int64_t)tp * U + u - 1) * W2;
+                                c[2 * j + 1] = (rd(tp, u - 1, back(d + 1)) + r[1]) + r[2 + j];
+                            }
+                        }
+                    }
+                }
+                v = (t == 0 && u == 0) ? 0.0f : lse_cands(c);
+            } else {
+                // push-side view: the cell's own weights, beta of the destinations; a blank to t + d == Tn from the
+                // last column is terminal (beta 0 after it)
+                const float *r = lp + ((int64_t)t * U + u) * W2;
+                const float b = r[0], l = r[1];
+                const bool has_label = u < Un - 1;
+                saw_nan |= (b != b) || (has_label && l != l);
+#pragma unroll
+                for (int j = 0; j < KD; ++j) {
+                    c[2 * j] = c[2 * j + 1] = -INFINITY;
+                    if (j < D) {
+                        const int d = a.dur.d[j], tq = t + d;
+                        const float ld = r[2 + j];
+                        saw_nan |= ld != ld;
+                        if (d > 0) {
+                            if (tq < Tn) c[2 * j] = (b + ld) + rd(tq, u, fwd(d));
+                            else if (tq == Tn && !has_label) c[2 * j] = b + ld;
+                        }
+                        if (has_label && tq < Tn) c[2 * j + 1] = (l + ld) + rd(tq, u + 1, fwd(d + 1));
+                    }
+                }
+                v = lse_cands(c);
+            }
+            if (R) ring[slot * U + u] = v;
+            out[(int64_t)t * U + u] = v;
+        }
+        __syncthreads();
+    }
+    if (!beta_side) return;
+    bool bad = false;
+    for (int u = threadIdx.x; u < Un - 1; u += blockDim.x) {
+        const int lab = a.labels[(int64_t)n * (U - 1) + u];
+        bad |= lab < 0 || lab >= a.V;
+    }
+    bad = __syncthreads_or(bad);
+    saw_nan = __syncthreads_or(saw_nan);
+    if (threadIdx.x == 0) {
+        const float lP = out[0];
+        const int st = bad ? kTdtInvalid : saw_nan ? kTdtNan : lattice_dead(lP) ? kTdtDead : kTdtOk;
+        a.status[n] = st;
+        a.ll[n] = lP;
+        a.costs[n] = st == kTdtOk ? -lP : st == kTdtDead ? INFINITY : NAN;
+    }
+}
+
+// Edge posteriors per cell: (Pb, Pl, Pd[0..D)), one thread per cell.  0 on padding and on lattices with invalid input
+// or no path; NaN on the live cells of a lattice with a NaN (or +inf, or all -inf) live row.
+template <int KD>
+__global__ void __launch_bounds__(kTdtRowThreads)
+k_tdt_post(const float *__restrict__ lp, const float *__restrict__ alpha, const float *__restrict__ beta,
+           const float *__restrict__ ll, const int *__restrict__ status, const int *__restrict__ xn,
+           const int *__restrict__ yn, int64_t cells, int T, int U, int D, TdtDurations dur, FastDiv divU,
+           FastDiv divTU, float *__restrict__ pg) {
+    const int W2 = 2 + D;
+    for (int64_t cell = (int64_t)blockIdx.x * kTdtRowThreads + threadIdx.x; cell < cells;
+         cell += (int64_t)gridDim.x * kTdtRowThreads) {
+        uint32_t n, rem, t, u;
+        divTU.divmod((uint32_t)cell, n, rem);
+        divU.divmod(rem, t, u);
+        float *g = pg + cell * W2;
+        const int Tn = xn[n], Un = yn[n] + 1;
+        const int st = status[n];
+        const bool live = st != kTdtInvalid && (int)t < Tn && (int)u < Un;   // status Invalid covers bad lengths
+        if (!live || st == kTdtDead || st == kTdtNan) {
+            const float z = (live && st == kTdtNan) ? NAN : 0.0f;
+            for (int k = 0; k < W2; ++k) g[k] = z;
+            continue;
+        }
+        const float *r = lp + cell * W2;
+        const float al = alpha[cell], lP = ll[n], b = r[0], l = r[1];
+        const bool has_label = (int)u < Un - 1;
+        float pb = 0.0f, pl = 0.0f;
+#pragma unroll
+        for (int j = 0; j < KD; ++j) {
+            if (j < D) {
+                const int d = dur.d[j], tq = (int)t + d;
+                const float ld = r[2 + j];
+                float gb = 0.0f, gl = 0.0f;
+                if (d > 0) {
+                    if (tq < Tn) gb = expf((((al + b) + ld) + beta[cell + (int64_t)d * U]) - lP);
+                    else if (tq == Tn && !has_label) gb = expf(((al + b) + ld) - lP);
+                }
+                if (has_label && tq < Tn) gl = expf((((al + l) + ld) + beta[cell + (int64_t)d * U + 1]) - lP);
+                pb += gb;
+                pl += gl;
+                g[2 + j] = gb + gl;
+            }
+        }
+        g[0] = pb;
+        g[1] = pl;
+    }
+}
+
+// The row data one gradient element needs.  zero: the row's posteriors are all 0 (padding, no path, or a cell no path
+// visits): the row is written as exact zeros and neither the logits nor lse are read.
+struct TdtRow {
+    const float *pd;
+    float occ, pb, pl, lt, ld, sc;
+    int lab;
+    bool zero;
+};
+__device__ __forceinline__ TdtRow tdt_row(int64_t row, const float2 *lse, const float *pg, const int *labels,
+                                          const float *grad_out, int U, int W2, const FastDiv &divU,
+                                          const FastDiv &divTU) {
+    TdtRow r;
+    r.pd = pg + row * W2;
+    r.pb = r.pd[0];
+    r.pl = r.pd[1];
+    r.zero = r.pb == 0.0f && r.pl == 0.0f;
+    r.occ = r.pb + r.pl;
+    r.lt = r.ld = r.sc = 0.0f;
+    r.lab = -1;
+    if (!r.zero) {
+        const float2 q = lse[row];
+        r.lt = q.x;
+        r.ld = q.y;
+        uint32_t n, rem, t, u;
+        divTU.divmod((uint32_t)row, n, rem);
+        divU.divmod(rem, t, u);
+        r.lab = ((int)u < U - 1) ? labels[(int64_t)n * (U - 1) + u] : -1;
+        r.sc = grad_out ? grad_out[n] : 1.0f;
+    }
+    return r;
+}
+__device__ __forceinline__ float tdt_elem(const TdtRow &r, int v, float xv, int V, int blank) {
+    if (r.zero) return 0.0f;
+    if (v < V) {
+        float sel = (v == blank) ? r.pb : 0.0f;
+        if (v == r.lab) sel += r.pl;
+        return (r.occ * expf(xv - r.lt) - sel) * r.sc;
+    }
+    return (r.occ * expf(xv - r.ld) - r.pd[2 + (v - V)]) * r.sc;
+}
+
+// Gradient emit: the flat (rows, W) output in vectors of VEC elements (16 bytes when `out` is 16-byte aligned, else 1),
+// which may straddle rows; XVEC: the logits are read with the same vectors (x aligned as out), else element by element.
+// Every element is computed the same way whatever VEC, XVEC and the element type; bf16 is rounded once on the store.
+template <typename IO, int VEC, bool XVEC>
+__global__ void __launch_bounds__(kTdtRowThreads)
+k_tdt_emit(const IO *__restrict__ x, const float2 *__restrict__ lse, const float *__restrict__ pg,
+           const int *__restrict__ labels, const float *__restrict__ grad_out, IO *__restrict__ out, int64_t total,
+           int V, int D, int blank, int U, FastDiv divU, FastDiv divTU, int64_t stride_rows, int stride_v) {
+    const int W = V + D, W2 = 2 + D;
+    int64_t f = ((int64_t)blockIdx.x * kTdtRowThreads + threadIdx.x) * VEC;
+    if (f >= total) return;
+    int64_t row = f / W;
+    int v0 = (int)(f - row * W);
+    const int64_t stride = stride_rows * W + stride_v;
+    for (; f < total; f += stride, row += stride_rows, v0 += stride_v) {
+        if (v0 >= W) { v0 -= W; ++row; }
+        float e[VEC];
+        TdtRow r = tdt_row(row, lse, pg, labels, grad_out, U, W2, divU, divTU);
+        if (f + VEC <= total) {
+            float xv[VEC];
+            const bool whole = v0 + VEC <= W;
+            if (XVEC && !(whole && r.zero)) {
+                ld_logits<VEC>(x + f, xv);
+            } else {
+#pragma unroll
+                for (int k = 0; k < VEC; ++k) xv[k] = 0.0f;
+            }
+            int64_t rw = row;
+            int v = v0;
+#pragma unroll
+            for (int k = 0; k < VEC; ++k) {
+                if (v == W) { v = 0; ++rw; r = tdt_row(rw, lse, pg, labels, grad_out, U, W2, divU, divTU); }
+                if (!XVEC && !r.zero) xv[k] = io_load(x + f + k);
+                e[k] = tdt_elem(r, v, xv[k], V, blank);
+                ++v;
+            }
+            if constexpr (VEC == 1) st_one(out + f, e[0]);
+            else st_vec(out + f, e);
+        } else {
+            // the last, partial vector of the tensor
+            int64_t rw = row;
+            int v = v0;
+            for (int64_t i = f; i < total; ++i) {
+                if (v == W) { v = 0; ++rw; r = tdt_row(rw, lse, pg, labels, grad_out, U, W2, divU, divTU); }
+                st_one(out + i, tdt_elem(r, v, r.zero ? 0.0f : io_load(x + i), V, blank));
+                ++v;
+            }
+        }
+    }
+}
+
+// Process-wide, unlike the loss' per-thread record (api.cu): autograd runs the backward on its own device thread, and
+// the record must see the emit of the same call.
+static std::mutex g_tdt_mu;
+static int32_t g_tdt_record[RNNT_TDT_RECORD_LEN];
+static int32_t g_tdt_seq;
+
+static int max_optin_smem(int dev) {
+    static std::atomic<int> cache[kMaxDevices];
+    if (dev < kMaxDevices) { const int c = cache[dev].load(std::memory_order_relaxed); if (c > 0) return c; }
+    int b = 48 << 10;
+    cudaDeviceGetAttribute(&b, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+    if (dev < kMaxDevices) cache[dev].store(b, std::memory_order_relaxed);
+    return b;
+}
+
+void tdt_launch_record(int32_t *out) {
+    std::lock_guard<std::mutex> lock(g_tdt_mu);
+    memcpy(out, g_tdt_record, sizeof(g_tdt_record));
+}
+
+TdtPlan tdt_plan(int U, const TdtDurations &dur, const void *x, int elem_bytes, int V) {
+    TdtPlan p;
+    const int W = V + dur.D;
+    const int eoff = (int)((reinterpret_cast<uintptr_t>(x) / (uintptr_t)elem_bytes) & 3u);   // element alignment
+    p.norm_group = (W % 4 == 0 && eoff == 0) ? 4 : (W % 2 == 0 && (eoff & 1) == 0) ? 2 : 1;
+    p.norm_lanes = W <= 64 ? 8 : 32;
+    p.kd = dur.D <= 5 ? 5 : kTdtMaxD;
+    p.warps = min((U + 31) / 32, kTdtMaxThreads / 32);
+    p.passes = (U + p.warps * 32 - 1) / (p.warps * 32);
+    p.ring = dur.dmax + 2;
+    const int64_t smem = (int64_t)p.ring * U * (int64_t)sizeof(float);
+    if (smem > max_optin_smem(current_device())) p.ring = 0;
+    p.smem = p.ring ? (int)smem : 0;
+    return p;
+}
+
+template <typename IN>
+static cudaError_t tdt_norm_as(cudaStream_t s, const TdtPlan &p, const IN *x, const TdtFwd &c, int64_t cells) {
+    const FastDiv divU((uint32_t)c.U), divTU((uint32_t)(c.T * c.U));
+    const int64_t per_block = kTdtRowThreads / p.norm_lanes;
+    const unsigned grid = (unsigned)min((cells + per_block - 1) / per_block, (int64_t)sm_count(current_device()) * 16);
+#define RNNT_TDT_NORM(SUB, G)                                                                                         \
+    k_tdt_norm<IN, SUB, G><<<grid, kTdtRowThreads, 0, s>>>(x, c.labels, c.xn, c.yn, cells, c.T, c.U, c.V, c.dur.D,     \
+                                                           c.blank, c.sigma, divU, divTU, c.lse, c.lp)
+    if (p.norm_lanes == 8) {
+        if (p.norm_group == 4) RNNT_TDT_NORM(8, 4); else if (p.norm_group == 2) RNNT_TDT_NORM(8, 2); else RNNT_TDT_NORM(8, 1);
+    } else {
+        if (p.norm_group == 4) RNNT_TDT_NORM(32, 4); else if (p.norm_group == 2) RNNT_TDT_NORM(32, 2); else RNNT_TDT_NORM(32, 1);
+    }
+#undef RNNT_TDT_NORM
+    count_launch();
+    return cudaGetLastError();
+}
+
+template <int KD>
+static cudaError_t tdt_recur_post(cudaStream_t s, const TdtPlan &p, const TdtFwd &c, int64_t cells) {
+    static std::atomic<bool> smem_set[kMaxDevices];
+    if (p.smem > (48 << 10)) {
+        const cudaError_t e = ensure_dyn_smem(k_tdt_recur<KD>, smem_set, max_optin_smem(current_device()));
+        if (e != cudaSuccess) return e;
+    }
+    TdtRec r = {c.lp, c.labels, c.xn, c.yn, c.alpha, c.beta, c.ll, c.costs, c.status, c.T, c.U, c.V, c.dur.D, p.ring,
+                c.dur};
+    k_tdt_recur<KD><<<dim3(c.N, 2), p.warps * 32, p.smem, s>>>(r);
+    count_launch();
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess || !c.pg) return e;
+    const FastDiv divU((uint32_t)c.U), divTU((uint32_t)(c.T * c.U));
+    const unsigned grid = (unsigned)min((cells + kTdtRowThreads - 1) / kTdtRowThreads,
+                                        (int64_t)sm_count(current_device()) * 16);
+    k_tdt_post<KD><<<grid, kTdtRowThreads, 0, s>>>(c.lp, c.alpha, c.beta, c.ll, c.status, c.xn, c.yn, cells, c.T, c.U,
+                                                   c.dur.D, c.dur, divU, divTU, c.pg);
+    count_launch();
+    return cudaGetLastError();
+}
+
+cudaError_t launch_tdt_forward(cudaStream_t s, const TdtFwd &c) {
+    const int64_t cells = (int64_t)c.N * c.T * c.U;
+    const TdtPlan p = tdt_plan(c.U, c.dur, c.x, c.io_bf16 ? 2 : 4, c.V);
+    {
+        std::lock_guard<std::mutex> lock(g_tdt_mu);
+        int32_t *rec = g_tdt_record;
+        memset(rec, 0, sizeof(g_tdt_record));
+        rec[RNNT_TDT_REC_SEQ] = ++g_tdt_seq;
+        rec[RNNT_TDT_REC_CLUSTER] = 0;
+        rec[RNNT_TDT_REC_WARPS] = p.warps;
+        rec[RNNT_TDT_REC_RING] = p.ring;
+        rec[RNNT_TDT_REC_PASSES] = p.passes;
+        rec[RNNT_TDT_REC_KD] = p.kd;
+        rec[RNNT_TDT_REC_NORM_GROUP] = p.norm_group;
+        rec[RNNT_TDT_REC_NORM_LANES] = p.norm_lanes;
+        rec[RNNT_TDT_REC_SMEM] = p.smem;
+    }
+    if (cells == 0) return cudaSuccess;
+    cudaError_t e = c.io_bf16 ? tdt_norm_as(s, p, static_cast<const __nv_bfloat16 *>(c.x), c, cells)
+                              : tdt_norm_as(s, p, static_cast<const float *>(c.x), c, cells);
+    if (e != cudaSuccess) return e;
+    return p.kd == 5 ? tdt_recur_post<5>(s, p, c, cells) : tdt_recur_post<kTdtMaxD>(s, p, c, cells);
+}
+
+template <typename IO>
+static cudaError_t tdt_emit_as(cudaStream_t s, const TdtBwd &c, const IO *x, IO *out) {
+    const int W = c.V + c.D;
+    const int64_t total = (int64_t)c.N * c.T * c.U * W;
+    constexpr int kVec = 16 / (int)sizeof(IO);
+    const bool ovec = (reinterpret_cast<uintptr_t>(out) & 15u) == 0;
+    const bool xvec = ovec && (reinterpret_cast<uintptr_t>(x) & 15u) == 0;
+    const int vec = ovec ? kVec : 1;
+    {
+        std::lock_guard<std::mutex> lock(g_tdt_mu);
+        g_tdt_record[RNNT_TDT_REC_EMIT_VEC] = vec;
+        g_tdt_record[RNNT_TDT_REC_EMIT_XVEC] = xvec;
+    }
+    if (total == 0) return cudaSuccess;
+    const FastDiv divU((uint32_t)c.U), divTU((uint32_t)(c.T * c.U));
+    const int64_t vecs = (total + vec - 1) / vec;
+    const unsigned grid = (unsigned)min((vecs + kTdtRowThreads - 1) / kTdtRowThreads,
+                                        (int64_t)sm_count(current_device()) * 32);
+    const int64_t stride = (int64_t)grid * kTdtRowThreads * vec;
+    const int64_t srows = stride / W;
+    const int sv = (int)(stride - srows * W);
+#define RNNT_TDT_EMIT(VEC, XV)                                                                                        \
+    k_tdt_emit<IO, VEC, XV><<<grid, kTdtRowThreads, 0, s>>>(x, c.lse, c.pg, c.labels, c.grad_out, out, total, c.V, c.D, \
+                                                            c.blank, c.U, divU, divTU, srows, sv)
+    if (!ovec) RNNT_TDT_EMIT(1, false);
+    else if (xvec) RNNT_TDT_EMIT(kVec, true);
+    else RNNT_TDT_EMIT(kVec, false);
+#undef RNNT_TDT_EMIT
+    count_launch();
+    return cudaGetLastError();
+}
+
+cudaError_t launch_tdt_backward(cudaStream_t s, const TdtBwd &c) {
+    if (c.io_bf16)
+        return tdt_emit_as(s, c, static_cast<const __nv_bfloat16 *>(c.x), static_cast<__nv_bfloat16 *>(c.out));
+    return tdt_emit_as(s, c, static_cast<const float *>(c.x), static_cast<float *>(c.out));
+}
+
+}  // namespace rnnt
