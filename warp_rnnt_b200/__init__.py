@@ -306,6 +306,32 @@ class RNNTLossTDT(torch.autograd.Function):
         return g, None, None, None, None, None, None
 
 
+class RNNTLossTDTCompact(torch.autograd.Function):
+    """``RNNTLossTDT`` on compact (STU,V+D) logits in ``joint_pack``'s row order: a packed TDT joint feeds the loss
+    without padding.  Forward keeps lse (STU,2), the posteriors (STU,2+D) and the compact prefix sums (16 bytes per
+    lattice); backward writes d loss / d logits, of the logits' dtype.  Inside ``compact_hints`` the forward has no host
+    sync (CUDA-graph capturable)."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, frames_lengths, labels_lengths, durations, sigma=0.0, blank=0):
+        need = ctx.needs_input_grad[0]
+        hints = _hints()
+        costs, lse, pg, prefix = _C.rnnt_tdt_compact_forward(logits, labels, frames_lengths, labels_lengths,
+                                                             list(durations), sigma, blank, need, hints[0], hints[1])
+        if need:
+            ctx.save_for_backward(logits, lse, pg, labels, frames_lengths, labels_lengths, prefix)
+            ctx.durations = list(durations)
+            ctx.blank = blank
+        return costs
+
+    @staticmethod
+    def backward(ctx, grads_output):
+        logits, lse, pg, labels, xn, yn, prefix = ctx.saved_tensors
+        go = grads_output.contiguous().to(torch.float32)
+        g = _C.rnnt_tdt_compact_backward(logits, lse, pg, labels, xn, yn, prefix, ctx.durations, go, ctx.blank)
+        return g, None, None, None, None, None, None
+
+
 def _tdt_durations(durations):
     if not isinstance(durations, (list, tuple)) or not durations or \
             any(isinstance(d, bool) or not isinstance(d, int) for d in durations):
@@ -318,20 +344,21 @@ def _tdt_durations(durations):
 
 
 def rnnt_loss_tdt(logits, labels, frames_lengths, labels_lengths, durations, sigma=0.0, average_frames=False,
-                  reduction="none", blank=0):
+                  reduction="none", blank=0, compact=False):
     """Token-and-Duration Transducer loss (TDT, Xu et al. 2023, arXiv:2304.06795), the loss of NeMo's Parakeet-TDT
     models, from the joint network's logits.  Follows NeMo's definition (``TDTLossPytorch``: the same alpha recursion
     and terminal sum); not tested against NeMo.
 
     Args:
         logits: (N, T, U, V + D) float32 or bfloat16, NeMo's layout: V token logits (blank included), then D duration
-            logits, D = len(durations).  U = labels.size(1) + 1.  Compact (ragged) input is not offered.
+            logits, D = len(durations).  U = labels.size(1) + 1.  ``compact=True``: (STU, V + D), see below.
         labels: (N, U-1) int32; frames_lengths, labels_lengths: (N,) int32, as for ``rnnt_loss_from_logits``.
         durations: list or tuple of ints, strictly increasing, in [0, 16], at least one > 0 (else ValueError), e.g.
             [0, 1, 2, 3, 4].  Host values: they reach the kernels as launch parameters.
         sigma: NeMo's logit under-normalisation, a finite float >= 0 (else ValueError).
         average_frames, reduction: as in ``rnnt_loss_from_logits``.
         blank: in [0, V).
+        compact: the ragged layout of ``rnnt_loss_from_logits(compact=True)``.
 
     Lattice n has Tn = frames_lengths[n] frames and Un = labels_lengths[n] + 1 columns.  Cell (t, u) has
     lt = log_softmax(logits[n,t,u,:V]) - sigma, the token log-probs, and ld = log_softmax(logits[n,t,u,V:]), the
@@ -363,6 +390,21 @@ def rnnt_loss_tdt(logits, labels, frames_lengths, labels_lengths, durations, sig
     the same values bit for bit, and the gradient is their float32 gradient rounded once.  Deterministic (no atomics),
     no host synchronisation: a step can be captured in a CUDA graph.  ``set_lse_mode`` does not apply.
 
+    ``compact=True``: ``logits`` is (STU, V + D), float32 or bfloat16, rows in ``joint_pack``'s order (row (n, t, u) at
+    sum_{m<n} Tm * Um + t * Un + u, STU = sum frames_lengths * (labels_lengths + 1)), and ``labels`` is
+    (sum labels_lengths,) int32, concatenated in lattice order.  Semantics, degenerate classes and gradient are those of
+    the dense call: costs, the normalisers, the posteriors and the gradient are bit for bit those of the same rows placed
+    in a padded tensor at the same element offset modulo 4.  Without ``compact_hints`` the call makes one small
+    device->host copy to check STU and ``labels.numel()`` against the lengths; inside ``compact_hints(max_T, max_U)`` it
+    makes none (forward and backward can be captured in a CUDA graph), and a sample exceeding the hints, or one whose
+    rows would run past STU, gets cost NaN and zero gradient rows.  Rows of no valid lattice get exact zeros.  A packed
+    TDT joint::
+
+        x = joint_pack(f, g, frames_lengths, labels_lengths)          # (STU, H), no padding
+        logits = joint(x)                                             # (STU, V + D)
+        loss = rnnt_loss_tdt(logits, labels_c, frames_lengths, labels_lengths, [0, 1, 2, 3, 4], compact=True,
+                             reduction="mean")
+
     Not offered: ``fastemit_lambda``, NeMo's ``omega`` mixing with the regular transducer loss, multi-blank, and a TDT
     variant of ``rnnt_align``."""
     assert average_frames is None or isinstance(average_frames, bool)
@@ -371,12 +413,14 @@ def rnnt_loss_tdt(logits, labels, frames_lengths, labels_lengths, durations, sig
     durations = _tdt_durations(durations)
     if isinstance(sigma, bool) or not isinstance(sigma, (int, float)) or not math.isfinite(sigma) or sigma < 0:
         raise ValueError("rnnt_loss_tdt: sigma must be a finite number >= 0, got %r" % (sigma,))
-    if logits.dim() != 4 or logits.size(-1) <= len(durations):
-        raise ValueError("rnnt_loss_tdt: logits must be (N, T, U, V + D) with V >= 1, D = len(durations) = %d, got "
-                         "shape %s" % (len(durations), tuple(logits.shape)))
+    assert isinstance(compact, bool)
+    if logits.dim() != (2 if compact else 4) or logits.size(-1) <= len(durations):
+        raise ValueError("rnnt_loss_tdt: logits must be %s with V >= 1, D = len(durations) = %d, got shape %s"
+                         % ("(STU, V + D)" if compact else "(N, T, U, V + D)", len(durations), tuple(logits.shape)))
     if isinstance(blank, bool) or not isinstance(blank, int) or not 0 <= blank < logits.size(-1) - len(durations):
         raise ValueError("rnnt_loss_tdt: blank must be an int in [0, V), got %r" % (blank,))
-    costs = RNNTLossTDT.apply(logits, labels, frames_lengths, labels_lengths, durations, float(sigma), blank)
+    fn = RNNTLossTDTCompact if compact else RNNTLossTDT
+    costs = fn.apply(logits, labels, frames_lengths, labels_lengths, durations, float(sigma), blank)
     return _reduce(costs, frames_lengths, average_frames, reduction)
 
 
@@ -671,6 +715,6 @@ def rnnt_align(log_probs, labels, frames_lengths, labels_lengths, blank=0, compa
 
 
 __all__ = ["rnnt_loss", "rnnt_align", "rnnt_loss_from_logits", "rnnt_loss_pruned", "RNNTLossPruned",
-           "rnnt_loss_simple", "RNNTLossSimple", "rnnt_loss_tdt", "RNNTLossTDT", "joint_pack",
+           "rnnt_loss_simple", "RNNTLossSimple", "rnnt_loss_tdt", "RNNTLossTDT", "RNNTLossTDTCompact", "joint_pack",
            "JointPack", "RNNTLossFromLogits", "RNNTLossFromLogitsCompact", "RNNTLoss", "RNNTLossGather", "RNNTLossEager",
            "RNNTLossCompact", "compact_hints", "set_lse_mode", "core", "_C", "__version__"]

@@ -617,8 +617,15 @@ static bool tdt_args_ok(int N, int T, int U, int V, int D, int blank, int elem_b
            N >= 0 && T >= 1 && U >= 1 && V >= 1 && (int64_t)V + D < ((int64_t)1 << 22) &&
            (int64_t)N * T * U < ((int64_t)1 << 31) && blank >= 0 && blank < V;
 }
-struct TdtWorkspace { float *lp, *alpha, *beta, *ll; int *status; size_t bytes; };
-static TdtWorkspace carve_tdt(void *base, int N, int T, int U, int D) {
+// the compact layout: N <= 65535 (the normaliser's grid holds one CTA row per lattice), STU < 2^31 in place of N*T*U
+static bool tdt_compact_args_ok(int N, int64_t STU, int V, int D, int blank, int elem_bytes, const void *logits) {
+    return (elem_bytes == 4 || elem_bytes == 2) && !(reinterpret_cast<uintptr_t>(logits) & (uintptr_t)(elem_bytes - 1)) &&
+           N >= 0 && N <= 65535 && STU >= 0 && STU < ((int64_t)1 << 31) && V >= 1 &&
+           (int64_t)V + D < ((int64_t)1 << 22) && blank >= 0 && blank < V;
+}
+// cells: N*T*U (dense) or STU (compact); the compact call also takes 4 ints for the totals it does not return
+struct TdtWorkspace { float *lp, *alpha, *beta, *ll; int *status, *totals; size_t bytes; };
+static TdtWorkspace carve_tdt(void *base, int64_t cells, int N, int D, bool compact) {
     TdtWorkspace w;
     size_t off = 0;
     auto take = [&](size_t bytes) {
@@ -626,12 +633,13 @@ static TdtWorkspace carve_tdt(void *base, int N, int T, int U, int D) {
         off += align_up(bytes, 256);
         return p;
     };
-    const size_t c = (size_t)max(N, 0) * (size_t)max(T, 0) * (size_t)max(U, 0), n = (size_t)max(N, 0);
+    const size_t c = (size_t)max(cells, (int64_t)0), n = (size_t)max(N, 0);
     w.lp = (float *)take(c * (size_t)(2 + max(D, 0)) * sizeof(float));
     w.alpha = (float *)take(c * sizeof(float));
     w.beta = (float *)take(c * sizeof(float));
     w.ll = (float *)take(n * sizeof(float));
     w.status = (int *)take(n * sizeof(int));
+    w.totals = compact ? (int *)take(4 * sizeof(int)) : nullptr;
     w.bytes = off;
     return w;
 }
@@ -868,7 +876,7 @@ int rnnt_b200_logits_pruned_backward(void *stream, const void *logits, const flo
 }
 
 size_t rnnt_b200_tdt_workspace_bytes(int N, int T, int U, int num_durations) {
-    return carve_tdt(nullptr, N, T, U, num_durations).bytes;
+    return carve_tdt(nullptr, (int64_t)max(N, 0) * max(T, 0) * max(U, 0), N, num_durations, false).bytes;
 }
 
 int rnnt_b200_tdt_forward(void *stream, void *workspace, size_t workspace_bytes, const void *logits, const int *labels,
@@ -883,7 +891,7 @@ int rnnt_b200_tdt_forward(void *stream, void *workspace, size_t workspace_bytes,
     if (N == 0) return RNNT_STATUS_SUCCESS;
     if (!workspace || workspace_bytes < rnnt_b200_tdt_workspace_bytes(N, T, U, num_durations))
         return RNNT_STATUS_WORKSPACE_TOO_SMALL;
-    const TdtWorkspace w = carve_tdt(workspace, N, T, U, num_durations);
+    const TdtWorkspace w = carve_tdt(workspace, (int64_t)N * T * U, N, num_durations, false);
     TdtFwd c = {};
     c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = costs;
     c.lse = reinterpret_cast<float2 *>(lse); c.pg = grads;
@@ -905,6 +913,57 @@ int rnnt_b200_tdt_backward(void *stream, const void *logits, const float *lse, c
     TdtBwd c = {};
     c.x = logits; c.lse = reinterpret_cast<const float2 *>(lse); c.pg = grads; c.labels = labels; c.grad_out = grad_out;
     c.out = out; c.N = N; c.T = T; c.U = U; c.V = V; c.D = num_durations; c.blank = blank; c.io_bf16 = elem_bytes == 2;
+    RNNT_TRY(launch_tdt_backward((cudaStream_t)stream, c), RNNT_STATUS_GRADS_BLANK_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+size_t rnnt_b200_tdt_compact_workspace_bytes(int64_t STU, int N, int num_durations) {
+    return carve_tdt(nullptr, STU, N, num_durations, true).bytes;
+}
+
+int rnnt_b200_tdt_compact_forward(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                  const int *labels, const int *xn, const int *yn, const int *durations,
+                                  int num_durations, float sigma, float *costs, float *lse, float *grads,
+                                  int64_t *prefix, int *totals, int64_t STU, int N, int V, int blank, int elem_bytes,
+                                  int max_T, int max_U) {
+    TdtDurations dur;
+    if (!tdt_durations(durations, num_durations, &dur) ||
+        !tdt_compact_args_ok(N, STU, V, num_durations, blank, elem_bytes, logits) || !std::isfinite(sigma) ||
+        sigma < 0.0f || !costs || !lse || !pairs_aligned(lse) || !workspace_aligned16(workspace) || !prefix ||
+        max_T < 1 || max_U < 1)
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    if (!workspace || workspace_bytes < rnnt_b200_tdt_compact_workspace_bytes(STU, N, num_durations))
+        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    cudaStream_t s = (cudaStream_t)stream;
+    const TdtWorkspace w = carve_tdt(workspace, STU, N, num_durations, true);
+    RNNT_TRY(launch_prefix(s, xn, yn, N, prefix, prefix + N, totals ? totals : w.totals), RNNT_STATUS_GATHER_FAILED);
+    TdtFwd c = {};
+    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = costs;
+    c.mem_pref = prefix; c.lab_pref = prefix + N; c.STU = STU;
+    c.lse = reinterpret_cast<float2 *>(lse); c.pg = grads;
+    c.lp = w.lp; c.alpha = w.alpha; c.beta = w.beta; c.ll = w.ll; c.status = w.status;
+    c.N = N; c.T = max_T; c.U = max_U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur;
+    c.io_bf16 = elem_bytes == 2;
+    RNNT_TRY(launch_tdt_forward(s, c), RNNT_STATUS_WARP_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+int rnnt_b200_tdt_compact_backward(void *stream, const void *logits, const float *lse, const float *grads,
+                                   const int *labels, const int *yn, const int *durations, int num_durations,
+                                   const int64_t *prefix, const float *grad_out, void *out, int64_t STU, int N, int V,
+                                   int blank, int elem_bytes) {
+    TdtDurations dur;
+    if (!tdt_durations(durations, num_durations, &dur) ||
+        !tdt_compact_args_ok(N, STU, V, num_durations, blank, elem_bytes, logits) ||
+        (reinterpret_cast<uintptr_t>(out) & (uintptr_t)(elem_bytes - 1)) || !lse || !pairs_aligned(lse) || !grads ||
+        !out || !prefix)
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0 || STU == 0) return RNNT_STATUS_SUCCESS;
+    TdtBwd c = {};
+    c.x = logits; c.lse = reinterpret_cast<const float2 *>(lse); c.pg = grads; c.labels = labels; c.grad_out = grad_out;
+    c.yn = yn; c.mem_pref = prefix; c.lab_pref = prefix + N; c.STU = STU;
+    c.out = out; c.N = N; c.V = V; c.D = num_durations; c.blank = blank; c.io_bf16 = elem_bytes == 2;
     RNNT_TRY(launch_tdt_backward((cudaStream_t)stream, c), RNNT_STATUS_GRADS_BLANK_FAILED);
     return RNNT_STATUS_SUCCESS;
 }

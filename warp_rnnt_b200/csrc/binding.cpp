@@ -584,6 +584,67 @@ at::Tensor rnnt_tdt_backward(const at::Tensor &xs, const at::Tensor &lse, const 
     return out;
 }
 
+// TDT loss from compact (STU,V+D) logits in joint_pack's row order, float32 or bfloat16, labels (sum yn): (costs (N),
+// lse (STU,2), grads (STU,2+D) or empty, prefix (2N) int64 = {mem_pref, lab_pref} for the backward).  Shapes are
+// validated as in rnnt_loss_compact: one 16-byte device->host copy, or none with hints (max_T, max_U > 0).
+std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor>
+rnnt_tdt_compact_forward(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
+                         const std::vector<int> &durations, double sigma, int blank, bool want_grads, int max_T,
+                         int max_U) {
+    const auto [N, STU, W, bf16, guard] = compact_front(xs, ys, xn, yn, blank, true);
+    const int64_t D = (int64_t)durations.size();
+    TORCH_CHECK(D >= 1 && W > D, "xs must have more than len(durations) logits per row (V + D)");
+    check_blank(blank, W - D);
+    void *stream = current_stream(xs);
+    const auto f32 = xs.options().dtype(at::kFloat);
+    at::Tensor costs = at::empty({N}, f32);
+    at::Tensor lse = at::empty({STU, 2}, f32);
+    at::Tensor pg = output(want_grads, {STU, 2 + D}, f32);
+    at::Tensor prefix = at::empty({2 * N}, xs.options().dtype(at::kLong));
+    if (N == 0) return std::make_tuple(costs, lse, pg, prefix);
+    std::tie(max_T, max_U) = compact_bounds(stream, xs, ys, xn, yn, max_T, max_U, prefix.data_ptr<int64_t>());
+    // a batch whose lengths are all 0: bounds of 1 (its lattices are invalid either way)
+    max_T = std::max(max_T, 1);
+    max_U = std::max(max_U, 1);
+    at::Tensor ws = workspace(xs, rnnt_b200_tdt_compact_workspace_bytes(STU, (int)N, (int)D));
+    check_status(rnnt_b200_tdt_compact_forward(stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
+                                               ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
+                                               durations.data(), (int)D, (float)sigma, costs.data_ptr<float>(),
+                                               lse.data_ptr<float>(), want_grads ? pg.data_ptr<float>() : nullptr,
+                                               prefix.data_ptr<int64_t>(), nullptr, STU, (int)N, (int)(W - D), blank,
+                                               bf16 ? 2 : 4, max_T, max_U));
+    return std::make_tuple(costs, lse, pg, prefix);
+}
+
+// d loss / d compact TDT logits (STU,V+D), of the dtype of xs
+at::Tensor rnnt_tdt_compact_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &grads,
+                                     const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
+                                     const at::Tensor &prefix, const std::vector<int> &durations,
+                                     const at::Tensor &grad_out, int blank) {
+    check_arg(xs, Dt::F32orBF16, xs, {kAny, kAny}, "xs must be a contiguous CUDA Float tensor of shape (STU, V+D)");
+    const int64_t STU = xs.size(0), W = xs.size(1), N = xn.numel(), D = (int64_t)durations.size();
+    TORCH_CHECK(D >= 1 && W > D, "xs must have more than len(durations) logits per row (V + D)");
+    check_arg(lse, Dt::F32, xs, {STU, 2}, "lse must be a contiguous Float tensor of shape (STU, 2) on the device of xs");
+    check_arg(grads, Dt::F32, xs, {STU, 2 + D},
+              "grads must be a contiguous Float tensor of shape (STU, 2+D) on the device of xs");
+    TORCH_CHECK(is_arg(ys, Dt::I32, xs), "ys must be a contiguous Int tensor on the device of xs");
+    const char *lengths = "xn and yn must be contiguous Int tensors of shape (N,) on the device of xs";
+    check_arg(xn, Dt::I32, xs, N, lengths);
+    check_arg(yn, Dt::I32, xs, N, lengths);
+    check_arg(prefix, Dt::I64, xs, 2 * N, "prefix must be a contiguous Long tensor of shape (2N,) on the device of xs");
+    check_arg(grad_out, Dt::F32, xs, N, "grad_out must be a contiguous Float tensor of shape (N,)");
+    check_blank(blank, W - D);
+    const c10::cuda::CUDAGuard guard(xs.device());
+    at::Tensor out = at::empty_like(xs);
+    if (N == 0 || STU == 0) return out;                 // empty tensors: nothing to write (and no data pointers)
+    check_status(rnnt_b200_tdt_compact_backward(current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(),
+                                                grads.data_ptr<float>(), ys.data_ptr<int>(), yn.data_ptr<int>(),
+                                                durations.data(), (int)D, prefix.data_ptr<int64_t>(),
+                                                grad_out.data_ptr<float>(), out.data_ptr(), STU, (int)N, (int)(W - D),
+                                                blank, xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
+    return out;
+}
+
 // am (N,T,V) and lm (N,U,V): dtypes, then contiguity and device, then shapes; then ys, xn and yn
 void check_simple_inputs(const at::Tensor &am, const at::Tensor &lm, const at::Tensor &ys, const at::Tensor &xn,
                          const at::Tensor &yn) {
@@ -835,6 +896,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("durations"), py::arg("sigma") = 0.0, py::arg("blank") = 0, py::arg("want_grads") = true);
     m.def("rnnt_tdt_backward", &rnnt_tdt_backward, py::arg("xs"), py::arg("lse"), py::arg("grads"), py::arg("ys"),
           py::arg("durations"), py::arg("grad_out"), py::arg("blank") = 0);
+    m.def("rnnt_tdt_compact_forward", &rnnt_tdt_compact_forward, py::arg("xs"), py::arg("ys"), py::arg("xn"),
+          py::arg("yn"), py::arg("durations"), py::arg("sigma"), py::arg("blank"), py::arg("want_grads"),
+          py::arg("max_T") = 0, py::arg("max_U") = 0);
+    m.def("rnnt_tdt_compact_backward", &rnnt_tdt_compact_backward, py::arg("xs"), py::arg("lse"), py::arg("grads"),
+          py::arg("ys"), py::arg("xn"), py::arg("yn"), py::arg("prefix"), py::arg("durations"), py::arg("grad_out"),
+          py::arg("blank"));
     m.def("rnnt_simple_forward", &rnnt_simple_forward, py::arg("am"), py::arg("lm"), py::arg("ys"), py::arg("xn"),
           py::arg("yn"), py::arg("blank") = 0, py::arg("want_grads") = true, py::arg("prune_range") = 0,
           py::arg("lse_mode") = 0, py::arg("lm_only_scale") = 0.0, py::arg("am_only_scale") = 0.0);

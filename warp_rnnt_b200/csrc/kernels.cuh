@@ -16,6 +16,14 @@ void begin_launch_record(int path);
 
 cudaError_t launch_prefix(cudaStream_t s, const int *xn, const int *yn, int N, int64_t *mem_pref,
                           int64_t *lab_pref, int *totals);
+// Compact grids are (gx, N): lattice lengths are on the device only, so gx covers twice the average lattice
+// (STU / N rows, as launch_gather sizes its grid) in CTAs of kCompactIters grid-stride iterations each; a larger lattice
+// is finished by the grid stride, the surplus CTAs of a smaller one return at once.
+constexpr int64_t kCompactIters = 4;
+inline int compact_gx(int64_t STU, int N, int64_t per_cta_rows) {
+    const int64_t per = (STU / (N > 0 ? N : 1)) * 2 + 1;
+    return (int)max((int64_t)1, min((per + per_cta_rows - 1) / per_cta_rows, (int64_t)65535));
+}
 // The LSE flavour of a launch: the fast one, else the reference's exact formula of the layout (dense or compact).
 inline int lse_kind(bool fast_lse, bool compact) { return fast_lse ? kFast : compact ? kExactCompact : kExactDense; }
 
@@ -164,9 +172,21 @@ struct TdtPlan {
     int ring, smem;                       // ring slots in shared memory (0: read back from global), its bytes
 };
 TdtPlan tdt_plan(int U, const TdtDurations &dur, const void *x, int elem_bytes, int V);
+// The compact layout of a TDT call (joint_pack's row order): lattice n is a Tn x Un slab at row mem_pref[n] with row
+// stride Un = yn[n] + 1, its labels start at lab_pref[n]; a lattice is ok when Tn <= max_T, Un <= max_U and its rows lie
+// inside [0, STU).  The backward takes max_T = max_U = 0 (it does not check lattices: the posteriors tell).
+struct TdtCompact {
+    const int64_t *mem_pref, *lab_pref;
+    int64_t STU;
+    int N, max_T, max_U;
+};
+// Every field below that names a (N,T,U,...) shape is (STU,...) in the compact layout (mem_pref set), where T and U are
+// the bounds max_T, max_U and labels is (sum yn).
 struct TdtFwd {
     const void *x;                        // logits (N,T,U,V+D), f32 or bf16
     const int *labels, *xn, *yn;
+    const int64_t *mem_pref, *lab_pref;   // compact: the prefix sums of xn * (yn + 1) and yn; null: dense
+    int64_t STU;                          // compact: rows
     float *costs;
     float2 *lse;                          // (N,T,U) (lse_tok, lse_dur) out
     float *pg;                            // (N,T,U,2+D) posteriors out, or null (costs only)
@@ -183,6 +203,9 @@ struct TdtBwd {
     const float2 *lse;
     const float *pg;                      // (N,T,U,2+D) posteriors of the forward
     const int *labels;
+    const int *yn;                        // compact only, with mem_pref, lab_pref and STU as in TdtFwd
+    const int64_t *mem_pref, *lab_pref;
+    int64_t STU;
     const float *grad_out;                // (N), or null (ones)
     void *out;                            // (N,T,U,V+D), of the logits' type
     int N, T, U, V, D, blank;

@@ -302,15 +302,7 @@ k_expand_logits_pruned(const IO *__restrict__ x, const float *__restrict__ lse, 
                                              stride_rows, stride_v, Problem{}, ranges);
 }
 
-// Compact grids are (gx, N): lattice lengths are on the device only, so gx covers twice the average lattice
-// (STU / N rows, as launch_gather sizes its grid) in CTAs of kCompactIters grid-stride iterations each; a larger lattice
-// is finished by the grid stride, the surplus CTAs of a smaller one return at once.
-constexpr int64_t kCompactIters = 4;
-static int compact_gx(int64_t STU, int N, int64_t per_cta_rows) {
-    const int64_t per = (STU / (N > 0 ? N : 1)) * 2 + 1;
-    return (int)max((int64_t)1, min((per + per_cta_rows - 1) / per_cta_rows, (int64_t)65535));
-}
-
+// compact grids: compact_gx (kernels.cuh)
 // lay == nullptr: dense (N,T,U,V) logits; else the compact (STU,V) rows of lattices lay->N, lay->T = lay->U = 0.
 // ranges != nullptr: the pruned (N,T,S,V) rows of windows ranges (N,T) on the full (N,T,U) lattice.
 template <typename IN>

@@ -20,6 +20,14 @@
 // value has one writer and a fixed operation order, so results are deterministic.  A bf16 row is read in exactly the
 // f32 row's order (branch and lanes depend on the row width and the element alignment only), so lse, lp, costs and the
 // posteriors are bit for bit those of the widened logits, and the bf16 gradient is the f32 gradient rounded once.
+//
+// Compact layout (joint_pack's row order, rnnt_b200_tdt_compact_*): the logits are (STU, V+D) and every intermediate
+// is compact too -- lse (STU,2), lp and the posteriors (STU,2+D), alpha / beta (STU).  Lattice n is a Tn x Un slab at
+// row mem_pref[n] with row stride Un, its labels start at lab_pref[n]; T and U are the bounds max_T, max_U.  Each
+// kernel body is shared by the two layouts and takes the layout as a template flag (COMPACT): only the cell ->
+// (n, t, u) mapping differs, so a compact row is computed exactly as the same row of a padded tensor.  The normaliser
+// runs one lattice per blockIdx.y (as logits.cu's compact rows); the posterior pass and the emit stay flat over the rows
+// and find a row's lattice by a binary search of mem_pref (tdt_find).
 #include "common.cuh"
 #include "kernels.cuh"
 
@@ -32,6 +40,31 @@ constexpr int kTdtMaxThreads = 512;   // k_tdt_recur: at most 16 warps over the 
 enum { kTdtOk = 0, kTdtInvalid = 1, kTdtNan = 2, kTdtDead = 3 };
 
 __device__ __forceinline__ float clamp_big(float v) { return v < kBig ? kBig : v; }   // NaN stays NaN
+
+// lattice n of a compact call: ok when its lengths are in [1, max_T] x [1, max_U] and its rows lie inside [0, STU)
+__device__ __forceinline__ Lattice tdt_lattice(const int *xn, const int *yn, const TdtCompact &cp, int n) {
+    Lattice L;
+    L.Tn = xn[n];
+    L.Un = yn[n] + 1;
+    L.stride = L.Un;
+    L.base = cp.mem_pref[n];
+    L.lab_base = cp.lab_pref[n];
+    L.ok = L.Tn >= 1 && L.Tn <= cp.max_T && L.Un >= 1 && L.Un <= cp.max_U && L.base >= 0 &&
+           L.base + (int64_t)L.Tn * L.Un <= cp.STU;
+    return L;
+}
+// the compact lattice holding row r: the last n with mem_pref[n] <= r (the prefix sums do not decrease, so an empty
+// lattice shares its first row with the next one and is passed over), -1 if there is none.  The caller still checks
+// that r lies inside it.
+__device__ __forceinline__ int tdt_find(const int64_t *__restrict__ mem_pref, int N, int64_t r) {
+    int lo = 0, hi = N;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (__ldg(mem_pref + mid) <= r) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo - 1;
+}
 
 // online max / sum: the running max m stays -inf while every element seen is -inf; until a finite one arrives the
 // sum subtracts 0 instead (exp(-inf) = 0), so -inf - -inf is never formed.  A NaN makes the sum NaN, +inf too.
@@ -51,21 +84,38 @@ __device__ __forceinline__ float online_lse(float m, float s) { return m == -INF
 // addresses, 2: the same for pairs, 1: any row); lanes stride over the groups, each lane keeps a token and a duration
 // accumulator (an element goes to the one of its column), then a butterfly merges the lanes.  Lane 0 writes lse and lp.
 // Rows outside the live lattice (padding, or a lattice with invalid lengths) are not read: lse (0, 0), lp untouched.
-template <typename IN, int SUB, int G>
-__global__ void __launch_bounds__(kTdtRowThreads)
-k_tdt_norm(const IN *__restrict__ x, const int *__restrict__ labels, const int *__restrict__ xn,
-           const int *__restrict__ yn, int64_t cells, int T, int U, int V, int D, int blank, float sigma, FastDiv divU,
-           FastDiv divTU, float2 *__restrict__ lse, float *__restrict__ lp) {
+// COMPACT: CTA row blockIdx.y streams over the Tn * Un rows of lattice n, the pointers rebased to its first row; the rows
+// of a lattice that is not ok are not read and lse / lp are not written there (the posteriors of those rows are 0).
+template <typename IN, int SUB, int G, bool COMPACT>
+__device__ __forceinline__ void
+tdt_norm_rows(const IN *__restrict__ x, const int *__restrict__ labels, const int *__restrict__ xn,
+              const int *__restrict__ yn, int64_t cells, int T, int U, int V, int D, int blank, float sigma,
+              FastDiv divU, FastDiv divTU, float2 *__restrict__ lse, float *__restrict__ lp, const TdtCompact &cp) {
     const int W = V + D, W2 = 2 + D;
+    Lattice L;
+    if constexpr (COMPACT) {
+        L = tdt_lattice(xn, yn, cp, blockIdx.y);
+        cells = L.ok ? (int64_t)L.Tn * L.Un : 0;
+        x += L.base * W; lse += L.base; lp += L.base * W2; labels += L.lab_base;
+    }
     const int sub = threadIdx.x % SUB;
     const int64_t per_block = kTdtRowThreads / SUB;
     for (int64_t base = (int64_t)blockIdx.x * per_block; base < cells; base += (int64_t)gridDim.x * per_block) {
         const int64_t cell = min(base + threadIdx.x / SUB, cells - 1);   // surplus groups redo the last row
         uint32_t n, rem, t, u;
-        divTU.divmod((uint32_t)cell, n, rem);
-        divU.divmod(rem, t, u);
-        const int Tn = xn[n], Un = yn[n] + 1;
-        const bool live = Tn >= 1 && Tn <= T && Un >= 1 && Un <= U && (int)t < Tn && (int)u < Un;
+        int Tn, Un;
+        bool live;
+        if constexpr (COMPACT) {
+            n = 0;                                                        // labels are rebased to the lattice's
+            Tn = L.Tn; Un = L.Un;
+            u = (uint32_t)cell % (uint32_t)Un;
+            live = true;
+        } else {
+            divTU.divmod((uint32_t)cell, n, rem);
+            divU.divmod(rem, t, u);
+            Tn = xn[n]; Un = yn[n] + 1;
+            live = Tn >= 1 && Tn <= T && Un >= 1 && Un <= U && (int)t < Tn && (int)u < Un;
+        }
         const IN *row = x + cell * W;
         float mt = -INFINITY, st = 0.0f, md = -INFINITY, sd = 0.0f;
         if (live) {
@@ -105,6 +155,25 @@ k_tdt_norm(const IN *__restrict__ x, const int *__restrict__ labels, const int *
     }
 }
 
+template <typename IN, int SUB, int G>
+__global__ void __launch_bounds__(kTdtRowThreads)
+k_tdt_norm(const IN *__restrict__ x, const int *__restrict__ labels, const int *__restrict__ xn,
+           const int *__restrict__ yn, int64_t cells, int T, int U, int V, int D, int blank, float sigma, FastDiv divU,
+           FastDiv divTU, float2 *__restrict__ lse, float *__restrict__ lp) {
+    tdt_norm_rows<IN, SUB, G, false>(x, labels, xn, yn, cells, T, U, V, D, blank, sigma, divU, divTU, lse, lp,
+                                     TdtCompact{});
+}
+
+// grid (gx, N): cells = STU
+template <typename IN, int SUB, int G>
+__global__ void __launch_bounds__(kTdtRowThreads)
+k_tdt_norm_compact(const IN *__restrict__ x, const int *__restrict__ labels, const int *__restrict__ xn,
+                   const int *__restrict__ yn, int V, int D, int blank, float sigma, float2 *__restrict__ lse,
+                   float *__restrict__ lp, TdtCompact cp) {
+    tdt_norm_rows<IN, SUB, G, true>(x, labels, xn, yn, cp.STU, cp.max_T, cp.max_U, V, D, blank, sigma, FastDiv(),
+                                    FastDiv(), lse, lp, cp);
+}
+
 struct TdtRec {
     const float *lp;
     const int *labels, *xn, *yn;
@@ -129,13 +198,25 @@ __device__ __forceinline__ float lse_cands(const float (&c)[C]) {
 }
 
 // alpha (blockIdx.y == 0) or beta (1) of lattice blockIdx.x.  KD >= D: the candidate arrays' compile-time size.
-template <int KD>
-__global__ void __launch_bounds__(kTdtMaxThreads) k_tdt_recur(TdtRec a) {
+// The ring holds U (dense: the padded width, compact: max_U) columns per diagonal; lp, alpha and beta are addressed
+// with the lattice's row stride ld (dense U, compact Un).
+template <int KD, bool COMPACT>
+__device__ __forceinline__ void tdt_recur(const TdtRec &a, const TdtCompact &cp) {
     extern __shared__ float ring[];
     const int n = blockIdx.x;
     const bool beta_side = blockIdx.y == 1;
-    const int Tn = a.xn[n], Un = a.yn[n] + 1;
-    if (!(Tn >= 1 && Tn <= a.T && Un >= 1 && Un <= a.U)) {
+    int Tn, Un;
+    bool ok;
+    int64_t base, lab_base;
+    if constexpr (COMPACT) {
+        const Lattice L = tdt_lattice(a.xn, a.yn, cp, n);
+        Tn = L.Tn; Un = L.Un; ok = L.ok; base = L.base; lab_base = L.lab_base;
+    } else {
+        Tn = a.xn[n]; Un = a.yn[n] + 1;
+        ok = Tn >= 1 && Tn <= a.T && Un >= 1 && Un <= a.U;
+        base = (int64_t)n * a.T * a.U; lab_base = (int64_t)n * (a.U - 1);
+    }
+    if (!ok) {
         if (beta_side && threadIdx.x == 0) {
             a.status[n] = kTdtInvalid;
             a.costs[n] = NAN;
@@ -144,11 +225,12 @@ __global__ void __launch_bounds__(kTdtMaxThreads) k_tdt_recur(TdtRec a) {
         return;
     }
     const int U = a.U, W2 = 2 + a.D, D = a.D, R = a.ring;
-    const int64_t base = (int64_t)n * a.T * U;
+    const int ld = COMPACT ? Un : U;
+    const int *labels = a.labels + lab_base;
     float *out = (beta_side ? a.beta : a.alpha) + base;
     const float *lp = a.lp + base * W2;
     // the value of cell (t, u) on the diagonal whose ring slot is sl (computed on an earlier step)
-    auto rd = [&](int t, int u, int sl) -> float { return R ? ring[sl * U + u] : out[(int64_t)t * U + u]; };
+    auto rd = [&](int t, int u, int sl) -> float { return R ? ring[sl * U + u] : out[(int64_t)t * ld + u]; };
     const int S = Tn + Un - 1;
     bool saw_nan = false;
     for (int step = 0; step < S; ++step) {
@@ -169,11 +251,11 @@ __global__ void __launch_bounds__(kTdtMaxThreads) k_tdt_recur(TdtRec a) {
                         const int d = a.dur.d[j], tp = t - d;
                         if (tp >= 0) {
                             if (d > 0) {
-                                const float *r = lp + ((int64_t)tp * U + u) * W2;
+                                const float *r = lp + ((int64_t)tp * ld + u) * W2;
                                 c[2 * j] = (rd(tp, u, back(d)) + r[0]) + r[2 + j];
                             }
                             if (u > 0) {
-                                const float *r = lp + ((int64_t)tp * U + u - 1) * W2;
+                                const float *r = lp + ((int64_t)tp * ld + u - 1) * W2;
                                 c[2 * j + 1] = (rd(tp, u - 1, back(d + 1)) + r[1]) + r[2 + j];
                             }
                         }
@@ -183,7 +265,7 @@ __global__ void __launch_bounds__(kTdtMaxThreads) k_tdt_recur(TdtRec a) {
             } else {
                 // push-side view: the cell's own weights, beta of the destinations; a blank to t + d == Tn from the
                 // last column is terminal (beta 0 after it)
-                const float *r = lp + ((int64_t)t * U + u) * W2;
+                const float *r = lp + ((int64_t)t * ld + u) * W2;
                 const float b = r[0], l = r[1];
                 const bool has_label = u < Un - 1;
                 saw_nan |= (b != b) || (has_label && l != l);
@@ -204,14 +286,14 @@ __global__ void __launch_bounds__(kTdtMaxThreads) k_tdt_recur(TdtRec a) {
                 v = lse_cands(c);
             }
             if (R) ring[slot * U + u] = v;
-            out[(int64_t)t * U + u] = v;
+            out[(int64_t)t * ld + u] = v;
         }
         __syncthreads();
     }
     if (!beta_side) return;
     bool bad = false;
     for (int u = threadIdx.x; u < Un - 1; u += blockDim.x) {
-        const int lab = a.labels[(int64_t)n * (U - 1) + u];
+        const int lab = labels[u];
         bad |= lab < 0 || lab >= a.V;
     }
     bad = __syncthreads_or(bad);
@@ -225,24 +307,51 @@ __global__ void __launch_bounds__(kTdtMaxThreads) k_tdt_recur(TdtRec a) {
     }
 }
 
-// Edge posteriors per cell: (Pb, Pl, Pd[0..D)), one thread per cell.  0 on padding and on lattices with invalid input
-// or no path; NaN on the live cells of a lattice with a NaN (or +inf, or all -inf) live row.
 template <int KD>
-__global__ void __launch_bounds__(kTdtRowThreads)
-k_tdt_post(const float *__restrict__ lp, const float *__restrict__ alpha, const float *__restrict__ beta,
-           const float *__restrict__ ll, const int *__restrict__ status, const int *__restrict__ xn,
-           const int *__restrict__ yn, int64_t cells, int T, int U, int D, TdtDurations dur, FastDiv divU,
-           FastDiv divTU, float *__restrict__ pg) {
+__global__ void __launch_bounds__(kTdtMaxThreads) k_tdt_recur(TdtRec a) {
+    tdt_recur<KD, false>(a, TdtCompact{});
+}
+
+// a.T, a.U = max_T, max_U
+template <int KD>
+__global__ void __launch_bounds__(kTdtMaxThreads) k_tdt_recur_compact(TdtRec a, TdtCompact cp) {
+    tdt_recur<KD, true>(a, cp);
+}
+
+// Edge posteriors per cell: (Pb, Pl, Pd[0..D)), one thread per cell.  0 on padding and on lattices with invalid input
+// or no path; NaN on the live cells of a lattice with a NaN (or +inf, or all -inf) live row.  COMPACT: cells = STU, and
+// a row that lies in no lattice, or in one that is not ok, is a padding row.
+template <int KD, bool COMPACT>
+__device__ __forceinline__ void
+tdt_post_rows(const float *__restrict__ lp, const float *__restrict__ alpha, const float *__restrict__ beta,
+              const float *__restrict__ ll, const int *__restrict__ status, const int *__restrict__ xn,
+              const int *__restrict__ yn, int64_t cells, int U, int D, const TdtDurations &dur, FastDiv divU,
+              FastDiv divTU, float *__restrict__ pg, const TdtCompact &cp) {
     const int W2 = 2 + D;
     for (int64_t cell = (int64_t)blockIdx.x * kTdtRowThreads + threadIdx.x; cell < cells;
          cell += (int64_t)gridDim.x * kTdtRowThreads) {
         uint32_t n, rem, t, u;
-        divTU.divmod((uint32_t)cell, n, rem);
-        divU.divmod(rem, t, u);
+        int Tn, Un, st, rs;                                      // rs: row stride
+        bool live;
         float *g = pg + cell * W2;
-        const int Tn = xn[n], Un = yn[n] + 1;
-        const int st = status[n];
-        const bool live = st != kTdtInvalid && (int)t < Tn && (int)u < Un;   // status Invalid covers bad lengths
+        if constexpr (COMPACT) {
+            const int m = tdt_find(cp.mem_pref, cp.N, cell);
+            n = max(m, 0);
+            Tn = xn[n]; Un = yn[n] + 1;
+            st = m < 0 ? kTdtInvalid : status[n];
+            const int64_t local = cell - cp.mem_pref[n];
+            live = st != kTdtInvalid && local < (int64_t)Tn * Un;     // an ok lattice: Un >= 1, rows inside STU
+            t = live ? (uint32_t)local / (uint32_t)Un : 0;
+            u = live ? (uint32_t)local % (uint32_t)Un : 0;
+            rs = Un;
+        } else {
+            divTU.divmod((uint32_t)cell, n, rem);
+            divU.divmod(rem, t, u);
+            Tn = xn[n]; Un = yn[n] + 1;
+            st = status[n];
+            live = st != kTdtInvalid && (int)t < Tn && (int)u < Un;   // status Invalid covers bad lengths
+            rs = U;
+        }
         if (!live || st == kTdtDead || st == kTdtNan) {
             const float z = (live && st == kTdtNan) ? NAN : 0.0f;
             for (int k = 0; k < W2; ++k) g[k] = z;
@@ -259,10 +368,10 @@ k_tdt_post(const float *__restrict__ lp, const float *__restrict__ alpha, const 
                 const float ld = r[2 + j];
                 float gb = 0.0f, gl = 0.0f;
                 if (d > 0) {
-                    if (tq < Tn) gb = expf((((al + b) + ld) + beta[cell + (int64_t)d * U]) - lP);
+                    if (tq < Tn) gb = expf((((al + b) + ld) + beta[cell + (int64_t)d * rs]) - lP);
                     else if (tq == Tn && !has_label) gb = expf(((al + b) + ld) - lP);
                 }
-                if (has_label && tq < Tn) gl = expf((((al + l) + ld) + beta[cell + (int64_t)d * U + 1]) - lP);
+                if (has_label && tq < Tn) gl = expf((((al + l) + ld) + beta[cell + (int64_t)d * rs + 1]) - lP);
                 pb += gb;
                 pl += gl;
                 g[2 + j] = gb + gl;
@@ -273,17 +382,37 @@ k_tdt_post(const float *__restrict__ lp, const float *__restrict__ alpha, const 
     }
 }
 
+template <int KD>
+__global__ void __launch_bounds__(kTdtRowThreads)
+k_tdt_post(const float *__restrict__ lp, const float *__restrict__ alpha, const float *__restrict__ beta,
+           const float *__restrict__ ll, const int *__restrict__ status, const int *__restrict__ xn,
+           const int *__restrict__ yn, int64_t cells, int T, int U, int D, TdtDurations dur, FastDiv divU,
+           FastDiv divTU, float *__restrict__ pg) {
+    tdt_post_rows<KD, false>(lp, alpha, beta, ll, status, xn, yn, cells, U, D, dur, divU, divTU, pg, TdtCompact{});
+}
+
+template <int KD>
+__global__ void __launch_bounds__(kTdtRowThreads)
+k_tdt_post_compact(const float *__restrict__ lp, const float *__restrict__ alpha, const float *__restrict__ beta,
+                   const float *__restrict__ ll, const int *__restrict__ status, const int *__restrict__ xn,
+                   const int *__restrict__ yn, int D, TdtDurations dur, float *__restrict__ pg, TdtCompact cp) {
+    tdt_post_rows<KD, true>(lp, alpha, beta, ll, status, xn, yn, cp.STU, cp.max_U, D, dur, FastDiv(), FastDiv(), pg,
+                            cp);
+}
+
 // The row data one gradient element needs.  zero: the row's posteriors are all 0 (padding, no path, or a cell no path
-// visits): the row is written as exact zeros and neither the logits nor lse are read.
+// visits): the row is written as exact zeros and neither the logits nor lse are read.  COMPACT: a row with posteriors
+// lies in an ok lattice, found by tdt_find (U, divU and divTU are not used).
 struct TdtRow {
     const float *pd;
     float occ, pb, pl, lt, ld, sc;
     int lab;
     bool zero;
 };
+template <bool COMPACT>
 __device__ __forceinline__ TdtRow tdt_row(int64_t row, const float2 *lse, const float *pg, const int *labels,
                                           const float *grad_out, int U, int W2, const FastDiv &divU,
-                                          const FastDiv &divTU) {
+                                          const FastDiv &divTU, const TdtCompact &cp, const int *yn) {
     TdtRow r;
     r.pd = pg + row * W2;
     r.pb = r.pd[0];
@@ -296,11 +425,18 @@ __device__ __forceinline__ TdtRow tdt_row(int64_t row, const float2 *lse, const 
         const float2 q = lse[row];
         r.lt = q.x;
         r.ld = q.y;
-        uint32_t n, rem, t, u;
-        divTU.divmod((uint32_t)row, n, rem);
-        divU.divmod(rem, t, u);
-        r.lab = ((int)u < U - 1) ? labels[(int64_t)n * (U - 1) + u] : -1;
-        r.sc = grad_out ? grad_out[n] : 1.0f;
+        if constexpr (COMPACT) {
+            const int n = tdt_find(cp.mem_pref, cp.N, row);
+            const int Un = yn[n] + 1, u = (int)((uint32_t)(row - cp.mem_pref[n]) % (uint32_t)Un);
+            r.lab = (u < Un - 1) ? labels[cp.lab_pref[n] + u] : -1;
+            r.sc = grad_out ? grad_out[n] : 1.0f;
+        } else {
+            uint32_t n, rem, t, u;
+            divTU.divmod((uint32_t)row, n, rem);
+            divU.divmod(rem, t, u);
+            r.lab = ((int)u < U - 1) ? labels[(int64_t)n * (U - 1) + u] : -1;
+            r.sc = grad_out ? grad_out[n] : 1.0f;
+        }
     }
     return r;
 }
@@ -316,22 +452,26 @@ __device__ __forceinline__ float tdt_elem(const TdtRow &r, int v, float xv, int 
 
 // Gradient emit: the flat (rows, W) output in vectors of VEC elements (16 bytes when `out` is 16-byte aligned, else 1),
 // which may straddle rows; XVEC: the logits are read with the same vectors (x aligned as out), else element by element.
-// Every element is computed the same way whatever VEC, XVEC and the element type; bf16 is rounded once on the store.
-template <typename IO, int VEC, bool XVEC>
-__global__ void __launch_bounds__(kTdtRowThreads)
-k_tdt_emit(const IO *__restrict__ x, const float2 *__restrict__ lse, const float *__restrict__ pg,
-           const int *__restrict__ labels, const float *__restrict__ grad_out, IO *__restrict__ out, int64_t total,
-           int V, int D, int blank, int U, FastDiv divU, FastDiv divTU, int64_t stride_rows, int stride_v) {
+// Every element is computed the same way whatever VEC, XVEC, the element type and the layout; bf16 is rounded once on
+// the store.  COMPACT: the rows are the (STU, W) rows of the compact layout, vectors straddle lattices as they
+// straddle rows.
+template <typename IO, int VEC, bool XVEC, bool COMPACT>
+__device__ __forceinline__ void
+tdt_emit_flat(const IO *__restrict__ x, const float2 *__restrict__ lse, const float *__restrict__ pg,
+              const int *__restrict__ labels, const float *__restrict__ grad_out, IO *__restrict__ out, int64_t total,
+              int V, int D, int blank, int U, FastDiv divU, FastDiv divTU, int64_t stride_rows, int stride_v,
+              const TdtCompact &cp, const int *__restrict__ yn) {
     const int W = V + D, W2 = 2 + D;
     int64_t f = ((int64_t)blockIdx.x * kTdtRowThreads + threadIdx.x) * VEC;
     if (f >= total) return;
     int64_t row = f / W;
     int v0 = (int)(f - row * W);
     const int64_t stride = stride_rows * W + stride_v;
+    auto row_at = [&](int64_t i) { return tdt_row<COMPACT>(i, lse, pg, labels, grad_out, U, W2, divU, divTU, cp, yn); };
     for (; f < total; f += stride, row += stride_rows, v0 += stride_v) {
         if (v0 >= W) { v0 -= W; ++row; }
         float e[VEC];
-        TdtRow r = tdt_row(row, lse, pg, labels, grad_out, U, W2, divU, divTU);
+        TdtRow r = row_at(row);
         if (f + VEC <= total) {
             float xv[VEC];
             const bool whole = v0 + VEC <= W;
@@ -345,7 +485,7 @@ k_tdt_emit(const IO *__restrict__ x, const float2 *__restrict__ lse, const float
             int v = v0;
 #pragma unroll
             for (int k = 0; k < VEC; ++k) {
-                if (v == W) { v = 0; ++rw; r = tdt_row(rw, lse, pg, labels, grad_out, U, W2, divU, divTU); }
+                if (v == W) { v = 0; ++rw; r = row_at(rw); }
                 if (!XVEC && !r.zero) xv[k] = io_load(x + f + k);
                 e[k] = tdt_elem(r, v, xv[k], V, blank);
                 ++v;
@@ -357,12 +497,32 @@ k_tdt_emit(const IO *__restrict__ x, const float2 *__restrict__ lse, const float
             int64_t rw = row;
             int v = v0;
             for (int64_t i = f; i < total; ++i) {
-                if (v == W) { v = 0; ++rw; r = tdt_row(rw, lse, pg, labels, grad_out, U, W2, divU, divTU); }
+                if (v == W) { v = 0; ++rw; r = row_at(rw); }
                 st_one(out + i, tdt_elem(r, v, r.zero ? 0.0f : io_load(x + i), V, blank));
                 ++v;
             }
         }
     }
+}
+
+template <typename IO, int VEC, bool XVEC>
+__global__ void __launch_bounds__(kTdtRowThreads)
+k_tdt_emit(const IO *__restrict__ x, const float2 *__restrict__ lse, const float *__restrict__ pg,
+           const int *__restrict__ labels, const float *__restrict__ grad_out, IO *__restrict__ out, int64_t total,
+           int V, int D, int blank, int U, FastDiv divU, FastDiv divTU, int64_t stride_rows, int stride_v) {
+    tdt_emit_flat<IO, VEC, XVEC, false>(x, lse, pg, labels, grad_out, out, total, V, D, blank, U, divU, divTU,
+                                        stride_rows, stride_v, TdtCompact{}, nullptr);
+}
+
+// total = STU * (V + D)
+template <typename IO, int VEC, bool XVEC>
+__global__ void __launch_bounds__(kTdtRowThreads)
+k_tdt_emit_compact(const IO *__restrict__ x, const float2 *__restrict__ lse, const float *__restrict__ pg,
+                   const int *__restrict__ labels, const int *__restrict__ yn, const float *__restrict__ grad_out,
+                   IO *__restrict__ out, int64_t total, int V, int D, int blank, int64_t stride_rows, int stride_v,
+                   TdtCompact cp) {
+    tdt_emit_flat<IO, VEC, XVEC, true>(x, lse, pg, labels, grad_out, out, total, V, D, blank, 0, FastDiv(), FastDiv(),
+                                       stride_rows, stride_v, cp, yn);
 }
 
 // Process-wide, unlike the loss' per-thread record (api.cu): autograd runs the backward on its own device thread, and
@@ -401,14 +561,25 @@ TdtPlan tdt_plan(int U, const TdtDurations &dur, const void *x, int elem_bytes, 
     return p;
 }
 
+// the compact layout of a forward (c.mem_pref set)
+static TdtCompact tdt_compact(const TdtFwd &c) { return {c.mem_pref, c.lab_pref, c.STU, c.N, c.T, c.U}; }
+
 template <typename IN>
 static cudaError_t tdt_norm_as(cudaStream_t s, const TdtPlan &p, const IN *x, const TdtFwd &c, int64_t cells) {
-    const FastDiv divU((uint32_t)c.U), divTU((uint32_t)(c.T * c.U));
+    // the dense cell -> (n, t, u) divisions (the compact kernels find lattices through mem_pref instead)
+    const FastDiv divU = c.mem_pref ? FastDiv() : FastDiv((uint32_t)c.U);
+    const FastDiv divTU = c.mem_pref ? FastDiv() : FastDiv((uint32_t)(c.T * c.U));
     const int64_t per_block = kTdtRowThreads / p.norm_lanes;
     const unsigned grid = (unsigned)min((cells + per_block - 1) / per_block, (int64_t)sm_count(current_device()) * 16);
+    // compact: CTA rows per lattice as logits.cu's compact normaliser sizes them
+    const dim3 cgrid(compact_gx(cells, c.N, per_block * kCompactIters), c.N);
 #define RNNT_TDT_NORM(SUB, G)                                                                                         \
-    k_tdt_norm<IN, SUB, G><<<grid, kTdtRowThreads, 0, s>>>(x, c.labels, c.xn, c.yn, cells, c.T, c.U, c.V, c.dur.D,     \
-                                                           c.blank, c.sigma, divU, divTU, c.lse, c.lp)
+    (c.mem_pref                                                                                                       \
+         ? k_tdt_norm_compact<IN, SUB, G><<<cgrid, kTdtRowThreads, 0, s>>>(x, c.labels, c.xn, c.yn, c.V, c.dur.D,     \
+                                                                           c.blank, c.sigma, c.lse, c.lp,             \
+                                                                           tdt_compact(c))                            \
+         : k_tdt_norm<IN, SUB, G><<<grid, kTdtRowThreads, 0, s>>>(x, c.labels, c.xn, c.yn, cells, c.T, c.U, c.V,      \
+                                                                  c.dur.D, c.blank, c.sigma, divU, divTU, c.lse, c.lp))
     if (p.norm_lanes == 8) {
         if (p.norm_group == 4) RNNT_TDT_NORM(8, 4); else if (p.norm_group == 2) RNNT_TDT_NORM(8, 2); else RNNT_TDT_NORM(8, 1);
     } else {
@@ -421,28 +592,37 @@ static cudaError_t tdt_norm_as(cudaStream_t s, const TdtPlan &p, const IN *x, co
 
 template <int KD>
 static cudaError_t tdt_recur_post(cudaStream_t s, const TdtPlan &p, const TdtFwd &c, int64_t cells) {
-    static std::atomic<bool> smem_set[kMaxDevices];
+    static std::atomic<bool> smem_set[kMaxDevices], smem_set_compact[kMaxDevices];
     if (p.smem > (48 << 10)) {
-        const cudaError_t e = ensure_dyn_smem(k_tdt_recur<KD>, smem_set, max_optin_smem(current_device()));
+        const cudaError_t e = c.mem_pref ? ensure_dyn_smem(k_tdt_recur_compact<KD>, smem_set_compact,
+                                                           max_optin_smem(current_device()))
+                                         : ensure_dyn_smem(k_tdt_recur<KD>, smem_set, max_optin_smem(current_device()));
         if (e != cudaSuccess) return e;
     }
     TdtRec r = {c.lp, c.labels, c.xn, c.yn, c.alpha, c.beta, c.ll, c.costs, c.status, c.T, c.U, c.V, c.dur.D, p.ring,
                 c.dur};
-    k_tdt_recur<KD><<<dim3(c.N, 2), p.warps * 32, p.smem, s>>>(r);
+    if (c.mem_pref) k_tdt_recur_compact<KD><<<dim3(c.N, 2), p.warps * 32, p.smem, s>>>(r, tdt_compact(c));
+    else k_tdt_recur<KD><<<dim3(c.N, 2), p.warps * 32, p.smem, s>>>(r);
     count_launch();
     cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess || !c.pg) return e;
-    const FastDiv divU((uint32_t)c.U), divTU((uint32_t)(c.T * c.U));
+    if (e != cudaSuccess || !c.pg || cells == 0) return e;
+    // the dense cell -> (n, t, u) divisions (the compact kernels find lattices through mem_pref instead)
+    const FastDiv divU = c.mem_pref ? FastDiv() : FastDiv((uint32_t)c.U);
+    const FastDiv divTU = c.mem_pref ? FastDiv() : FastDiv((uint32_t)(c.T * c.U));
     const unsigned grid = (unsigned)min((cells + kTdtRowThreads - 1) / kTdtRowThreads,
                                         (int64_t)sm_count(current_device()) * 16);
-    k_tdt_post<KD><<<grid, kTdtRowThreads, 0, s>>>(c.lp, c.alpha, c.beta, c.ll, c.status, c.xn, c.yn, cells, c.T, c.U,
-                                                   c.dur.D, c.dur, divU, divTU, c.pg);
+    if (c.mem_pref)
+        k_tdt_post_compact<KD><<<grid, kTdtRowThreads, 0, s>>>(c.lp, c.alpha, c.beta, c.ll, c.status, c.xn, c.yn,
+                                                               c.dur.D, c.dur, c.pg, tdt_compact(c));
+    else
+        k_tdt_post<KD><<<grid, kTdtRowThreads, 0, s>>>(c.lp, c.alpha, c.beta, c.ll, c.status, c.xn, c.yn, cells, c.T,
+                                                       c.U, c.dur.D, c.dur, divU, divTU, c.pg);
     count_launch();
     return cudaGetLastError();
 }
 
 cudaError_t launch_tdt_forward(cudaStream_t s, const TdtFwd &c) {
-    const int64_t cells = (int64_t)c.N * c.T * c.U;
+    const int64_t cells = c.mem_pref ? c.STU : (int64_t)c.N * c.T * c.U;
     const TdtPlan p = tdt_plan(c.U, c.dur, c.x, c.io_bf16 ? 2 : 4, c.V);
     {
         std::lock_guard<std::mutex> lock(g_tdt_mu);
@@ -458,7 +638,7 @@ cudaError_t launch_tdt_forward(cudaStream_t s, const TdtFwd &c) {
         rec[RNNT_TDT_REC_NORM_LANES] = p.norm_lanes;
         rec[RNNT_TDT_REC_SMEM] = p.smem;
     }
-    if (cells == 0) return cudaSuccess;
+    if (cells == 0 && !c.mem_pref) return cudaSuccess;   // compact: with no rows the recurrence still gives the costs
     cudaError_t e = c.io_bf16 ? tdt_norm_as(s, p, static_cast<const __nv_bfloat16 *>(c.x), c, cells)
                               : tdt_norm_as(s, p, static_cast<const float *>(c.x), c, cells);
     if (e != cudaSuccess) return e;
@@ -468,7 +648,7 @@ cudaError_t launch_tdt_forward(cudaStream_t s, const TdtFwd &c) {
 template <typename IO>
 static cudaError_t tdt_emit_as(cudaStream_t s, const TdtBwd &c, const IO *x, IO *out) {
     const int W = c.V + c.D;
-    const int64_t total = (int64_t)c.N * c.T * c.U * W;
+    const int64_t total = (c.mem_pref ? c.STU : (int64_t)c.N * c.T * c.U) * W;
     constexpr int kVec = 16 / (int)sizeof(IO);
     const bool ovec = (reinterpret_cast<uintptr_t>(out) & 15u) == 0;
     const bool xvec = ovec && (reinterpret_cast<uintptr_t>(x) & 15u) == 0;
@@ -479,16 +659,23 @@ static cudaError_t tdt_emit_as(cudaStream_t s, const TdtBwd &c, const IO *x, IO 
         g_tdt_record[RNNT_TDT_REC_EMIT_XVEC] = xvec;
     }
     if (total == 0) return cudaSuccess;
-    const FastDiv divU((uint32_t)c.U), divTU((uint32_t)(c.T * c.U));
+    // the dense cell -> (n, t, u) divisions (the compact kernels find lattices through mem_pref instead)
+    const FastDiv divU = c.mem_pref ? FastDiv() : FastDiv((uint32_t)c.U);
+    const FastDiv divTU = c.mem_pref ? FastDiv() : FastDiv((uint32_t)(c.T * c.U));
     const int64_t vecs = (total + vec - 1) / vec;
     const unsigned grid = (unsigned)min((vecs + kTdtRowThreads - 1) / kTdtRowThreads,
                                         (int64_t)sm_count(current_device()) * 32);
     const int64_t stride = (int64_t)grid * kTdtRowThreads * vec;
     const int64_t srows = stride / W;
     const int sv = (int)(stride - srows * W);
+    const TdtCompact cp = {c.mem_pref, c.lab_pref, c.STU, c.N, 0, 0};
 #define RNNT_TDT_EMIT(VEC, XV)                                                                                        \
-    k_tdt_emit<IO, VEC, XV><<<grid, kTdtRowThreads, 0, s>>>(x, c.lse, c.pg, c.labels, c.grad_out, out, total, c.V, c.D, \
-                                                            c.blank, c.U, divU, divTU, srows, sv)
+    (c.mem_pref                                                                                                       \
+         ? k_tdt_emit_compact<IO, VEC, XV><<<grid, kTdtRowThreads, 0, s>>>(x, c.lse, c.pg, c.labels, c.yn, c.grad_out, \
+                                                                           out, total, c.V, c.D, c.blank, srows, sv,  \
+                                                                           cp)                                        \
+         : k_tdt_emit<IO, VEC, XV><<<grid, kTdtRowThreads, 0, s>>>(x, c.lse, c.pg, c.labels, c.grad_out, out, total,  \
+                                                                   c.V, c.D, c.blank, c.U, divU, divTU, srows, sv))
     if (!ovec) RNNT_TDT_EMIT(1, false);
     else if (xvec) RNNT_TDT_EMIT(kVec, true);
     else RNNT_TDT_EMIT(kVec, false);
