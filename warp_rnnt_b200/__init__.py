@@ -145,10 +145,11 @@ class RNNTLossFromLogits(torch.autograd.Function):
     logits; the gradient has the logits' dtype, costs are float32."""
 
     @staticmethod
-    def forward(ctx, logits, labels, frames_lengths, labels_lengths, blank=0, fastemit_lambda=0.0):
+    def forward(ctx, logits, labels, frames_lengths, labels_lengths, blank=0, fastemit_lambda=0.0, rnnt_type=0,
+                delay_penalty=0.0):
         need = ctx.needs_input_grad[0]
         costs, lse, pg = _C.rnnt_logits_forward(logits, labels, frames_lengths, labels_lengths, blank,
-                                                fastemit_lambda, need, 0)
+                                                fastemit_lambda, need, 0, rnnt_type, delay_penalty)
         if need:
             ctx.save_for_backward(logits, lse, pg, labels)
             ctx.blank = blank
@@ -158,7 +159,7 @@ class RNNTLossFromLogits(torch.autograd.Function):
     def backward(ctx, grads_output):
         logits, lse, pg, labels = ctx.saved_tensors
         go = grads_output.contiguous().to(torch.float32)
-        return _C.rnnt_logits_backward(logits, lse, pg, labels, go, ctx.blank), None, None, None, None, None
+        return _C.rnnt_logits_backward(logits, lse, pg, labels, go, ctx.blank), None, None, None, None, None, None, None
 
 
 class RNNTLossFromLogitsCompact(torch.autograd.Function):
@@ -198,8 +199,26 @@ def _reduce(costs, frames_lengths, average_frames, reduction):
     return costs
 
 
+_RNNT_TYPES = {"regular": 0, "modified": 1, "constrained": 2}
+
+
+def _path_type(fn, rnnt_type, delay_penalty, fastemit_lambda=0.0, compact=False):
+    """k2's ``rnnt_type`` and ``delay_penalty`` checked on the host: (type id, penalty), or ValueError."""
+    if not isinstance(rnnt_type, str) or rnnt_type not in _RNNT_TYPES:
+        raise ValueError("%s: rnnt_type must be 'regular', 'modified' or 'constrained', got %r" % (fn, rnnt_type))
+    if isinstance(delay_penalty, bool) or not isinstance(delay_penalty, (int, float)) \
+            or not math.isfinite(delay_penalty) or delay_penalty < 0:
+        raise ValueError("%s: delay_penalty must be a finite number >= 0, got %r" % (fn, delay_penalty))
+    if rnnt_type != "regular" and fastemit_lambda != 0:
+        raise ValueError("%s: fastemit_lambda is only offered with rnnt_type='regular', got %r with %r"
+                         % (fn, fastemit_lambda, rnnt_type))
+    if compact and (rnnt_type != "regular" or delay_penalty != 0):
+        raise ValueError("%s: compact=True takes rnnt_type='regular' and delay_penalty=0 only" % fn)
+    return _RNNT_TYPES[rnnt_type], float(delay_penalty)
+
+
 def rnnt_loss_from_logits(logits, labels, frames_lengths, labels_lengths, average_frames=False, reduction="none",
-                          blank=0, fastemit_lambda=0.0, compact=False):
+                          blank=0, fastemit_lambda=0.0, compact=False, rnnt_type="regular", delay_penalty=0.0):
     """``rnnt_loss(log_softmax(logits, -1), ...)`` in three dense passes instead of seven; the gradient is w.r.t. the
     LOGITS.  Dense (N,T,U,V) layout, float32 or bfloat16 (what ``torch.autocast(dtype=torch.bfloat16)`` makes of the
     joint network's output); other arguments as in ``rnnt_loss``.  Agrees with ``torch.log_softmax`` + the reference
@@ -212,14 +231,31 @@ def rnnt_loss_from_logits(logits, labels, frames_lengths, labels_lengths, averag
     ``compact=True``: ``logits`` is (STU, V), float32 or bfloat16, rows in ``joint_pack``'s order
     (STU = sum frames_lengths * (labels_lengths + 1)); ``labels`` is (sum labels_lengths,) int32, as for
     ``rnnt_loss(compact=True)``, and so are the shape checks and ``compact_hints``.  Costs are float32, the gradient is
-    w.r.t. the packed logits and has their dtype."""
+    w.r.t. the packed logits and has their dtype.
+
+    ``rnnt_type`` and ``delay_penalty`` are k2's (``rnnt_loss(..., rnnt_type=, delay_penalty=)``), dense layout only:
+      - ``"regular"`` (default): the lattice above, a label edge stays in its frame.
+      - ``"modified"``: one symbol per frame, a label edge (t,u)->(t+1,u+1) also leaves the frame; a lattice with more
+        labels than frames has no path (cost +inf).
+      - ``"constrained"``: modified, with each label edge weighted by its log-prob plus the blank log-prob of the cell it
+        reaches in the same frame (k2's ``px += py[:, 1:, :]``).
+      - ``delay_penalty`` (lambda >= 0): adds lambda * ((T_n - 1) / 2 - t) to every label log-prob of frame t, so that
+        paths emitting earlier score higher (icefall's streaming recipes).  The costs include the penalty, as k2's do.
+    Non-regular types take no FastEmit (k2 has none); regular + penalty + FastEmit compose.  A lattice with invalid
+    lengths gets cost NaN, one without a finite path +inf, one with a NaN in its live log-probs NaN, with zero, zero and
+    NaN gradients; the one-symbol-per-frame types take label dimensions up to 25599 (include/rnnt_b200.h).  Bad values
+    raise ValueError before any launch."""
     assert average_frames is None or isinstance(average_frames, bool)
     assert reduction is None or reduction in ("none", "mean", "sum")
     assert isinstance(blank, int)
     assert isinstance(compact, bool)
     assert not labels.requires_grad and not frames_lengths.requires_grad and not labels_lengths.requires_grad
-    fn = RNNTLossFromLogitsCompact if compact else RNNTLossFromLogits
-    costs = fn.apply(logits, labels, frames_lengths, labels_lengths, blank, fastemit_lambda)
+    kind, lam = _path_type("rnnt_loss_from_logits", rnnt_type, delay_penalty, fastemit_lambda, compact)
+    if compact:
+        costs = RNNTLossFromLogitsCompact.apply(logits, labels, frames_lengths, labels_lengths, blank, fastemit_lambda)
+    else:
+        costs = RNNTLossFromLogits.apply(logits, labels, frames_lengths, labels_lengths, blank, fastemit_lambda, kind,
+                                         lam)
     return _reduce(costs, frames_lengths, average_frames, reduction)
 
 
@@ -230,10 +266,11 @@ class RNNTLossPruned(torch.autograd.Function):
     d logits (N,T,S,V), of the logits' dtype."""
 
     @staticmethod
-    def forward(ctx, logits, labels, frames_lengths, labels_lengths, ranges, blank=0, fastemit_lambda=0.0):
+    def forward(ctx, logits, labels, frames_lengths, labels_lengths, ranges, blank=0, fastemit_lambda=0.0, rnnt_type=0,
+                delay_penalty=0.0):
         need = ctx.needs_input_grad[0]
         costs, lse, pg = _C.rnnt_logits_pruned_forward(logits, labels, frames_lengths, labels_lengths, ranges, blank,
-                                                       fastemit_lambda, need, 0)
+                                                       fastemit_lambda, need, 0, rnnt_type, delay_penalty)
         if need:
             ctx.save_for_backward(logits, lse, pg, labels, ranges)
             ctx.blank = blank
@@ -244,11 +281,11 @@ class RNNTLossPruned(torch.autograd.Function):
         logits, lse, pg, labels, ranges = ctx.saved_tensors
         go = grads_output.contiguous().to(torch.float32)
         g = _C.rnnt_logits_pruned_backward(logits, lse, pg, labels, ranges, go, ctx.blank)
-        return g, None, None, None, None, None, None
+        return g, None, None, None, None, None, None, None, None
 
 
 def rnnt_loss_pruned(logits, labels, frames_lengths, labels_lengths, ranges, average_frames=False, reduction="none",
-                     blank=0, fastemit_lambda=0.0):
+                     blank=0, fastemit_lambda=0.0, rnnt_type="regular", delay_penalty=0.0):
     """Pruned RNN-T loss: the transducer loss from a joint network evaluated only in a window of S label columns per
     frame, which takes about U/S times less memory and traffic than the full (N,T,U,V) joint output.
 
@@ -258,6 +295,9 @@ def rnnt_loss_pruned(logits, labels, frames_lengths, labels_lengths, ranges, ave
         frames_lengths, labels_lengths: (N,) int32.
         ranges: (N, T) int32; ranges[n, t] is the first label column of frame t's window.
         average_frames, reduction, blank, fastemit_lambda: as in ``rnnt_loss_from_logits``.
+        rnnt_type, delay_penalty: k2's, as in ``rnnt_loss_from_logits``, on the full lattice with the edges out of the
+            cells outside the windows removed.  A constrained label edge also reads the blank of the cell it
+            reaches, so it is removed when that cell lies outside its frame's window.
 
     Row (n, t, s) of ``logits`` is lattice cell (t, u = ranges[n, t] + s) when t < frames_lengths[n] and
     0 <= u <= labels_lengths[n]; any other row is padding.  Frame t's window is {u : r <= u < r + S} clipped to the
@@ -277,7 +317,9 @@ def rnnt_loss_pruned(logits, labels, frames_lengths, labels_lengths, ranges, ave
     assert isinstance(blank, int)
     assert not labels.requires_grad and not frames_lengths.requires_grad and not labels_lengths.requires_grad
     assert not ranges.requires_grad
-    costs = RNNTLossPruned.apply(logits, labels, frames_lengths, labels_lengths, ranges, blank, fastemit_lambda)
+    kind, lam = _path_type("rnnt_loss_pruned", rnnt_type, delay_penalty, fastemit_lambda)
+    costs = RNNTLossPruned.apply(logits, labels, frames_lengths, labels_lengths, ranges, blank, fastemit_lambda, kind,
+                                 lam)
     return _reduce(costs, frames_lengths, average_frames, reduction)
 
 
@@ -434,10 +476,11 @@ class RNNTLossSimple(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, am, lm, labels, frames_lengths, labels_lengths, blank=0, prune_range=0, lm_only_scale=0.0,
-                am_only_scale=0.0):
+                am_only_scale=0.0, rnnt_type=0, delay_penalty=0.0):
         need = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
         costs, saved, pg, ranges = _C.rnnt_simple_forward(am, lm, labels, frames_lengths, labels_lengths, blank, need,
-                                                          prune_range, 0, lm_only_scale, am_only_scale)
+                                                          prune_range, 0, lm_only_scale, am_only_scale, rnnt_type,
+                                                          delay_penalty)
         if need:
             ctx.save_for_backward(am, lm, labels, frames_lengths, labels_lengths, saved, pg)
             ctx.blank = blank
@@ -451,7 +494,7 @@ class RNNTLossSimple(torch.autograd.Function):
         go = grads_output.contiguous().to(torch.float32)
         dam, dlm = _C.rnnt_simple_backward(am, lm, labels, xn, yn, saved, pg, go, ctx.blank, *ctx.scales)
         return (dam if ctx.needs_input_grad[0] else None), (dlm if ctx.needs_input_grad[1] else None), \
-            None, None, None, None, None, None, None
+            None, None, None, None, None, None, None, None, None
 
 
 def _smoothing_scale(name, x):
@@ -461,7 +504,7 @@ def _smoothing_scale(name, x):
 
 
 def rnnt_loss_simple(am, lm, labels, frames_lengths, labels_lengths, average_frames=False, reduction="none", blank=0,
-                     prune_range=None, lm_only_scale=0.0, am_only_scale=0.0):
+                     prune_range=None, lm_only_scale=0.0, am_only_scale=0.0, rnnt_type="regular", delay_penalty=0.0):
     """Simple transducer loss of the pruned recipe, and the windows ``rnnt_loss_pruned`` takes.  Follows k2's
     ``rnnt_loss_simple`` + ``get_rnnt_prune_ranges`` (regular lattice), and with ``lm_only_scale`` /
     ``am_only_scale`` k2's ``rnnt_loss_smoothed``; not tested against k2.
@@ -475,6 +518,11 @@ def rnnt_loss_simple(am, lm, labels, frames_lengths, labels_lengths, average_fra
             ``rnnt_loss_pruned(..., ranges)`` with windows of S labels.
         lm_only_scale, am_only_scale: k2's smoothing scales sl, sa: finite, >= 0, sl + sa < 1 (else ValueError).
             Both 0 (the default) is the plain simple loss, with the same kernels and the same bits.
+        rnnt_type, delay_penalty: k2's, as in ``rnnt_loss_from_logits`` (the penalty goes on the smoothed pairs).
+            With "modified" / "constrained", ``prune_range`` may be 1 and the windows move by at most one column a frame
+            (k2's ``_adjust_pruning_lower_bound(s_begin, 2)``); they are scored from the raw edge occupations, for
+            "constrained" the blank edges' before their label-edge share is folded in.  The last frame's window then
+            holds the last label whenever labels_lengths - prune_range + 1 <= frames_lengths - 1.
 
     The loss is the RNN-T loss of lattice n in which cell (t, u) has the log-probs log_softmax(am[n,t] + lm[n,u]) at
     ``blank`` and at labels[n,u].  Its normaliser is log(sum_v exp(am[n,t,v]) exp(lm[n,u,v])), a fp32 contraction over
@@ -516,15 +564,18 @@ def rnnt_loss_simple(am, lm, labels, frames_lengths, labels_lengths, average_fra
     if am.dtype != torch.float32 or lm.dtype != torch.float32:
         raise TypeError("rnnt_loss_simple: am and lm must be float32, got %s and %s (bfloat16 is not supported; "
                         "run this loss outside autocast or cast with .float())" % (am.dtype, lm.dtype))
+    kind, lam = _path_type("rnnt_loss_simple", rnnt_type, delay_penalty)
+    least = 2 if kind == 0 else 1
     if prune_range is not None and (isinstance(prune_range, bool) or not isinstance(prune_range, int)
-                                    or prune_range < 2):
-        raise ValueError("rnnt_loss_simple: prune_range must be None or an int >= 2, got %r" % (prune_range,))
+                                    or prune_range < least):
+        raise ValueError("rnnt_loss_simple: prune_range must be None or an int >= %d, got %r" % (least, prune_range))
     sl = _smoothing_scale("lm_only_scale", lm_only_scale)
     sa = _smoothing_scale("am_only_scale", am_only_scale)
     # the kernels take the scales as float32: the check is on the values they see
     if torch.tensor(sl, dtype=torch.float32).item() + torch.tensor(sa, dtype=torch.float32).item() >= 1.0:
         raise ValueError("rnnt_loss_simple: lm_only_scale + am_only_scale must be < 1, got %r + %r" % (sl, sa))
-    costs, ranges = RNNTLossSimple.apply(am, lm, labels, frames_lengths, labels_lengths, blank, prune_range or 0, sl, sa)
+    costs, ranges = RNNTLossSimple.apply(am, lm, labels, frames_lengths, labels_lengths, blank, prune_range or 0, sl, sa,
+                                         kind, lam)
     costs = _reduce(costs, frames_lengths, average_frames, reduction)
     return costs if prune_range is None else (costs, ranges)
 

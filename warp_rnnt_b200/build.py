@@ -21,7 +21,8 @@ LIB = os.path.join(LIBDIR, "librnnt_b200.so")
 EXT = os.path.join(LIBDIR, "_C.so")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
-CU_SOURCES = ["wavefront.cu", "expand.cu", "fused.cu", "logits.cu", "joint.cu", "simple.cu", "tdt.cu", "api.cu"]
+CU_SOURCES = ["wavefront.cu", "expand.cu", "fused.cu", "logits.cu", "joint.cu", "simple.cu", "tdt.cu", "frames.cu",
+              "api.cu"]
 CU_HEADERS = ["common.cuh", "kernels.cuh", os.path.join(INCLUDE, "rnnt_b200.h")]
 
 

@@ -466,6 +466,33 @@ static int run_loss(cudaStream_t s, void *workspace, size_t workspace_bytes, con
     return RNNT_STATUS_SUCCESS;
 }
 
+// k2's lattice type and delay penalty (include/rnnt_b200.h): 0 regular, 1 modified, 2 constrained; lam finite, >= 0.
+// The one-symbol-per-frame types take no FastEmit and rows of at most kFramesMaxU columns.
+static bool path_type_ok(int rnnt_type, float delay_penalty, float fastemit_lambda, int U) {
+    if (rnnt_type < 0 || rnnt_type > 2 || !std::isfinite(delay_penalty) || delay_penalty < 0.0f) return false;
+    return rnnt_type == 0 || (fastemit_lambda == 0.0f && U <= kFramesMaxU);
+}
+
+// A dense k2-family call on its pairs c.pairs (the workspace's, or the caller's): the delay penalty into the workspace's
+// pairs, then the regular driver (run_loss) or the frame sweep.  raw_blank: k_frames_grads' unfolded blank slots, or null.
+static int run_typed(cudaStream_t s, void *workspace, size_t workspace_bytes, const Workspace &w, LossCall c,
+                     int rnnt_type, float delay_penalty, float *raw_blank) {
+    const bool delayed = delay_penalty != 0.0f;
+    if (delayed) {
+        RNNT_TRY(launch_delay_pairs(s, c.pairs, w.pairs, c.p.xn, c.p.yn, c.p.N, c.T, c.U, delay_penalty),
+                 RNNT_STATUS_GATHER_FAILED);
+        c.pairs = w.pairs;
+    }
+    if (rnnt_type == 0) return run_loss(s, workspace, workspace_bytes, c);
+    FramesCall f = {};
+    f.pairs = c.pairs; f.xn = c.p.xn; f.yn = c.p.yn;
+    f.alphas = w.alphas; f.betas = w.betas; f.ll = w.ll; f.status = w.bad;
+    f.costs = c.costs; f.pair_grads = c.pair_grads; f.raw_blank = c.pair_grads ? raw_blank : nullptr;
+    f.N = c.p.N; f.T = c.T; f.U = c.U; f.constrained = rnnt_type == 2;
+    RNNT_TRY(launch_frames(s, f, delayed), RNNT_STATUS_WARP_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
 // dense layout, log_probs / grads of 4-byte (f32) or 2-byte (bf16) elements
 static int loss_dense_any(void *stream, void *workspace, size_t workspace_bytes, const void *log_probs,
                           const int *labels, const int *xn, const int *yn, float *costs, void *grads,
@@ -484,8 +511,10 @@ static int loss_dense_any(void *stream, void *workspace, size_t workspace_bytes,
 static int logits_forward_any(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
                               const int *labels, const int *xn, const int *yn, float *costs, float *lse,
                               float *pair_grads, int N, int T, int U, int V, int blank, float fastemit_lambda,
-                              int lse_mode, int io_bf16) {
-    if (!dense_args_ok(N, T, U, V, blank) || !lse || !pairs_aligned(pair_grads)) return RNNT_STATUS_INVALID_ARGUMENT;
+                              int lse_mode, int io_bf16, int rnnt_type, float delay_penalty) {
+    if (!dense_args_ok(N, T, U, V, blank) || !lse || !pairs_aligned(pair_grads) ||
+        !path_type_ok(rnnt_type, delay_penalty, fastemit_lambda, U))
+        return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
     cudaStream_t s = (cudaStream_t)stream;
     LossCall c = dense_call(xn, yn, N, T, U, costs, fastemit_lambda, lse_mode);
@@ -494,7 +523,7 @@ static int logits_forward_any(void *stream, void *workspace, size_t workspace_by
     // one pass over the logits: normaliser per cell + the two normalised log-probs the recurrence needs
     RNNT_TRY(launch_lse_pairs(s, logits, labels, N, T, U, V, blank, w.pairs, lse, io_bf16), RNNT_STATUS_GATHER_FAILED);
     c.pairs = w.pairs; c.pair_grads = reinterpret_cast<float2 *>(pair_grads);
-    return run_loss(s, workspace, workspace_bytes, c);
+    return run_typed(s, workspace, workspace_bytes, w, c, rnnt_type, delay_penalty, nullptr);
 }
 
 static int logits_backward_any(void *stream, const void *logits, const float *lse, const float *pair_grads,
@@ -725,12 +754,24 @@ int rnnt_b200_rescale(void *stream, void *grads, const float *grad_out, int grad
 int rnnt_b200_loss_pairs(void *stream, void *workspace, size_t workspace_bytes, const float *pairs, const int *xn,
                          const int *yn, float *costs, float *pair_grads, int N, int T, int U,
                          float fastemit_lambda, int lse_mode) {
-    if (!dense_args_ok(N, T, U, 2, 0) || !pairs_aligned(pairs) || !pairs_aligned(pair_grads))
+    return rnnt_b200_loss_pairs_ex(stream, workspace, workspace_bytes, pairs, xn, yn, costs, pair_grads, N, T, U,
+                                   fastemit_lambda, lse_mode, 0, 0.0f);
+}
+
+int rnnt_b200_loss_pairs_ex(void *stream, void *workspace, size_t workspace_bytes, const float *pairs, const int *xn,
+                            const int *yn, float *costs, float *pair_grads, int N, int T, int U, float fastemit_lambda,
+                            int lse_mode, int rnnt_type, float delay_penalty) {
+    if (!dense_args_ok(N, T, U, 2, 0) || !pairs_aligned(pairs) || !pairs_aligned(pair_grads) ||
+        !path_type_ok(rnnt_type, delay_penalty, fastemit_lambda, U))
         return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
     LossCall c = dense_call(xn, yn, N, T, U, costs, fastemit_lambda, lse_mode);
     c.pairs = reinterpret_cast<const float2 *>(pairs); c.pair_grads = reinterpret_cast<float2 *>(pair_grads);
-    return run_loss((cudaStream_t)stream, workspace, workspace_bytes, c);
+    if (rnnt_type == 0 && delay_penalty == 0.0f)        // the regular loss: the fused kernel needs no workspace
+        return run_loss((cudaStream_t)stream, workspace, workspace_bytes, c);
+    Workspace w;
+    if (!carve_ok(workspace, workspace_bytes, c.cells, N, &w)) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    return run_typed((cudaStream_t)stream, workspace, workspace_bytes, w, c, rnnt_type, delay_penalty, nullptr);
 }
 
 int rnnt_b200_gather_forward(void *stream, void *workspace, size_t workspace_bytes, const float *log_probs,
@@ -747,8 +788,16 @@ int rnnt_b200_logits_forward(void *stream, void *workspace, size_t workspace_byt
                               const int *labels, const int *xn, const int *yn, float *costs, float *lse,
                               float *pair_grads, int N, int T, int U, int V, int blank, float fastemit_lambda,
                               int lse_mode) {
+    return rnnt_b200_logits_forward_ex(stream, workspace, workspace_bytes, logits, labels, xn, yn, costs, lse,
+                                       pair_grads, N, T, U, V, blank, fastemit_lambda, lse_mode, 0, 0.0f);
+}
+
+int rnnt_b200_logits_forward_ex(void *stream, void *workspace, size_t workspace_bytes, const float *logits,
+                                const int *labels, const int *xn, const int *yn, float *costs, float *lse,
+                                float *pair_grads, int N, int T, int U, int V, int blank, float fastemit_lambda,
+                                int lse_mode, int rnnt_type, float delay_penalty) {
     return logits_forward_any(stream, workspace, workspace_bytes, logits, labels, xn, yn, costs, lse, pair_grads, N, T,
-                              U, V, blank, fastemit_lambda, lse_mode, 0);
+                              U, V, blank, fastemit_lambda, lse_mode, 0, rnnt_type, delay_penalty);
 }
 
 int rnnt_b200_logits_backward(void *stream, const float *logits, const float *lse, const float *pair_grads,
@@ -761,9 +810,17 @@ int rnnt_b200_logits_forward_bf16(void *stream, void *workspace, size_t workspac
                                   const int *labels, const int *xn, const int *yn, float *costs, float *lse,
                                   float *pair_grads, int N, int T, int U, int V, int blank, float fastemit_lambda,
                                   int lse_mode) {
+    return rnnt_b200_logits_forward_bf16_ex(stream, workspace, workspace_bytes, logits_bf16, labels, xn, yn, costs, lse,
+                                            pair_grads, N, T, U, V, blank, fastemit_lambda, lse_mode, 0, 0.0f);
+}
+
+int rnnt_b200_logits_forward_bf16_ex(void *stream, void *workspace, size_t workspace_bytes, const void *logits_bf16,
+                                     const int *labels, const int *xn, const int *yn, float *costs, float *lse,
+                                     float *pair_grads, int N, int T, int U, int V, int blank, float fastemit_lambda,
+                                     int lse_mode, int rnnt_type, float delay_penalty) {
     if (reinterpret_cast<uintptr_t>(logits_bf16) & 1u) return RNNT_STATUS_INVALID_ARGUMENT;
     return logits_forward_any(stream, workspace, workspace_bytes, logits_bf16, labels, xn, yn, costs, lse, pair_grads,
-                              N, T, U, V, blank, fastemit_lambda, lse_mode, 1);
+                              N, T, U, V, blank, fastemit_lambda, lse_mode, 1, rnnt_type, delay_penalty);
 }
 
 int rnnt_b200_logits_backward_bf16(void *stream, const void *logits_bf16, const float *lse, const float *pair_grads,
@@ -845,9 +902,19 @@ int rnnt_b200_logits_pruned_forward(void *stream, void *workspace, size_t worksp
                                     const int *labels, const int *xn, const int *yn, const int *ranges, float *costs,
                                     float *lse, float *pair_grads, int N, int T, int S, int U, int V, int blank,
                                     float fastemit_lambda, int lse_mode, int elem_bytes) {
+    return rnnt_b200_logits_pruned_forward_ex(stream, workspace, workspace_bytes, logits, labels, xn, yn, ranges, costs,
+                                              lse, pair_grads, N, T, S, U, V, blank, fastemit_lambda, lse_mode,
+                                              elem_bytes, 0, 0.0f);
+}
+
+int rnnt_b200_logits_pruned_forward_ex(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                       const int *labels, const int *xn, const int *yn, const int *ranges,
+                                       float *costs, float *lse, float *pair_grads, int N, int T, int S, int U, int V,
+                                       int blank, float fastemit_lambda, int lse_mode, int elem_bytes, int rnnt_type,
+                                       float delay_penalty) {
     if ((elem_bytes != 4 && elem_bytes != 2) || (reinterpret_cast<uintptr_t>(logits) & (uintptr_t)(elem_bytes - 1)) ||
         !pruned_args_ok(N, T, S, U, V, blank) || !lse || !pairs_aligned(pair_grads) ||
-        !workspace_aligned16(workspace))
+        !workspace_aligned16(workspace) || !path_type_ok(rnnt_type, delay_penalty, fastemit_lambda, U))
         return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
     cudaStream_t s = (cudaStream_t)stream;
@@ -858,7 +925,7 @@ int rnnt_b200_logits_pruned_forward(void *stream, void *workspace, size_t worksp
     RNNT_TRY(launch_lse_pairs_pruned(s, logits, labels, ranges, N, T, S, U, V, blank, w.pairs, lse, elem_bytes == 2),
              RNNT_STATUS_GATHER_FAILED);
     c.pairs = w.pairs; c.pair_grads = reinterpret_cast<float2 *>(pair_grads);
-    return run_loss(s, workspace, workspace_bytes, c);
+    return run_typed(s, workspace, workspace_bytes, w, c, rnnt_type, delay_penalty, nullptr);
 }
 
 int rnnt_b200_logits_pruned_backward(void *stream, const void *logits, const float *lse, const float *pair_grads,
@@ -972,6 +1039,10 @@ void rnnt_b200_debug_last_tdt_launch(int32_t *out) {
     if (out) rnnt::tdt_launch_record(out);
 }
 
+void rnnt_b200_debug_last_frames_launch(int32_t *out) {
+    if (out) rnnt::frames_launch_record(out);
+}
+
 size_t rnnt_b200_simple_workspace_bytes(int N, int T, int U) {
     return carve(nullptr, (int64_t)max(N, 0) * max(T, 0) * max(U, 0), N).bytes;
 }
@@ -999,8 +1070,19 @@ int rnnt_b200_simple_smoothed_forward(void *stream, void *workspace, size_t work
                                       const float *lm, const int *labels, const int *xn, const int *yn, float *costs,
                                       float *saved, float *pair_grads, int N, int T, int U, int V, int blank,
                                       int lse_mode, float lm_only_scale, float am_only_scale) {
+    return rnnt_b200_simple_smoothed_forward_ex(stream, workspace, workspace_bytes, am, lm, labels, xn, yn, costs, saved,
+                                                pair_grads, N, T, U, V, blank, lse_mode, lm_only_scale, am_only_scale,
+                                                0, 0.0f, nullptr);
+}
+
+int rnnt_b200_simple_smoothed_forward_ex(void *stream, void *workspace, size_t workspace_bytes, const float *am,
+                                         const float *lm, const int *labels, const int *xn, const int *yn,
+                                         float *costs, float *saved, float *pair_grads, int N, int T, int U, int V,
+                                         int blank, int lse_mode, float lm_only_scale, float am_only_scale,
+                                         int rnnt_type, float delay_penalty, float *raw_blank_grads) {
     if (!simple_args_ok(N, T, U, V, blank) || !smooth_scales_ok(lm_only_scale, am_only_scale) || !saved ||
-        !pairs_aligned(pair_grads) || !pairs_aligned(workspace))
+        !pairs_aligned(pair_grads) || !pairs_aligned(workspace) ||
+        !path_type_ok(rnnt_type, delay_penalty, 0.0f, U) || (raw_blank_grads && !pair_grads))
         return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
     const bool smooth = smoothed(lm_only_scale, am_only_scale);
@@ -1022,7 +1104,7 @@ int rnnt_b200_simple_smoothed_forward(void *stream, void *workspace, size_t work
         RNNT_TRY(launch_simple_smoothed_forward(s, m), RNNT_STATUS_GATHER_FAILED);
     }
     c.pairs = w.pairs; c.pair_grads = reinterpret_cast<float2 *>(pair_grads);
-    return run_loss(s, workspace, workspace_bytes, c);
+    return run_typed(s, workspace, workspace_bytes, w, c, rnnt_type, delay_penalty, raw_blank_grads);
 }
 
 int rnnt_b200_simple_smoothed_backward(void *stream, void *workspace, size_t workspace_bytes, const float *am,
@@ -1053,11 +1135,17 @@ int rnnt_b200_simple_smoothed_backward(void *stream, void *workspace, size_t wor
 
 int rnnt_b200_prune_ranges(void *stream, const float *pair_grads, const int *xn, const int *yn, int N, int T, int U,
                            int S, int *ranges) {
-    if (!simple_args_ok(N, T, U, 1, 0) || S < 2 || !pair_grads || !pairs_aligned(pair_grads) || !ranges)
+    return rnnt_b200_prune_ranges_ex(stream, pair_grads, nullptr, xn, yn, N, T, U, S, 0, ranges);
+}
+
+int rnnt_b200_prune_ranges_ex(void *stream, const float *pair_grads, const float *raw_blank_grads, const int *xn,
+                              const int *yn, int N, int T, int U, int S, int rnnt_type, int *ranges) {
+    if (!simple_args_ok(N, T, U, 1, 0) || rnnt_type < 0 || rnnt_type > 2 || S < (rnnt_type == 0 ? 2 : 1) ||
+        !pair_grads || !pairs_aligned(pair_grads) || !ranges || (rnnt_type == 2 && !raw_blank_grads))
         return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
-    RNNT_TRY(launch_prune_ranges((cudaStream_t)stream, reinterpret_cast<const float2 *>(pair_grads), xn, yn, N, T, U, S,
-                                 ranges),
+    RNNT_TRY(launch_prune_ranges((cudaStream_t)stream, reinterpret_cast<const float2 *>(pair_grads), raw_blank_grads, xn,
+                                 yn, N, T, U, S, rnnt_type, ranges),
              RNNT_STATUS_GATHER_FAILED);
     return RNNT_STATUS_SUCCESS;
 }

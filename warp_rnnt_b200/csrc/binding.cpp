@@ -366,7 +366,7 @@ std::tuple<at::Tensor, at::Tensor> rnnt_gather_forward(const at::Tensor &xs, con
 std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_logits_forward(const at::Tensor &xs, const at::Tensor &ys,
                                                                    const at::Tensor &xn, const at::Tensor &yn,
                                                                    int blank, float fastemit_lambda, bool want_grads,
-                                                                   int lse_mode) {
+                                                                   int lse_mode, int rnnt_type, double delay_penalty) {
     const auto [N, T, U, V, bf16, guard] = dense_front(xs, ys, xn, yn, true);
     check_blank(blank, V);
     const auto f32 = xs.options().dtype(at::kFloat);
@@ -377,15 +377,17 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_logits_forward(const at::Ten
     at::Tensor ws = workspace(xs, rnnt_b200_workspace_bytes(N * T * U, (int)N));
     float *pgp = want_grads ? pg.data_ptr<float>() : nullptr;
     if (bf16)
-        check_status(rnnt_b200_logits_forward_bf16(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
-                                                   ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
-                                                   costs.data_ptr<float>(), lse.data_ptr<float>(), pgp, (int)N, (int)T,
-                                                   (int)U, (int)V, blank, fastemit_lambda, lse_mode));
+        check_status(rnnt_b200_logits_forward_bf16_ex(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(),
+                                                      xs.data_ptr(), ys.data_ptr<int>(), xn.data_ptr<int>(),
+                                                      yn.data_ptr<int>(), costs.data_ptr<float>(), lse.data_ptr<float>(),
+                                                      pgp, (int)N, (int)T, (int)U, (int)V, blank, fastemit_lambda,
+                                                      lse_mode, rnnt_type, (float)delay_penalty));
     else
-        check_status(rnnt_b200_logits_forward(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr<float>(),
-                                              ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
-                                              costs.data_ptr<float>(), lse.data_ptr<float>(), pgp, (int)N, (int)T, (int)U,
-                                              (int)V, blank, fastemit_lambda, lse_mode));
+        check_status(rnnt_b200_logits_forward_ex(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(),
+                                                 xs.data_ptr<float>(), ys.data_ptr<int>(), xn.data_ptr<int>(),
+                                                 yn.data_ptr<int>(), costs.data_ptr<float>(), lse.data_ptr<float>(), pgp,
+                                                 (int)N, (int)T, (int)U, (int)V, blank, fastemit_lambda, lse_mode,
+                                                 rnnt_type, (float)delay_penalty));
     return std::make_tuple(costs, lse, pg);
 }
 
@@ -483,7 +485,8 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_logits_pruned_forward(const 
                                                                           const at::Tensor &xn, const at::Tensor &yn,
                                                                           const at::Tensor &ranges, int blank,
                                                                           float fastemit_lambda, bool want_grads,
-                                                                          int lse_mode) {
+                                                                          int lse_mode, int rnnt_type,
+                                                                          double delay_penalty) {
     check4(xs, ys, xn, yn, true);
     check_batch4(xs, xn, yn);
     TORCH_CHECK(ys.dim() == 2 && ys.size(0) == xs.size(0), "ys shape must be (N, U-1)");
@@ -497,12 +500,11 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_logits_pruned_forward(const 
     at::Tensor pg = output(want_grads, {N, T, U, 2}, f32);
     if (N == 0) return std::make_tuple(costs, lse, pg);
     at::Tensor ws = workspace(xs, rnnt_b200_workspace_bytes(N * T * U, (int)N));
-    check_status(rnnt_b200_logits_pruned_forward(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
-                                                 ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
-                                                 ranges.data_ptr<int>(), costs.data_ptr<float>(), lse.data_ptr<float>(),
-                                                 want_grads ? pg.data_ptr<float>() : nullptr, (int)N, (int)T, (int)S,
-                                                 (int)U, (int)V, blank, fastemit_lambda, lse_mode,
-                                                 xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
+    check_status(rnnt_b200_logits_pruned_forward_ex(
+        current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(), ys.data_ptr<int>(), xn.data_ptr<int>(),
+        yn.data_ptr<int>(), ranges.data_ptr<int>(), costs.data_ptr<float>(), lse.data_ptr<float>(),
+        want_grads ? pg.data_ptr<float>() : nullptr, (int)N, (int)T, (int)S, (int)U, (int)V, blank, fastemit_lambda,
+        lse_mode, xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4, rnnt_type, (float)delay_penalty));
     return std::make_tuple(costs, lse, pg);
 }
 
@@ -673,11 +675,12 @@ int64_t simple_saved_len(int64_t N, int64_t T, int64_t U, int64_t V, bool smooth
 std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor>
 rnnt_simple_forward(const at::Tensor &am, const at::Tensor &lm, const at::Tensor &ys, const at::Tensor &xn,
                     const at::Tensor &yn, int blank, bool want_grads, int prune_range, int lse_mode,
-                    double lm_only_scale, double am_only_scale) {
+                    double lm_only_scale, double am_only_scale, int rnnt_type, double delay_penalty) {
     check_simple_inputs(am, lm, ys, xn, yn);
     const int64_t N = am.size(0), T = am.size(1), U = lm.size(1), V = am.size(2);
     check_blank(blank, V);
-    TORCH_CHECK(prune_range == 0 || prune_range >= 2, "prune_range must be an int >= 2");
+    TORCH_CHECK(prune_range == 0 || prune_range >= (rnnt_type == 0 ? 2 : 1),
+                rnnt_type == 0 ? "prune_range must be an int >= 2" : "prune_range must be an int >= 1");
     const float sl = (float)lm_only_scale, sa = (float)am_only_scale;
     const bool smooth = sl != 0.0f || sa != 0.0f;
     const c10::cuda::CUDAGuard guard(am.device());
@@ -687,18 +690,21 @@ rnnt_simple_forward(const at::Tensor &am, const at::Tensor &lm, const at::Tensor
     at::Tensor saved = at::empty({simple_saved_len(N, T, U, V, smooth)}, f32);
     at::Tensor pg = output(pairs, {N, T, U, 2}, f32);
     at::Tensor ranges = at::empty({prune_range > 0 ? N : 0, prune_range > 0 ? T : 0}, am.options().dtype(at::kInt));
+    // the constrained ranges score the blank edges before the fold: their gradient slots, kept for the ranges only
+    at::Tensor raw = at::empty({rnnt_type == 2 && prune_range > 0 ? N * T * U : 0}, f32);
+    float *rawp = raw.numel() ? raw.data_ptr<float>() : nullptr;
     if (N == 0) return std::make_tuple(costs, saved, pg, ranges);
     void *stream = current_stream(am);
     at::Tensor ws = workspace(am, smooth ? rnnt_b200_simple_smoothed_workspace_bytes((int)N, (int)T, (int)U, (int)V)
                                          : rnnt_b200_simple_workspace_bytes((int)N, (int)T, (int)U));
-    check_status(rnnt_b200_simple_smoothed_forward(stream, ws.data_ptr(), (size_t)ws.numel(), am.data_ptr<float>(),
-                                                   lm.data_ptr<float>(), ys.data_ptr<int>(), xn.data_ptr<int>(),
-                                                   yn.data_ptr<int>(), costs.data_ptr<float>(), saved.data_ptr<float>(),
-                                                   pairs ? pg.data_ptr<float>() : nullptr, (int)N, (int)T, (int)U,
-                                                   (int)V, blank, lse_mode, sl, sa));
+    check_status(rnnt_b200_simple_smoothed_forward_ex(
+        stream, ws.data_ptr(), (size_t)ws.numel(), am.data_ptr<float>(), lm.data_ptr<float>(), ys.data_ptr<int>(),
+        xn.data_ptr<int>(), yn.data_ptr<int>(), costs.data_ptr<float>(), saved.data_ptr<float>(),
+        pairs ? pg.data_ptr<float>() : nullptr, (int)N, (int)T, (int)U, (int)V, blank, lse_mode, sl, sa, rnnt_type,
+        (float)delay_penalty, rawp));
     if (prune_range > 0)
-        check_status(rnnt_b200_prune_ranges(stream, pg.data_ptr<float>(), xn.data_ptr<int>(), yn.data_ptr<int>(), (int)N,
-                                            (int)T, (int)U, prune_range, ranges.data_ptr<int>()));
+        check_status(rnnt_b200_prune_ranges_ex(stream, pg.data_ptr<float>(), rawp, xn.data_ptr<int>(), yn.data_ptr<int>(),
+                                               (int)N, (int)T, (int)U, prune_range, rnnt_type, ranges.data_ptr<int>()));
     return std::make_tuple(costs, saved, pg, ranges);
 }
 
@@ -734,19 +740,29 @@ std::tuple<at::Tensor, at::Tensor> rnnt_simple_backward(const at::Tensor &am, co
 }
 
 // prune ranges (N,T) int32 from pair gradients (N,T,U,2) of a loss call
-at::Tensor rnnt_prune_ranges(const at::Tensor &pair_grads, const at::Tensor &xn, const at::Tensor &yn, int S) {
+at::Tensor rnnt_prune_ranges(const at::Tensor &pair_grads, const at::Tensor &xn, const at::Tensor &yn, int S,
+                             int rnnt_type, const c10::optional<at::Tensor> &raw_blank) {
     check_arg(pair_grads, Dt::F32, pair_grads, {kAny, kAny, kAny, 2},
               "pair_grads must be a contiguous CUDA Float tensor of shape (N, T, U, 2)");
     const int64_t N = pair_grads.size(0), T = pair_grads.size(1), U = pair_grads.size(2);
     const char *lengths = "xn and yn must be contiguous Int tensors of shape (N,) on the device of pair_grads";
     check_arg(xn, Dt::I32, pair_grads, N, lengths);
     check_arg(yn, Dt::I32, pair_grads, N, lengths);
-    TORCH_CHECK(S >= 2, "prune_range must be an int >= 2");
+    TORCH_CHECK(rnnt_type >= 0 && rnnt_type <= 2, "rnnt_type must be 0, 1 or 2");
+    TORCH_CHECK(S >= (rnnt_type == 0 ? 2 : 1),
+                rnnt_type == 0 ? "prune_range must be an int >= 2" : "prune_range must be an int >= 1");
+    const bool use_raw = rnnt_type == 2;
+    TORCH_CHECK(!use_raw || raw_blank.has_value(), "rnnt_type 2 needs raw_blank");
+    if (use_raw)
+        check_arg(*raw_blank, Dt::F32, pair_grads, N * T * U,
+                  "raw_blank must be a contiguous Float tensor of shape (N, T, U) on the device of pair_grads");
     const c10::cuda::CUDAGuard guard(pair_grads.device());
     at::Tensor ranges = at::empty({N, T}, pair_grads.options().dtype(at::kInt));
     if (N == 0) return ranges;
-    check_status(rnnt_b200_prune_ranges(current_stream(pair_grads), pair_grads.data_ptr<float>(), xn.data_ptr<int>(),
-                                        yn.data_ptr<int>(), (int)N, (int)T, (int)U, S, ranges.data_ptr<int>()));
+    check_status(rnnt_b200_prune_ranges_ex(current_stream(pair_grads), pair_grads.data_ptr<float>(),
+                                           use_raw ? raw_blank->data_ptr<float>() : nullptr, xn.data_ptr<int>(),
+                                           yn.data_ptr<int>(), (int)N, (int)T, (int)U, S, rnnt_type,
+                                           ranges.data_ptr<int>()));
     return ranges;
 }
 
@@ -878,7 +894,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("want_grads") = true, py::arg("lse_mode") = 0);
     m.def("rnnt_rescale_", &rnnt_rescale_, py::arg("grads"), py::arg("grad_out"), py::arg("applied") = py::none());
     m.def("rnnt_logits_forward", &rnnt_logits_forward, py::arg("xs"), py::arg("ys"), py::arg("xn"), py::arg("yn"),
-          py::arg("blank") = 0, py::arg("fastemit_lambda") = 0.0, py::arg("want_grads") = true, py::arg("lse_mode") = 0);
+          py::arg("blank") = 0, py::arg("fastemit_lambda") = 0.0, py::arg("want_grads") = true, py::arg("lse_mode") = 0,
+          py::arg("rnnt_type") = 0, py::arg("delay_penalty") = 0.0);
     m.def("rnnt_logits_backward", &rnnt_logits_backward, py::arg("xs"), py::arg("lse"), py::arg("pair_grads"),
           py::arg("ys"), py::arg("grad_out"), py::arg("blank") = 0);
     m.def("rnnt_logits_compact_forward", &rnnt_logits_compact_forward, py::arg("xs"), py::arg("ys"), py::arg("xn"),
@@ -889,7 +906,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("blank") = 0);
     m.def("rnnt_logits_pruned_forward", &rnnt_logits_pruned_forward, py::arg("xs"), py::arg("ys"), py::arg("xn"),
           py::arg("yn"), py::arg("ranges"), py::arg("blank") = 0, py::arg("fastemit_lambda") = 0.0,
-          py::arg("want_grads") = true, py::arg("lse_mode") = 0);
+          py::arg("want_grads") = true, py::arg("lse_mode") = 0, py::arg("rnnt_type") = 0,
+          py::arg("delay_penalty") = 0.0);
     m.def("rnnt_logits_pruned_backward", &rnnt_logits_pruned_backward, py::arg("xs"), py::arg("lse"),
           py::arg("pair_grads"), py::arg("ys"), py::arg("ranges"), py::arg("grad_out"), py::arg("blank") = 0);
     m.def("rnnt_tdt_forward", &rnnt_tdt_forward, py::arg("xs"), py::arg("ys"), py::arg("xn"), py::arg("yn"),
@@ -904,11 +922,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("blank"));
     m.def("rnnt_simple_forward", &rnnt_simple_forward, py::arg("am"), py::arg("lm"), py::arg("ys"), py::arg("xn"),
           py::arg("yn"), py::arg("blank") = 0, py::arg("want_grads") = true, py::arg("prune_range") = 0,
-          py::arg("lse_mode") = 0, py::arg("lm_only_scale") = 0.0, py::arg("am_only_scale") = 0.0);
+          py::arg("lse_mode") = 0, py::arg("lm_only_scale") = 0.0, py::arg("am_only_scale") = 0.0,
+          py::arg("rnnt_type") = 0, py::arg("delay_penalty") = 0.0);
     m.def("rnnt_simple_backward", &rnnt_simple_backward, py::arg("am"), py::arg("lm"), py::arg("ys"), py::arg("xn"),
           py::arg("yn"), py::arg("saved"), py::arg("pair_grads"), py::arg("grad_out"), py::arg("blank") = 0,
           py::arg("lm_only_scale") = 0.0, py::arg("am_only_scale") = 0.0);
-    m.def("rnnt_prune_ranges", &rnnt_prune_ranges, py::arg("pair_grads"), py::arg("xn"), py::arg("yn"), py::arg("S"));
+    m.def("rnnt_prune_ranges", &rnnt_prune_ranges, py::arg("pair_grads"), py::arg("xn"), py::arg("yn"), py::arg("S"),
+          py::arg("rnnt_type") = 0, py::arg("raw_blank") = py::none());
     m.def("rnnt_joint_pack", &rnnt_joint_pack, py::arg("f"), py::arg("g"), py::arg("lf"), py::arg("lg"), py::arg("stu") = -1);
     m.def("rnnt_joint_pack_backward", &rnnt_joint_pack_backward, py::arg("dx"), py::arg("lf"), py::arg("lg"),
           py::arg("mem_pref"), py::arg("T"), py::arg("U1"));

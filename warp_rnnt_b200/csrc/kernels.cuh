@@ -122,9 +122,30 @@ cudaError_t launch_simple_smoothed_forward(cudaStream_t s, const SmoothArgs &m);
 // terms added to dam, dlm
 cudaError_t launch_simple_smoothed_backward(cudaStream_t s, const SimpleArgs &a, const SmoothArgs &m, float *dam,
                                             float *dlm);
-// ranges (N,T) from the pair gradients (N,T,U,2) of a loss call; S >= 2
-cudaError_t launch_prune_ranges(cudaStream_t s, const float2 *pg, const int *xn, const int *yn, int N, int T, int U,
-                                int S, int *ranges);
+// ranges (N,T) from the pair gradients (N,T,U,2) of a loss call; rnnt_type 0 (S >= 2), 1 or 2 (S >= 1); raw_blank:
+// the constrained call's blank slots before the fold (N,T,U), read for rnnt_type 2 only
+cudaError_t launch_prune_ranges(cudaStream_t s, const float2 *pg, const float *raw_blank, const int *xn, const int *yn,
+                                int N, int T, int U, int S, int rnnt_type, int *ranges);
+
+// frames.cu -- k2's modified / constrained lattices and delay penalty on the dense (N,T,U,2) pairs
+constexpr int kFramesMaxU = 25600;        // k_frames keeps two rows of U floats in shared memory
+struct FramesCall {
+    const float2 *pairs;                  // (N,T,U,2) (blank, label) log-probs
+    const int *xn, *yn;
+    float *alphas, *betas, *ll;           // workspace: (N,T,U), (N,T,U), (N)
+    int *status;                          // workspace: (N) lattice class
+    float *costs;
+    float2 *pair_grads;                   // (N,T,U,2) out, or null (costs only)
+    float *raw_blank;                     // (N,T,U) out: blank slots before the constrained fold, or null
+    int N, T, U;
+    bool constrained;
+};
+// pairs_out = pairs_in with lam * ((Tn-1)/2 - t) added to every live label slot (in place when they are the same)
+cudaError_t launch_delay_pairs(cudaStream_t s, const float2 *pairs_in, float2 *pairs_out, const int *xn, const int *yn,
+                               int N, int T, int U, float lam);
+// k_frames then, with pair_grads, k_frames_grads; `delayed` is recorded (the call ran launch_delay_pairs first)
+cudaError_t launch_frames(cudaStream_t s, const FramesCall &c, bool delayed);
+void frames_launch_record(int32_t *out);  // copy of the last k_frames launch's record (rnntFramesLaunchRecord_t)
 
 // joint.cu -- compact packing of the joint network's input (caller side of compact=True)
 cudaError_t launch_joint_pack(cudaStream_t s, const float *f, const float *g, const int *lf, const int *lg,

@@ -214,10 +214,13 @@ __global__ void __launch_bounds__(kRowThreads) k_simple_sparse(SimpleArgs a, flo
 // score(t,r) = (ob[t,r] + ... + ob[t,r+S-1]) - (r > 0 ? ol[t,r-1] : 0), ob = -gb, ol = -gl, the sum added in increasing
 // u and the subtraction last; a NaN score never wins, and r = 0 when every score is NaN.  Frames t >= Tn-1 take Un-S.
 // One warp per frame, lane l scoring r = l, l+32, ...  Then, over all T frames: b = suffix minimum of r0,
-// c = (S-1) t - b, c' = suffix minimum of c, r = (S-1) t - max(c', 0) -- computed in place in `ranges` by warp 0.
+// c = k t - b, c' = suffix minimum of c, r = k t - max(c', 0) -- computed in place in `ranges` by warp 0.  TYPE is the
+// lattice type: k = S-1 for 0 (regular), 1 for 1 and 2 (modified, constrained); type 2 takes gb from raw (the blank
+// slots before the constrained fold), the others from pg.
+template <int TYPE>
 __global__ void __launch_bounds__(kRangeThreads)
 k_prune_ranges(const float2 *__restrict__ pg, const int *__restrict__ xn, const int *__restrict__ yn, int T, int U,
-               int S, int *__restrict__ ranges) {
+               int S, int *__restrict__ ranges, const float *__restrict__ raw) {
     const int n = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int Tn, Un;
     simple_lengths(xn, yn, n, T, U, Tn, Un);
@@ -236,7 +239,12 @@ k_prune_ranges(const float2 *__restrict__ pg, const int *__restrict__ xn, const 
             best_r = 0;
             for (int r = lane; r <= top; r += 32) {
                 float sc = 0.0f;
-                for (int u = r; u < r + S; ++u) sc += -q[u].x;
+                if constexpr (TYPE == 2) {
+                    const float *qb = raw + ((int64_t)n * T + t) * U;
+                    for (int u = r; u < r + S; ++u) sc += -qb[u];
+                } else {
+                    for (int u = r; u < r + S; ++u) sc += -q[u].x;
+                }
                 if (r > 0) sc = sc - (-q[r - 1].y);
                 if (sc == sc && (!have || sc > best)) { best = sc; best_r = r; have = true; }
             }
@@ -265,7 +273,7 @@ k_prune_ranges(const float2 *__restrict__ pg, const int *__restrict__ xn, const 
         }
         b = min(b, carry_b);
         carry_b = __shfl_sync(0xffffffffu, b, 0);
-        int c = t < T ? (S - 1) * t - b : INT_MAX;
+        int c = t < T ? (TYPE == 0 ? S - 1 : 1) * t - b : INT_MAX;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) {
             const int y = __shfl_down_sync(0xffffffffu, c, o);
@@ -273,7 +281,7 @@ k_prune_ranges(const float2 *__restrict__ pg, const int *__restrict__ xn, const 
         }
         c = min(c, carry_c);
         carry_c = __shfl_sync(0xffffffffu, c, 0);
-        if (t < T) out[t] = (S - 1) * t - max(c, 0);
+        if (t < T) out[t] = (TYPE == 0 ? S - 1 : 1) * t - max(c, 0);
     }
 }
 
@@ -638,9 +646,11 @@ cudaError_t launch_simple_smoothed_backward(cudaStream_t s, const SimpleArgs &a,
     return cudaGetLastError();
 }
 
-cudaError_t launch_prune_ranges(cudaStream_t s, const float2 *pg, const int *xn, const int *yn, int N, int T, int U,
-                                int S, int *ranges) {
-    k_prune_ranges<<<N, kRangeThreads, 0, s>>>(pg, xn, yn, T, U, S, ranges);
+cudaError_t launch_prune_ranges(cudaStream_t s, const float2 *pg, const float *raw_blank, const int *xn, const int *yn,
+                                int N, int T, int U, int S, int rnnt_type, int *ranges) {
+    if (rnnt_type == 2) k_prune_ranges<2><<<N, kRangeThreads, 0, s>>>(pg, xn, yn, T, U, S, ranges, raw_blank);
+    else if (rnnt_type == 1) k_prune_ranges<1><<<N, kRangeThreads, 0, s>>>(pg, xn, yn, T, U, S, ranges, nullptr);
+    else k_prune_ranges<0><<<N, kRangeThreads, 0, s>>>(pg, xn, yn, T, U, S, ranges, nullptr);
     count_launch();
     return cudaGetLastError();
 }
