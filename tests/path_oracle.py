@@ -5,12 +5,17 @@ lattice() gives costs, the pair gradients in the kernels' convention (d cost / d
 occupation folded into the blank slot of the cell it reaches) and the blank slots before that fold.  Log-probs at or
 below -1e30 (the kernels' removed-edge sentinel) count as -inf.  penalise() is the delay penalty in the kernels' f32
 operation order, and prune_ranges() the windows rule with the step bound of each type, beside simple_oracle's.
-brute_force() enumerates every path, for small lattices."""
+brute_force() enumerates every path, for small lattices.
+
+stream() is lattice() for one modified / constrained lattice in O(U) memory, frame by frame from a function that makes
+each frame's pair row, so that it reaches the largest lattice the frame sweep takes (U = 25600, 655 M cells);
+stream_grads() gives the pair gradients of the frames it kept.  pruned() restates rnnt_loss_pruned for every type:
+window rows -> log_softmax -> full pairs with the edges off the windows removed -> penalty -> lattice()."""
 import itertools
 
 import numpy as np
 
-from tests.pruned_oracle import _alphas, _betas
+from tests.pruned_oracle import _alphas, _betas, log_softmax, window_rows
 
 KBIG = -1.0e30
 TYPES = ("regular", "modified", "constrained")
@@ -192,3 +197,111 @@ def window_pairs(pairs, ranges, S):
     inside = (u[None, None, :] >= ranges[:, :, None]) & (u[None, None, :] < ranges[:, :, None] + S)
     p[~inside] = KBIG
     return p
+
+
+# ------------------------------------------------------------------------------------------ streaming, O(U) memory
+def _frame_ops(row, Un, t, Tn, lam, constrained):
+    """(B (Un,), label weight l' (Un-1,)) of one frame from its (Un, 2) pair row, fp64, the penalty added in fp64."""
+    r = np.asarray(row, np.float64)[:Un]
+    r = np.where(r <= KBIG, -np.inf, r)
+    B, L = r[:, 0], r[:Un - 1, 1]
+    if lam:
+        L = L + lam * ((Tn - 1) / 2.0 - t)
+    return B, (L + B[1:] if constrained else L)
+
+
+def stream(row_fn, Tn, Un, rnnt_type, keep=(), lam=0.0):
+    """-> (cost, {t: alpha of frame t}, {t: beta of frame t + 1}) of one modified or constrained lattice, fp64, each
+    alpha / beta an (Un,) row, for t in keep.  row_fn(t) gives frame t's (Un, 2) (blank, label) pair row (more columns
+    are ignored); it is called twice per frame, once per direction, so the pairs never exist whole.  lam: the delay
+    penalty, added in fp64.  Cost +inf when no finite path is left; NaN in a live pair is not classified (see
+    lattice())."""
+    assert rnnt_type in ("modified", "constrained") and Tn >= 1 and Un >= 1
+    con = rnnt_type == "constrained"
+    keep = set(int(t) for t in keep)
+    alphas, betas = {}, {}
+    a = np.full(Un, -np.inf)
+    a[0] = 0.0
+    with np.errstate(invalid="ignore", divide="ignore"):
+        for t in range(Tn):
+            if t in keep:
+                alphas[t] = a.copy()
+            B, Lw = _frame_ops(row_fn(t), Un, t, Tn, lam, con)
+            nxt = a + B
+            nxt[1:] = np.logaddexp(nxt[1:], a[:-1] + Lw)
+            a = nxt
+        b = np.full(Un, -np.inf)
+        b[Un - 1] = 0.0
+        for t in range(Tn - 1, -1, -1):
+            if t in keep:
+                betas[t] = b.copy()
+            B, Lw = _frame_ops(row_fn(t), Un, t, Tn, lam, con)
+            nxt = B + b
+            nxt[:-1] = np.logaddexp(nxt[:-1], Lw + b[1:])
+            b = nxt
+    ll = b[0]
+    return (-ll if np.isfinite(ll) else np.inf), alphas, betas
+
+
+def stream_grads(row_fn, Tn, Un, rnnt_type, keep, lam=0.0):
+    """-> (cost, {t: (Un, 2) pair gradients of frame t in lattice()'s convention}, the largest |alpha| of the kept
+    frames' cells that lie on a path: finite alpha and a finite beta one frame on) from stream()'s rows."""
+    cost, alphas, betas = stream(row_fn, Tn, Un, rnnt_type, keep, lam)
+    con = rnnt_type == "constrained"
+    out = {}
+    top = 0.0
+    for t in sorted(alphas):
+        a, b = alphas[t], betas[t]
+        fin = np.isfinite(a) & np.isfinite(b)
+        top = max(top, float(np.abs(a[fin]).max()) if fin.any() else 0.0)
+        g = np.zeros((Un, 2))
+        if np.isfinite(cost):
+            B, Lw = _frame_ops(row_fn(t), Un, t, Tn, lam, con)
+            with np.errstate(invalid="ignore"):
+                ob = np.exp(a + B + b + cost)
+                ol = np.exp(a[:-1] + Lw + b[1:] + cost)
+            g[:, 0] = -ob
+            g[:Un - 1, 1] = -ol
+            if con:
+                g[1:, 0] -= ol
+        out[t] = g
+    return cost, out, top
+
+
+# ------------------------------------------------------------------------------------------ pruned, every type
+def pruned(logits, labels, xn, yn, ranges, blank=0, rnnt_type="regular", delay_penalty=0.0, fastemit_lambda=0.0,
+           grad_output=None):
+    """rnnt_loss_pruned restated for every type: -> (costs (N,), d sum_n grad_output[n] cost[n] / d logits
+    (N, T, S, V)), fp64.  The window rows' log_softmax go to their cells of full (N,T,U,2) pairs that are -inf
+    everywhere else (window_pairs()), the penalty is added there in fp64, lattice() gives the costs and the pair
+    gradients, and each row's gradient is the vector-Jacobian product of log_softmax, gb (e_blank - p) + gl (e_y - p).
+    FastEmit (regular only) scales the label gradients by 1 + lambda and leaves the costs, as pruned_oracle.lattice
+    does.  Classes are lattice()'s: NaN for invalid lengths, +inf and zero rows when no path is left."""
+    assert rnnt_type == "regular" or not fastemit_lambda
+    lp = log_softmax(logits)
+    labels = np.asarray(labels)
+    N, T, S, V = lp.shape
+    U = labels.shape[1] + 1
+    lab = np.concatenate([labels.astype(np.int64), np.full((N, 1), blank, np.int64)], axis=1)
+    n, t, s, u = window_rows(ranges, xn, yn, S)
+    cl = lab[n, u]
+    P = np.full((N, T, U, 2), -np.inf)
+    P[n, t, u, 0] = lp[n, t, s, blank]
+    P[n, t, u, 1] = lp[n, t, s, cl]
+    if delay_penalty:
+        for k in range(N):
+            Tn, Un = int(xn[k]), int(yn[k]) + 1
+            if lengths_ok(Tn, Un, T, U):
+                P[k, :Tn, :Un - 1, 1] += delay_penalty * ((Tn - 1) / 2.0 - np.arange(Tn))[:, None]
+    costs, g, _ = lattice(P, xn, yn, rnnt_type)
+    g[..., 1] *= 1.0 + fastemit_lambda
+    go = np.ones(N) if grad_output is None else np.asarray(grad_output, np.float64)
+    qb, ql = g[n, t, u, 0], g[n, t, u, 1]
+    grads = np.zeros_like(lp)
+    with np.errstate(invalid="ignore"):
+        rows = -np.exp(lp[n, t, s]) * (qb + ql)[:, None]
+        k = np.arange(len(n))
+        rows[k, blank] += qb
+        rows[k, cl] += ql
+        grads[n, t, s] = rows * go[n][:, None]
+    return costs, grads

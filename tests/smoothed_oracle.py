@@ -14,9 +14,13 @@ and takes no part in the objective, but with sa > 0 its lm rows still enter the 
 smoothed() takes norm as a logsumexp over the (N,T,U,V) joint and runs autograd through a per-lattice alpha loop, so it
 only reaches toy sizes.  factorised() is the same loss from the same pair formula (pairs()) without that tensor: the
 normaliser as a per-lattice matrix product, alpha and beta in numpy over anti-diagonals for every lattice at once, and
-autograd through the pair formula alone; it reaches the shapes the loss is used at (N=64 T=1500 U=300 V=50)."""
+autograd through the pair formula alone; it reaches the shapes the loss is used at (N=64 T=1500 U=300 V=50).  It
+also takes k2's rnnt_type and delay_penalty: the penalty on the fp64 pairs' live label slots, the pair gradients of
+the modified and constrained lattices from path_oracle.lattice."""
 import numpy as np
 import torch
+
+from tests import path_oracle as pa
 
 FLT_MIN = float(np.finfo(np.float32).tiny)
 SENTINEL = -1e30            # alpha outside the lattice: finite, so that logaddexp never meets -inf - (-inf)
@@ -192,14 +196,19 @@ def lattice_grads(B, L, Tn, Un):
 
 
 def factorised(am, lm, labels, xn, yn, blank=0, lm_only_scale=0.0, am_only_scale=0.0, grad_output=None,
-               detach_unigram=False, round_pairs=False):
+               detach_unigram=False, round_pairs=False, rnnt_type="regular", delay_penalty=0.0):
     """smoothed(..., want_pairs=True) without the (N,T,U,V) tensor: -> (costs, d am, d lm, pair gradients), fp64.
 
     The normaliser is log(exp(am - oa) @ exp(lm - ol)^T) + oa + ol per lattice (oa, ol the rows' maxima, held
     constant: their gradient cancels), the pairs are pairs() above, and the recurrence runs in numpy over
     anti-diagonals for all lattices at once (lattice_grads).  d am and d lm then come from autograd through the pair
     formula with grad_output * (gb, gl) as the pairs' gradient, so the chain rule through the normaliser, Ll and the
-    unigram is torch's, not the kernels'.  Arguments and meaning as smoothed()'s."""
+    unigram is torch's, not the kernels'.  Arguments and meaning as smoothed()'s.
+
+    rnnt_type, delay_penalty: rnnt_loss_simple's.  The penalty delay_penalty * ((Tn-1)/2 - t) is added in fp64 to the
+    label pair of every live label slot (t < Tn, u < Un - 1), a constant that leaves the pairs' gradient alone; the
+    modified and constrained lattices take their costs and pair gradients (folded, as the kernels write them) from
+    path_oracle.lattice.  At the defaults this is the regular loss, unchanged."""
     a = torch.tensor(np.asarray(am, np.float64), requires_grad=True)
     l = torch.tensor(np.asarray(lm, np.float64), requires_grad=True)
     N, T, V = a.shape
@@ -217,7 +226,16 @@ def factorised(am, lm, labels, xn, yn, blank=0, lm_only_scale=0.0, am_only_scale
     xn, yn = np.asarray(xn, np.int64), np.asarray(yn, np.int64)
     ok = (xn >= 1) & (xn <= T) & (yn >= 0) & (yn < U)
     Tn, Un = np.where(ok, xn, 0), np.where(ok, yn + 1, 0)
-    costs, gb, gl = lattice_grads(pb.detach().numpy(), pl.detach().numpy(), Tn, Un)
+    if delay_penalty:
+        t, u = np.arange(T)[None, :, None], np.arange(U)[None, None, :]
+        tt, uu = Tn[:, None, None], Un[:, None, None]
+        pen = np.where((t < tt) & (u < uu - 1), delay_penalty * ((tt - 1) / 2.0 - t), 0.0)
+        pl = pl + torch.from_numpy(pen)
+    if rnnt_type == "regular":
+        costs, gb, gl = lattice_grads(pb.detach().numpy(), pl.detach().numpy(), Tn, Un)
+    else:
+        costs, g, _ = pa.lattice(np.stack([pb.detach().numpy(), pl.detach().numpy()], -1), xn, yn, rnnt_type)
+        gb, gl = g[..., 0], g[..., 1]
     w = go[:, None, None]
     torch.autograd.backward([pb, pl], [torch.from_numpy(w * gb), torch.from_numpy(w * gl)])
     return costs, a.grad.numpy(), l.grad.numpy(), np.stack([gb, gl], axis=-1)

@@ -116,3 +116,54 @@ def test_windows_keep_a_path(kind, S):
         reach = (yn <= xn)
         assert np.isfinite(c[reach]).all(), (xn[reach], yn[reach], c[reach])
         assert (c[~reach] == np.inf).all()
+
+
+# ------------------------------------------------------------------------------------------ stream
+def penalise64(p, xn, yn, lam):
+    """the delay penalty added in fp64 (stream()'s), beside penalise()'s f32 order"""
+    q = np.array(p, np.float64, copy=True)
+    for n in range(len(xn)):
+        Tn, Un = int(xn[n]), int(yn[n]) + 1
+        q[n, :Tn, :Un - 1, 1] += lam * ((Tn - 1) / 2.0 - np.arange(Tn))[:, None]
+    return q
+
+
+@pytest.mark.parametrize("kind", ["modified", "constrained"])
+@pytest.mark.parametrize("lam", [0.0, 0.05])
+def test_stream_is_the_lattice(kind, lam):
+    """stream() / stream_grads() on every class of small lattice -- live, one frame, one column, Un - 1 = Tn, more
+    labels than frames, every path cut by removed edges, -inf log-probs -- give lattice()'s cost and, at the kept
+    frames, its pair gradients to 1e-12, with rows wider than the lattice (padding columns ignored)."""
+    T, U = 7, 6
+    p, _, _ = make_pairs(8, T, U, 21)
+    xn = np.array([7, 1, 5, 4, 3, 6, 7, 6], np.int32)
+    yn = np.array([5, 0, 0, 4, 4, 3, 5, 2], np.int32)
+    p[5, :, :, 0] = pa.KBIG                                  # lattice 5: no blank edge left, no path
+    rng = np.random.RandomState(2)
+    p[6][rng.rand(T, U, 2) < 0.15] = -np.inf                 # lattice 6: masked log-probs
+    q = penalise64(p, xn, yn, lam)
+    c0, g0, _ = pa.lattice(q, xn, yn, kind)
+    assert np.isinf(c0[[4, 5]]).all() and np.isfinite(c0[[0, 1, 2, 3]]).all()
+    for n in range(len(xn)):
+        Tn, Un = int(xn[n]), int(yn[n]) + 1
+        calls = []
+
+        def row(t):
+            calls.append(t)
+            return p[n, t]                                   # (U, 2): the columns past Un are padding
+
+        keep = range(Tn)
+        c, g, top = pa.stream_grads(row, Tn, Un, kind, keep, lam)
+        assert sorted(calls[:2 * Tn]) == sorted(list(range(Tn)) * 2)
+        if np.isinf(c0[n]):
+            assert c == np.inf and all(not v.any() for v in g.values())
+            continue
+        assert abs(c - c0[n]) <= 1e-12 * max(1.0, abs(c0[n])) and top >= 0
+        for t in keep:
+            np.testing.assert_allclose(g[t], g0[n, t, :Un], rtol=0, atol=1e-12)
+    # a few kept frames only: the same rows, alpha / beta the lattice's recurrence
+    n, Tn, Un = 0, 7, 6
+    c, a, b = pa.stream(lambda t: p[n, t], Tn, Un, kind, keep=[0, 3, 6], lam=lam)
+    assert sorted(a) == [0, 3, 6] and sorted(b) == [0, 3, 6]
+    assert a[0][0] == 0 and np.isneginf(a[0][1:]).all() and b[6][Un - 1] == 0 and np.isneginf(b[6][:-1]).all()
+    assert abs(c - c0[n]) <= 1e-12 * abs(c0[n])

@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 
 from oracle import oracle
+from tests import path_oracle as pa
 from tests import pruned_oracle as po
 
 
@@ -180,3 +181,67 @@ def test_live_windows_clip_on_both_sides_and_are_not_monotone():
     x, ys = make(N, T, S, U, 6, seed=1)
     c, _ = po.lattice(x, ys, xn, yn, r)
     assert np.isfinite(c).all()
+
+
+# ------------------------------------------------------------------------------------------ every type (path_oracle)
+def test_pruned_every_type_is_the_regular_lattice():
+    """path_oracle.pruned with rnnt_type regular, no penalty, is pruned_oracle.lattice: costs and window-logit
+    gradients to 1e-10, FastEmit and a non-uniform grad_output included."""
+    rng = np.random.RandomState(17)
+    N, T, S, U, V = 5, 9, 3, 7, 6
+    x = rng.randn(N, T, S, V) * 2
+    ys = rng.randint(1, V, (N, U - 1)).astype(np.int32)
+    xn = np.array([9, 7, 5, 9, 3], np.int32)
+    yn = np.array([6, 4, 2, 5, 1], np.int32)
+    r = po.live_windows(rng, xn, yn, T, S)
+    go = np.linspace(0.5, 1.5, N)
+    for lam in (0.0, 0.3):
+        c0, g0 = po.lattice(x, ys, xn, yn, r, 0, lam, grad_output=go)
+        c1, g1 = pa.pruned(x, ys, xn, yn, r, 0, "regular", 0.0, lam, grad_output=go)
+        assert np.isfinite(c0).all()
+        np.testing.assert_allclose(c1, c0, rtol=1e-10, atol=0)
+        np.testing.assert_allclose(g1, g0, rtol=0, atol=1e-10)
+
+
+@pytest.mark.parametrize("kind", ["modified", "constrained"])
+def test_pruned_every_type_against_brute_force(kind):
+    """path_oracle.pruned on tiny modified / constrained lattices with a penalty: the costs are path enumeration's
+    (path_oracle.brute_force on the windowed, penalised pairs), the window-logit gradient the central differences of
+    its own costs; windows that cut every path give +inf and zero rows."""
+    rng = np.random.RandomState(5 if kind == "modified" else 6)
+    N, T, S, U, V = 4, 5, 2, 4, 5
+    x = rng.randn(N, T, S, V)
+    ys = rng.randint(1, V, (N, U - 1)).astype(np.int32)
+    xn = np.array([5, 4, 5, 3], np.int32)
+    yn = np.array([3, 2, 3, 1], np.int32)
+    r = np.zeros((N, T), np.int32)
+    for n in range(N):                                           # windows that move by at most 1 around a path
+        r[n, 1:] = np.minimum(np.cumsum(rng.randint(0, 2, T - 1)), max(int(yn[n]) + 1 - S, 0))
+    r[2, 2:] = 3                                                 # a gap: lattice 2 has no path
+    lam, go = 0.2, np.array([0.5, 1.0, 1.5, 0.7])
+    c, g = pa.pruned(x, ys, xn, yn, r, 0, kind, lam, grad_output=go)
+    lp = po.log_softmax(x)
+    lab = np.concatenate([ys, np.zeros((N, 1), np.int32)], axis=1)
+    P = np.full((N, T, U, 2), -np.inf)
+    n, t, s, u = po.window_rows(r, xn, yn, S)
+    P[n, t, u, 0] = lp[n, t, s, 0]
+    P[n, t, u, 1] = lp[n, t, s, lab[n, u]]
+    for k in range(N):
+        P[k, :xn[k], :yn[k], 1] += lam * ((xn[k] - 1) / 2.0 - np.arange(xn[k]))[:, None]
+    cb, _ = pa.brute_force(P, xn, yn, kind)
+    assert c[2] == np.inf and cb[2] == np.inf and not g[2].any()
+    live = np.isfinite(cb)
+    assert live.sum() >= 2
+    np.testing.assert_allclose(c[live], cb[live], rtol=1e-12)
+    h = 1e-6
+    num = np.zeros_like(x)
+    for idx in np.ndindex(x.shape):
+        if not live[idx[0]]:
+            continue
+        xp, xm = x.copy(), x.copy()
+        xp[idx] += h
+        xm[idx] -= h
+        k = idx[0]
+        num[idx] = go[k] * (pa.pruned(xp, ys, xn, yn, r, 0, kind, lam)[0][k] -
+                            pa.pruned(xm, ys, xn, yn, r, 0, kind, lam)[0][k]) / (2 * h)
+    np.testing.assert_allclose(g[live], num[live], rtol=0, atol=1e-7)

@@ -4,7 +4,9 @@ costs (padding lm rows and an invalid lattice included), its costs do not move w
 constant, and a padding row of lm reaches another lattice's cost exactly when am_only_scale > 0."""
 import numpy as np
 import pytest
+import torch
 
+from tests import path_oracle as pa
 from tests import pruned_oracle as po
 from tests import simple_oracle as so
 from tests import smoothed_oracle as sm
@@ -169,3 +171,64 @@ def test_vectorised_recurrences_are_the_per_lattice_ones():
         assert costs[n] == -b[n, 0, 0]
         assert gb[n, t - 1, u - 1] == pytest.approx(-1.0, abs=1e-12)
     assert (a[N - 1] == -np.inf).all() and np.isnan(costs[N - 1]) and not gb[N - 1].any()
+
+
+# ------------------------------------------------------------------------------------------ rnnt_type, delay_penalty
+def test_factorised_regular_without_penalty_is_unchanged():
+    am, lm, ys, xn, yn = edge_inputs(3, 9, 6, 5, 2, seed=12)
+    go = np.linspace(0.5, 1.5, 3)
+    for scales in [(0.0, 0.0), (0.1, 0.1)]:
+        a = sm.factorised(am, lm, ys, xn, yn, 2, *scales, grad_output=go)
+        b = sm.factorised(am, lm, ys, xn, yn, 2, *scales, grad_output=go, rnnt_type="regular", delay_penalty=0.0)
+        for x, y in zip(a, b):
+            assert np.array_equal(x, y, equal_nan=True)
+
+
+@pytest.mark.parametrize("kind", ["regular", "modified", "constrained"])
+@pytest.mark.parametrize("scales", [(0.0, 0.0), (0.25, 0.0), (0.1, 0.1)])
+def test_factorised_types_are_the_path_oracle_on_its_pairs(kind, scales):
+    """The costs and pair gradients factorised() returns are path_oracle.lattice's on its own pairs (pairs() with the
+    penalty added in fp64), lattices with invalid lengths and more labels than frames included."""
+    N, T, U, V = 4, 8, 6, 5
+    am, lm, ys, xn, yn = make(N, T, U, V, seed=31)
+    xn[:] = [8, 5, 9, 3]                                     # lattice 2: invalid lengths
+    yn[:] = [5, 4, 2, 5]                                     # lattice 3: Un - 1 = 5 > Tn = 3
+    lam = 0.05
+    c, _, _, pg = sm.factorised(am, lm, ys, xn, yn, 0, *scales, rnnt_type=kind, delay_penalty=lam)
+    a, l = torch.tensor(am), torch.tensor(lm)
+    norm = torch.logsumexp(a[:, :, None, :] + l[:, None, :, :], dim=-1)
+    pb, pl = sm.pairs(a, l, norm, ys, yn, 0, *scales)
+    P = np.stack([pb.numpy(), pl.numpy()], -1)
+    for n in range(N):
+        if 1 <= xn[n] <= T:
+            P[n, :xn[n], :yn[n], 1] += lam * ((xn[n] - 1) / 2.0 - np.arange(xn[n]))[:, None]
+    c0, g0, _ = pa.lattice(P, xn, yn, kind)
+    assert np.isnan(c[2]) and np.isnan(c0[2])
+    assert (c[3] == np.inf) == (kind != "regular")
+    np.testing.assert_allclose(c, c0, rtol=1e-12)
+    np.testing.assert_allclose(pg, g0, rtol=0, atol=1e-12)
+
+
+@pytest.mark.parametrize("kind", ["regular", "modified", "constrained"])
+def test_factorised_types_gradients_are_central_differences(kind):
+    """d am and d lm of factorised() with a penalty and smoothing are the central differences of its costs."""
+    N, T, U, V = 2, 5, 4, 4
+    am, lm, ys, xn, yn = make(N, T, U, V, seed=9)
+    xn[:], yn[:] = [5, 4], [3, 2]
+    go = np.array([0.7, 1.3])
+    sl, sa, lam = 0.1, 0.1, 0.2
+    c, dam, dlm, _ = sm.factorised(am, lm, ys, xn, yn, 0, sl, sa, grad_output=go, rnnt_type=kind, delay_penalty=lam)
+    assert np.isfinite(c).all()
+
+    def obj(a, l):
+        return float((sm.factorised(a, l, ys, xn, yn, 0, sl, sa, rnnt_type=kind, delay_penalty=lam)[0] * go).sum())
+
+    h = 1e-6
+    for x, g in ((am, dam), (lm, dlm)):
+        num = np.zeros_like(x)
+        for idx in np.ndindex(x.shape):
+            xp, xm = x.copy(), x.copy()
+            xp[idx] += h
+            xm[idx] -= h
+            num[idx] = (obj(xp, lm) - obj(xm, lm) if x is am else obj(am, xp) - obj(am, xm)) / (2 * h)
+        np.testing.assert_allclose(g, num, rtol=0, atol=2e-6)

@@ -310,8 +310,9 @@ def rnnt_loss_pruned(logits, labels, frames_lengths, labels_lengths, ranges, ave
 
     Costs are float32; the gradient is w.r.t. ``logits``, of their dtype (bfloat16: the float32 gradient of the
     widened logits rounded once).  Padding rows get exact zeros, or NaN where the row's normaliser is NaN.  A lattice
-    with no path left gets the dense classes of ``rnnt_loss_from_logits``: cost NaN, +inf when it has one frame or no
-    labels.  No host synchronisation: the step can be captured in a CUDA graph."""
+    with no path left gets, with ``rnnt_type="regular"``, the dense classes of ``rnnt_loss_from_logits``: cost NaN
+    (+inf when it has one frame or no labels); with "modified" or "constrained", cost +inf and exactly zero gradient
+    rows, as for more labels than frames.  No host synchronisation: the step can be captured in a CUDA graph."""
     assert average_frames is None or isinstance(average_frames, bool)
     assert reduction is None or reduction in ("none", "mean", "sum")
     assert isinstance(blank, int)
