@@ -375,14 +375,25 @@ class RNNTLossTDTCompact(torch.autograd.Function):
         return g, None, None, None, None, None, None
 
 
-def _tdt_durations(durations):
+def _tdt_args(fn, logits, durations, sigma, blank, compact):
+    """The argument checks of ``rnnt_loss_tdt`` and ``rnnt_align_tdt`` (``fn`` names the caller in the messages):
+    durations, sigma, the logits' shape and blank.  Returns the durations as a tuple."""
     if not isinstance(durations, (list, tuple)) or not durations or \
             any(isinstance(d, bool) or not isinstance(d, int) for d in durations):
-        raise ValueError("rnnt_loss_tdt: durations must be a non-empty list or tuple of ints, got %r" % (durations,))
+        raise ValueError("%s: durations must be a non-empty list or tuple of ints, got %r" % (fn, durations))
     if any(d < 0 or d > 16 for d in durations) or any(b <= a for a, b in zip(durations, durations[1:])) \
             or max(durations) == 0:
-        raise ValueError("rnnt_loss_tdt: durations must be strictly increasing, in [0, 16], with at least one > 0, "
-                         "got %r" % (durations,))
+        raise ValueError("%s: durations must be strictly increasing, in [0, 16], with at least one > 0, "
+                         "got %r" % (fn, durations))
+    if isinstance(sigma, bool) or not isinstance(sigma, (int, float)) or not math.isfinite(sigma) or sigma < 0:
+        raise ValueError("%s: sigma must be a finite number >= 0, got %r" % (fn, sigma))
+    assert isinstance(compact, bool)
+    if logits.dim() != (2 if compact else 4) or logits.size(-1) <= len(durations):
+        raise ValueError("%s: logits must be %s with V >= 1, D = len(durations) = %d, got shape %s"
+                         % (fn, "(STU, V + D)" if compact else "(N, T, U, V + D)", len(durations),
+                            tuple(logits.shape)))
+    if isinstance(blank, bool) or not isinstance(blank, int) or not 0 <= blank < logits.size(-1) - len(durations):
+        raise ValueError("%s: blank must be an int in [0, V), got %r" % (fn, blank))
     return tuple(durations)
 
 
@@ -448,20 +459,12 @@ def rnnt_loss_tdt(logits, labels, frames_lengths, labels_lengths, durations, sig
         loss = rnnt_loss_tdt(logits, labels_c, frames_lengths, labels_lengths, [0, 1, 2, 3, 4], compact=True,
                              reduction="mean")
 
-    Not offered: ``fastemit_lambda``, NeMo's ``omega`` mixing with the regular transducer loss, multi-blank, and a TDT
-    variant of ``rnnt_align``."""
+    Not offered: ``fastemit_lambda``, NeMo's ``omega`` mixing with the regular transducer loss, and multi-blank.  The
+    best path itself (token frames and durations) is ``rnnt_align_tdt``."""
     assert average_frames is None or isinstance(average_frames, bool)
     assert reduction is None or reduction in ("none", "mean", "sum")
     assert not labels.requires_grad and not frames_lengths.requires_grad and not labels_lengths.requires_grad
-    durations = _tdt_durations(durations)
-    if isinstance(sigma, bool) or not isinstance(sigma, (int, float)) or not math.isfinite(sigma) or sigma < 0:
-        raise ValueError("rnnt_loss_tdt: sigma must be a finite number >= 0, got %r" % (sigma,))
-    assert isinstance(compact, bool)
-    if logits.dim() != (2 if compact else 4) or logits.size(-1) <= len(durations):
-        raise ValueError("rnnt_loss_tdt: logits must be %s with V >= 1, D = len(durations) = %d, got shape %s"
-                         % ("(STU, V + D)" if compact else "(N, T, U, V + D)", len(durations), tuple(logits.shape)))
-    if isinstance(blank, bool) or not isinstance(blank, int) or not 0 <= blank < logits.size(-1) - len(durations):
-        raise ValueError("rnnt_loss_tdt: blank must be an int in [0, V), got %r" % (blank,))
+    durations = _tdt_args("rnnt_loss_tdt", logits, durations, sigma, blank, compact)
     fn = RNNTLossTDTCompact if compact else RNNTLossTDT
     costs = fn.apply(logits, labels, frames_lengths, labels_lengths, durations, float(sigma), blank)
     return _reduce(costs, frames_lengths, average_frames, reduction)
@@ -766,7 +769,49 @@ def rnnt_align(log_probs, labels, frames_lengths, labels_lengths, blank=0, compa
     return _C.rnnt_align_dense(log_probs, labels, frames_lengths, labels_lengths, blank)
 
 
-__all__ = ["rnnt_loss", "rnnt_align", "rnnt_loss_from_logits", "rnnt_loss_pruned", "RNNTLossPruned",
-           "rnnt_loss_simple", "RNNTLossSimple", "rnnt_loss_tdt", "RNNTLossTDT", "RNNTLossTDTCompact", "joint_pack",
+def rnnt_align_tdt(logits, labels, frames_lengths, labels_lengths, durations, sigma=0.0, blank=0, compact=False):
+    """Viterbi forced alignment on the Token-and-Duration Transducer lattice of ``rnnt_loss_tdt``: the single best
+    path, with the frame and the duration of each label, for word timings, segmentation and emission latency.
+
+    Inputs and argument checks are those of ``rnnt_loss_tdt``: dense (N, T, U, V + D) logits, float32 or bfloat16, with
+    labels (N, U-1); or ``compact=True``: (STU, V + D) rows in ``joint_pack``'s order with labels
+    (sum(labels_lengths),), honouring ``compact_hints``.  durations, sigma and blank as there.  No autograd: the
+    outputs are not differentiable and ``logits.requires_grad`` is ignored.
+
+    The lattice, its edges and their weights are ``rnnt_loss_tdt``'s with the same sigma, each log-prob clamped below
+    at -1e30 (a masked -inf becomes that finite sentinel).  A path runs from (0, 0) to a terminal blank edge; its score
+    is the float32 left fold over its edges in path order, each edge adding its token log-prob and then its duration
+    log-prob, ``acc = (acc + lt) + ld``.  The max-plus recurrence adds in that order and so gives the largest such
+    score exactly (float32 rounding is monotone).  Ties: the larger candidate wins; on equal values a blank edge beats
+    a label edge, and within one kind the shorter duration wins (also for the terminal edge).
+
+    Returns ``(scores, frames, label_durations)``:
+      * ``scores`` (N,) float32: the best path's score.
+      * ``frames`` int32, dense (N, U-1), compact (sum(labels_lengths),) in the labels' order: frames[n, u] is the frame
+        t of the best path's label edge for label u, (t, u) -> (t + d, u + 1).
+      * ``label_durations`` int32, the same shape: that edge's duration d, a value of ``durations`` (not an index).
+      Both are -1 for u >= labels_lengths[n] and on every lattice without an alignment.
+
+    Lattices without an alignment, in the classes of ``rnnt_loss_tdt`` on the same input: invalid lengths (compact:
+    also outside ``compact_hints``, or rows running past STU) or a live label outside [0, V) give score NaN; a NaN or
+    +inf in a live row, or a live row whose token or duration logits are all -inf, gives NaN (even for a row no path
+    visits); no path above the loss's dead threshold (best score at or below -5e29, e.g. Tn < min(d > 0)) gives -inf.
+    Padding rows are never read.  Deterministic; no host synchronisation in the dense layout and, inside
+    ``compact_hints``, in the compact one (CUDA-graph capturable); without hints the compact call makes one 16-byte
+    device->host copy.  bfloat16 results equal those of the float32 call on the widened logits, and compact results
+    equal those of the dense call on the same rows placed in a padded tensor."""
+    assert isinstance(compact, bool)
+    durations = _tdt_args("rnnt_align_tdt", logits, durations, sigma, blank, compact)
+    with torch.no_grad():
+        if compact:
+            hints = _hints()
+            return _C.rnnt_tdt_align_compact(logits, labels, frames_lengths, labels_lengths, list(durations),
+                                             float(sigma), blank, hints[0], hints[1])
+        return _C.rnnt_tdt_align_dense(logits, labels, frames_lengths, labels_lengths, list(durations), float(sigma),
+                                       blank)
+
+
+__all__ = ["rnnt_loss", "rnnt_align", "rnnt_align_tdt", "rnnt_loss_from_logits", "rnnt_loss_pruned",
+           "RNNTLossPruned", "rnnt_loss_simple", "RNNTLossSimple", "rnnt_loss_tdt", "RNNTLossTDT", "RNNTLossTDTCompact", "joint_pack",
            "JointPack", "RNNTLossFromLogits", "RNNTLossFromLogitsCompact", "RNNTLoss", "RNNTLossGather", "RNNTLossEager",
            "RNNTLossCompact", "compact_hints", "set_lse_mode", "core", "_C", "__version__"]

@@ -672,6 +672,36 @@ static TdtWorkspace carve_tdt(void *base, int64_t cells, int N, int D, bool comp
     w.bytes = off;
     return w;
 }
+// The TDT alignment (rnnt_b200_tdt_align_*), one size for both layouts: lse (cells,2), lp (cells,2+D), alpha (cells),
+// the decision bytes (cells), status (N), then the compact call's prefix sums (2N) and totals (4).
+struct TdtAlignWorkspace {
+    float2 *lse;
+    float *lp, *alpha;
+    uint8_t *dec;
+    int *status;
+    int64_t *prefix;
+    int *totals;
+    size_t bytes;
+};
+static TdtAlignWorkspace carve_tdt_align(void *base, int64_t cells, int N, int D) {
+    TdtAlignWorkspace w;
+    size_t off = 0;
+    auto take = [&](size_t bytes) {
+        void *p = base ? (void *)((char *)base + off) : nullptr;
+        off += align_up(bytes, 256);
+        return p;
+    };
+    const size_t c = (size_t)max(cells, (int64_t)0), n = (size_t)max(N, 0);
+    w.lse = (float2 *)take(c * sizeof(float2));
+    w.lp = (float *)take(c * (size_t)(2 + max(D, 0)) * sizeof(float));
+    w.alpha = (float *)take(c * sizeof(float));
+    w.dec = (uint8_t *)take(c);
+    w.status = (int *)take(n * sizeof(int));
+    w.prefix = (int64_t *)take(2 * n * sizeof(int64_t));
+    w.totals = (int *)take(4 * sizeof(int));
+    w.bytes = off;
+    return w;
+}
 
 extern "C" {
 
@@ -1032,6 +1062,58 @@ int rnnt_b200_tdt_compact_backward(void *stream, const void *logits, const float
     c.yn = yn; c.mem_pref = prefix; c.lab_pref = prefix + N; c.STU = STU;
     c.out = out; c.N = N; c.V = V; c.D = num_durations; c.blank = blank; c.io_bf16 = elem_bytes == 2;
     RNNT_TRY(launch_tdt_backward((cudaStream_t)stream, c), RNNT_STATUS_GRADS_BLANK_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+size_t rnnt_b200_tdt_align_workspace_bytes(int64_t cells, int N, int num_durations) {
+    return carve_tdt_align(nullptr, cells, N, num_durations).bytes;
+}
+
+int rnnt_b200_tdt_align_dense(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                              const int *labels, const int *xn, const int *yn, const int *durations, int num_durations,
+                              float sigma, float *scores, int *frames, int *label_durations, int N, int T, int U,
+                              int V, int blank, int elem_bytes) {
+    TdtDurations dur;
+    if (!tdt_durations(durations, num_durations, &dur) || !tdt_args_ok(N, T, U, V, num_durations, blank, elem_bytes, logits) ||
+        !std::isfinite(sigma) || sigma < 0.0f || !scores || !frames || !label_durations ||
+        !workspace_aligned16(workspace))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    const int64_t cells = (int64_t)N * T * U;
+    if (!workspace || workspace_bytes < rnnt_b200_tdt_align_workspace_bytes(cells, N, num_durations))
+        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    const TdtAlignWorkspace w = carve_tdt_align(workspace, cells, N, num_durations);
+    TdtFwd c = {};
+    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = scores;
+    c.lse = w.lse; c.lp = w.lp; c.alpha = w.alpha; c.status = w.status;
+    c.N = N; c.T = T; c.U = U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur; c.io_bf16 = elem_bytes == 2;
+    RNNT_TRY(launch_tdt_align((cudaStream_t)stream, c, w.dec, frames, label_durations), RNNT_STATUS_WARP_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+int rnnt_b200_tdt_align_compact(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                const int *labels, const int *xn, const int *yn, const int *durations,
+                                int num_durations, float sigma, float *scores, int *frames, int *label_durations,
+                                int64_t STU, int N, int V, int blank, int elem_bytes, int max_T, int max_U) {
+    TdtDurations dur;
+    if (!tdt_durations(durations, num_durations, &dur) ||
+        !tdt_compact_args_ok(N, STU, V, num_durations, blank, elem_bytes, logits) || !std::isfinite(sigma) ||
+        sigma < 0.0f || !scores || !frames || !label_durations || !workspace_aligned16(workspace) || max_T < 1 ||
+        max_U < 1)
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    if (!workspace || workspace_bytes < rnnt_b200_tdt_align_workspace_bytes(STU, N, num_durations))
+        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    cudaStream_t s = (cudaStream_t)stream;
+    const TdtAlignWorkspace w = carve_tdt_align(workspace, STU, N, num_durations);
+    RNNT_TRY(launch_prefix(s, xn, yn, N, w.prefix, w.prefix + N, w.totals), RNNT_STATUS_GATHER_FAILED);
+    TdtFwd c = {};
+    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = scores;
+    c.mem_pref = w.prefix; c.lab_pref = w.prefix + N; c.STU = STU;
+    c.lse = w.lse; c.lp = w.lp; c.alpha = w.alpha; c.status = w.status;
+    c.N = N; c.T = max_T; c.U = max_U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur;
+    c.io_bf16 = elem_bytes == 2;
+    RNNT_TRY(launch_tdt_align(s, c, w.dec, frames, label_durations), RNNT_STATUS_WARP_FAILED);
     return RNNT_STATUS_SUCCESS;
 }
 

@@ -233,6 +233,10 @@ struct TdtBwd {
     int io_bf16;
 };
 cudaError_t launch_tdt_backward(cudaStream_t s, const TdtBwd &c);
+// The Viterbi alignment on the TDT lattice (rnnt_b200_tdt_align_*): c as for the forward, with costs = the scores
+// (N) and pg, beta, ll unused; the normaliser writes lse and lp, then k_tdt_align writes alpha, dec (cells bytes, the
+// decision per cell), status, the scores, and frames and fdur (dense (N,U-1), compact (sum yn)).
+cudaError_t launch_tdt_align(cudaStream_t s, const TdtFwd &c, uint8_t *dec, int *frames, int *fdur);
 void tdt_launch_record(int32_t *out);     // copy of the last TDT launch's record (rnntTdtLaunchRecord_t)
 
 // expand.cu -- small helpers of the python-level API

@@ -14,6 +14,9 @@
 //                CTA also classifies the lattice and writes its cost.
 //   k_tdt_post   per cell, the edge posteriors -> (Pb, Pl, Pd[0..D)) (N,T,U,2+D), unscaled
 //   k_tdt_emit   (backward) one read of the logits and one write of d loss / d logits (N,T,U,V+D), every element once
+//   k_tdt_align  (rnnt_b200_tdt_align_*, after k_tdt_norm) the Viterbi alignment: one CTA per lattice (grid (N, 1)),
+//                tdt_recur's alpha side in max-plus form with a decision byte per cell, then the class, the score and
+//                the backtrace in the same kernel
 //
 // Every LSE is one max-then-sum over all candidate terms of a cell.  All candidates are finite (kBig sentinels) or NaN,
 // absent ones are -inf and only ever subtracted from a finite maximum: -inf - -inf is never formed.  No atomics: every
@@ -197,14 +200,72 @@ __device__ __forceinline__ float lse_cands(const float (&c)[C]) {
     return m + logf(s);
 }
 
+// The Viterbi alignment's outputs (k_tdt_align): the alpha side of tdt_recur in max-plus form.  Per cell, the index k
+// in [0, 2 KD) of the candidate it took (2j: blank edge of duration d[j], 2j + 1: label edge), kTdtNoPred for (0, 0)
+// and for a cell without a predecessor; frames / fdur: dense (N,U-1), compact (sum yn) in the labels' order.
+constexpr int kTdtNoPred = 0xff;
+struct TdtAlignOut {
+    uint8_t *dec;                         // decisions, addressed as alpha
+    int *frames, *fdur;
+};
+
+// The largest of C candidates and its index in `arg`: blank edges (even k) first, then label edges (odd k), each by
+// increasing duration, and only a strictly larger value replaces the one held, so on a tie blank beats label and the
+// shorter duration wins.  Absent candidates are -inf and never taken.  No candidate: kBig and kTdtNoPred, as lse_cands.
+// A NaN candidate is never taken either (the lattice is classed NaN whatever the sweep gives).
+template <int C>
+__device__ __forceinline__ float max_cands(const float (&c)[C], int &arg) {
+    float m = -INFINITY;
+    arg = kTdtNoPred;
+#pragma unroll
+    for (int k = 0; k < C; k += 2)
+        if (c[k] > m) { m = c[k]; arg = k; }
+#pragma unroll
+    for (int k = 1; k < C; k += 2)
+        if (c[k] > m) { m = c[k]; arg = k; }
+    return arg == kTdtNoPred ? kBig : m;
+}
+
+// ALIGN, after the sweep, every thread of the CTA: the lattice's `slots` label slots at lab_base are set to -1; then,
+// for a lattice classed ok, thread 0 follows the decisions back from the best terminal edge's source (t0, Un - 1) to
+// (0, 0) and writes frame t and duration d of each label edge (t, u) -> (t + d, u + 1) into slot u.  A decision only
+// ever names a predecessor that exists, so the walk stays inside the lattice; it is bounded by Tn + Un - 1 steps all
+// the same (a path has at most Tn - 1 blank edges inside the lattice and Un - 1 label edges).
+__device__ __forceinline__ void tdt_backtrace(const TdtRec &a, const TdtAlignOut &o, int64_t base, int ld,
+                                              int64_t lab_base, int slots, int Tn, int Un, int t0, bool ok) {
+    int *fr = o.frames + lab_base, *fd = o.fdur + lab_base;
+    for (int u = threadIdx.x; u < slots; u += blockDim.x) {
+        fr[u] = -1;
+        fd[u] = -1;
+    }
+    __syncthreads();
+    if (!ok || threadIdx.x != 0) return;
+    int t = t0, u = Un - 1;
+    for (int step = 0; step < Tn + Un - 1; ++step) {
+        const int k = o.dec[base + (int64_t)t * ld + u];
+        if (k == kTdtNoPred) break;
+        const int d = a.dur.d[k >> 1];
+        t -= d;
+        if (k & 1) {
+            --u;
+            fr[u] = t;
+            fd[u] = d;
+        }
+    }
+}
+
 // alpha (blockIdx.y == 0) or beta (1) of lattice blockIdx.x.  KD >= D: the candidate arrays' compile-time size.
 // The ring holds U (dense: the padded width, compact: max_U) columns per diagonal; lp, alpha and beta are addressed
 // with the lattice's row stride ld (dense U, compact Un).
-template <int KD, bool COMPACT>
-__device__ __forceinline__ void tdt_recur(const TdtRec &a, const TdtCompact &cp) {
+// ALIGN (k_tdt_align, grid (N, 1)): the alpha side only, with max_cands in place of lse_cands and a decision byte per
+// cell; it also checks every live cell's own lp row for NaN, as the beta side does.  After the sweep, the class and
+// the score (a.costs) of the lattice, then the backtrace (tdt_backtrace).
+template <int KD, bool COMPACT, bool ALIGN = false>
+__device__ __forceinline__ void tdt_recur(const TdtRec &a, const TdtCompact &cp,
+                                          const TdtAlignOut &o = TdtAlignOut{}) {
     extern __shared__ float ring[];
     const int n = blockIdx.x;
-    const bool beta_side = blockIdx.y == 1;
+    const bool beta_side = !ALIGN && blockIdx.y == 1;
     int Tn, Un;
     bool ok;
     int64_t base, lab_base;
@@ -217,7 +278,14 @@ __device__ __forceinline__ void tdt_recur(const TdtRec &a, const TdtCompact &cp)
         base = (int64_t)n * a.T * a.U; lab_base = (int64_t)n * (a.U - 1);
     }
     if (!ok) {
-        if (beta_side && threadIdx.x == 0) {
+        if constexpr (ALIGN) {
+            if (threadIdx.x == 0) {
+                a.status[n] = kTdtInvalid;
+                a.costs[n] = NAN;
+            }
+            // the label slots of lattice n: dense U - 1, compact yn[n] (none when it is negative)
+            tdt_backtrace(a, o, 0, 0, lab_base, COMPACT ? max(Un - 1, 0) : a.U - 1, 0, 0, 0, false);
+        } else if (beta_side && threadIdx.x == 0) {
             a.status[n] = kTdtInvalid;
             a.costs[n] = NAN;
             a.ll[n] = NAN;
@@ -261,7 +329,19 @@ __device__ __forceinline__ void tdt_recur(const TdtRec &a, const TdtCompact &cp)
                         }
                     }
                 }
-                v = (t == 0 && u == 0) ? 0.0f : lse_cands(c);
+                if constexpr (ALIGN) {
+                    // the cell's own row, for the NaN class (the beta side's check, here on the alpha side)
+                    const float *r = lp + ((int64_t)t * ld + u) * W2;
+                    saw_nan |= (r[0] != r[0]) || (u < Un - 1 && r[1] != r[1]);
+#pragma unroll
+                    for (int j = 0; j < KD; ++j)
+                        if (j < D) saw_nan |= r[2 + j] != r[2 + j];
+                    int k = kTdtNoPred;
+                    v = (t == 0 && u == 0) ? 0.0f : max_cands(c, k);
+                    o.dec[base + (int64_t)t * ld + u] = (uint8_t)k;
+                } else {
+                    v = (t == 0 && u == 0) ? 0.0f : lse_cands(c);
+                }
             } else {
                 // push-side view: the cell's own weights, beta of the destinations; a blank to t + d == Tn from the
                 // last column is terminal (beta 0 after it)
@@ -290,7 +370,7 @@ __device__ __forceinline__ void tdt_recur(const TdtRec &a, const TdtCompact &cp)
         }
         __syncthreads();
     }
-    if (!beta_side) return;
+    if (!beta_side && !ALIGN) return;
     bool bad = false;
     for (int u = threadIdx.x; u < Un - 1; u += blockDim.x) {
         const int lab = labels[u];
@@ -298,6 +378,28 @@ __device__ __forceinline__ void tdt_recur(const TdtRec &a, const TdtCompact &cp)
     }
     bad = __syncthreads_or(bad);
     saw_nan = __syncthreads_or(saw_nan);
+    if constexpr (ALIGN) {
+        // the terminal step: the best blank edge of duration d > 0 from (Tn - d, Un - 1), by the tie rule of
+        // max_cands (the shorter duration wins).  Every thread computes it alike from alpha in global memory (the
+        // sweep ended on a barrier), so the choice needs no broadcast and the ring keeps all of shared memory.
+        float best = -INFINITY;
+        int t0 = 0;
+        for (int j = 0; j < D; ++j) {
+            const int d = a.dur.d[j], tp = Tn - d;
+            if (d > 0 && tp >= 0) {
+                const float *r = lp + ((int64_t)tp * ld + Un - 1) * W2;
+                const float cand = (out[(int64_t)tp * ld + Un - 1] + r[0]) + r[2 + j];
+                if (cand > best) { best = cand; t0 = tp; }
+            }
+        }
+        const int st = bad ? kTdtInvalid : saw_nan ? kTdtNan : lattice_dead(best) ? kTdtDead : kTdtOk;
+        if (threadIdx.x == 0) {
+            a.status[n] = st;
+            a.costs[n] = st == kTdtOk ? best : st == kTdtDead ? -INFINITY : NAN;
+        }
+        tdt_backtrace(a, o, base, ld, lab_base, COMPACT ? Un - 1 : U - 1, Tn, Un, t0, st == kTdtOk);
+        return;
+    }
     if (threadIdx.x == 0) {
         const float lP = out[0];
         const int st = bad ? kTdtInvalid : saw_nan ? kTdtNan : lattice_dead(lP) ? kTdtDead : kTdtOk;
@@ -310,6 +412,16 @@ __device__ __forceinline__ void tdt_recur(const TdtRec &a, const TdtCompact &cp)
 template <int KD>
 __global__ void __launch_bounds__(kTdtMaxThreads) k_tdt_recur(TdtRec a) {
     tdt_recur<KD, false>(a, TdtCompact{});
+}
+
+// The Viterbi alignment, one CTA per lattice (grid (N, 1)): a.costs = the scores; a.beta, a.ll unused
+template <int KD>
+__global__ void __launch_bounds__(kTdtMaxThreads) k_tdt_align(TdtRec a, TdtAlignOut o) {
+    tdt_recur<KD, false, true>(a, TdtCompact{}, o);
+}
+template <int KD>
+__global__ void __launch_bounds__(kTdtMaxThreads) k_tdt_align_compact(TdtRec a, TdtCompact cp, TdtAlignOut o) {
+    tdt_recur<KD, true, true>(a, cp, o);
 }
 
 // a.T, a.U = max_T, max_U
@@ -621,28 +733,59 @@ static cudaError_t tdt_recur_post(cudaStream_t s, const TdtPlan &p, const TdtFwd
     return cudaGetLastError();
 }
 
+// The plan of a forward or alignment call, recorded for rnnt_b200_debug_last_tdt_launch (the emit fields 0)
+static TdtPlan tdt_plan_recorded(const TdtFwd &c) {
+    const TdtPlan p = tdt_plan(c.U, c.dur, c.x, c.io_bf16 ? 2 : 4, c.V);
+    std::lock_guard<std::mutex> lock(g_tdt_mu);
+    int32_t *rec = g_tdt_record;
+    memset(rec, 0, sizeof(g_tdt_record));
+    rec[RNNT_TDT_REC_SEQ] = ++g_tdt_seq;
+    rec[RNNT_TDT_REC_CLUSTER] = 0;
+    rec[RNNT_TDT_REC_WARPS] = p.warps;
+    rec[RNNT_TDT_REC_RING] = p.ring;
+    rec[RNNT_TDT_REC_PASSES] = p.passes;
+    rec[RNNT_TDT_REC_KD] = p.kd;
+    rec[RNNT_TDT_REC_NORM_GROUP] = p.norm_group;
+    rec[RNNT_TDT_REC_NORM_LANES] = p.norm_lanes;
+    rec[RNNT_TDT_REC_SMEM] = p.smem;
+    return p;
+}
+
 cudaError_t launch_tdt_forward(cudaStream_t s, const TdtFwd &c) {
     const int64_t cells = c.mem_pref ? c.STU : (int64_t)c.N * c.T * c.U;
-    const TdtPlan p = tdt_plan(c.U, c.dur, c.x, c.io_bf16 ? 2 : 4, c.V);
-    {
-        std::lock_guard<std::mutex> lock(g_tdt_mu);
-        int32_t *rec = g_tdt_record;
-        memset(rec, 0, sizeof(g_tdt_record));
-        rec[RNNT_TDT_REC_SEQ] = ++g_tdt_seq;
-        rec[RNNT_TDT_REC_CLUSTER] = 0;
-        rec[RNNT_TDT_REC_WARPS] = p.warps;
-        rec[RNNT_TDT_REC_RING] = p.ring;
-        rec[RNNT_TDT_REC_PASSES] = p.passes;
-        rec[RNNT_TDT_REC_KD] = p.kd;
-        rec[RNNT_TDT_REC_NORM_GROUP] = p.norm_group;
-        rec[RNNT_TDT_REC_NORM_LANES] = p.norm_lanes;
-        rec[RNNT_TDT_REC_SMEM] = p.smem;
-    }
+    const TdtPlan p = tdt_plan_recorded(c);
     if (cells == 0 && !c.mem_pref) return cudaSuccess;   // compact: with no rows the recurrence still gives the costs
     cudaError_t e = c.io_bf16 ? tdt_norm_as(s, p, static_cast<const __nv_bfloat16 *>(c.x), c, cells)
                               : tdt_norm_as(s, p, static_cast<const float *>(c.x), c, cells);
     if (e != cudaSuccess) return e;
     return p.kd == 5 ? tdt_recur_post<5>(s, p, c, cells) : tdt_recur_post<kTdtMaxD>(s, p, c, cells);
+}
+
+template <int KD>
+static cudaError_t tdt_align_as(cudaStream_t s, const TdtPlan &p, const TdtFwd &c, const TdtAlignOut &o) {
+    static std::atomic<bool> smem_set[kMaxDevices], smem_set_compact[kMaxDevices];
+    if (p.smem > (48 << 10)) {
+        const cudaError_t e = c.mem_pref ? ensure_dyn_smem(k_tdt_align_compact<KD>, smem_set_compact,
+                                                           max_optin_smem(current_device()))
+                                         : ensure_dyn_smem(k_tdt_align<KD>, smem_set, max_optin_smem(current_device()));
+        if (e != cudaSuccess) return e;
+    }
+    const TdtRec r = {c.lp, c.labels, c.xn, c.yn, c.alpha, nullptr, nullptr, c.costs, c.status, c.T, c.U, c.V,
+                      c.dur.D, p.ring, c.dur};
+    if (c.mem_pref) k_tdt_align_compact<KD><<<dim3(c.N, 1), p.warps * 32, p.smem, s>>>(r, tdt_compact(c), o);
+    else k_tdt_align<KD><<<dim3(c.N, 1), p.warps * 32, p.smem, s>>>(r, o);
+    count_launch();
+    return cudaGetLastError();
+}
+
+cudaError_t launch_tdt_align(cudaStream_t s, const TdtFwd &c, uint8_t *dec, int *frames, int *fdur) {
+    const int64_t cells = c.mem_pref ? c.STU : (int64_t)c.N * c.T * c.U;
+    const TdtPlan p = tdt_plan_recorded(c);
+    cudaError_t e = c.io_bf16 ? tdt_norm_as(s, p, static_cast<const __nv_bfloat16 *>(c.x), c, cells)
+                              : tdt_norm_as(s, p, static_cast<const float *>(c.x), c, cells);
+    if (e != cudaSuccess) return e;
+    const TdtAlignOut o = {dec, frames, fdur};
+    return p.kd == 5 ? tdt_align_as<5>(s, p, c, o) : tdt_align_as<kTdtMaxD>(s, p, c, o);
 }
 
 template <typename IO>
