@@ -459,13 +459,145 @@ def rnnt_loss_tdt(logits, labels, frames_lengths, labels_lengths, durations, sig
         loss = rnnt_loss_tdt(logits, labels_c, frames_lengths, labels_lengths, [0, 1, 2, 3, 4], compact=True,
                              reduction="mean")
 
-    Not offered: ``fastemit_lambda``, NeMo's ``omega`` mixing with the regular transducer loss, and multi-blank.  The
-    best path itself (token frames and durations) is ``rnnt_align_tdt``."""
+    Not offered: ``fastemit_lambda`` and NeMo's ``omega`` mixing with the regular transducer loss.  The multi-blank
+    transducer loss is ``rnnt_loss_multiblank``.  The best path itself (token frames and durations) is
+    ``rnnt_align_tdt``."""
     assert average_frames is None or isinstance(average_frames, bool)
     assert reduction is None or reduction in ("none", "mean", "sum")
     assert not labels.requires_grad and not frames_lengths.requires_grad and not labels_lengths.requires_grad
     durations = _tdt_args("rnnt_loss_tdt", logits, durations, sigma, blank, compact)
     fn = RNNTLossTDTCompact if compact else RNNTLossTDT
+    costs = fn.apply(logits, labels, frames_lengths, labels_lengths, durations, float(sigma), blank)
+    return _reduce(costs, frames_lengths, average_frames, reduction)
+
+
+class RNNTLossMultiblank(torch.autograd.Function):
+    """The multi-blank transducer loss from (N,T,U,V) joint logits.  Forward reads the logits once (one normaliser per
+    cell, the 2 + B log-probs the recurrence needs), runs alpha and beta on the lattice and keeps lse (N,T,U) and the
+    per-cell edge posteriors (N,T,U,2+B); backward reads the logits again and writes d loss / d logits, of their
+    dtype."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, frames_lengths, labels_lengths, big_blank_durations, sigma, blank):
+        need = ctx.needs_input_grad[0]
+        costs, lse, pg = _C.rnnt_multiblank_forward(logits, labels, frames_lengths, labels_lengths,
+                                                    list(big_blank_durations), sigma, blank, need)
+        if need:
+            ctx.save_for_backward(logits, lse, pg, labels)
+            ctx.durations = list(big_blank_durations)
+            ctx.blank = blank
+        return costs
+
+    @staticmethod
+    def backward(ctx, grads_output):
+        logits, lse, pg, labels = ctx.saved_tensors
+        go = grads_output.contiguous().to(torch.float32)
+        g = _C.rnnt_multiblank_backward(logits, lse, pg, labels, ctx.durations, go, ctx.blank)
+        return g, None, None, None, None, None, None
+
+
+class RNNTLossMultiblankCompact(torch.autograd.Function):
+    """``RNNTLossMultiblank`` on compact (STU,V) logits in ``joint_pack``'s row order.  Forward keeps lse (STU), the
+    posteriors (STU,2+B) and the compact prefix sums (16 bytes per lattice).  Inside ``compact_hints`` the forward has
+    no host sync (CUDA-graph capturable)."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, frames_lengths, labels_lengths, big_blank_durations, sigma, blank):
+        need = ctx.needs_input_grad[0]
+        hints = _hints()
+        costs, lse, pg, prefix = _C.rnnt_multiblank_compact_forward(logits, labels, frames_lengths, labels_lengths,
+                                                                    list(big_blank_durations), sigma, blank, need,
+                                                                    hints[0], hints[1])
+        if need:
+            ctx.save_for_backward(logits, lse, pg, labels, frames_lengths, labels_lengths, prefix)
+            ctx.durations = list(big_blank_durations)
+            ctx.blank = blank
+        return costs
+
+    @staticmethod
+    def backward(ctx, grads_output):
+        logits, lse, pg, labels, xn, yn, prefix = ctx.saved_tensors
+        go = grads_output.contiguous().to(torch.float32)
+        g = _C.rnnt_multiblank_compact_backward(logits, lse, pg, labels, xn, yn, prefix, ctx.durations, go, ctx.blank)
+        return g, None, None, None, None, None, None
+
+
+def _multiblank_args(fn, logits, big_blank_durations, sigma, blank, compact):
+    """The argument checks of ``rnnt_loss_multiblank``: the durations, sigma, the logits' shape and blank.  Returns
+    (durations as a tuple, the standard blank's column)."""
+    d = big_blank_durations
+    if not isinstance(d, (list, tuple)) or not d or any(isinstance(x, bool) or not isinstance(x, int) for x in d):
+        raise ValueError("%s: big_blank_durations must be a non-empty list or tuple of ints, got %r" % (fn, d))
+    if any(x < 2 or x > 16 for x in d) or any(b <= a for a, b in zip(d, d[1:])):
+        raise ValueError("%s: big_blank_durations must be strictly increasing, each in [2, 16], got %r" % (fn, d))
+    if isinstance(sigma, bool) or not isinstance(sigma, (int, float)) or not math.isfinite(sigma) or sigma < 0:
+        raise ValueError("%s: sigma must be a finite number >= 0, got %r" % (fn, sigma))
+    assert isinstance(compact, bool)
+    if logits.dim() != (2 if compact else 4) or logits.size(-1) <= len(d):
+        raise ValueError("%s: logits must be %s with V > B = len(big_blank_durations) = %d, got shape %s"
+                         % (fn, "(STU, V)" if compact else "(N, T, U, V)", len(d), tuple(logits.shape)))
+    V = logits.size(-1)
+    if blank is None:
+        blank = V - 1
+    if isinstance(blank, bool) or not isinstance(blank, int) or not len(d) <= blank < V:
+        raise ValueError("%s: blank must be None or an int in [B, V) = [%d, %d), got %r" % (fn, len(d), V, blank))
+    return tuple(d), blank
+
+
+def rnnt_loss_multiblank(logits, labels, frames_lengths, labels_lengths, big_blank_durations, sigma=0.0,
+                         average_frames=False, reduction="none", blank=None, compact=False):
+    """Multi-blank transducer loss (Xu et al. 2022, "Multi-blank Transducers for Speech Recognition",
+    arXiv:2211.03541), the loss of NeMo's multi-blank Conformer-Transducer, from the joint network's logits.  Follows
+    NeMo's definition (``MultiblankRNNTLossPytorch``: the same alpha recursion, terminal sum, column layout and sigma);
+    not tested against NeMo.
+
+    Args:
+        logits: (N, T, U, V) float32 or bfloat16.  V is the whole row: the tokens, the big blanks and the standard
+            blank.  U = labels.size(1) + 1.  ``compact=True``: (STU, V), see below.
+        labels: (N, U-1) int32; frames_lengths, labels_lengths: (N,) int32, as for ``rnnt_loss_from_logits``.
+        big_blank_durations: list or tuple of B >= 1 ints, strictly increasing, each in [2, 16] (else ValueError),
+            e.g. [2, 4, 8].  Host values: they reach the kernels as launch parameters.
+        sigma: NeMo's logit under-normalisation, a finite float >= 0 (else ValueError).
+        average_frames, reduction: as in ``rnnt_loss_from_logits``.
+        blank: the standard blank's column; None (default) means V - 1, NeMo's layout.  Big blank i sits in column
+            blank - 1 - i.  An explicit blank must lie in [B, V).
+        compact: the ragged layout of ``rnnt_loss_from_logits(compact=True)``.
+
+    Lattice n has Tn = frames_lengths[n] frames and Un = labels_lengths[n] + 1 columns.  Every edge weight is
+    lp = log_softmax(logits[n,t,u,:]) - sigma at the edge's column.  Edges out of cell (t, u), with t < Tn and u < Un:
+
+    * standard blank, weight lp[blank]: to (t + 1, u) if t + 1 < Tn; terminal if u = Un - 1 and t + 1 = Tn;
+    * big blank i, d = big_blank_durations[i], weight lp[blank - 1 - i]: to (t + d, u) if t + d < Tn; terminal if
+      u = Un - 1 and t + d = Tn; otherwise no edge;
+    * label, for u < Un - 1, weight lp[labels[n,u]]: to (t, u + 1).
+
+    P is the sum, over paths from (0, 0) to a terminal edge, of exp(sum of edge weights); cost[n] = -log P.  Per cell,
+    the edge posteriors are P_std, P_big[i] and Pl, and occ is their sum.  The gradient of the cost w.r.t. the logits,
+    times grad_output[n] (and the reduction's weights), is
+    occ * softmax[v] - P_std [v = blank] - sum_i P_big[i] [v = blank - 1 - i] - Pl [v = label]; a label equal to a
+    blank column gets both terms, as autograd gives.
+
+    Degenerate input, without host synchronisation: padding rows are never read and get exact zeros; invalid lengths or
+    a live label outside [0, V) give cost NaN and zero gradient rows; a NaN or +inf in a live row, or a live row that is
+    all -inf, gives cost NaN and NaN on that lattice's live rows (every other lattice is bit-identical to a batch
+    without it); no path of finite log-probability (only through -inf logits, as the standard blank always gives a
+    path) gives cost +inf and zero gradient rows.
+
+    Costs are float32; ``logits.grad`` has the logits' dtype.  bfloat16: costs equal those of the float32 logits with
+    the same values bit for bit, and the gradient is their float32 gradient rounded once.  Deterministic (no atomics),
+    no host synchronisation: a step can be captured in a CUDA graph.  ``set_lse_mode`` does not apply.
+
+    ``compact=True``: ``logits`` is (STU, V), rows in ``joint_pack``'s order, and ``labels`` is (sum labels_lengths,)
+    int32, as for ``rnnt_loss_tdt(compact=True)``, with the same ``compact_hints`` behaviour and classes: costs, the
+    posteriors and the gradient are bit for bit those of the same rows placed in a padded tensor at the same element
+    offset modulo 4.
+
+    Not offered: ``fastemit_lambda``, ``rnnt_type``, ``delay_penalty`` and TDT's ``omega``."""
+    assert average_frames is None or isinstance(average_frames, bool)
+    assert reduction is None or reduction in ("none", "mean", "sum")
+    assert not labels.requires_grad and not frames_lengths.requires_grad and not labels_lengths.requires_grad
+    durations, blank = _multiblank_args("rnnt_loss_multiblank", logits, big_blank_durations, sigma, blank, compact)
+    fn = RNNTLossMultiblankCompact if compact else RNNTLossMultiblank
     costs = fn.apply(logits, labels, frames_lengths, labels_lengths, durations, float(sigma), blank)
     return _reduce(costs, frames_lengths, average_frames, reduction)
 
@@ -812,6 +944,7 @@ def rnnt_align_tdt(logits, labels, frames_lengths, labels_lengths, durations, si
 
 
 __all__ = ["rnnt_loss", "rnnt_align", "rnnt_align_tdt", "rnnt_loss_from_logits", "rnnt_loss_pruned",
+           "rnnt_loss_multiblank", "RNNTLossMultiblank", "RNNTLossMultiblankCompact",
            "RNNTLossPruned", "rnnt_loss_simple", "RNNTLossSimple", "rnnt_loss_tdt", "RNNTLossTDT", "RNNTLossTDTCompact", "joint_pack",
            "JointPack", "RNNTLossFromLogits", "RNNTLossFromLogitsCompact", "RNNTLoss", "RNNTLossGather", "RNNTLossEager",
            "RNNTLossCompact", "compact_hints", "set_lse_mode", "core", "_C", "__version__"]

@@ -652,6 +652,26 @@ static bool tdt_compact_args_ok(int N, int64_t STU, int V, int D, int blank, int
            N >= 0 && N <= 65535 && STU >= 0 && STU < ((int64_t)1 << 31) && V >= 1 &&
            (int64_t)V + D < ((int64_t)1 << 22) && blank >= 0 && blank < V;
 }
+// Multi-blank: B big blanks with durations strictly increasing in [2, 16] (so B <= 15), in the durations' place
+static bool mb_durations(const int *durations, int B, TdtDurations *out) {
+    if (!durations || B < 1 || B > kTdtMaxD - 2) return false;
+    *out = {};
+    out->D = B;
+    for (int j = 0; j < B; ++j) {
+        const int d = durations[j];
+        if (d < 2 || d > 16 || (j > 0 && d <= durations[j - 1])) return false;
+        out->d[j] = d;
+    }
+    out->dmax = durations[B - 1];
+    return true;
+}
+// the row is V logits: the standard blank at `blank`, big blank i at blank - 1 - i, so blank in [B, V)
+static bool mb_args_ok(int N, int T, int U, int V, int B, int blank, int elem_bytes, const void *logits) {
+    return tdt_args_ok(N, T, U, V, 0, blank, elem_bytes, logits) && blank >= B;
+}
+static bool mb_compact_args_ok(int N, int64_t STU, int V, int B, int blank, int elem_bytes, const void *logits) {
+    return tdt_compact_args_ok(N, STU, V, 0, blank, elem_bytes, logits) && blank >= B;
+}
 // cells: N*T*U (dense) or STU (compact); the compact call also takes 4 ints for the totals it does not return
 struct TdtWorkspace { float *lp, *alpha, *beta, *ll; int *status, *totals; size_t bytes; };
 static TdtWorkspace carve_tdt(void *base, int64_t cells, int N, int D, bool compact) {
@@ -1114,6 +1134,99 @@ int rnnt_b200_tdt_align_compact(void *stream, void *workspace, size_t workspace_
     c.N = N; c.T = max_T; c.U = max_U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur;
     c.io_bf16 = elem_bytes == 2;
     RNNT_TRY(launch_tdt_align(s, c, w.dec, frames, label_durations), RNNT_STATUS_WARP_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+size_t rnnt_b200_multiblank_workspace_bytes(int N, int T, int U, int num_big_blanks) {
+    return carve_tdt(nullptr, (int64_t)max(N, 0) * max(T, 0) * max(U, 0), N, num_big_blanks, false).bytes;
+}
+
+int rnnt_b200_multiblank_forward(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                 const int *labels, const int *xn, const int *yn, const int *big_blank_durations,
+                                 int num_big_blanks, float sigma, float *costs, float *lse, float *grads, int N, int T,
+                                 int U, int V, int blank, int elem_bytes) {
+    TdtDurations dur;
+    if (!mb_durations(big_blank_durations, num_big_blanks, &dur) ||
+        !mb_args_ok(N, T, U, V, num_big_blanks, blank, elem_bytes, logits) || !std::isfinite(sigma) || sigma < 0.0f ||
+        !costs || !lse || !workspace_aligned16(workspace))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    if (!workspace || workspace_bytes < rnnt_b200_multiblank_workspace_bytes(N, T, U, num_big_blanks))
+        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    const TdtWorkspace w = carve_tdt(workspace, (int64_t)N * T * U, N, num_big_blanks, false);
+    TdtFwd c = {};
+    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = costs;
+    c.multiblank = true; c.lse_mb = lse; c.pg = grads;
+    c.lp = w.lp; c.alpha = w.alpha; c.beta = w.beta; c.ll = w.ll; c.status = w.status;
+    c.N = N; c.T = T; c.U = U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur; c.io_bf16 = elem_bytes == 2;
+    RNNT_TRY(launch_tdt_forward((cudaStream_t)stream, c), RNNT_STATUS_WARP_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+int rnnt_b200_multiblank_backward(void *stream, const void *logits, const float *lse, const float *grads,
+                                  const int *labels, const int *big_blank_durations, int num_big_blanks,
+                                  const float *grad_out, void *out, int N, int T, int U, int V, int blank,
+                                  int elem_bytes) {
+    TdtDurations dur;
+    if (!mb_durations(big_blank_durations, num_big_blanks, &dur) ||
+        !mb_args_ok(N, T, U, V, num_big_blanks, blank, elem_bytes, logits) ||
+        (reinterpret_cast<uintptr_t>(out) & (uintptr_t)(elem_bytes - 1)) || !lse || !grads || !out)
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    TdtBwd c = {};
+    c.x = logits; c.multiblank = true; c.lse_mb = lse; c.pg = grads; c.labels = labels; c.grad_out = grad_out;
+    c.out = out; c.N = N; c.T = T; c.U = U; c.V = V; c.D = num_big_blanks; c.blank = blank;
+    c.io_bf16 = elem_bytes == 2;
+    RNNT_TRY(launch_tdt_backward((cudaStream_t)stream, c), RNNT_STATUS_GRADS_BLANK_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+size_t rnnt_b200_multiblank_compact_workspace_bytes(int64_t STU, int N, int num_big_blanks) {
+    return carve_tdt(nullptr, STU, N, num_big_blanks, true).bytes;
+}
+
+int rnnt_b200_multiblank_compact_forward(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                         const int *labels, const int *xn, const int *yn,
+                                         const int *big_blank_durations, int num_big_blanks, float sigma,
+                                         float *costs, float *lse, float *grads, int64_t *prefix, int *totals,
+                                         int64_t STU, int N, int V, int blank, int elem_bytes, int max_T, int max_U) {
+    TdtDurations dur;
+    if (!mb_durations(big_blank_durations, num_big_blanks, &dur) ||
+        !mb_compact_args_ok(N, STU, V, num_big_blanks, blank, elem_bytes, logits) || !std::isfinite(sigma) ||
+        sigma < 0.0f || !costs || !lse || !workspace_aligned16(workspace) || !prefix || max_T < 1 || max_U < 1)
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    if (!workspace || workspace_bytes < rnnt_b200_multiblank_compact_workspace_bytes(STU, N, num_big_blanks))
+        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    cudaStream_t s = (cudaStream_t)stream;
+    const TdtWorkspace w = carve_tdt(workspace, STU, N, num_big_blanks, true);
+    RNNT_TRY(launch_prefix(s, xn, yn, N, prefix, prefix + N, totals ? totals : w.totals), RNNT_STATUS_GATHER_FAILED);
+    TdtFwd c = {};
+    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = costs;
+    c.mem_pref = prefix; c.lab_pref = prefix + N; c.STU = STU;
+    c.multiblank = true; c.lse_mb = lse; c.pg = grads;
+    c.lp = w.lp; c.alpha = w.alpha; c.beta = w.beta; c.ll = w.ll; c.status = w.status;
+    c.N = N; c.T = max_T; c.U = max_U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur;
+    c.io_bf16 = elem_bytes == 2;
+    RNNT_TRY(launch_tdt_forward(s, c), RNNT_STATUS_WARP_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+int rnnt_b200_multiblank_compact_backward(void *stream, const void *logits, const float *lse, const float *grads,
+                                          const int *labels, const int *yn, const int *big_blank_durations,
+                                          int num_big_blanks, const int64_t *prefix, const float *grad_out, void *out,
+                                          int64_t STU, int N, int V, int blank, int elem_bytes) {
+    TdtDurations dur;
+    if (!mb_durations(big_blank_durations, num_big_blanks, &dur) ||
+        !mb_compact_args_ok(N, STU, V, num_big_blanks, blank, elem_bytes, logits) ||
+        (reinterpret_cast<uintptr_t>(out) & (uintptr_t)(elem_bytes - 1)) || !lse || !grads || !out || !prefix)
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0 || STU == 0) return RNNT_STATUS_SUCCESS;
+    TdtBwd c = {};
+    c.x = logits; c.multiblank = true; c.lse_mb = lse; c.pg = grads; c.labels = labels; c.grad_out = grad_out;
+    c.yn = yn; c.mem_pref = prefix; c.lab_pref = prefix + N; c.STU = STU;
+    c.out = out; c.N = N; c.V = V; c.D = num_big_blanks; c.blank = blank; c.io_bf16 = elem_bytes == 2;
+    RNNT_TRY(launch_tdt_backward((cudaStream_t)stream, c), RNNT_STATUS_GRADS_BLANK_FAILED);
     return RNNT_STATUS_SUCCESS;
 }
 

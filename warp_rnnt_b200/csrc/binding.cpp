@@ -647,6 +647,122 @@ at::Tensor rnnt_tdt_compact_backward(const at::Tensor &xs, const at::Tensor &lse
     return out;
 }
 
+// Multi-blank: B = big_blank_durations.size() big blanks in the row of V, the standard blank in [B, V)
+void check_multiblank(int64_t B, int blank, int64_t V) {
+    TORCH_CHECK(B >= 1 && V > B, "xs must have more than len(big_blank_durations) logits per cell");
+    TORCH_CHECK(blank >= B && blank < V, "blank must be in [len(big_blank_durations), V)");
+}
+
+// Multi-blank transducer loss from (N,T,U,V) logits, float32 or bfloat16, B = durations.size(): (costs (N),
+// lse (N,T,U), grads (N,T,U,2+B) or empty), all float32.  No host sync.
+std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_multiblank_forward(const at::Tensor &xs, const at::Tensor &ys,
+                                                                       const at::Tensor &xn, const at::Tensor &yn,
+                                                                       const std::vector<int> &durations,
+                                                                       double sigma, int blank, bool want_grads) {
+    check4(xs, ys, xn, yn, true);
+    check_batch4(xs, xn, yn);
+    const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), V = xs.size(3), B = (int64_t)durations.size();
+    check_arg(ys, Dt::I32, xs, {N, U - 1}, "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
+    check_multiblank(B, blank, V);
+    const c10::cuda::CUDAGuard guard(xs.device());
+    const auto f32 = xs.options().dtype(at::kFloat);
+    at::Tensor costs = at::empty({N}, f32);
+    at::Tensor lse = at::empty({N, T, U}, f32);
+    at::Tensor pg = output(want_grads, {N, T, U, 2 + B}, f32);
+    if (N == 0) return std::make_tuple(costs, lse, pg);
+    at::Tensor ws = workspace(xs, rnnt_b200_multiblank_workspace_bytes((int)N, (int)T, (int)U, (int)B));
+    check_status(rnnt_b200_multiblank_forward(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
+                                              ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
+                                              durations.data(), (int)B, (float)sigma, costs.data_ptr<float>(),
+                                              lse.data_ptr<float>(), want_grads ? pg.data_ptr<float>() : nullptr,
+                                              (int)N, (int)T, (int)U, (int)V, blank,
+                                              xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
+    return std::make_tuple(costs, lse, pg);
+}
+
+// d loss / d multi-blank logits (N,T,U,V), of the dtype of xs
+at::Tensor rnnt_multiblank_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &grads,
+                                    const at::Tensor &ys, const std::vector<int> &durations,
+                                    const at::Tensor &grad_out, int blank) {
+    check_arg(xs, Dt::F32orBF16, xs, {kAny, kAny, kAny, kAny},
+              "xs must be a contiguous CUDA Float tensor of shape (N, T, U, V)");
+    const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), V = xs.size(3), B = (int64_t)durations.size();
+    check_multiblank(B, blank, V);
+    check_arg(lse, Dt::F32, xs, {N, T, U}, "lse must be a contiguous Float tensor of shape (N, T, U) on the device of xs");
+    check_arg(grads, Dt::F32, xs, {N, T, U, 2 + B},
+              "grads must be a contiguous Float tensor of shape (N, T, U, 2+B) on the device of xs");
+    check_arg(ys, Dt::I32, xs, {N, U - 1}, "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
+    check_arg(grad_out, Dt::F32, xs, N, "grad_out must be a contiguous Float tensor of shape (N,)");
+    const c10::cuda::CUDAGuard guard(xs.device());
+    at::Tensor out = at::empty_like(xs);
+    if (N == 0) return out;
+    check_status(rnnt_b200_multiblank_backward(current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(),
+                                               grads.data_ptr<float>(), ys.data_ptr<int>(), durations.data(), (int)B,
+                                               grad_out.data_ptr<float>(), out.data_ptr(), (int)N, (int)T, (int)U,
+                                               (int)V, blank, xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
+    return out;
+}
+
+// Multi-blank loss from compact (STU,V) logits in joint_pack's row order, float32 or bfloat16, labels (sum yn):
+// (costs (N), lse (STU), grads (STU,2+B) or empty, prefix (2N) int64 for the backward).  Shapes are validated as in
+// rnnt_tdt_compact_forward: one 16-byte device->host copy, or none with hints (max_T, max_U > 0).
+std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor>
+rnnt_multiblank_compact_forward(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn,
+                                const at::Tensor &yn, const std::vector<int> &durations, double sigma, int blank,
+                                bool want_grads, int max_T, int max_U) {
+    const auto [N, STU, V, bf16, guard] = compact_front(xs, ys, xn, yn, blank, true);
+    const int64_t B = (int64_t)durations.size();
+    check_multiblank(B, blank, V);
+    void *stream = current_stream(xs);
+    const auto f32 = xs.options().dtype(at::kFloat);
+    at::Tensor costs = at::empty({N}, f32);
+    at::Tensor lse = at::empty({STU}, f32);
+    at::Tensor pg = output(want_grads, {STU, 2 + B}, f32);
+    at::Tensor prefix = at::empty({2 * N}, xs.options().dtype(at::kLong));
+    if (N == 0) return std::make_tuple(costs, lse, pg, prefix);
+    std::tie(max_T, max_U) = compact_bounds(stream, xs, ys, xn, yn, max_T, max_U, prefix.data_ptr<int64_t>());
+    // a batch whose lengths are all 0: bounds of 1 (its lattices are invalid either way)
+    max_T = std::max(max_T, 1);
+    max_U = std::max(max_U, 1);
+    at::Tensor ws = workspace(xs, rnnt_b200_multiblank_compact_workspace_bytes(STU, (int)N, (int)B));
+    check_status(rnnt_b200_multiblank_compact_forward(stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
+                                                      ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
+                                                      durations.data(), (int)B, (float)sigma, costs.data_ptr<float>(),
+                                                      lse.data_ptr<float>(),
+                                                      want_grads ? pg.data_ptr<float>() : nullptr,
+                                                      prefix.data_ptr<int64_t>(), nullptr, STU, (int)N, (int)V, blank,
+                                                      bf16 ? 2 : 4, max_T, max_U));
+    return std::make_tuple(costs, lse, pg, prefix);
+}
+
+// d loss / d compact multi-blank logits (STU,V), of the dtype of xs
+at::Tensor rnnt_multiblank_compact_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &grads,
+                                            const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
+                                            const at::Tensor &prefix, const std::vector<int> &durations,
+                                            const at::Tensor &grad_out, int blank) {
+    check_arg(xs, Dt::F32orBF16, xs, {kAny, kAny}, "xs must be a contiguous CUDA Float tensor of shape (STU, V)");
+    const int64_t STU = xs.size(0), V = xs.size(1), N = xn.numel(), B = (int64_t)durations.size();
+    check_multiblank(B, blank, V);
+    check_arg(lse, Dt::F32, xs, {STU}, "lse must be a contiguous Float tensor of shape (STU,) on the device of xs");
+    check_arg(grads, Dt::F32, xs, {STU, 2 + B},
+              "grads must be a contiguous Float tensor of shape (STU, 2+B) on the device of xs");
+    TORCH_CHECK(is_arg(ys, Dt::I32, xs), "ys must be a contiguous Int tensor on the device of xs");
+    const char *lengths = "xn and yn must be contiguous Int tensors of shape (N,) on the device of xs";
+    check_arg(xn, Dt::I32, xs, N, lengths);
+    check_arg(yn, Dt::I32, xs, N, lengths);
+    check_arg(prefix, Dt::I64, xs, 2 * N, "prefix must be a contiguous Long tensor of shape (2N,) on the device of xs");
+    check_arg(grad_out, Dt::F32, xs, N, "grad_out must be a contiguous Float tensor of shape (N,)");
+    const c10::cuda::CUDAGuard guard(xs.device());
+    at::Tensor out = at::empty_like(xs);
+    if (N == 0 || STU == 0) return out;                 // empty tensors: nothing to write (and no data pointers)
+    check_status(rnnt_b200_multiblank_compact_backward(current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(),
+                                                       grads.data_ptr<float>(), ys.data_ptr<int>(), yn.data_ptr<int>(),
+                                                       durations.data(), (int)B, prefix.data_ptr<int64_t>(),
+                                                       grad_out.data_ptr<float>(), out.data_ptr(), STU, (int)N, (int)V,
+                                                       blank, xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
+    return out;
+}
+
 // An (n,) int32 output of the TDT alignment: a view of at least one element, so that the C ABI, which refuses NULL
 // outputs, gets a pointer also when there are no label slots (U = 1, or no labels in the batch)
 at::Tensor label_slots(int64_t n, const at::Tensor &like) {
@@ -981,6 +1097,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("rnnt_tdt_compact_backward", &rnnt_tdt_compact_backward, py::arg("xs"), py::arg("lse"), py::arg("grads"),
           py::arg("ys"), py::arg("xn"), py::arg("yn"), py::arg("prefix"), py::arg("durations"), py::arg("grad_out"),
           py::arg("blank"));
+    m.def("rnnt_multiblank_forward", &rnnt_multiblank_forward, py::arg("xs"), py::arg("ys"), py::arg("xn"),
+          py::arg("yn"), py::arg("big_blank_durations"), py::arg("sigma"), py::arg("blank"), py::arg("want_grads") = true);
+    m.def("rnnt_multiblank_backward", &rnnt_multiblank_backward, py::arg("xs"), py::arg("lse"), py::arg("grads"),
+          py::arg("ys"), py::arg("big_blank_durations"), py::arg("grad_out"), py::arg("blank"));
+    m.def("rnnt_multiblank_compact_forward", &rnnt_multiblank_compact_forward, py::arg("xs"), py::arg("ys"),
+          py::arg("xn"), py::arg("yn"), py::arg("big_blank_durations"), py::arg("sigma"), py::arg("blank"),
+          py::arg("want_grads"), py::arg("max_T") = 0, py::arg("max_U") = 0);
+    m.def("rnnt_multiblank_compact_backward", &rnnt_multiblank_compact_backward, py::arg("xs"), py::arg("lse"),
+          py::arg("grads"), py::arg("ys"), py::arg("xn"), py::arg("yn"), py::arg("prefix"),
+          py::arg("big_blank_durations"), py::arg("grad_out"), py::arg("blank"));
     m.def("rnnt_tdt_align_dense", &rnnt_tdt_align_dense, "Viterbi forced alignment on the TDT lattice, dense layout.",
           py::arg("xs"), py::arg("ys"), py::arg("xn"), py::arg("yn"), py::arg("durations"), py::arg("sigma") = 0.0,
           py::arg("blank") = 0);

@@ -182,7 +182,8 @@ struct FusedCall {
 };
 cudaError_t launch_fused(cudaStream_t s, const FusedPlan &plan, const FusedCall &c);
 
-// tdt.cu -- the Token-and-Duration Transducer loss from (N,T,U,V+D) joint logits (include/rnnt_b200.h)
+// tdt.cu -- the Token-and-Duration Transducer loss from (N,T,U,V+D) joint logits, and on the same kernels the
+// multi-blank transducer loss from (N,T,U,V) logits (include/rnnt_b200.h)
 constexpr int kTdtMaxD = 17;              // durations are distinct values in [0, 16]
 struct TdtDurations { int d[kTdtMaxD]; int D, dmax; };
 // the launch shape the planner picks (recorded by rnnt_b200_debug_last_tdt_launch)
@@ -192,7 +193,8 @@ struct TdtPlan {
     int warps, passes;                    // recurrence: warps per CTA, column passes per diagonal
     int ring, smem;                       // ring slots in shared memory (0: read back from global), its bytes
 };
-TdtPlan tdt_plan(int U, const TdtDurations &dur, const void *x, int elem_bytes, int V);
+// multiblank: dur holds the big blanks' durations and V is the whole row
+TdtPlan tdt_plan(int U, const TdtDurations &dur, const void *x, int elem_bytes, int V, bool multiblank = false);
 // The compact layout of a TDT call (joint_pack's row order): lattice n is a Tn x Un slab at row mem_pref[n] with row
 // stride Un = yn[n] + 1, its labels start at lab_pref[n]; a lattice is ok when Tn <= max_T, Un <= max_U and its rows lie
 // inside [0, STU).  The backward takes max_T = max_U = 0 (it does not check lattices: the posteriors tell).
@@ -202,7 +204,9 @@ struct TdtCompact {
     int N, max_T, max_U;
 };
 // Every field below that names a (N,T,U,...) shape is (STU,...) in the compact layout (mem_pref set), where T and U are
-// the bounds max_T, max_U and labels is (sum yn).
+// the bounds max_T, max_U and labels is (sum yn).  multiblank: the multi-blank lattice, with dur the big blanks'
+// durations (D = B), V the whole row (blank in [B, V)), lse_mb (N,T,U) out in place of lse, and pg (N,T,U,2+B) =
+// (P_std, Pl, P_big[0..B)).
 struct TdtFwd {
     const void *x;                        // logits (N,T,U,V+D), f32 or bf16
     const int *labels, *xn, *yn;
@@ -217,6 +221,8 @@ struct TdtFwd {
     float sigma;
     TdtDurations dur;
     int io_bf16;
+    bool multiblank;
+    float *lse_mb;                        // multiblank: (N,T,U) lse out
 };
 cudaError_t launch_tdt_forward(cudaStream_t s, const TdtFwd &c);
 struct TdtBwd {
@@ -231,6 +237,8 @@ struct TdtBwd {
     void *out;                            // (N,T,U,V+D), of the logits' type
     int N, T, U, V, D, blank;
     int io_bf16;
+    bool multiblank;                      // as in TdtFwd: V the whole row, D = B
+    const float *lse_mb;                  // multiblank: (N,T,U) lse of the forward
 };
 cudaError_t launch_tdt_backward(cudaStream_t s, const TdtBwd &c);
 // The Viterbi alignment on the TDT lattice (rnnt_b200_tdt_align_*): c as for the forward, with costs = the scores

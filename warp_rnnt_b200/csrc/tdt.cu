@@ -31,6 +31,14 @@
 // (n, t, u) mapping differs, so a compact row is computed exactly as the same row of a padded tensor.  The normaliser
 // runs one lattice per blockIdx.y (as logits.cu's compact rows); the posterior pass and the emit stay flat over the rows
 // and find a row's lattice by a binary search of mem_pref (tdt_find).
+//
+// Multi-blank transducer (Xu et al. 2022, arXiv:2211.03541; rnnt_b200_multiblank_*): the same four stages on the same
+// bodies, under the template flag MB, with B big blanks of durations d[0..B) in the durations' place (D = B).  The row
+// is V logits with one normaliser (W = V), lse is (cells) floats and lp, the posteriors (cells, 2 + B) = (standard
+// blank, label, big blank [0..B)), big blank i at column blank - 1 - i.  The edges out of (t, u): the standard blank to
+// (t + 1, u), the label to (t, u + 1) and big blank i to (t + d[i], u), so alpha's sources lie on diagonals s - 1 and
+// s - d[i] and the ring keeps max(d) + 1 diagonals.  Kernels k_mb_norm, k_mb_recur, k_mb_post, k_mb_emit (and their
+// _compact twins); every TDT instantiation is the code it was.
 #include "common.cuh"
 #include "kernels.cuh"
 
@@ -89,12 +97,13 @@ __device__ __forceinline__ float online_lse(float m, float s) { return m == -INF
 // Rows outside the live lattice (padding, or a lattice with invalid lengths) are not read: lse (0, 0), lp untouched.
 // COMPACT: CTA row blockIdx.y streams over the Tn * Un rows of lattice n, the pointers rebased to its first row; the rows
 // of a lattice that is not ok are not read and lse / lp are not written there (the posteriors of those rows are 0).
-template <typename IN, int SUB, int G, bool COMPACT>
+// MB (LSE = float): one accumulator over the whole row of V; lp = (blank, label, big blanks) each minus sigma.
+template <typename IN, int SUB, int G, bool COMPACT, bool MB = false, typename LSE = float2>
 __device__ __forceinline__ void
 tdt_norm_rows(const IN *__restrict__ x, const int *__restrict__ labels, const int *__restrict__ xn,
               const int *__restrict__ yn, int64_t cells, int T, int U, int V, int D, int blank, float sigma,
-              FastDiv divU, FastDiv divTU, float2 *__restrict__ lse, float *__restrict__ lp, const TdtCompact &cp) {
-    const int W = V + D, W2 = 2 + D;
+              FastDiv divU, FastDiv divTU, LSE *__restrict__ lse, float *__restrict__ lp, const TdtCompact &cp) {
+    const int W = MB ? V : V + D, W2 = 2 + D;
     Lattice L;
     if constexpr (COMPACT) {
         L = tdt_lattice(xn, yn, cp, blockIdx.y);
@@ -127,25 +136,44 @@ tdt_norm_rows(const IN *__restrict__ x, const int *__restrict__ labels, const in
                 ld_logits<G>(row + q * G, v);
 #pragma unroll
                 for (int k = 0; k < G; ++k) {
-                    if (q * G + k < V) online_add(mt, st, v[k]);
+                    if (MB || q * G + k < V) online_add(mt, st, v[k]);
                     else online_add(md, sd, v[k]);
                 }
             }
         }
+        if constexpr (MB) {
 #pragma unroll
-        for (int o = SUB / 2; o > 0; o >>= 1) {
-            const float mt2 = __shfl_xor_sync(0xffffffffu, mt, o), st2 = __shfl_xor_sync(0xffffffffu, st, o);
-            const float md2 = __shfl_xor_sync(0xffffffffu, md, o), sd2 = __shfl_xor_sync(0xffffffffu, sd, o);
-            online_merge(mt, st, mt2, st2);
-            online_merge(md, sd, md2, sd2);
+            for (int o = SUB / 2; o > 0; o >>= 1) {
+                const float mt2 = __shfl_xor_sync(0xffffffffu, mt, o), st2 = __shfl_xor_sync(0xffffffffu, st, o);
+                online_merge(mt, st, mt2, st2);
+            }
+            if (sub != 0) continue;
+            if (!live) {
+                lse[cell] = 0.0f;
+                continue;
+            }
+        } else {
+#pragma unroll
+            for (int o = SUB / 2; o > 0; o >>= 1) {
+                const float mt2 = __shfl_xor_sync(0xffffffffu, mt, o), st2 = __shfl_xor_sync(0xffffffffu, st, o);
+                const float md2 = __shfl_xor_sync(0xffffffffu, md, o), sd2 = __shfl_xor_sync(0xffffffffu, sd, o);
+                online_merge(mt, st, mt2, st2);
+                online_merge(md, sd, md2, sd2);
+            }
+            if (sub != 0) continue;
+            if (!live) {
+                lse[cell] = make_float2(0.0f, 0.0f);
+                continue;
+            }
         }
-        if (sub != 0) continue;
-        if (!live) {
-            lse[cell] = make_float2(0.0f, 0.0f);
-            continue;
+        const float lt = online_lse(mt, st);
+        float ld = 0.0f;
+        if constexpr (MB) {
+            lse[cell] = lt;
+        } else {
+            ld = online_lse(md, sd);
+            lse[cell] = make_float2(lt, ld);
         }
-        const float lt = online_lse(mt, st), ld = online_lse(md, sd);
-        lse[cell] = make_float2(lt, ld);
         float *o = lp + cell * W2;
         o[0] = clamp_big((io_load(row + blank) - lt) - sigma);
         float l = kBig;                                         // the last column has no label edge
@@ -154,7 +182,11 @@ tdt_norm_rows(const IN *__restrict__ x, const int *__restrict__ labels, const in
             l = (lab >= 0 && lab < V) ? clamp_big((io_load(row + lab) - lt) - sigma) : NAN;   // bad label: k_tdt_recur
         }
         o[1] = l;
-        for (int j = 0; j < D; ++j) o[2 + j] = clamp_big(io_load(row + V + j) - ld);
+        if constexpr (MB) {
+            for (int j = 0; j < D; ++j) o[2 + j] = clamp_big((io_load(row + blank - 1 - j) - lt) - sigma);
+        } else {
+            for (int j = 0; j < D; ++j) o[2 + j] = clamp_big(io_load(row + V + j) - ld);
+        }
     }
 }
 
@@ -177,13 +209,31 @@ k_tdt_norm_compact(const IN *__restrict__ x, const int *__restrict__ labels, con
                                     FastDiv(), lse, lp, cp);
 }
 
+// The multi-blank normaliser: lse (N,T,U), lp (N,T,U,2+B); D = B
+template <typename IN, int SUB, int G>
+__global__ void __launch_bounds__(kTdtRowThreads)
+k_mb_norm(const IN *__restrict__ x, const int *__restrict__ labels, const int *__restrict__ xn,
+          const int *__restrict__ yn, int64_t cells, int T, int U, int V, int D, int blank, float sigma, FastDiv divU,
+          FastDiv divTU, float *__restrict__ lse, float *__restrict__ lp) {
+    tdt_norm_rows<IN, SUB, G, false, true>(x, labels, xn, yn, cells, T, U, V, D, blank, sigma, divU, divTU, lse, lp,
+                                           TdtCompact{});
+}
+template <typename IN, int SUB, int G>
+__global__ void __launch_bounds__(kTdtRowThreads)
+k_mb_norm_compact(const IN *__restrict__ x, const int *__restrict__ labels, const int *__restrict__ xn,
+                  const int *__restrict__ yn, int V, int D, int blank, float sigma, float *__restrict__ lse,
+                  float *__restrict__ lp, TdtCompact cp) {
+    tdt_norm_rows<IN, SUB, G, true, true>(x, labels, xn, yn, cp.STU, cp.max_T, cp.max_U, V, D, blank, sigma,
+                                          FastDiv(), FastDiv(), lse, lp, cp);
+}
+
 struct TdtRec {
     const float *lp;
     const int *labels, *xn, *yn;
     float *alpha, *beta, *ll, *costs;
     int *status;
     int T, U, V, D;
-    int ring;                 // ring slots in shared memory (max(d) + 2), or 0: read back from alpha / beta
+    int ring;                 // ring slots in shared memory (max(d) + 2, MB max(d) + 1), or 0: read back from alpha / beta
     TdtDurations dur;
 };
 
@@ -260,7 +310,8 @@ __device__ __forceinline__ void tdt_backtrace(const TdtRec &a, const TdtAlignOut
 // ALIGN (k_tdt_align, grid (N, 1)): the alpha side only, with max_cands in place of lse_cands and a decision byte per
 // cell; it also checks every live cell's own lp row for NaN, as the beta side does.  After the sweep, the class and
 // the score (a.costs) of the lattice, then the backtrace (tdt_backtrace).
-template <int KD, bool COMPACT, bool ALIGN = false>
+// MB (k_mb_recur): the multi-blank edges; KD >= 2 + B is the candidate array's size (standard blank, label, big blanks).
+template <int KD, bool COMPACT, bool ALIGN = false, bool MB = false>
 __device__ __forceinline__ void tdt_recur(const TdtRec &a, const TdtCompact &cp,
                                           const TdtAlignOut &o = TdtAlignOut{}) {
     extern __shared__ float ring[];
@@ -308,9 +359,47 @@ __device__ __forceinline__ void tdt_recur(const TdtRec &a, const TdtCompact &cp,
         auto fwd = [&](int k) { const int q = slot + k; return q >= R ? q - R : q; };
         for (int u = max(0, s - Tn + 1) + (int)threadIdx.x; u <= min(s, Un - 1); u += blockDim.x) {
             const int t = s - u;
-            float c[2 * KD];
+            float c[MB ? KD : 2 * KD];
             float v;
-            if (!beta_side) {
+            if constexpr (MB) {
+                if (!beta_side) {
+                    // pull: standard blank from (t-1, u) and label from (t, u-1), both on diagonal s-1; big blank j
+                    // from (t-d[j], u) on s-d[j]; weights at the source cell
+                    c[0] = c[1] = -INFINITY;
+                    if (t > 0) c[0] = rd(t - 1, u, back(1)) + lp[((int64_t)(t - 1) * ld + u) * W2];
+                    if (u > 0) c[1] = rd(t, u - 1, back(1)) + lp[((int64_t)t * ld + u - 1) * W2 + 1];
+#pragma unroll
+                    for (int j = 0; j < KD - 2; ++j) {
+                        c[2 + j] = -INFINITY;
+                        if (j < D) {
+                            const int d = a.dur.d[j], tp = t - d;
+                            if (tp >= 0) c[2 + j] = rd(tp, u, back(d)) + lp[((int64_t)tp * ld + u) * W2 + 2 + j];
+                        }
+                    }
+                    v = (t == 0 && u == 0) ? 0.0f : lse_cands(c);
+                } else {
+                    // push: the cell's own weights, beta of the destinations; a blank that reaches t = Tn from the
+                    // last column is terminal (beta 0 after it)
+                    const float *r = lp + ((int64_t)t * ld + u) * W2;
+                    const float b = r[0], l = r[1];
+                    const bool has_label = u < Un - 1;
+                    saw_nan |= (b != b) || (has_label && l != l);
+                    c[0] = t + 1 < Tn ? b + rd(t + 1, u, fwd(1)) : has_label ? -INFINITY : b;
+                    c[1] = has_label ? l + rd(t, u + 1, fwd(1)) : -INFINITY;
+#pragma unroll
+                    for (int j = 0; j < KD - 2; ++j) {
+                        c[2 + j] = -INFINITY;
+                        if (j < D) {
+                            const int d = a.dur.d[j], tq = t + d;
+                            const float lb = r[2 + j];
+                            saw_nan |= lb != lb;
+                            if (tq < Tn) c[2 + j] = lb + rd(tq, u, fwd(d));
+                            else if (tq == Tn && !has_label) c[2 + j] = lb;
+                        }
+                    }
+                    v = lse_cands(c);
+                }
+            } else if (!beta_side) {
                 // pull: blank from (t-d, u) for d > 0, label from (t-d, u-1) for every d; weights at the source cell
 #pragma unroll
                 for (int j = 0; j < KD; ++j) {
@@ -414,6 +503,17 @@ __global__ void __launch_bounds__(kTdtMaxThreads) k_tdt_recur(TdtRec a) {
     tdt_recur<KD, false>(a, TdtCompact{});
 }
 
+// The multi-blank alpha / beta, grid (N, 2): a.D = B, a.dur the big blanks' durations.  One CTA per SM is all the
+// bound promises: without it ptxas holds the compact KD = 17 body to 40 registers and spills.
+template <int KD>
+__global__ void __launch_bounds__(kTdtMaxThreads, 1) k_mb_recur(TdtRec a) {
+    tdt_recur<KD, false, false, true>(a, TdtCompact{});
+}
+template <int KD>
+__global__ void __launch_bounds__(kTdtMaxThreads, 1) k_mb_recur_compact(TdtRec a, TdtCompact cp) {
+    tdt_recur<KD, true, false, true>(a, cp);
+}
+
 // The Viterbi alignment, one CTA per lattice (grid (N, 1)): a.costs = the scores; a.beta, a.ll unused
 template <int KD>
 __global__ void __launch_bounds__(kTdtMaxThreads) k_tdt_align(TdtRec a, TdtAlignOut o) {
@@ -432,8 +532,9 @@ __global__ void __launch_bounds__(kTdtMaxThreads) k_tdt_recur_compact(TdtRec a, 
 
 // Edge posteriors per cell: (Pb, Pl, Pd[0..D)), one thread per cell.  0 on padding and on lattices with invalid input
 // or no path; NaN on the live cells of a lattice with a NaN (or +inf, or all -inf) live row.  COMPACT: cells = STU, and
-// a row that lies in no lattice, or in one that is not ok, is a padding row.
-template <int KD, bool COMPACT>
+// a row that lies in no lattice, or in one that is not ok, is a padding row.  MB: (P_std, Pl, P_big[0..B)), the
+// posterior of each of the cell's edges.
+template <int KD, bool COMPACT, bool MB = false>
 __device__ __forceinline__ void
 tdt_post_rows(const float *__restrict__ lp, const float *__restrict__ alpha, const float *__restrict__ beta,
               const float *__restrict__ ll, const int *__restrict__ status, const int *__restrict__ xn,
@@ -472,6 +573,25 @@ tdt_post_rows(const float *__restrict__ lp, const float *__restrict__ alpha, con
         const float *r = lp + cell * W2;
         const float al = alpha[cell], lP = ll[n], b = r[0], l = r[1];
         const bool has_label = (int)u < Un - 1;
+        if constexpr (MB) {
+            float ps = 0.0f, pl = 0.0f;
+            if ((int)t + 1 < Tn) ps = expf(((al + b) + beta[cell + rs]) - lP);
+            else if (!has_label) ps = expf((al + b) - lP);
+            if (has_label) pl = expf(((al + l) + beta[cell + 1]) - lP);
+            g[0] = ps;
+            g[1] = pl;
+#pragma unroll
+            for (int j = 0; j < KD - 2; ++j) {
+                if (j < D) {
+                    const int d = dur.d[j], tq = (int)t + d;
+                    float pj = 0.0f;
+                    if (tq < Tn) pj = expf(((al + r[2 + j]) + beta[cell + (int64_t)d * rs]) - lP);
+                    else if (tq == Tn && !has_label) pj = expf((al + r[2 + j]) - lP);
+                    g[2 + j] = pj;
+                }
+            }
+            continue;
+        }
         float pb = 0.0f, pl = 0.0f;
 #pragma unroll
         for (int j = 0; j < KD; ++j) {
@@ -505,6 +625,24 @@ k_tdt_post(const float *__restrict__ lp, const float *__restrict__ alpha, const 
 
 template <int KD>
 __global__ void __launch_bounds__(kTdtRowThreads)
+k_mb_post(const float *__restrict__ lp, const float *__restrict__ alpha, const float *__restrict__ beta,
+          const float *__restrict__ ll, const int *__restrict__ status, const int *__restrict__ xn,
+          const int *__restrict__ yn, int64_t cells, int T, int U, int D, TdtDurations dur, FastDiv divU,
+          FastDiv divTU, float *__restrict__ pg) {
+    tdt_post_rows<KD, false, true>(lp, alpha, beta, ll, status, xn, yn, cells, U, D, dur, divU, divTU, pg,
+                                   TdtCompact{});
+}
+template <int KD>
+__global__ void __launch_bounds__(kTdtRowThreads)
+k_mb_post_compact(const float *__restrict__ lp, const float *__restrict__ alpha, const float *__restrict__ beta,
+                  const float *__restrict__ ll, const int *__restrict__ status, const int *__restrict__ xn,
+                  const int *__restrict__ yn, int D, TdtDurations dur, float *__restrict__ pg, TdtCompact cp) {
+    tdt_post_rows<KD, true, true>(lp, alpha, beta, ll, status, xn, yn, cp.STU, cp.max_U, D, dur, FastDiv(), FastDiv(),
+                                  pg, cp);
+}
+
+template <int KD>
+__global__ void __launch_bounds__(kTdtRowThreads)
 k_tdt_post_compact(const float *__restrict__ lp, const float *__restrict__ alpha, const float *__restrict__ beta,
                    const float *__restrict__ ll, const int *__restrict__ status, const int *__restrict__ xn,
                    const int *__restrict__ yn, int D, TdtDurations dur, float *__restrict__ pg, TdtCompact cp) {
@@ -514,29 +652,41 @@ k_tdt_post_compact(const float *__restrict__ lp, const float *__restrict__ alpha
 
 // The row data one gradient element needs.  zero: the row's posteriors are all 0 (padding, no path, or a cell no path
 // visits): the row is written as exact zeros and neither the logits nor lse are read.  COMPACT: a row with posteriors
-// lies in an ok lattice, found by tdt_find (U, divU and divTU are not used).
+// lies in an ok lattice, found by tdt_find (U, divU and divTU are not used).  MB (LSE = float): occ is the sum of all
+// 2 + B posteriors and zero says it is 0 (each is >= 0 or NaN); ld is not used.
 struct TdtRow {
     const float *pd;
     float occ, pb, pl, lt, ld, sc;
     int lab;
     bool zero;
 };
-template <bool COMPACT>
-__device__ __forceinline__ TdtRow tdt_row(int64_t row, const float2 *lse, const float *pg, const int *labels,
+template <bool COMPACT, bool MB = false, typename LSE = float2>
+__device__ __forceinline__ TdtRow tdt_row(int64_t row, const LSE *lse, const float *pg, const int *labels,
                                           const float *grad_out, int U, int W2, const FastDiv &divU,
                                           const FastDiv &divTU, const TdtCompact &cp, const int *yn) {
     TdtRow r;
     r.pd = pg + row * W2;
     r.pb = r.pd[0];
     r.pl = r.pd[1];
-    r.zero = r.pb == 0.0f && r.pl == 0.0f;
-    r.occ = r.pb + r.pl;
+    if constexpr (MB) {
+        float occ = r.pb + r.pl;
+        for (int k = 2; k < W2; ++k) occ += r.pd[k];
+        r.occ = occ;
+        r.zero = occ == 0.0f;
+    } else {
+        r.zero = r.pb == 0.0f && r.pl == 0.0f;
+        r.occ = r.pb + r.pl;
+    }
     r.lt = r.ld = r.sc = 0.0f;
     r.lab = -1;
     if (!r.zero) {
-        const float2 q = lse[row];
-        r.lt = q.x;
-        r.ld = q.y;
+        if constexpr (MB) {
+            r.lt = lse[row];
+        } else {
+            const float2 q = lse[row];
+            r.lt = q.x;
+            r.ld = q.y;
+        }
         if constexpr (COMPACT) {
             const int n = tdt_find(cp.mem_pref, cp.N, row);
             const int Un = yn[n] + 1, u = (int)((uint32_t)(row - cp.mem_pref[n]) % (uint32_t)Un);
@@ -561,25 +711,40 @@ __device__ __forceinline__ float tdt_elem(const TdtRow &r, int v, float xv, int 
     }
     return (r.occ * expf(xv - r.ld) - r.pd[2 + (v - V)]) * r.sc;
 }
+// the multi-blank gradient element of column v < V; big blank j = blank - 1 - v when 0 <= j < B
+__device__ __forceinline__ float mb_elem(const TdtRow &r, int v, float xv, int B, int blank) {
+    if (r.zero) return 0.0f;
+    float sel = (v == blank) ? r.pb : 0.0f;
+    const int j = blank - 1 - v;
+    if (j >= 0 && j < B) sel += r.pd[2 + j];
+    if (v == r.lab) sel += r.pl;
+    return (r.occ * expf(xv - r.lt) - sel) * r.sc;
+}
 
 // Gradient emit: the flat (rows, W) output in vectors of VEC elements (16 bytes when `out` is 16-byte aligned, else 1),
 // which may straddle rows; XVEC: the logits are read with the same vectors (x aligned as out), else element by element.
 // Every element is computed the same way whatever VEC, XVEC, the element type and the layout; bf16 is rounded once on
 // the store.  COMPACT: the rows are the (STU, W) rows of the compact layout, vectors straddle lattices as they
-// straddle rows.
-template <typename IO, int VEC, bool XVEC, bool COMPACT>
+// straddle rows.  MB: rows of W = V (mb_elem), lse (rows) floats.
+template <typename IO, int VEC, bool XVEC, bool COMPACT, bool MB = false, typename LSE = float2>
 __device__ __forceinline__ void
-tdt_emit_flat(const IO *__restrict__ x, const float2 *__restrict__ lse, const float *__restrict__ pg,
+tdt_emit_flat(const IO *__restrict__ x, const LSE *__restrict__ lse, const float *__restrict__ pg,
               const int *__restrict__ labels, const float *__restrict__ grad_out, IO *__restrict__ out, int64_t total,
               int V, int D, int blank, int U, FastDiv divU, FastDiv divTU, int64_t stride_rows, int stride_v,
               const TdtCompact &cp, const int *__restrict__ yn) {
-    const int W = V + D, W2 = 2 + D;
+    const int W = MB ? V : V + D, W2 = 2 + D;
     int64_t f = ((int64_t)blockIdx.x * kTdtRowThreads + threadIdx.x) * VEC;
     if (f >= total) return;
     int64_t row = f / W;
     int v0 = (int)(f - row * W);
     const int64_t stride = stride_rows * W + stride_v;
-    auto row_at = [&](int64_t i) { return tdt_row<COMPACT>(i, lse, pg, labels, grad_out, U, W2, divU, divTU, cp, yn); };
+    auto row_at = [&](int64_t i) {
+        return tdt_row<COMPACT, MB>(i, lse, pg, labels, grad_out, U, W2, divU, divTU, cp, yn);
+    };
+    auto elem = [&](const TdtRow &r, int v, float xv) {
+        if constexpr (MB) return mb_elem(r, v, xv, D, blank);
+        else return tdt_elem(r, v, xv, V, blank);
+    };
     for (; f < total; f += stride, row += stride_rows, v0 += stride_v) {
         if (v0 >= W) { v0 -= W; ++row; }
         float e[VEC];
@@ -599,7 +764,7 @@ tdt_emit_flat(const IO *__restrict__ x, const float2 *__restrict__ lse, const fl
             for (int k = 0; k < VEC; ++k) {
                 if (v == W) { v = 0; ++rw; r = row_at(rw); }
                 if (!XVEC && !r.zero) xv[k] = io_load(x + f + k);
-                e[k] = tdt_elem(r, v, xv[k], V, blank);
+                e[k] = elem(r, v, xv[k]);
                 ++v;
             }
             if constexpr (VEC == 1) st_one(out + f, e[0]);
@@ -610,7 +775,7 @@ tdt_emit_flat(const IO *__restrict__ x, const float2 *__restrict__ lse, const fl
             int v = v0;
             for (int64_t i = f; i < total; ++i) {
                 if (v == W) { v = 0; ++rw; r = row_at(rw); }
-                st_one(out + i, tdt_elem(r, v, r.zero ? 0.0f : io_load(x + i), V, blank));
+                st_one(out + i, elem(r, v, r.zero ? 0.0f : io_load(x + i)));
                 ++v;
             }
         }
@@ -637,6 +802,24 @@ k_tdt_emit_compact(const IO *__restrict__ x, const float2 *__restrict__ lse, con
                                        stride_rows, stride_v, cp, yn);
 }
 
+template <typename IO, int VEC, bool XVEC>
+__global__ void __launch_bounds__(kTdtRowThreads)
+k_mb_emit(const IO *__restrict__ x, const float *__restrict__ lse, const float *__restrict__ pg,
+          const int *__restrict__ labels, const float *__restrict__ grad_out, IO *__restrict__ out, int64_t total,
+          int V, int D, int blank, int U, FastDiv divU, FastDiv divTU, int64_t stride_rows, int stride_v) {
+    tdt_emit_flat<IO, VEC, XVEC, false, true>(x, lse, pg, labels, grad_out, out, total, V, D, blank, U, divU, divTU,
+                                              stride_rows, stride_v, TdtCompact{}, nullptr);
+}
+template <typename IO, int VEC, bool XVEC>
+__global__ void __launch_bounds__(kTdtRowThreads)
+k_mb_emit_compact(const IO *__restrict__ x, const float *__restrict__ lse, const float *__restrict__ pg,
+                  const int *__restrict__ labels, const int *__restrict__ yn, const float *__restrict__ grad_out,
+                  IO *__restrict__ out, int64_t total, int V, int D, int blank, int64_t stride_rows, int stride_v,
+                  TdtCompact cp) {
+    tdt_emit_flat<IO, VEC, XVEC, true, true>(x, lse, pg, labels, grad_out, out, total, V, D, blank, 0, FastDiv(),
+                                             FastDiv(), stride_rows, stride_v, cp, yn);
+}
+
 // Process-wide, unlike the loss' per-thread record (api.cu): autograd runs the backward on its own device thread, and
 // the record must see the emit of the same call.
 static std::mutex g_tdt_mu;
@@ -657,16 +840,17 @@ void tdt_launch_record(int32_t *out) {
     memcpy(out, g_tdt_record, sizeof(g_tdt_record));
 }
 
-TdtPlan tdt_plan(int U, const TdtDurations &dur, const void *x, int elem_bytes, int V) {
+TdtPlan tdt_plan(int U, const TdtDurations &dur, const void *x, int elem_bytes, int V, bool multiblank) {
     TdtPlan p;
-    const int W = V + dur.D;
+    const int W = multiblank ? V : V + dur.D;
     const int eoff = (int)((reinterpret_cast<uintptr_t>(x) / (uintptr_t)elem_bytes) & 3u);   // element alignment
     p.norm_group = (W % 4 == 0 && eoff == 0) ? 4 : (W % 2 == 0 && (eoff & 1) == 0) ? 2 : 1;
     p.norm_lanes = W <= 64 ? 8 : 32;
-    p.kd = dur.D <= 5 ? 5 : kTdtMaxD;
+    // TDT: D candidate pairs; multi-blank: 2 + B candidates
+    p.kd = (multiblank ? 2 + dur.D : dur.D) <= 5 ? 5 : kTdtMaxD;
     p.warps = min((U + 31) / 32, kTdtMaxThreads / 32);
     p.passes = (U + p.warps * 32 - 1) / (p.warps * 32);
-    p.ring = dur.dmax + 2;
+    p.ring = dur.dmax + (multiblank ? 1 : 2);
     const int64_t smem = (int64_t)p.ring * U * (int64_t)sizeof(float);
     if (smem > max_optin_smem(current_device())) p.ring = 0;
     p.smem = p.ring ? (int)smem : 0;
@@ -676,7 +860,7 @@ TdtPlan tdt_plan(int U, const TdtDurations &dur, const void *x, int elem_bytes, 
 // the compact layout of a forward (c.mem_pref set)
 static TdtCompact tdt_compact(const TdtFwd &c) { return {c.mem_pref, c.lab_pref, c.STU, c.N, c.T, c.U}; }
 
-template <typename IN>
+template <bool MB, typename IN>
 static cudaError_t tdt_norm_as(cudaStream_t s, const TdtPlan &p, const IN *x, const TdtFwd &c, int64_t cells) {
     // the dense cell -> (n, t, u) divisions (the compact kernels find lattices through mem_pref instead)
     const FastDiv divU = c.mem_pref ? FastDiv() : FastDiv((uint32_t)c.U);
@@ -686,6 +870,16 @@ static cudaError_t tdt_norm_as(cudaStream_t s, const TdtPlan &p, const IN *x, co
     // compact: CTA rows per lattice as logits.cu's compact normaliser sizes them
     const dim3 cgrid(compact_gx(cells, c.N, per_block * kCompactIters), c.N);
 #define RNNT_TDT_NORM(SUB, G)                                                                                         \
+    if constexpr (MB) {                                                                                               \
+        if (c.mem_pref)                                                                                               \
+            k_mb_norm_compact<IN, SUB, G><<<cgrid, kTdtRowThreads, 0, s>>>(x, c.labels, c.xn, c.yn, c.V, c.dur.D,     \
+                                                                           c.blank, c.sigma, c.lse_mb, c.lp,          \
+                                                                           tdt_compact(c));                           \
+        else                                                                                                          \
+            k_mb_norm<IN, SUB, G><<<grid, kTdtRowThreads, 0, s>>>(x, c.labels, c.xn, c.yn, cells, c.T, c.U, c.V,      \
+                                                                  c.dur.D, c.blank, c.sigma, divU, divTU, c.lse_mb,   \
+                                                                  c.lp);                                              \
+    } else                                                                                                            \
     (c.mem_pref                                                                                                       \
          ? k_tdt_norm_compact<IN, SUB, G><<<cgrid, kTdtRowThreads, 0, s>>>(x, c.labels, c.xn, c.yn, c.V, c.dur.D,     \
                                                                            c.blank, c.sigma, c.lse, c.lp,             \
@@ -693,28 +887,30 @@ static cudaError_t tdt_norm_as(cudaStream_t s, const TdtPlan &p, const IN *x, co
          : k_tdt_norm<IN, SUB, G><<<grid, kTdtRowThreads, 0, s>>>(x, c.labels, c.xn, c.yn, cells, c.T, c.U, c.V,      \
                                                                   c.dur.D, c.blank, c.sigma, divU, divTU, c.lse, c.lp))
     if (p.norm_lanes == 8) {
-        if (p.norm_group == 4) RNNT_TDT_NORM(8, 4); else if (p.norm_group == 2) RNNT_TDT_NORM(8, 2); else RNNT_TDT_NORM(8, 1);
+        if (p.norm_group == 4) { RNNT_TDT_NORM(8, 4); } else if (p.norm_group == 2) { RNNT_TDT_NORM(8, 2); } else { RNNT_TDT_NORM(8, 1); }
     } else {
-        if (p.norm_group == 4) RNNT_TDT_NORM(32, 4); else if (p.norm_group == 2) RNNT_TDT_NORM(32, 2); else RNNT_TDT_NORM(32, 1);
+        if (p.norm_group == 4) { RNNT_TDT_NORM(32, 4); } else if (p.norm_group == 2) { RNNT_TDT_NORM(32, 2); } else { RNNT_TDT_NORM(32, 1); }
     }
 #undef RNNT_TDT_NORM
     count_launch();
     return cudaGetLastError();
 }
 
-template <int KD>
+template <int KD, bool MB>
 static cudaError_t tdt_recur_post(cudaStream_t s, const TdtPlan &p, const TdtFwd &c, int64_t cells) {
     static std::atomic<bool> smem_set[kMaxDevices], smem_set_compact[kMaxDevices];
+    const auto recur = MB ? k_mb_recur<KD> : k_tdt_recur<KD>;
+    const auto recur_compact = MB ? k_mb_recur_compact<KD> : k_tdt_recur_compact<KD>;
     if (p.smem > (48 << 10)) {
-        const cudaError_t e = c.mem_pref ? ensure_dyn_smem(k_tdt_recur_compact<KD>, smem_set_compact,
+        const cudaError_t e = c.mem_pref ? ensure_dyn_smem(recur_compact, smem_set_compact,
                                                            max_optin_smem(current_device()))
-                                         : ensure_dyn_smem(k_tdt_recur<KD>, smem_set, max_optin_smem(current_device()));
+                                         : ensure_dyn_smem(recur, smem_set, max_optin_smem(current_device()));
         if (e != cudaSuccess) return e;
     }
     TdtRec r = {c.lp, c.labels, c.xn, c.yn, c.alpha, c.beta, c.ll, c.costs, c.status, c.T, c.U, c.V, c.dur.D, p.ring,
                 c.dur};
-    if (c.mem_pref) k_tdt_recur_compact<KD><<<dim3(c.N, 2), p.warps * 32, p.smem, s>>>(r, tdt_compact(c));
-    else k_tdt_recur<KD><<<dim3(c.N, 2), p.warps * 32, p.smem, s>>>(r);
+    if (c.mem_pref) recur_compact<<<dim3(c.N, 2), p.warps * 32, p.smem, s>>>(r, tdt_compact(c));
+    else recur<<<dim3(c.N, 2), p.warps * 32, p.smem, s>>>(r);
     count_launch();
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess || !c.pg || cells == 0) return e;
@@ -723,19 +919,21 @@ static cudaError_t tdt_recur_post(cudaStream_t s, const TdtPlan &p, const TdtFwd
     const FastDiv divTU = c.mem_pref ? FastDiv() : FastDiv((uint32_t)(c.T * c.U));
     const unsigned grid = (unsigned)min((cells + kTdtRowThreads - 1) / kTdtRowThreads,
                                         (int64_t)sm_count(current_device()) * 16);
+    const auto post = MB ? k_mb_post<KD> : k_tdt_post<KD>;
+    const auto post_compact = MB ? k_mb_post_compact<KD> : k_tdt_post_compact<KD>;
     if (c.mem_pref)
-        k_tdt_post_compact<KD><<<grid, kTdtRowThreads, 0, s>>>(c.lp, c.alpha, c.beta, c.ll, c.status, c.xn, c.yn,
-                                                               c.dur.D, c.dur, c.pg, tdt_compact(c));
+        post_compact<<<grid, kTdtRowThreads, 0, s>>>(c.lp, c.alpha, c.beta, c.ll, c.status, c.xn, c.yn, c.dur.D, c.dur,
+                                                     c.pg, tdt_compact(c));
     else
-        k_tdt_post<KD><<<grid, kTdtRowThreads, 0, s>>>(c.lp, c.alpha, c.beta, c.ll, c.status, c.xn, c.yn, cells, c.T,
-                                                       c.U, c.dur.D, c.dur, divU, divTU, c.pg);
+        post<<<grid, kTdtRowThreads, 0, s>>>(c.lp, c.alpha, c.beta, c.ll, c.status, c.xn, c.yn, cells, c.T, c.U,
+                                             c.dur.D, c.dur, divU, divTU, c.pg);
     count_launch();
     return cudaGetLastError();
 }
 
 // The plan of a forward or alignment call, recorded for rnnt_b200_debug_last_tdt_launch (the emit fields 0)
 static TdtPlan tdt_plan_recorded(const TdtFwd &c) {
-    const TdtPlan p = tdt_plan(c.U, c.dur, c.x, c.io_bf16 ? 2 : 4, c.V);
+    const TdtPlan p = tdt_plan(c.U, c.dur, c.x, c.io_bf16 ? 2 : 4, c.V, c.multiblank);
     std::lock_guard<std::mutex> lock(g_tdt_mu);
     int32_t *rec = g_tdt_record;
     memset(rec, 0, sizeof(g_tdt_record));
@@ -755,10 +953,16 @@ cudaError_t launch_tdt_forward(cudaStream_t s, const TdtFwd &c) {
     const int64_t cells = c.mem_pref ? c.STU : (int64_t)c.N * c.T * c.U;
     const TdtPlan p = tdt_plan_recorded(c);
     if (cells == 0 && !c.mem_pref) return cudaSuccess;   // compact: with no rows the recurrence still gives the costs
-    cudaError_t e = c.io_bf16 ? tdt_norm_as(s, p, static_cast<const __nv_bfloat16 *>(c.x), c, cells)
-                              : tdt_norm_as(s, p, static_cast<const float *>(c.x), c, cells);
+    if (c.multiblank) {
+        const cudaError_t e = c.io_bf16 ? tdt_norm_as<true>(s, p, static_cast<const __nv_bfloat16 *>(c.x), c, cells)
+                                        : tdt_norm_as<true>(s, p, static_cast<const float *>(c.x), c, cells);
+        if (e != cudaSuccess) return e;
+        return p.kd == 5 ? tdt_recur_post<5, true>(s, p, c, cells) : tdt_recur_post<kTdtMaxD, true>(s, p, c, cells);
+    }
+    cudaError_t e = c.io_bf16 ? tdt_norm_as<false>(s, p, static_cast<const __nv_bfloat16 *>(c.x), c, cells)
+                              : tdt_norm_as<false>(s, p, static_cast<const float *>(c.x), c, cells);
     if (e != cudaSuccess) return e;
-    return p.kd == 5 ? tdt_recur_post<5>(s, p, c, cells) : tdt_recur_post<kTdtMaxD>(s, p, c, cells);
+    return p.kd == 5 ? tdt_recur_post<5, false>(s, p, c, cells) : tdt_recur_post<kTdtMaxD, false>(s, p, c, cells);
 }
 
 template <int KD>
@@ -781,16 +985,16 @@ static cudaError_t tdt_align_as(cudaStream_t s, const TdtPlan &p, const TdtFwd &
 cudaError_t launch_tdt_align(cudaStream_t s, const TdtFwd &c, uint8_t *dec, int *frames, int *fdur) {
     const int64_t cells = c.mem_pref ? c.STU : (int64_t)c.N * c.T * c.U;
     const TdtPlan p = tdt_plan_recorded(c);
-    cudaError_t e = c.io_bf16 ? tdt_norm_as(s, p, static_cast<const __nv_bfloat16 *>(c.x), c, cells)
-                              : tdt_norm_as(s, p, static_cast<const float *>(c.x), c, cells);
+    cudaError_t e = c.io_bf16 ? tdt_norm_as<false>(s, p, static_cast<const __nv_bfloat16 *>(c.x), c, cells)
+                              : tdt_norm_as<false>(s, p, static_cast<const float *>(c.x), c, cells);
     if (e != cudaSuccess) return e;
     const TdtAlignOut o = {dec, frames, fdur};
     return p.kd == 5 ? tdt_align_as<5>(s, p, c, o) : tdt_align_as<kTdtMaxD>(s, p, c, o);
 }
 
-template <typename IO>
+template <bool MB, typename IO>
 static cudaError_t tdt_emit_as(cudaStream_t s, const TdtBwd &c, const IO *x, IO *out) {
-    const int W = c.V + c.D;
+    const int W = MB ? c.V : c.V + c.D;
     const int64_t total = (c.mem_pref ? c.STU : (int64_t)c.N * c.T * c.U) * W;
     constexpr int kVec = 16 / (int)sizeof(IO);
     const bool ovec = (reinterpret_cast<uintptr_t>(out) & 15u) == 0;
@@ -813,24 +1017,39 @@ static cudaError_t tdt_emit_as(cudaStream_t s, const TdtBwd &c, const IO *x, IO 
     const int sv = (int)(stride - srows * W);
     const TdtCompact cp = {c.mem_pref, c.lab_pref, c.STU, c.N, 0, 0};
 #define RNNT_TDT_EMIT(VEC, XV)                                                                                        \
+    if constexpr (MB) {                                                                                               \
+        if (c.mem_pref)                                                                                               \
+            k_mb_emit_compact<IO, VEC, XV><<<grid, kTdtRowThreads, 0, s>>>(x, c.lse_mb, c.pg, c.labels, c.yn,         \
+                                                                           c.grad_out, out, total, c.V, c.D, c.blank, \
+                                                                           srows, sv, cp);                            \
+        else                                                                                                          \
+            k_mb_emit<IO, VEC, XV><<<grid, kTdtRowThreads, 0, s>>>(x, c.lse_mb, c.pg, c.labels, c.grad_out, out,      \
+                                                                   total, c.V, c.D, c.blank, c.U, divU, divTU, srows, \
+                                                                   sv);                                               \
+    } else                                                                                                            \
     (c.mem_pref                                                                                                       \
          ? k_tdt_emit_compact<IO, VEC, XV><<<grid, kTdtRowThreads, 0, s>>>(x, c.lse, c.pg, c.labels, c.yn, c.grad_out, \
                                                                            out, total, c.V, c.D, c.blank, srows, sv,  \
                                                                            cp)                                        \
          : k_tdt_emit<IO, VEC, XV><<<grid, kTdtRowThreads, 0, s>>>(x, c.lse, c.pg, c.labels, c.grad_out, out, total,  \
                                                                    c.V, c.D, c.blank, c.U, divU, divTU, srows, sv))
-    if (!ovec) RNNT_TDT_EMIT(1, false);
-    else if (xvec) RNNT_TDT_EMIT(kVec, true);
-    else RNNT_TDT_EMIT(kVec, false);
+    if (!ovec) { RNNT_TDT_EMIT(1, false); }
+    else if (xvec) { RNNT_TDT_EMIT(kVec, true); }
+    else { RNNT_TDT_EMIT(kVec, false); }
 #undef RNNT_TDT_EMIT
     count_launch();
     return cudaGetLastError();
 }
 
 cudaError_t launch_tdt_backward(cudaStream_t s, const TdtBwd &c) {
+    if (c.multiblank) {
+        if (c.io_bf16)
+            return tdt_emit_as<true>(s, c, static_cast<const __nv_bfloat16 *>(c.x), static_cast<__nv_bfloat16 *>(c.out));
+        return tdt_emit_as<true>(s, c, static_cast<const float *>(c.x), static_cast<float *>(c.out));
+    }
     if (c.io_bf16)
-        return tdt_emit_as(s, c, static_cast<const __nv_bfloat16 *>(c.x), static_cast<__nv_bfloat16 *>(c.out));
-    return tdt_emit_as(s, c, static_cast<const float *>(c.x), static_cast<float *>(c.out));
+        return tdt_emit_as<false>(s, c, static_cast<const __nv_bfloat16 *>(c.x), static_cast<__nv_bfloat16 *>(c.out));
+    return tdt_emit_as<false>(s, c, static_cast<const float *>(c.x), static_cast<float *>(c.out));
 }
 
 }  // namespace rnnt
