@@ -523,7 +523,8 @@ class RNNTLossMultiblankCompact(torch.autograd.Function):
 
 
 def _multiblank_args(fn, logits, big_blank_durations, sigma, blank, compact):
-    """The argument checks of ``rnnt_loss_multiblank``: the durations, sigma, the logits' shape and blank.  Returns
+    """The argument checks of ``rnnt_loss_multiblank`` and ``rnnt_align_multiblank`` (``fn`` names the caller in the
+    messages): the durations, sigma, the logits' shape and blank.  Returns
     (durations as a tuple, the standard blank's column)."""
     d = big_blank_durations
     if not isinstance(d, (list, tuple)) or not d or any(isinstance(x, bool) or not isinstance(x, int) for x in d):
@@ -592,7 +593,8 @@ def rnnt_loss_multiblank(logits, labels, frames_lengths, labels_lengths, big_bla
     posteriors and the gradient are bit for bit those of the same rows placed in a padded tensor at the same element
     offset modulo 4.
 
-    Not offered: ``fastemit_lambda``, ``rnnt_type``, ``delay_penalty`` and TDT's ``omega``."""
+    Not offered: ``fastemit_lambda``, ``rnnt_type``, ``delay_penalty`` and TDT's ``omega``.  The best path itself
+    (token frames and blank counts) is ``rnnt_align_multiblank``."""
     assert average_frames is None or isinstance(average_frames, bool)
     assert reduction is None or reduction in ("none", "mean", "sum")
     assert not labels.requires_grad and not frames_lengths.requires_grad and not labels_lengths.requires_grad
@@ -943,7 +945,57 @@ def rnnt_align_tdt(logits, labels, frames_lengths, labels_lengths, durations, si
                                        blank)
 
 
-__all__ = ["rnnt_loss", "rnnt_align", "rnnt_align_tdt", "rnnt_loss_from_logits", "rnnt_loss_pruned",
+def rnnt_align_multiblank(logits, labels, frames_lengths, labels_lengths, big_blank_durations, sigma=0.0, blank=None,
+                          compact=False):
+    """Viterbi forced alignment on the multi-blank transducer lattice of ``rnnt_loss_multiblank``: the single best
+    path, with the frame of each label and how often it takes each blank, for token timings and for how much a trained
+    model relies on its big blanks.
+
+    Inputs and argument checks are those of ``rnnt_loss_multiblank``: dense (N, T, U, V) logits, float32 or bfloat16,
+    with labels (N, U-1); or ``compact=True``: (STU, V) rows in ``joint_pack``'s order with labels
+    (sum(labels_lengths),), honouring ``compact_hints``.  big_blank_durations, sigma and blank as there (blank None:
+    V - 1; big blank i in column blank - 1 - i).  No autograd: the outputs are not differentiable and
+    ``logits.requires_grad`` is ignored.
+
+    The lattice, its edges and their weights are ``rnnt_loss_multiblank``'s with the same sigma, each weight
+    lp = log_softmax(row) - sigma clamped below at -1e30 (a masked -inf becomes that finite sentinel).  A path runs from
+    (0, 0) up to and including a terminal edge (the standard blank from (Tn-1, Un-1), or big blank i from
+    (Tn-d_i, Un-1)); its score is the float32 left fold ``acc = acc + lp`` over its edges in path order.  The max-plus
+    recurrence adds in that order and so gives the largest such score exactly (float32 rounding is monotone).  Ties:
+    only a strictly larger candidate replaces the one held, the candidates taken as the standard blank, then the big
+    blanks by increasing duration, then the label; so on equal values a blank beats a label and the shorter blank wins
+    (also for the terminal edge).  A NaN candidate is never taken.
+
+    Returns ``(scores, frames, blank_counts)``:
+      * ``scores`` (N,) float32: the best path's score.
+      * ``frames`` int32, dense (N, U-1), compact (sum(labels_lengths),) in the labels' order: frames[n, u] is the
+        frame t of the best path's label edge (t, u) -> (t, u+1); non-decreasing, in [0, Tn-1], and -1 for
+        u >= labels_lengths[n].
+      * ``blank_counts`` (N, 1 + B) int32 in both layouts: column 0 counts the best path's standard-blank edges
+        (the terminal edge included), column 1 + i its uses of big blank i; counts[0] + sum_i d_i counts[1+i] = Tn.
+      Both are -1 throughout on every lattice without an alignment.
+
+    Lattices without an alignment, in the classes of ``rnnt_loss_multiblank`` on the same input: invalid lengths
+    (compact: also outside ``compact_hints``, or rows running past STU) or a live label outside [0, V) give score NaN;
+    a NaN or +inf in a live row, or a live row that is all -inf, gives NaN (even for a row no path visits); a best score
+    at or below the loss's dead threshold (-5e29) gives -inf, which only masked logits can cause, as the standard blank
+    always leaves a path.  Padding rows are never read.  Deterministic; no host synchronisation in the dense layout
+    and, inside ``compact_hints``, in the compact one (CUDA-graph capturable); without hints the compact call makes one
+    16-byte device->host copy.  bfloat16 results equal those of the float32 call on the widened logits, and compact
+    results equal those of the dense call on the same rows placed in a padded tensor."""
+    assert isinstance(compact, bool)
+    durations, blank = _multiblank_args("rnnt_align_multiblank", logits, big_blank_durations, sigma, blank, compact)
+    with torch.no_grad():
+        if compact:
+            hints = _hints()
+            return _C.rnnt_multiblank_align_compact(logits, labels, frames_lengths, labels_lengths, list(durations),
+                                                    float(sigma), blank, hints[0], hints[1])
+        return _C.rnnt_multiblank_align_dense(logits, labels, frames_lengths, labels_lengths, list(durations),
+                                              float(sigma), blank)
+
+
+__all__ = ["rnnt_loss", "rnnt_align", "rnnt_align_tdt", "rnnt_align_multiblank", "rnnt_loss_from_logits",
+           "rnnt_loss_pruned",
            "rnnt_loss_multiblank", "RNNTLossMultiblank", "RNNTLossMultiblankCompact",
            "RNNTLossPruned", "rnnt_loss_simple", "RNNTLossSimple", "rnnt_loss_tdt", "RNNTLossTDT", "RNNTLossTDTCompact", "joint_pack",
            "JointPack", "RNNTLossFromLogits", "RNNTLossFromLogitsCompact", "RNNTLoss", "RNNTLossGather", "RNNTLossEager",

@@ -1137,6 +1137,63 @@ int rnnt_b200_tdt_align_compact(void *stream, void *workspace, size_t workspace_
     return RNNT_STATUS_SUCCESS;
 }
 
+// The multi-blank alignment carves the TDT alignment's workspace with D = B; its lse is one float per cell, held in
+// the first half of the lse slot.
+size_t rnnt_b200_multiblank_align_workspace_bytes(int64_t cells, int N, int num_big_blanks) {
+    return carve_tdt_align(nullptr, cells, N, num_big_blanks).bytes;
+}
+
+int rnnt_b200_multiblank_align_dense(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                     const int *labels, const int *xn, const int *yn, const int *big_blank_durations,
+                                     int num_big_blanks, float sigma, float *scores, int *frames, int *blank_counts,
+                                     int N, int T, int U, int V, int blank, int elem_bytes) {
+    TdtDurations dur;
+    if (!mb_durations(big_blank_durations, num_big_blanks, &dur) ||
+        !mb_args_ok(N, T, U, V, num_big_blanks, blank, elem_bytes, logits) || !std::isfinite(sigma) || sigma < 0.0f ||
+        !scores || !frames || !blank_counts || !workspace_aligned16(workspace))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    const int64_t cells = (int64_t)N * T * U;
+    if (!workspace || workspace_bytes < rnnt_b200_multiblank_align_workspace_bytes(cells, N, num_big_blanks))
+        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    const TdtAlignWorkspace w = carve_tdt_align(workspace, cells, N, num_big_blanks);
+    TdtFwd c = {};
+    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = scores;
+    c.multiblank = true; c.lse_mb = (float *)w.lse;
+    c.lp = w.lp; c.alpha = w.alpha; c.status = w.status;
+    c.N = N; c.T = T; c.U = U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur; c.io_bf16 = elem_bytes == 2;
+    RNNT_TRY(launch_mb_align((cudaStream_t)stream, c, w.dec, frames, blank_counts), RNNT_STATUS_WARP_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+int rnnt_b200_multiblank_align_compact(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                       const int *labels, const int *xn, const int *yn,
+                                       const int *big_blank_durations, int num_big_blanks, float sigma, float *scores,
+                                       int *frames, int *blank_counts, int64_t STU, int N, int V, int blank,
+                                       int elem_bytes, int max_T, int max_U) {
+    TdtDurations dur;
+    if (!mb_durations(big_blank_durations, num_big_blanks, &dur) ||
+        !mb_compact_args_ok(N, STU, V, num_big_blanks, blank, elem_bytes, logits) || !std::isfinite(sigma) ||
+        sigma < 0.0f || !scores || !frames || !blank_counts || !workspace_aligned16(workspace) || max_T < 1 ||
+        max_U < 1)
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    if (!workspace || workspace_bytes < rnnt_b200_multiblank_align_workspace_bytes(STU, N, num_big_blanks))
+        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    cudaStream_t s = (cudaStream_t)stream;
+    const TdtAlignWorkspace w = carve_tdt_align(workspace, STU, N, num_big_blanks);
+    RNNT_TRY(launch_prefix(s, xn, yn, N, w.prefix, w.prefix + N, w.totals), RNNT_STATUS_GATHER_FAILED);
+    TdtFwd c = {};
+    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = scores;
+    c.mem_pref = w.prefix; c.lab_pref = w.prefix + N; c.STU = STU;
+    c.multiblank = true; c.lse_mb = (float *)w.lse;
+    c.lp = w.lp; c.alpha = w.alpha; c.status = w.status;
+    c.N = N; c.T = max_T; c.U = max_U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur;
+    c.io_bf16 = elem_bytes == 2;
+    RNNT_TRY(launch_mb_align(s, c, w.dec, frames, blank_counts), RNNT_STATUS_WARP_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
 size_t rnnt_b200_multiblank_workspace_bytes(int N, int T, int U, int num_big_blanks) {
     return carve_tdt(nullptr, (int64_t)max(N, 0) * max(T, 0) * max(U, 0), N, num_big_blanks, false).bytes;
 }

@@ -824,6 +824,59 @@ rnnt_tdt_align_compact(const at::Tensor &xs, const at::Tensor &ys, const at::Ten
     return std::make_tuple(scores, frames, fdur);
 }
 
+// Viterbi alignment on the multi-blank lattice, dense (N,T,U,V) f32 or bf16 logits, B = durations.size(): (scores (N)
+// f32, frames (N,U-1) i32, blank counts (N,1+B) i32).  No host sync.
+std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_multiblank_align_dense(const at::Tensor &xs, const at::Tensor &ys,
+                                                                           const at::Tensor &xn, const at::Tensor &yn,
+                                                                           const std::vector<int> &durations,
+                                                                           double sigma, int blank) {
+    check4(xs, ys, xn, yn, true);
+    check_batch4(xs, xn, yn);
+    const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), V = xs.size(3), B = (int64_t)durations.size();
+    check_arg(ys, Dt::I32, xs, {N, U - 1}, "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
+    check_multiblank(B, blank, V);
+    const c10::cuda::CUDAGuard guard(xs.device());
+    at::Tensor scores = at::empty({N}, xs.options().dtype(at::kFloat));
+    at::Tensor frames = label_slots(N * (U - 1), xs).view({N, U - 1});
+    at::Tensor counts = at::empty({N, 1 + B}, xs.options().dtype(at::kInt));
+    if (N == 0) return std::make_tuple(scores, frames, counts);
+    at::Tensor ws = workspace(xs, rnnt_b200_multiblank_align_workspace_bytes(N * T * U, (int)N, (int)B));
+    check_status(rnnt_b200_multiblank_align_dense(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
+                                                  ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
+                                                  durations.data(), (int)B, (float)sigma, scores.data_ptr<float>(),
+                                                  frames.data_ptr<int>(), counts.data_ptr<int>(), (int)N, (int)T,
+                                                  (int)U, (int)V, blank,
+                                                  xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
+    return std::make_tuple(scores, frames, counts);
+}
+
+// Viterbi alignment on the multi-blank lattice, compact (STU,V) f32 or bf16 logits in joint_pack's row order, labels
+// (sum yn): (scores (N) f32, frames (sum yn) i32, blank counts (N,1+B) i32).  The bounds are the hints when given (no
+// host sync), else one 16-byte device->host copy, as in rnnt_multiblank_compact_forward.
+std::tuple<at::Tensor, at::Tensor, at::Tensor>
+rnnt_multiblank_align_compact(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
+                              const std::vector<int> &durations, double sigma, int blank, int max_T, int max_U) {
+    const auto [N, STU, V, bf16, guard] = compact_front(xs, ys, xn, yn, blank, true);
+    const int64_t B = (int64_t)durations.size();
+    check_multiblank(B, blank, V);
+    void *stream = current_stream(xs);
+    at::Tensor scores = at::empty({N}, xs.options().dtype(at::kFloat));
+    at::Tensor frames = label_slots(ys.numel(), xs);
+    at::Tensor counts = at::empty({N, 1 + B}, xs.options().dtype(at::kInt));
+    if (N == 0) return std::make_tuple(scores, frames, counts);
+    std::tie(max_T, max_U) = compact_bounds(stream, xs, ys, xn, yn, max_T, max_U, nullptr);
+    // a batch whose lengths are all 0: bounds of 1 (its lattices are invalid either way)
+    max_T = std::max(max_T, 1);
+    max_U = std::max(max_U, 1);
+    at::Tensor ws = workspace(xs, rnnt_b200_multiblank_align_workspace_bytes(STU, (int)N, (int)B));
+    check_status(rnnt_b200_multiblank_align_compact(stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
+                                                    ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
+                                                    durations.data(), (int)B, (float)sigma, scores.data_ptr<float>(),
+                                                    frames.data_ptr<int>(), counts.data_ptr<int>(), STU, (int)N,
+                                                    (int)V, blank, bf16 ? 2 : 4, max_T, max_U));
+    return std::make_tuple(scores, frames, counts);
+}
+
 // am (N,T,V) and lm (N,U,V): dtypes, then contiguity and device, then shapes; then ys, xn and yn
 void check_simple_inputs(const at::Tensor &am, const at::Tensor &lm, const at::Tensor &ys, const at::Tensor &xn,
                          const at::Tensor &yn) {
@@ -1114,6 +1167,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           "Viterbi forced alignment on the TDT lattice, compact layout.", py::arg("xs"), py::arg("ys"), py::arg("xn"),
           py::arg("yn"), py::arg("durations"), py::arg("sigma") = 0.0, py::arg("blank") = 0, py::arg("max_T") = 0,
           py::arg("max_U") = 0);
+    m.def("rnnt_multiblank_align_dense", &rnnt_multiblank_align_dense,
+          "Viterbi forced alignment on the multi-blank lattice, dense layout.", py::arg("xs"), py::arg("ys"),
+          py::arg("xn"), py::arg("yn"), py::arg("big_blank_durations"), py::arg("sigma"), py::arg("blank"));
+    m.def("rnnt_multiblank_align_compact", &rnnt_multiblank_align_compact,
+          "Viterbi forced alignment on the multi-blank lattice, compact layout.", py::arg("xs"), py::arg("ys"),
+          py::arg("xn"), py::arg("yn"), py::arg("big_blank_durations"), py::arg("sigma"), py::arg("blank"),
+          py::arg("max_T") = 0, py::arg("max_U") = 0);
     m.def("rnnt_simple_forward", &rnnt_simple_forward, py::arg("am"), py::arg("lm"), py::arg("ys"), py::arg("xn"),
           py::arg("yn"), py::arg("blank") = 0, py::arg("want_grads") = true, py::arg("prune_range") = 0,
           py::arg("lse_mode") = 0, py::arg("lm_only_scale") = 0.0, py::arg("am_only_scale") = 0.0,

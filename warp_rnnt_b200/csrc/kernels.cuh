@@ -245,6 +245,10 @@ cudaError_t launch_tdt_backward(cudaStream_t s, const TdtBwd &c);
 // (N) and pg, beta, ll unused; the normaliser writes lse and lp, then k_tdt_align writes alpha, dec (cells bytes, the
 // decision per cell), status, the scores, and frames and fdur (dense (N,U-1), compact (sum yn)).
 cudaError_t launch_tdt_align(cudaStream_t s, const TdtFwd &c, uint8_t *dec, int *frames, int *fdur);
+// The Viterbi alignment on the multi-blank lattice (rnnt_b200_multiblank_align_*): c as for the multiblank forward
+// (lse_mb the normaliser's (cells) floats), costs = the scores (N), pg, beta, ll unused; k_mb_align writes alpha, dec,
+// status, the scores, frames (dense (N,U-1), compact (sum yn)) and counts (N, 1 + B).
+cudaError_t launch_mb_align(cudaStream_t s, const TdtFwd &c, uint8_t *dec, int *frames, int *counts);
 void tdt_launch_record(int32_t *out);     // copy of the last TDT launch's record (rnntTdtLaunchRecord_t)
 
 // expand.cu -- small helpers of the python-level API

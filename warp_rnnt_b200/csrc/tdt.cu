@@ -38,7 +38,9 @@
 // blank, label, big blank [0..B)), big blank i at column blank - 1 - i.  The edges out of (t, u): the standard blank to
 // (t + 1, u), the label to (t, u + 1) and big blank i to (t + d[i], u), so alpha's sources lie on diagonals s - 1 and
 // s - d[i] and the ring keeps max(d) + 1 diagonals.  Kernels k_mb_norm, k_mb_recur, k_mb_post, k_mb_emit (and their
-// _compact twins); every TDT instantiation is the code it was.
+// _compact twins); every TDT instantiation is the code it was.  k_mb_align (rnnt_b200_multiblank_align_*, after
+// k_mb_norm) is the Viterbi alignment on this lattice: k_mb_recur's alpha side in max-plus form, as k_tdt_align is
+// k_tdt_recur's, with the blank counts of the best path beside its label frames.
 #include "common.cuh"
 #include "kernels.cuh"
 
@@ -258,6 +260,13 @@ struct TdtAlignOut {
     uint8_t *dec;                         // decisions, addressed as alpha
     int *frames, *fdur;
 };
+// The multi-blank alignment's outputs (k_mb_align): per cell the index k in [0, 2 + B) of the candidate it took (0:
+// standard blank, 1: label, 2 + j: big blank j), kTdtNoPred as above; frames as above; counts (N, 1 + B): the standard
+// blank's and each big blank's edges on the best path.
+struct MbAlignOut {
+    uint8_t *dec;
+    int *frames, *counts;
+};
 
 // The largest of C candidates and its index in `arg`: blank edges (even k) first, then label edges (odd k), each by
 // increasing duration, and only a strictly larger value replaces the one held, so on a tie blank beats label and the
@@ -273,6 +282,20 @@ __device__ __forceinline__ float max_cands(const float (&c)[C], int &arg) {
 #pragma unroll
     for (int k = 1; k < C; k += 2)
         if (c[k] > m) { m = c[k]; arg = k; }
+    return arg == kTdtNoPred ? kBig : m;
+}
+// max_cands over the multi-blank layout (c[0] standard blank, c[1] label, c[2 + j] big blank j): the standard blank
+// first, then the big blanks by increasing duration, then the label, so on a tie a blank beats the label and the
+// shorter blank wins.  Absent and NaN candidates are never taken; no candidate: kBig and kTdtNoPred.
+template <int C>
+__device__ __forceinline__ float max_cands_mb(const float (&c)[C], int &arg) {
+    float m = -INFINITY;
+    arg = kTdtNoPred;
+    if (c[0] > m) { m = c[0]; arg = 0; }
+#pragma unroll
+    for (int k = 2; k < C; ++k)
+        if (c[k] > m) { m = c[k]; arg = k; }
+    if (c[1] > m) { m = c[1]; arg = 1; }
     return arg == kTdtNoPred ? kBig : m;
 }
 
@@ -304,6 +327,47 @@ __device__ __forceinline__ void tdt_backtrace(const TdtRec &a, const TdtAlignOut
     }
 }
 
+// ALIGN && MB, after the sweep: as tdt_backtrace, the lattice's label slots set to -1 and, for a lattice classed ok,
+// thread 0 follows the decisions back from the terminal edge k0 (0: the standard blank, 2 + j: big blank j) out of
+// (t0, Un - 1) to (0, 0): k = 0 moves t back by 1, k = 1 moves u back by 1 and writes the label edge's frame, k = 2 + j
+// moves t back by d[j].  The edge counts (terminal edge included) are kept in registers and written once to row n of
+// o.counts; a lattice that is not ok gets -1 there.
+template <int KD>
+__device__ __forceinline__ void mb_backtrace(const TdtRec &a, const MbAlignOut &o, int64_t base, int ld,
+                                             int64_t lab_base, int slots, int n, int Un, int t0, int k0, bool ok) {
+    int *fr = o.frames + lab_base, *cnt = o.counts + (int64_t)n * (1 + a.D);
+    for (int u = threadIdx.x; u < slots; u += blockDim.x) fr[u] = -1;
+    __syncthreads();
+    if (threadIdx.x != 0) return;
+    if (!ok) {
+        for (int k = 0; k <= a.D; ++k) cnt[k] = -1;
+        return;
+    }
+    int n_std = 0, n_big[KD - 2];
+#pragma unroll
+    for (int j = 0; j < KD - 2; ++j) n_big[j] = 0;
+    int t = t0, u = Un - 1, k = k0;
+    for (int step = 0; step <= t0 + Un - 1; ++step) {
+        n_std += k == 0;
+#pragma unroll
+        for (int j = 0; j < KD - 2; ++j) n_big[j] += k == 2 + j;
+        k = o.dec[base + (int64_t)t * ld + u];
+        if (k == kTdtNoPred) break;
+        if (k == 0) {
+            --t;
+        } else if (k == 1) {
+            --u;
+            fr[u] = t;
+        } else {
+            t -= a.dur.d[k - 2];
+        }
+    }
+    cnt[0] = n_std;
+#pragma unroll
+    for (int j = 0; j < KD - 2; ++j)
+        if (j < a.D) cnt[1 + j] = n_big[j];
+}
+
 // alpha (blockIdx.y == 0) or beta (1) of lattice blockIdx.x.  KD >= D: the candidate arrays' compile-time size.
 // The ring holds U (dense: the padded width, compact: max_U) columns per diagonal; lp, alpha and beta are addressed
 // with the lattice's row stride ld (dense U, compact Un).
@@ -311,9 +375,10 @@ __device__ __forceinline__ void tdt_backtrace(const TdtRec &a, const TdtAlignOut
 // cell; it also checks every live cell's own lp row for NaN, as the beta side does.  After the sweep, the class and
 // the score (a.costs) of the lattice, then the backtrace (tdt_backtrace).
 // MB (k_mb_recur): the multi-blank edges; KD >= 2 + B is the candidate array's size (standard blank, label, big blanks).
-template <int KD, bool COMPACT, bool ALIGN = false, bool MB = false>
-__device__ __forceinline__ void tdt_recur(const TdtRec &a, const TdtCompact &cp,
-                                          const TdtAlignOut &o = TdtAlignOut{}) {
+// ALIGN && MB (k_mb_align, OUT = MbAlignOut): the same alpha side with max_cands_mb, the cell's own row checked for
+// NaN, then the terminal step by max_cands_mb's tie rule and mb_backtrace.
+template <int KD, bool COMPACT, bool ALIGN = false, bool MB = false, typename OUT = TdtAlignOut>
+__device__ __forceinline__ void tdt_recur(const TdtRec &a, const TdtCompact &cp, const OUT &o = OUT{}) {
     extern __shared__ float ring[];
     const int n = blockIdx.x;
     const bool beta_side = !ALIGN && blockIdx.y == 1;
@@ -335,7 +400,9 @@ __device__ __forceinline__ void tdt_recur(const TdtRec &a, const TdtCompact &cp,
                 a.costs[n] = NAN;
             }
             // the label slots of lattice n: dense U - 1, compact yn[n] (none when it is negative)
-            tdt_backtrace(a, o, 0, 0, lab_base, COMPACT ? max(Un - 1, 0) : a.U - 1, 0, 0, 0, false);
+            const int slots = COMPACT ? max(Un - 1, 0) : a.U - 1;
+            if constexpr (MB) mb_backtrace<KD>(a, o, 0, 0, lab_base, slots, n, 0, 0, 0, false);
+            else tdt_backtrace(a, o, 0, 0, lab_base, slots, 0, 0, 0, false);
         } else if (beta_side && threadIdx.x == 0) {
             a.status[n] = kTdtInvalid;
             a.costs[n] = NAN;
@@ -376,7 +443,19 @@ __device__ __forceinline__ void tdt_recur(const TdtRec &a, const TdtCompact &cp,
                             if (tp >= 0) c[2 + j] = rd(tp, u, back(d)) + lp[((int64_t)tp * ld + u) * W2 + 2 + j];
                         }
                     }
-                    v = (t == 0 && u == 0) ? 0.0f : lse_cands(c);
+                    if constexpr (ALIGN) {
+                        // the cell's own row, for the NaN class (the beta side's check, here on the alpha side)
+                        const float *r = lp + ((int64_t)t * ld + u) * W2;
+                        saw_nan |= (r[0] != r[0]) || (u < Un - 1 && r[1] != r[1]);
+#pragma unroll
+                        for (int j = 0; j < KD - 2; ++j)
+                            if (j < D) saw_nan |= r[2 + j] != r[2 + j];
+                        int k = kTdtNoPred;
+                        v = (t == 0 && u == 0) ? 0.0f : max_cands_mb(c, k);
+                        o.dec[base + (int64_t)t * ld + u] = (uint8_t)k;
+                    } else {
+                        v = (t == 0 && u == 0) ? 0.0f : lse_cands(c);
+                    }
                 } else {
                     // push: the cell's own weights, beta of the destinations; a blank that reaches t = Tn from the
                     // last column is terminal (beta 0 after it)
@@ -467,7 +546,30 @@ __device__ __forceinline__ void tdt_recur(const TdtRec &a, const TdtCompact &cp,
     }
     bad = __syncthreads_or(bad);
     saw_nan = __syncthreads_or(saw_nan);
-    if constexpr (ALIGN) {
+    if constexpr (ALIGN && MB) {
+        // the terminal step, by the tie rule of max_cands_mb: the standard blank from (Tn - 1, Un - 1), then big blank
+        // j from (Tn - d[j], Un - 1) by increasing duration.  Every thread computes it alike, as below.
+        float best = -INFINITY;
+        int t0 = 0, k0 = kTdtNoPred;
+        const int64_t last = (int64_t)(Tn - 1) * ld + Un - 1;
+        const float cs = out[last] + lp[last * W2];
+        if (cs > best) { best = cs; t0 = Tn - 1; k0 = 0; }
+        for (int j = 0; j < D; ++j) {
+            const int tp = Tn - a.dur.d[j];
+            if (tp >= 0) {
+                const int64_t src = (int64_t)tp * ld + Un - 1;
+                const float cand = out[src] + lp[src * W2 + 2 + j];
+                if (cand > best) { best = cand; t0 = tp; k0 = 2 + j; }
+            }
+        }
+        const int st = bad ? kTdtInvalid : saw_nan ? kTdtNan : lattice_dead(best) ? kTdtDead : kTdtOk;
+        if (threadIdx.x == 0) {
+            a.status[n] = st;
+            a.costs[n] = st == kTdtOk ? best : st == kTdtDead ? -INFINITY : NAN;
+        }
+        mb_backtrace<KD>(a, o, base, ld, lab_base, COMPACT ? Un - 1 : U - 1, n, Un, t0, k0, st == kTdtOk);
+        return;
+    } else if constexpr (ALIGN) {
         // the terminal step: the best blank edge of duration d > 0 from (Tn - d, Un - 1), by the tie rule of
         // max_cands (the shorter duration wins).  Every thread computes it alike from alpha in global memory (the
         // sweep ended on a barrier), so the choice needs no broadcast and the ring keeps all of shared memory.
@@ -522,6 +624,16 @@ __global__ void __launch_bounds__(kTdtMaxThreads) k_tdt_align(TdtRec a, TdtAlign
 template <int KD>
 __global__ void __launch_bounds__(kTdtMaxThreads) k_tdt_align_compact(TdtRec a, TdtCompact cp, TdtAlignOut o) {
     tdt_recur<KD, true, true>(a, cp, o);
+}
+
+// The multi-blank Viterbi alignment, grid (N, 1): a.D = B, a.costs = the scores.  The bound of k_mb_recur.
+template <int KD>
+__global__ void __launch_bounds__(kTdtMaxThreads, 1) k_mb_align(TdtRec a, MbAlignOut o) {
+    tdt_recur<KD, false, true, true>(a, TdtCompact{}, o);
+}
+template <int KD>
+__global__ void __launch_bounds__(kTdtMaxThreads, 1) k_mb_align_compact(TdtRec a, TdtCompact cp, MbAlignOut o) {
+    tdt_recur<KD, true, true, true>(a, cp, o);
 }
 
 // a.T, a.U = max_T, max_U
@@ -990,6 +1102,33 @@ cudaError_t launch_tdt_align(cudaStream_t s, const TdtFwd &c, uint8_t *dec, int 
     if (e != cudaSuccess) return e;
     const TdtAlignOut o = {dec, frames, fdur};
     return p.kd == 5 ? tdt_align_as<5>(s, p, c, o) : tdt_align_as<kTdtMaxD>(s, p, c, o);
+}
+
+template <int KD>
+static cudaError_t mb_align_as(cudaStream_t s, const TdtPlan &p, const TdtFwd &c, const MbAlignOut &o) {
+    static std::atomic<bool> smem_set[kMaxDevices], smem_set_compact[kMaxDevices];
+    if (p.smem > (48 << 10)) {
+        const cudaError_t e = c.mem_pref ? ensure_dyn_smem(k_mb_align_compact<KD>, smem_set_compact,
+                                                           max_optin_smem(current_device()))
+                                         : ensure_dyn_smem(k_mb_align<KD>, smem_set, max_optin_smem(current_device()));
+        if (e != cudaSuccess) return e;
+    }
+    const TdtRec r = {c.lp, c.labels, c.xn, c.yn, c.alpha, nullptr, nullptr, c.costs, c.status, c.T, c.U, c.V,
+                      c.dur.D, p.ring, c.dur};
+    if (c.mem_pref) k_mb_align_compact<KD><<<dim3(c.N, 1), p.warps * 32, p.smem, s>>>(r, tdt_compact(c), o);
+    else k_mb_align<KD><<<dim3(c.N, 1), p.warps * 32, p.smem, s>>>(r, o);
+    count_launch();
+    return cudaGetLastError();
+}
+
+cudaError_t launch_mb_align(cudaStream_t s, const TdtFwd &c, uint8_t *dec, int *frames, int *counts) {
+    const int64_t cells = c.mem_pref ? c.STU : (int64_t)c.N * c.T * c.U;
+    const TdtPlan p = tdt_plan_recorded(c);
+    cudaError_t e = c.io_bf16 ? tdt_norm_as<true>(s, p, static_cast<const __nv_bfloat16 *>(c.x), c, cells)
+                              : tdt_norm_as<true>(s, p, static_cast<const float *>(c.x), c, cells);
+    if (e != cudaSuccess) return e;
+    const MbAlignOut o = {dec, frames, counts};
+    return p.kd == 5 ? mb_align_as<5>(s, p, c, o) : mb_align_as<kTdtMaxD>(s, p, c, o);
 }
 
 template <bool MB, typename IO>
