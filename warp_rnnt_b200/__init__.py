@@ -244,7 +244,7 @@ def rnnt_loss_from_logits(logits, labels, frames_lengths, labels_lengths, averag
     Non-regular types take no FastEmit (k2 has none); regular + penalty + FastEmit compose.  A lattice with invalid
     lengths gets cost NaN, one without a finite path +inf, one with a NaN in its live log-probs NaN, with zero, zero and
     NaN gradients; the one-symbol-per-frame types take label dimensions up to 25599 (include/rnnt_b200.h).  Bad values
-    raise ValueError before any launch."""
+    raise ValueError before any launch.  ``rnnt_align_from_logits`` gives the best path on the same lattice."""
     assert average_frames is None or isinstance(average_frames, bool)
     assert reduction is None or reduction in ("none", "mean", "sum")
     assert isinstance(blank, int)
@@ -894,13 +894,57 @@ def rnnt_align(log_probs, labels, frames_lengths, labels_lengths, blank=0, compa
     emitted as early as the ties allow.  A lattice with no path above -inf gets score -inf, one whose every path is NaN
     gets NaN; lengths outside (1..T, 1..U-1 labels; compact: outside ``compact_hints``) get score NaN.  All of these
     get frames -1.  No autograd.  No host synchronisation in the dense layout and, inside ``compact_hints``, in the
-    compact one (CUDA-graph capturable); without hints the compact call makes one 16-byte device->host copy."""
+    compact one (CUDA-graph capturable); without hints the compact call makes one 16-byte device->host copy.
+
+    From joint logits, ``rnnt_align_from_logits`` gives the same result without a dense ``log_softmax`` tensor, and
+    also on k2's "modified" and "constrained" lattices and with ``delay_penalty``."""
     assert isinstance(blank, int)
     assert isinstance(compact, bool)
     if compact:
         hints = _hints()
         return _C.rnnt_align_compact(log_probs, labels, frames_lengths, labels_lengths, blank, hints[0], hints[1])
     return _C.rnnt_align_dense(log_probs, labels, frames_lengths, labels_lengths, blank)
+
+
+def rnnt_align_from_logits(logits, labels, frames_lengths, labels_lengths, blank=0, compact=False,
+                           rnnt_type="regular", delay_penalty=0.0):
+    """Viterbi forced alignment straight from joint logits, on the lattice of ``rnnt_loss_from_logits`` with the same
+    ``rnnt_type`` and ``delay_penalty``: the single best path of each lattice and the frame of each label, without the
+    dense ``log_softmax`` tensor that ``rnnt_align`` needs.  For the one-symbol-per-frame types this is the alignment
+    of the lattice the model was trained on, and with a penalty it shows the emission latency the penalty tunes.
+
+    Inputs and argument checks are those of ``rnnt_loss_from_logits``: dense (N, T, U, V) logits, float32 or bfloat16,
+    with labels (N, U-1) int32; or ``compact=True``: (STU, V) rows in ``joint_pack``'s order with labels
+    (sum(labels_lengths),), honouring ``compact_hints`` (``rnnt_type="regular"`` and ``delay_penalty=0`` only, as for
+    the loss).  No autograd: the outputs are not differentiable and ``logits.requires_grad`` is ignored.
+
+    Edge weights: cell (t, u) has the pair b = logit[blank] - lse and l = logit[label] - lse in float32, lse the
+    normaliser of the loss's own pass, so they are bit for bit the loss's; a penalty is added to them exactly as the
+    loss adds it; the constrained label weight is l(t, u) + b(t, u+1).  A path's score is the float32 left fold
+    ``acc = acc + w`` over its edges; the max-plus recurrence adds in that order and so gives the largest one exactly.
+      - ``"regular"``: ``rnnt_align``'s lattice, tie rule, classes and frames on these pairs, so the result equals
+        ``rnnt_align(logits.float() - lse[..., None])`` bit for bit (with the penalty on the label columns).
+      - ``"modified"`` / ``"constrained"``: a label edge (t, u) -> (t+1, u+1) also leaves the frame; alpha(0, 0) = 0,
+        the score is alpha(Tn, Un-1), and the label edge wins iff its candidate is larger or the blank one is NaN.
+        Frames are strictly increasing, in [0, Tn-1]; a lattice with more labels than frames gets score -inf.  Dense
+        only, with U <= 25600.
+
+    Returns ``(scores, frames)``: ``scores`` (N,) float32, the best path's score; ``frames`` int32, dense (N, U-1),
+    compact (sum(labels_lengths),): frames[n, u] is the frame of the best path's edge for label u, -1 for
+    u >= labels_lengths[n].  A lattice with no path above -inf gets score -inf, one whose every path is NaN gets NaN,
+    invalid lengths (compact: also outside ``compact_hints``) get NaN, all with frames -1.  Deterministic; no host
+    synchronisation in the dense layout and, inside ``compact_hints``, in the compact one (CUDA-graph capturable).
+    bfloat16 results equal those of the float32 call on the widened logits, and compact results equal those of the
+    dense call on the same rows placed in a padded tensor.  Bad values raise ValueError before any launch."""
+    assert isinstance(blank, int)
+    assert isinstance(compact, bool)
+    kind, lam = _path_type("rnnt_align_from_logits", rnnt_type, delay_penalty, 0.0, compact)
+    with torch.no_grad():
+        if compact:
+            hints = _hints()
+            return _C.rnnt_align_logits_compact(logits, labels, frames_lengths, labels_lengths, blank, hints[0],
+                                                hints[1])
+        return _C.rnnt_align_logits_dense(logits, labels, frames_lengths, labels_lengths, blank, kind, lam)
 
 
 def rnnt_align_tdt(logits, labels, frames_lengths, labels_lengths, durations, sigma=0.0, blank=0, compact=False):
@@ -994,7 +1038,7 @@ def rnnt_align_multiblank(logits, labels, frames_lengths, labels_lengths, big_bl
                                               float(sigma), blank)
 
 
-__all__ = ["rnnt_loss", "rnnt_align", "rnnt_align_tdt", "rnnt_align_multiblank", "rnnt_loss_from_logits",
+__all__ = ["rnnt_loss", "rnnt_align", "rnnt_align_from_logits", "rnnt_align_tdt", "rnnt_align_multiblank", "rnnt_loss_from_logits",
            "rnnt_loss_pruned",
            "rnnt_loss_multiblank", "RNNTLossMultiblank", "RNNTLossMultiblankCompact",
            "RNNTLossPruned", "rnnt_loss_simple", "RNNTLossSimple", "rnnt_loss_tdt", "RNNTLossTDT", "RNNTLossTDTCompact", "joint_pack",

@@ -613,6 +613,44 @@ static int run_align(cudaStream_t s, void *workspace, size_t workspace_bytes, Al
     return RNNT_STATUS_SUCCESS;
 }
 
+// The alignment from logits (rnnt_b200_align_logits_*): run_align's workspace, then the normaliser's lse (cells).  Its
+// decision words (N, ceil(U/32), T+31) also hold k_frames_align's (N, ceil(U/32), T).
+static size_t align_logits_bytes(int64_t cells, int N, int T, int U) {
+    return carve_align(nullptr, cells, N, T, U).bytes + align_up((size_t)(cells > 0 ? cells : 0) * sizeof(float), 256);
+}
+
+// compact prefix sums, the normaliser pass into the workspace's pairs and lse, the delay penalty in place, then k_align
+// (regular) or k_frames_align (modified, constrained); c.lp holds the logits
+static int run_align_logits(cudaStream_t s, void *workspace, size_t workspace_bytes, AlignCall c, int rnnt_type,
+                            float delay_penalty) {
+    if (!workspace || workspace_bytes < align_logits_bytes(c.cells, c.p.N, c.T, c.U))
+        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    const AlignWorkspace w = carve_align(workspace, c.cells, c.p.N, c.T, c.U);
+    float *lse = reinterpret_cast<float *>(static_cast<char *>(workspace) + w.bytes);
+    if (c.p.compact) {
+        RNNT_TRY(launch_prefix(s, c.p.xn, c.p.yn, c.p.N, w.mem_pref, w.lab_pref, w.totals), RNNT_STATUS_GATHER_FAILED);
+        c.p.mem_pref = w.mem_pref;
+        c.p.lab_pref = w.lab_pref;
+        RNNT_TRY(launch_lse_pairs_compact(s, c.lp, c.p, c.labels, c.cells, c.V, c.blank, w.pairs, lse, c.io_bf16),
+                 RNNT_STATUS_GATHER_FAILED);
+    } else {
+        RNNT_TRY(launch_lse_pairs(s, c.lp, c.labels, c.p.N, c.T, c.U, c.V, c.blank, w.pairs, lse, c.io_bf16),
+                 RNNT_STATUS_GATHER_FAILED);
+    }
+    if (delay_penalty != 0.0f)
+        RNNT_TRY(launch_delay_pairs(s, w.pairs, w.pairs, c.p.xn, c.p.yn, c.p.N, c.T, c.U, delay_penalty),
+                 RNNT_STATUS_GATHER_FAILED);
+    if (rnnt_type == 0) {
+        RNNT_TRY(launch_align(s, c.p, w.pairs, w.alphas, w.dec, c.T, c.U, c.scores, c.frames), RNNT_STATUS_WARP_FAILED);
+        return RNNT_STATUS_SUCCESS;
+    }
+    FramesAlignCall f = {};
+    f.pairs = w.pairs; f.xn = c.p.xn; f.yn = c.p.yn; f.dec = w.dec; f.scores = c.scores; f.frames = c.frames;
+    f.N = c.p.N; f.T = c.T; f.U = c.U; f.constrained = rnnt_type == 2; f.delayed = delay_penalty != 0.0f;
+    RNNT_TRY(launch_frames_align(s, f), RNNT_STATUS_WARP_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
 static int logits_compact_backward_any(void *stream, const void *logits, const float *lse, const float *pair_grads,
                                        const int *ys, const int *xn, const int *yn, const int64_t *prefix,
                                        const float *grad_out, void *out, int64_t STU, int N, int V, int blank,
@@ -1295,6 +1333,10 @@ void rnnt_b200_debug_last_frames_launch(int32_t *out) {
     if (out) rnnt::frames_launch_record(out);
 }
 
+void rnnt_b200_debug_last_frames_align_launch(int32_t *out) {
+    if (out) rnnt::frames_align_launch_record(out);
+}
+
 size_t rnnt_b200_simple_workspace_bytes(int N, int T, int U) {
     return carve(nullptr, (int64_t)max(N, 0) * max(T, 0) * max(U, 0), N).bytes;
 }
@@ -1434,6 +1476,42 @@ int rnnt_b200_align_compact(void *stream, void *workspace, size_t workspace_byte
     c.lp = log_probs; c.labels = labels; c.V = V; c.blank = blank; c.io_bf16 = elem_bytes == 2;
     c.scores = scores; c.frames = frames;
     return run_align((cudaStream_t)stream, workspace, workspace_bytes, c);
+}
+
+size_t rnnt_b200_align_logits_workspace_bytes(int64_t cells, int N, int T, int U) {
+    return align_logits_bytes(cells, N, T, U);
+}
+
+int rnnt_b200_align_logits_dense(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                 const int *labels, const int *xn, const int *yn, float *scores, int *frames, int N,
+                                 int T, int U, int V, int blank, int elem_bytes, int rnnt_type, float delay_penalty) {
+    if ((elem_bytes != 4 && elem_bytes != 2) || !dense_args_ok(N, T, U, V, blank) ||
+        (reinterpret_cast<uintptr_t>(logits) & (uintptr_t)(elem_bytes - 1)) ||
+        !path_type_ok(rnnt_type, delay_penalty, 0.0f, U) || !scores || !frames || !workspace_aligned16(workspace))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    AlignCall c = {};
+    c.p = {xn, yn, nullptr, nullptr, N, T, U, 0};
+    c.T = T; c.U = U; c.cells = (int64_t)N * T * U;
+    c.lp = logits; c.labels = labels; c.V = V; c.blank = blank; c.io_bf16 = elem_bytes == 2;
+    c.scores = scores; c.frames = frames;
+    return run_align_logits((cudaStream_t)stream, workspace, workspace_bytes, c, rnnt_type, delay_penalty);
+}
+
+int rnnt_b200_align_logits_compact(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                   const int *labels, const int *xn, const int *yn, float *scores, int *frames,
+                                   int64_t STU, int N, int V, int blank, int elem_bytes, int max_T, int max_U) {
+    if ((elem_bytes != 4 && elem_bytes != 2) || !compact_args_ok(N, STU, V, blank) || max_T <= 0 || max_U <= 0 ||
+        (reinterpret_cast<uintptr_t>(logits) & (uintptr_t)(elem_bytes - 1)) || !scores || !frames ||
+        !workspace_aligned16(workspace))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    AlignCall c = {};
+    c.p = {xn, yn, nullptr, nullptr, N, 0, 0, 1};
+    c.T = max_T; c.U = max_U; c.cells = STU;
+    c.lp = logits; c.labels = labels; c.V = V; c.blank = blank; c.io_bf16 = elem_bytes == 2;
+    c.scores = scores; c.frames = frames;
+    return run_align_logits((cudaStream_t)stream, workspace, workspace_bytes, c, 0, 0.0f);
 }
 
 int rnnt_b200_compact_totals(void *stream, const int *xn, const int *yn, int N, int64_t *scratch, int *totals) {

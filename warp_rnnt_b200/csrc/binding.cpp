@@ -1104,6 +1104,45 @@ std::tuple<at::Tensor, at::Tensor> rnnt_align_compact(const at::Tensor &xs, cons
     return std::make_tuple(scores, frames);
 }
 
+// Viterbi alignment from dense (N,T,U,V) f32 or bf16 logits on k2's lattices (rnnt_type 0, 1, 2, delay_penalty):
+// (scores (N) f32, frames (N,U-1) i32).  No host sync.
+std::tuple<at::Tensor, at::Tensor> rnnt_align_logits_dense(const at::Tensor &xs, const at::Tensor &ys,
+                                                           const at::Tensor &xn, const at::Tensor &yn, int blank,
+                                                           int rnnt_type, double delay_penalty) {
+    const auto [N, T, U, V, bf16, guard] = dense_front(xs, ys, xn, yn, true);
+    check_blank(blank, V);
+    at::Tensor scores = at::empty({N}, xs.options().dtype(at::kFloat));
+    at::Tensor frames = label_slots(N * (U - 1), xs).view({N, U - 1});
+    if (N == 0) return std::make_tuple(scores, frames);
+    at::Tensor ws = workspace(xs, rnnt_b200_align_logits_workspace_bytes(N * T * U, (int)N, (int)T, (int)U));
+    check_status(rnnt_b200_align_logits_dense(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
+                                              ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
+                                              scores.data_ptr<float>(), frames.data_ptr<int>(), (int)N, (int)T, (int)U,
+                                              (int)V, blank, bf16 ? 2 : 4, rnnt_type, (float)delay_penalty));
+    return std::make_tuple(scores, frames);
+}
+
+// Viterbi alignment from compact (STU,V) f32 or bf16 logits in joint_pack's row order (regular lattice): (scores (N)
+// f32, frames (sum yn) i32).  The bounds are the hints when given (no host sync), else one 16-byte device->host copy.
+std::tuple<at::Tensor, at::Tensor> rnnt_align_logits_compact(const at::Tensor &xs, const at::Tensor &ys,
+                                                             const at::Tensor &xn, const at::Tensor &yn, int blank,
+                                                             int max_T, int max_U) {
+    const auto [N, STU, V, bf16, guard] = compact_front(xs, ys, xn, yn, blank, true);
+    void *stream = current_stream(xs);
+    at::Tensor scores = at::empty({N}, xs.options().dtype(at::kFloat));
+    at::Tensor frames = label_slots(ys.numel(), xs);
+    if (N == 0) return std::make_tuple(scores, frames);
+    std::tie(max_T, max_U) = compact_bounds(stream, xs, ys, xn, yn, max_T, max_U, nullptr);
+    max_T = std::max(max_T, 1);              // lengths of 0 or less: the lattice is outside any bounds (score NaN)
+    max_U = std::max(max_U, 1);
+    at::Tensor ws = workspace(xs, rnnt_b200_align_logits_workspace_bytes(STU, (int)N, max_T, max_U));
+    check_status(rnnt_b200_align_logits_compact(stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
+                                                ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
+                                                scores.data_ptr<float>(), frames.data_ptr<int>(), STU, (int)N, (int)V,
+                                                blank, bf16 ? 2 : 4, max_T, max_U));
+    return std::make_tuple(scores, frames);
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -1196,6 +1235,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("rnnt_align_compact", &rnnt_align_compact, "Viterbi forced alignment, compact layout.", py::arg("xs"),
           py::arg("ys"), py::arg("xn"), py::arg("yn"), py::arg("blank") = 0, py::arg("max_T") = 0,
           py::arg("max_U") = 0);
+    m.def("rnnt_align_logits_dense", &rnnt_align_logits_dense,
+          "Viterbi forced alignment from logits on k2's lattices, dense layout.", py::arg("xs"), py::arg("ys"),
+          py::arg("xn"), py::arg("yn"), py::arg("blank") = 0, py::arg("rnnt_type") = 0, py::arg("delay_penalty") = 0.0);
+    m.def("rnnt_align_logits_compact", &rnnt_align_logits_compact,
+          "Viterbi forced alignment from logits, compact layout.", py::arg("xs"), py::arg("ys"), py::arg("xn"),
+          py::arg("yn"), py::arg("blank") = 0, py::arg("max_T") = 0, py::arg("max_U") = 0);
     m.def("set_lse_mode", [](int mode) { rnnt_b200_set_lse_mode(mode); }, py::arg("mode"));
     m.def("get_lse_mode", []() { return rnnt_b200_get_lse_mode(); });
     m.def("launch_count", []() { return rnnt_b200_launch_count(); });

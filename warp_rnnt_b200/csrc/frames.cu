@@ -11,6 +11,8 @@
 //                  path, so that every backward kernel consumes them unchanged.  Constrained: the label weight is
 //                  l(t,u) + b(t,u+1), so the label edge's occupation is also added to the blank slot of (t,u+1); the
 //                  blank slot before that fold can be written on its own for the prune ranges.
+//   k_frames_align k_frames' alpha side in max-plus form, with one decision word per warp and frame, then the
+//                  backtrace in the same CTA: the Viterbi alignment on these lattices (rnnt_b200_align_logits_dense).
 //
 // Every operand is clamped below at kBig (a -inf log-prob becomes the finite sentinel) and every LSE is the exact
 // max + log1pf(expf(-|d|)) of two finite values or NaN, so -inf - -inf is never formed; a lattice with no finite path
@@ -199,6 +201,125 @@ __global__ void __launch_bounds__(kFramesMaxThreads) k_frames(FramesArgs a) {
     }
 }
 
+// Viterbi alignment on the modified / constrained lattice (rnnt_b200_align_logits_dense, rnnt_type 1 or 2): alpha in
+// max-plus form, alpha(0,0) = 0, alpha(0,u>0) = -inf, alpha(t+1,u) = skip = alpha(t,u) + b(t,u), or emit =
+// alpha(t,u-1) + l'(t,u-1) iff emit > skip or skip is NaN (column 0: skip).  The weights are not clamped: max-plus
+// never subtracts, so -inf stays -inf.  The sweep and its operand prefetch are k_frames' alpha side, one frame per
+// step; each warp also stores the __ballot_sync of its 32 columns' choices as one word of dec (N, ceil(U/32), T), so
+// that one coalesced load serves 32 frames of a column block.  Then warp 0 walks the path back from (Tn, Un-1): the
+// walk leaves one frame per step and at most one column, so 32 steps need the words of the current column block and
+// of the one to its left; those of the next 32 frames are loaded while the walk runs on shuffled copies.
+struct FramesAlignArgs {
+    const float2 *pairs;
+    const int *xn, *yn;
+    uint32_t *dec;
+    float *scores;
+    int *frames;                    // (N, U-1)
+    int T, U;
+};
+
+template <bool CONSTRAINED>
+__global__ void __launch_bounds__(kFramesMaxThreads) k_frames_align(FramesAlignArgs a) {
+    extern __shared__ float rows[];                 // two row buffers of a.U floats
+    const int n = blockIdx.x;
+    const int U = a.U, bd = blockDim.x, lane = threadIdx.x & 31;
+    int *fr = a.frames + (int64_t)n * (U - 1);
+    int Tn, Un;
+    const bool ok = fr_lengths(a.xn, a.yn, n, a.T, U, Tn, Un);
+    if (!ok || Un - 1 > Tn) {                       // invalid lengths: NaN; more labels than frames: no path, -inf
+        for (int u = threadIdx.x; u < U - 1; u += bd) fr[u] = -1;
+        if (threadIdx.x == 0) a.scores[n] = ok ? -INFINITY : NAN;
+        return;
+    }
+    const float2 *pr = a.pairs + (int64_t)n * a.T * U;
+    uint32_t *dec = a.dec + (int64_t)n * ((U + 31) >> 5) * a.T;
+    auto buf = [&](int t) { return rows + (t & 1) * U; };   // the row buffer of frame t
+    for (int u = threadIdx.x; u < Un; u += bd) buf(0)[u] = u == 0 ? 0.0f : -INFINITY;
+    FrOps pf[kFramesPrefetch];
+#pragma unroll
+    for (int k = 0; k < kFramesPrefetch; ++k)
+        if (threadIdx.x + k * bd < Un) pf[k] = fr_ops<false, CONSTRAINED>(pr, threadIdx.x + k * bd, Un);
+    __syncthreads();
+    for (int t = 0; t < Tn; ++t) {
+        const float *prev = buf(t);
+        float *cur = buf(t + 1);
+        const float2 *row = pr + (int64_t)t * U;
+        auto step = [&](int u, const FrOps &o) {
+            const float skip = prev[u] + o.b;
+            bool e = false;
+            float v = skip;
+            if (u > 0) {
+                const float emit = prev[u - 1] + (CONSTRAINED ? o.l + o.b : o.l);
+                e = emit > skip || isnan(skip);
+                if (e) v = emit;
+            }
+            cur[u] = v;
+            return e;
+        };
+        // u0: the warp's first column (warp-uniform), below Un
+        auto store = [&](int u0, bool e) {
+            const unsigned word = __ballot_sync(0xffffffffu, e);
+            if (lane == 0) dec[(int64_t)(u0 >> 5) * a.T + t] = word;
+        };
+#pragma unroll
+        for (int k = 0; k < kFramesPrefetch; ++k) {
+            const int u = threadIdx.x + k * bd;
+            if (u - lane < Un) {
+                bool e = false;
+                if (u < Un) {
+                    const FrOps o = pf[k];
+                    if (t + 1 < Tn) pf[k] = fr_ops<false, CONSTRAINED>(row + U, u, Un);
+                    e = step(u, o);
+                }
+                store(u - lane, e);
+            }
+        }
+        for (int u0 = threadIdx.x - lane + kFramesPrefetch * bd; u0 < Un; u0 += bd) {
+            const int u = u0 + lane;
+            store(u0, u < Un && step(u, fr_ops<false, CONSTRAINED>(row, u, Un)));
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x >= 32) return;
+    const float score = buf(Tn)[Un - 1];
+    const bool live = score > -INFINITY;            // -inf: no path above -inf; NaN: every path NaN
+    for (int u = (live ? Un - 1 : 0) + lane; u < U - 1; u += 32) fr[u] = -1;
+    if (lane == 0) a.scores[n] = score;
+    if (!live) return;
+    // Backtrace over chunks of 32 frames: lane k holds the words of frame s_hi - k of column blocks w (cur) and w - 1
+    // (left); ul is the column inside block w, negative once the walk has entered block w - 1.  Lane k keeps its
+    // step's column and bit and writes that label's frame after the chunk.  Frames below 0 read as zero words.
+    auto ld = [&](int blk, int s) -> uint32_t {
+        return (blk >= 0 && s - lane >= 0) ? dec[(int64_t)blk * a.T + s - lane] : 0u;
+    };
+    int u = Un - 1, s_hi = Tn - 1, w = u >> 5;
+    uint32_t cur = ld(w, s_hi), left = ld(w - 1, s_hi);
+    while (true) {
+        const int s_next = s_hi - 32;
+        const uint32_t ncur = ld(w, s_next), nleft = ld(w - 1, s_next);
+        int ul = u - 32 * w, my_u = 0, my_b = 0;
+#pragma unroll
+        for (int k = 0; k < 32; ++k) {
+            const uint32_t wc = __shfl_sync(0xffffffffu, cur, k), wl = __shfl_sync(0xffffffffu, left, k);
+            const int b = (int)(((ul >= 0 ? wc : wl) >> (ul & 31)) & 1u);
+            if (lane == k) { my_u = 32 * w + ul; my_b = b; }
+            ul -= b;
+        }
+        if (my_b) fr[my_u - 1] = s_hi - lane;       // label edge (t, my_u - 1) -> (t + 1, my_u)
+        u = 32 * w + ul;
+        if (s_next < 0) break;
+        s_hi = s_next;
+        if (ul < 0) {                               // entered block w - 1: its words are the prefetched left ones
+            --w;
+            cur = nleft;
+            left = ld(w - 1, s_hi);
+        } else {
+            cur = ncur;
+            left = nleft;
+        }
+    }
+}
+
 // occupation of the label edge out of (t,u), u < Un-1: exp(alpha + l' + beta(t+1,u+1) - ll), with beta(Tn,Un-1) = 0
 // and no edge into (Tn, u+1 < Un-1)
 template <bool CONSTRAINED>
@@ -304,6 +425,38 @@ cudaError_t launch_frames(cudaStream_t s, const FramesCall &c, bool delayed) {
     memset(t_frames_record, 0, sizeof(t_frames_record));
     t_frames_record[RNNT_FRAMES_REC_DELAY] = delayed;
     return c.constrained ? launch_frames_c<true>(s, c) : launch_frames_c<false>(s, c);
+}
+
+static thread_local int32_t t_frames_align_record[RNNT_FRAMES_ALIGN_RECORD_LEN];
+static thread_local int32_t t_frames_align_seq;
+void frames_align_launch_record(int32_t *out) {
+    memcpy(out, t_frames_align_record, sizeof(t_frames_align_record));
+}
+
+template <bool C>
+static cudaError_t launch_frames_align_c(cudaStream_t s, const FramesAlignCall &c) {
+    static std::atomic<bool> attr_done[kMaxDevices];
+    const cudaError_t e = ensure_dyn_smem(k_frames_align<C>, attr_done, (int)frames_smem_bytes(kFramesMaxU));
+    if (e != cudaSuccess) return e;
+    const int threads = min(kFramesMaxThreads, max(32, (c.U + 31) / 32 * 32));
+    const size_t smem = frames_smem_bytes(c.U);
+    FramesAlignArgs a = {c.pairs, c.xn, c.yn, c.dec, c.scores, c.frames, c.T, c.U};
+    k_frames_align<C><<<c.N, threads, smem, s>>>(a);
+    count_launch();
+    int32_t *rec = t_frames_align_record;
+    memset(rec, 0, sizeof(t_frames_align_record));
+    rec[RNNT_FRAMES_ALIGN_REC_SEQ] = ++t_frames_align_seq;
+    rec[RNNT_FRAMES_ALIGN_REC_CONSTRAINED] = C;
+    rec[RNNT_FRAMES_ALIGN_REC_THREADS] = threads;
+    rec[RNNT_FRAMES_ALIGN_REC_PASSES] = (c.U + threads - 1) / threads;
+    rec[RNNT_FRAMES_ALIGN_REC_SMEM] = (int32_t)smem;
+    rec[RNNT_FRAMES_ALIGN_REC_BLOCKS] = (c.U + 31) / 32;
+    rec[RNNT_FRAMES_ALIGN_REC_DELAY] = c.delayed;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_frames_align(cudaStream_t s, const FramesAlignCall &c) {
+    return c.constrained ? launch_frames_align_c<true>(s, c) : launch_frames_align_c<false>(s, c);
 }
 
 }  // namespace rnnt

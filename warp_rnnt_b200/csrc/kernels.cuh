@@ -146,6 +146,22 @@ cudaError_t launch_delay_pairs(cudaStream_t s, const float2 *pairs_in, float2 *p
 // k_frames then, with pair_grads, k_frames_grads; `delayed` is recorded (the call ran launch_delay_pairs first)
 cudaError_t launch_frames(cudaStream_t s, const FramesCall &c, bool delayed);
 void frames_launch_record(int32_t *out);  // copy of the last k_frames launch's record (rnntFramesLaunchRecord_t)
+// Viterbi alignment on the modified / constrained lattice (k_frames_align): pairs -> decision words dec
+// (N, ceil(U/32), T), scores (N) and frames (N, U-1)
+struct FramesAlignCall {
+    const float2 *pairs;                  // (N,T,U,2) (blank, label) log-probs, penalised already when `delayed`
+    const int *xn, *yn;
+    uint32_t *dec;                        // workspace: frames_align_words(N, T, U) words
+    float *scores;
+    int *frames;
+    int N, T, U;
+    bool constrained, delayed;            // `delayed` is only recorded
+};
+inline size_t frames_align_words(int N, int T, int U) {
+    return (size_t)max(N, 0) * (size_t)((max(U, 0) + 31) / 32) * (size_t)max(T, 0);
+}
+cudaError_t launch_frames_align(cudaStream_t s, const FramesAlignCall &c);
+void frames_align_launch_record(int32_t *out);   // copy of the last k_frames_align launch's record
 
 // joint.cu -- compact packing of the joint network's input (caller side of compact=True)
 cudaError_t launch_joint_pack(cudaStream_t s, const float *f, const float *g, const int *lf, const int *lg,
