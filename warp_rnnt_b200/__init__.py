@@ -142,49 +142,54 @@ class RNNTLossFromLogits(torch.autograd.Function):
     benchmark.py:65): seven dense passes over (N,T,U,V) per step.  Here forward reads the logits once (per-cell
     normaliser + the two log-probs the recurrence needs) and keeps a (N,T,U,2) gradient; backward reads them once more
     and writes d loss / d LOGITS, applying log_softmax's backward on the fly: three dense passes.  float32 or bfloat16
-    logits; the gradient has the logits' dtype, costs are float32."""
+    logits; the gradient has the logits' dtype, costs are float32.  ``hat``: the HAT normalisation in place of
+    log_softmax (``rnnt_loss_from_logits(use_hat_loss=True)``)."""
 
     @staticmethod
     def forward(ctx, logits, labels, frames_lengths, labels_lengths, blank=0, fastemit_lambda=0.0, rnnt_type=0,
-                delay_penalty=0.0):
+                delay_penalty=0.0, hat=False):
         need = ctx.needs_input_grad[0]
         costs, lse, pg = _C.rnnt_logits_forward(logits, labels, frames_lengths, labels_lengths, blank,
-                                                fastemit_lambda, need, 0, rnnt_type, delay_penalty)
+                                                fastemit_lambda, need, 0, rnnt_type, delay_penalty, hat)
         if need:
             ctx.save_for_backward(logits, lse, pg, labels)
             ctx.blank = blank
+            ctx.hat = hat
         return costs
 
     @staticmethod
     def backward(ctx, grads_output):
         logits, lse, pg, labels = ctx.saved_tensors
         go = grads_output.contiguous().to(torch.float32)
-        return _C.rnnt_logits_backward(logits, lse, pg, labels, go, ctx.blank), None, None, None, None, None, None, None
+        g = _C.rnnt_logits_backward(logits, lse, pg, labels, go, ctx.blank, ctx.hat)
+        return g, None, None, None, None, None, None, None, None
 
 
 class RNNTLossFromLogitsCompact(torch.autograd.Function):
     """``RNNTLossFromLogits`` on compact (STU,V) logits in ``joint_pack``'s row order: a packed joint network feeds
     the fused loss without padding.  Forward keeps lse (4 bytes per row), the (STU,2) pair gradients (8 bytes per row)
     and the compact prefix sums (16 bytes per lattice); backward writes d loss / d logits, of the logits' dtype.  Inside
-    ``compact_hints`` the forward has no host sync (CUDA-graph capturable), as ``rnnt_loss(compact=True)``."""
+    ``compact_hints`` the forward has no host sync (CUDA-graph capturable), as ``rnnt_loss(compact=True)``.  ``hat``:
+    the HAT normalisation in place of log_softmax."""
 
     @staticmethod
-    def forward(ctx, logits, labels, frames_lengths, labels_lengths, blank=0, fastemit_lambda=0.0):
+    def forward(ctx, logits, labels, frames_lengths, labels_lengths, blank=0, fastemit_lambda=0.0, hat=False):
         need = ctx.needs_input_grad[0]
         hints = _hints()
         costs, lse, pg, prefix = _C.rnnt_logits_compact_forward(logits, labels, frames_lengths, labels_lengths, blank,
-                                                                fastemit_lambda, need, 0, hints[0], hints[1])
+                                                                fastemit_lambda, need, 0, hints[0], hints[1], hat)
         if need:
             ctx.save_for_backward(logits, lse, pg, labels, frames_lengths, labels_lengths, prefix)
             ctx.blank = blank
+            ctx.hat = hat
         return costs
 
     @staticmethod
     def backward(ctx, grads_output):
         logits, lse, pg, labels, xn, yn, prefix = ctx.saved_tensors
         go = grads_output.contiguous().to(torch.float32)
-        g = _C.rnnt_logits_compact_backward(logits, lse, pg, labels, xn, yn, prefix, go, ctx.blank)
-        return g, None, None, None, None, None
+        g = _C.rnnt_logits_compact_backward(logits, lse, pg, labels, xn, yn, prefix, go, ctx.blank, ctx.hat)
+        return g, None, None, None, None, None, None
 
 
 def _reduce(costs, frames_lengths, average_frames, reduction):
@@ -217,8 +222,19 @@ def _path_type(fn, rnnt_type, delay_penalty, fastemit_lambda=0.0, compact=False)
     return _RNNT_TYPES[rnnt_type], float(delay_penalty)
 
 
+def _use_hat(fn, use_hat_loss, logits):
+    """k2's ``use_hat_loss`` checked on the host: a bool, and V >= 2 when set (the labels need a column besides the
+    blank); ValueError otherwise."""
+    if not isinstance(use_hat_loss, bool):
+        raise ValueError("%s: use_hat_loss must be a bool, got %r" % (fn, use_hat_loss))
+    if use_hat_loss and logits.dim() > 0 and logits.size(-1) < 2:
+        raise ValueError("%s: use_hat_loss=True needs V >= 2, got V = %d" % (fn, logits.size(-1)))
+    return use_hat_loss
+
+
 def rnnt_loss_from_logits(logits, labels, frames_lengths, labels_lengths, average_frames=False, reduction="none",
-                          blank=0, fastemit_lambda=0.0, compact=False, rnnt_type="regular", delay_penalty=0.0):
+                          blank=0, fastemit_lambda=0.0, compact=False, rnnt_type="regular", delay_penalty=0.0,
+                          use_hat_loss=False):
     """``rnnt_loss(log_softmax(logits, -1), ...)`` in three dense passes instead of seven; the gradient is w.r.t. the
     LOGITS.  Dense (N,T,U,V) layout, float32 or bfloat16 (what ``torch.autocast(dtype=torch.bfloat16)`` makes of the
     joint network's output); other arguments as in ``rnnt_loss``.  Agrees with ``torch.log_softmax`` + the reference
@@ -244,18 +260,37 @@ def rnnt_loss_from_logits(logits, labels, frames_lengths, labels_lengths, averag
     Non-regular types take no FastEmit (k2 has none); regular + penalty + FastEmit compose.  A lattice with invalid
     lengths gets cost NaN, one without a finite path +inf, one with a NaN in its live log-probs NaN, with zero, zero and
     NaN gradients; the one-symbol-per-frame types take label dimensions up to 25599 (include/rnnt_b200.h).  Bad values
-    raise ValueError before any launch.  ``rnnt_align_from_logits`` gives the best path on the same lattice."""
+    raise ValueError before any launch.  ``rnnt_align_from_logits`` gives the best path on the same lattice.
+
+    ``use_hat_loss=True`` (k2's name): the Hybrid Autoregressive Transducer's normalisation (HAT; Variani et al. 2020,
+    arXiv:2003.07705) in place of log_softmax, as k2's ``get_hat_logprobs`` (and NeMo's ``HATJoint``) factorise the
+    joint: P(blank) = sigmoid(x[blank]) and P(y | not blank) a softmax over the non-blank logits.  In float32 per row
+    x, with lse_nb the normaliser over the columns v != blank (summed as a row whose blank logit is -inf, so every
+    non-blank logit -inf gives NaN), s = log1p(exp(-|x[blank]|)):
+      - blank log-prob b = min(x[blank], 0) - s = logsigmoid(x[blank]);
+      - label log-prob l = (x[y] - lse_nb) + (min(-x[blank], 0) - s) = log_softmax_nb(x)[y] + logsigmoid(-x[blank]).
+    Everything downstream of (b, l) is unchanged: ``rnnt_type``, ``delay_penalty``, FastEmit, the classes, the compact
+    layout and the hints.  The gradient applies the HAT Jacobian to the (blank, label) gradients (gb, gl):
+    gl * ([v == y] - exp(x[v] - lse_nb)) at a non-blank column, gb * sigmoid(-x[blank]) - gl * sigmoid(x[blank]) at
+    the blank column (plus gl where the label is the blank); a row without gradient gets zeros, NaN at the non-blank
+    columns where lse_nb is NaN and at the blank column where x[blank] is NaN, as autograd of the composition gives.
+    One difference from log_softmax follows: a NaN confined to the non-blank columns of a last-column row (u = U_n - 1)
+    reaches only l, which no lattice reads there, so the cost stays finite.  Needs V >= 2 (else ValueError); a
+    ``use_hat_loss`` that is not a bool is a ValueError.  The implementation follows k2's ``get_hat_logprobs``; it was
+    not tested against k2 or NeMo."""
     assert average_frames is None or isinstance(average_frames, bool)
     assert reduction is None or reduction in ("none", "mean", "sum")
     assert isinstance(blank, int)
     assert isinstance(compact, bool)
     assert not labels.requires_grad and not frames_lengths.requires_grad and not labels_lengths.requires_grad
     kind, lam = _path_type("rnnt_loss_from_logits", rnnt_type, delay_penalty, fastemit_lambda, compact)
+    hat = _use_hat("rnnt_loss_from_logits", use_hat_loss, logits)
     if compact:
-        costs = RNNTLossFromLogitsCompact.apply(logits, labels, frames_lengths, labels_lengths, blank, fastemit_lambda)
+        costs = RNNTLossFromLogitsCompact.apply(logits, labels, frames_lengths, labels_lengths, blank, fastemit_lambda,
+                                                hat)
     else:
         costs = RNNTLossFromLogits.apply(logits, labels, frames_lengths, labels_lengths, blank, fastemit_lambda, kind,
-                                         lam)
+                                         lam, hat)
     return _reduce(costs, frames_lengths, average_frames, reduction)
 
 
@@ -263,29 +298,30 @@ class RNNTLossPruned(torch.autograd.Function):
     """``RNNTLossFromLogits`` on the (N,T,S,V) logits of a joint evaluated in a window of S labels per frame.  Forward
     reads the window rows once and runs the recurrence on the full (N,T,U) lattice, with the edges out of the cells
     outside the windows removed; it keeps lse (N,T,S) and the (N,T,U,2) pair gradients.  Backward writes d loss /
-    d logits (N,T,S,V), of the logits' dtype."""
+    d logits (N,T,S,V), of the logits' dtype.  ``hat``: the HAT normalisation in place of log_softmax."""
 
     @staticmethod
     def forward(ctx, logits, labels, frames_lengths, labels_lengths, ranges, blank=0, fastemit_lambda=0.0, rnnt_type=0,
-                delay_penalty=0.0):
+                delay_penalty=0.0, hat=False):
         need = ctx.needs_input_grad[0]
         costs, lse, pg = _C.rnnt_logits_pruned_forward(logits, labels, frames_lengths, labels_lengths, ranges, blank,
-                                                       fastemit_lambda, need, 0, rnnt_type, delay_penalty)
+                                                       fastemit_lambda, need, 0, rnnt_type, delay_penalty, hat)
         if need:
             ctx.save_for_backward(logits, lse, pg, labels, ranges)
             ctx.blank = blank
+            ctx.hat = hat
         return costs
 
     @staticmethod
     def backward(ctx, grads_output):
         logits, lse, pg, labels, ranges = ctx.saved_tensors
         go = grads_output.contiguous().to(torch.float32)
-        g = _C.rnnt_logits_pruned_backward(logits, lse, pg, labels, ranges, go, ctx.blank)
-        return g, None, None, None, None, None, None, None, None
+        g = _C.rnnt_logits_pruned_backward(logits, lse, pg, labels, ranges, go, ctx.blank, ctx.hat)
+        return g, None, None, None, None, None, None, None, None, None
 
 
 def rnnt_loss_pruned(logits, labels, frames_lengths, labels_lengths, ranges, average_frames=False, reduction="none",
-                     blank=0, fastemit_lambda=0.0, rnnt_type="regular", delay_penalty=0.0):
+                     blank=0, fastemit_lambda=0.0, rnnt_type="regular", delay_penalty=0.0, use_hat_loss=False):
     """Pruned RNN-T loss: the transducer loss from a joint network evaluated only in a window of S label columns per
     frame, which takes about U/S times less memory and traffic than the full (N,T,U,V) joint output.
 
@@ -298,6 +334,9 @@ def rnnt_loss_pruned(logits, labels, frames_lengths, labels_lengths, ranges, ave
         rnnt_type, delay_penalty: k2's, as in ``rnnt_loss_from_logits``, on the full lattice with the edges out of the
             cells outside the windows removed.  A constrained label edge also reads the blank of the cell it
             reaches, so it is removed when that cell lies outside its frame's window.
+        use_hat_loss: k2's flag, as in ``rnnt_loss_from_logits``: the HAT normalisation of each window row in place of
+            log_softmax (lse then holds the non-blank normaliser).  A HAT pipeline takes its ``ranges`` from the
+            regular ``rnnt_loss_simple``, which is unchanged.
 
     Row (n, t, s) of ``logits`` is lattice cell (t, u = ranges[n, t] + s) when t < frames_lengths[n] and
     0 <= u <= labels_lengths[n]; any other row is padding.  Frame t's window is {u : r <= u < r + S} clipped to the
@@ -319,8 +358,9 @@ def rnnt_loss_pruned(logits, labels, frames_lengths, labels_lengths, ranges, ave
     assert not labels.requires_grad and not frames_lengths.requires_grad and not labels_lengths.requires_grad
     assert not ranges.requires_grad
     kind, lam = _path_type("rnnt_loss_pruned", rnnt_type, delay_penalty, fastemit_lambda)
+    hat = _use_hat("rnnt_loss_pruned", use_hat_loss, logits)
     costs = RNNTLossPruned.apply(logits, labels, frames_lengths, labels_lengths, ranges, blank, fastemit_lambda, kind,
-                                 lam)
+                                 lam, hat)
     return _reduce(costs, frames_lengths, average_frames, reduction)
 
 
@@ -907,7 +947,7 @@ def rnnt_align(log_probs, labels, frames_lengths, labels_lengths, blank=0, compa
 
 
 def rnnt_align_from_logits(logits, labels, frames_lengths, labels_lengths, blank=0, compact=False,
-                           rnnt_type="regular", delay_penalty=0.0):
+                           rnnt_type="regular", delay_penalty=0.0, use_hat_loss=False):
     """Viterbi forced alignment straight from joint logits, on the lattice of ``rnnt_loss_from_logits`` with the same
     ``rnnt_type`` and ``delay_penalty``: the single best path of each lattice and the frame of each label, without the
     dense ``log_softmax`` tensor that ``rnnt_align`` needs.  For the one-symbol-per-frame types this is the alignment
@@ -935,16 +975,21 @@ def rnnt_align_from_logits(logits, labels, frames_lengths, labels_lengths, blank
     invalid lengths (compact: also outside ``compact_hints``) get NaN, all with frames -1.  Deterministic; no host
     synchronisation in the dense layout and, inside ``compact_hints``, in the compact one (CUDA-graph capturable).
     bfloat16 results equal those of the float32 call on the widened logits, and compact results equal those of the
-    dense call on the same rows placed in a padded tensor.  Bad values raise ValueError before any launch."""
+    dense call on the same rows placed in a padded tensor.  Bad values raise ValueError before any launch.
+
+    ``use_hat_loss=True``: the edge weights are the HAT pairs (b, l) of ``rnnt_loss_from_logits(use_hat_loss=True)``,
+    bit for bit the loss's, with everything above unchanged (``"regular"`` then equals ``rnnt_align`` on those pairs).
+    Needs V >= 2.  The implementation follows k2's ``get_hat_logprobs``; it was not tested against k2 or NeMo."""
     assert isinstance(blank, int)
     assert isinstance(compact, bool)
     kind, lam = _path_type("rnnt_align_from_logits", rnnt_type, delay_penalty, 0.0, compact)
+    hat = _use_hat("rnnt_align_from_logits", use_hat_loss, logits)
     with torch.no_grad():
         if compact:
             hints = _hints()
             return _C.rnnt_align_logits_compact(logits, labels, frames_lengths, labels_lengths, blank, hints[0],
-                                                hints[1])
-        return _C.rnnt_align_logits_dense(logits, labels, frames_lengths, labels_lengths, blank, kind, lam)
+                                                hints[1], hat)
+        return _C.rnnt_align_logits_dense(logits, labels, frames_lengths, labels_lengths, blank, kind, lam, hat)
 
 
 def rnnt_align_tdt(logits, labels, frames_lengths, labels_lengths, durations, sigma=0.0, blank=0, compact=False):

@@ -506,14 +506,22 @@ static int loss_dense_any(void *stream, void *workspace, size_t workspace_bytes,
     return run_loss((cudaStream_t)stream, workspace, workspace_bytes, c);
 }
 
+// the HAT normalisation needs a label column besides the blank
+static bool hat_ok(int hat, int V) { return !hat || V >= 2; }
+
+// a 4-byte (f32) or 2-byte (bf16) element size, and p aligned to it
+static bool elem_ok(const void *p, int elem_bytes) {
+    return (elem_bytes == 4 || elem_bytes == 2) && !(reinterpret_cast<uintptr_t>(p) & (uintptr_t)(elem_bytes - 1));
+}
+
 // loss from logits of 4-byte (f32) or 2-byte (bf16) elements: the normaliser pass reads them, the recurrence and
-// everything after it run on the f32 (cells,2) pairs and do not see the element type
+// everything after it run on the f32 (cells,2) pairs and do not see the element type (nor the normalisation: hat)
 static int logits_forward_any(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
                               const int *labels, const int *xn, const int *yn, float *costs, float *lse,
                               float *pair_grads, int N, int T, int U, int V, int blank, float fastemit_lambda,
-                              int lse_mode, int io_bf16, int rnnt_type, float delay_penalty) {
+                              int lse_mode, int io_bf16, int rnnt_type, float delay_penalty, int hat = 0) {
     if (!dense_args_ok(N, T, U, V, blank) || !lse || !pairs_aligned(pair_grads) ||
-        !path_type_ok(rnnt_type, delay_penalty, fastemit_lambda, U))
+        !path_type_ok(rnnt_type, delay_penalty, fastemit_lambda, U) || !hat_ok(hat, V))
         return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
     cudaStream_t s = (cudaStream_t)stream;
@@ -521,18 +529,20 @@ static int logits_forward_any(void *stream, void *workspace, size_t workspace_by
     Workspace w;
     if (!carve_ok(workspace, workspace_bytes, c.cells, N, &w)) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
     // one pass over the logits: normaliser per cell + the two normalised log-probs the recurrence needs
-    RNNT_TRY(launch_lse_pairs(s, logits, labels, N, T, U, V, blank, w.pairs, lse, io_bf16), RNNT_STATUS_GATHER_FAILED);
+    RNNT_TRY(launch_lse_pairs(s, logits, labels, N, T, U, V, blank, w.pairs, lse, io_bf16, hat),
+             RNNT_STATUS_GATHER_FAILED);
     c.pairs = w.pairs; c.pair_grads = reinterpret_cast<float2 *>(pair_grads);
     return run_typed(s, workspace, workspace_bytes, w, c, rnnt_type, delay_penalty, nullptr);
 }
 
 static int logits_backward_any(void *stream, const void *logits, const float *lse, const float *pair_grads,
                                const int *labels, const float *grad_out, void *out, int N, int T, int U, int V,
-                               int blank, int io_bf16) {
-    if (!dense_args_ok(N, T, U, V, blank) || !pairs_aligned(pair_grads)) return RNNT_STATUS_INVALID_ARGUMENT;
+                               int blank, int io_bf16, int hat = 0) {
+    if (!dense_args_ok(N, T, U, V, blank) || !pairs_aligned(pair_grads) || !hat_ok(hat, V))
+        return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
     RNNT_TRY(launch_expand_logits((cudaStream_t)stream, logits, lse, reinterpret_cast<const float2 *>(pair_grads), labels,
-                                  grad_out, out, N, T, U, V, blank, io_bf16),
+                                  grad_out, out, N, T, U, V, blank, io_bf16, hat),
              RNNT_STATUS_GRADS_BLANK_FAILED);
     return RNNT_STATUS_SUCCESS;
 }
@@ -543,8 +553,8 @@ static int logits_compact_forward_any(void *stream, void *workspace, size_t work
                                       const int *ys, const int *xn, const int *yn, float *costs, float *lse,
                                       float *pair_grads, int64_t *prefix, int *totals, int64_t STU, int N, int V,
                                       int blank, float fastemit_lambda, int lse_mode, int max_T, int max_U,
-                                      int io_bf16) {
-    if (!compact_args_ok(N, STU, V, blank) || !lse || !prefix || !pairs_aligned(pair_grads))
+                                      int io_bf16, int hat = 0) {
+    if (!compact_args_ok(N, STU, V, blank) || !lse || !prefix || !pairs_aligned(pair_grads) || !hat_ok(hat, V))
         return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0) return RNNT_STATUS_SUCCESS;
     cudaStream_t s = (cudaStream_t)stream;
@@ -552,7 +562,8 @@ static int logits_compact_forward_any(void *stream, void *workspace, size_t work
     if (!carve_ok(workspace, workspace_bytes, STU, N, &w)) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
     RNNT_TRY(launch_prefix(s, xn, yn, N, prefix, prefix + N, totals ? totals : w.totals), RNNT_STATUS_GATHER_FAILED);
     LossCall c = compact_call(xn, yn, prefix, prefix + N, N, STU, max_T, max_U, costs, fastemit_lambda, lse_mode);
-    RNNT_TRY(launch_lse_pairs_compact(s, logits, c.p, ys, STU, V, blank, w.pairs, lse, io_bf16), RNNT_STATUS_GATHER_FAILED);
+    RNNT_TRY(launch_lse_pairs_compact(s, logits, c.p, ys, STU, V, blank, w.pairs, lse, io_bf16, hat),
+             RNNT_STATUS_GATHER_FAILED);
     c.pairs = w.pairs; c.pair_grads = reinterpret_cast<float2 *>(pair_grads);
     return run_loss(s, workspace, workspace_bytes, c);
 }
@@ -566,6 +577,7 @@ struct AlignCall {
     const void *lp;
     const int *labels;
     int V, blank, io_bf16;
+    int hat;                     // alignment from logits: the HAT normalisation instead of log_softmax
     float *scores;
     int *frames;
 };
@@ -631,10 +643,11 @@ static int run_align_logits(cudaStream_t s, void *workspace, size_t workspace_by
         RNNT_TRY(launch_prefix(s, c.p.xn, c.p.yn, c.p.N, w.mem_pref, w.lab_pref, w.totals), RNNT_STATUS_GATHER_FAILED);
         c.p.mem_pref = w.mem_pref;
         c.p.lab_pref = w.lab_pref;
-        RNNT_TRY(launch_lse_pairs_compact(s, c.lp, c.p, c.labels, c.cells, c.V, c.blank, w.pairs, lse, c.io_bf16),
+        RNNT_TRY(launch_lse_pairs_compact(s, c.lp, c.p, c.labels, c.cells, c.V, c.blank, w.pairs, lse, c.io_bf16,
+                                          c.hat),
                  RNNT_STATUS_GATHER_FAILED);
     } else {
-        RNNT_TRY(launch_lse_pairs(s, c.lp, c.labels, c.p.N, c.T, c.U, c.V, c.blank, w.pairs, lse, c.io_bf16),
+        RNNT_TRY(launch_lse_pairs(s, c.lp, c.labels, c.p.N, c.T, c.U, c.V, c.blank, w.pairs, lse, c.io_bf16, c.hat),
                  RNNT_STATUS_GATHER_FAILED);
     }
     if (delay_penalty != 0.0f)
@@ -651,16 +664,86 @@ static int run_align_logits(cudaStream_t s, void *workspace, size_t workspace_by
     return RNNT_STATUS_SUCCESS;
 }
 
+// the alignment from dense (N,T,U,V) logits of 4- or 2-byte elements (hat: the HAT normalisation)
+static int align_logits_dense_any(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                  const int *labels, const int *xn, const int *yn, float *scores, int *frames, int N,
+                                  int T, int U, int V, int blank, int elem_bytes, int rnnt_type, float delay_penalty,
+                                  int hat) {
+    if (!elem_ok(logits, elem_bytes) || !dense_args_ok(N, T, U, V, blank) || !hat_ok(hat, V) ||
+        !path_type_ok(rnnt_type, delay_penalty, 0.0f, U) || !scores || !frames || !workspace_aligned16(workspace))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    AlignCall c = {};
+    c.p = {xn, yn, nullptr, nullptr, N, T, U, 0};
+    c.T = T; c.U = U; c.cells = (int64_t)N * T * U;
+    c.lp = logits; c.labels = labels; c.V = V; c.blank = blank; c.io_bf16 = elem_bytes == 2; c.hat = hat;
+    c.scores = scores; c.frames = frames;
+    return run_align_logits((cudaStream_t)stream, workspace, workspace_bytes, c, rnnt_type, delay_penalty);
+}
+
+// ... and from compact (STU,V) logits in joint_pack's row order (regular lattice, no penalty)
+static int align_logits_compact_any(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                    const int *labels, const int *xn, const int *yn, float *scores, int *frames,
+                                    int64_t STU, int N, int V, int blank, int elem_bytes, int max_T, int max_U,
+                                    int hat) {
+    if (!elem_ok(logits, elem_bytes) || !compact_args_ok(N, STU, V, blank) || !hat_ok(hat, V) || max_T <= 0 ||
+        max_U <= 0 || !scores || !frames || !workspace_aligned16(workspace))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    AlignCall c = {};
+    c.p = {xn, yn, nullptr, nullptr, N, 0, 0, 1};
+    c.T = max_T; c.U = max_U; c.cells = STU;
+    c.lp = logits; c.labels = labels; c.V = V; c.blank = blank; c.io_bf16 = elem_bytes == 2; c.hat = hat;
+    c.scores = scores; c.frames = frames;
+    return run_align_logits((cudaStream_t)stream, workspace, workspace_bytes, c, 0, 0.0f);
+}
+
 static int logits_compact_backward_any(void *stream, const void *logits, const float *lse, const float *pair_grads,
                                        const int *ys, const int *xn, const int *yn, const int64_t *prefix,
                                        const float *grad_out, void *out, int64_t STU, int N, int V, int blank,
-                                       int io_bf16) {
-    if (!compact_args_ok(N, STU, V, blank) || !lse || !prefix || !pairs_aligned(pair_grads))
+                                       int io_bf16, int hat = 0) {
+    if (!compact_args_ok(N, STU, V, blank) || !lse || !prefix || !pairs_aligned(pair_grads) || !hat_ok(hat, V))
         return RNNT_STATUS_INVALID_ARGUMENT;
     if (N == 0 || STU == 0) return RNNT_STATUS_SUCCESS;
     const Problem p = {xn, yn, prefix, prefix + N, N, 0, 0, 1};
     RNNT_TRY(launch_expand_logits_compact((cudaStream_t)stream, logits, lse, reinterpret_cast<const float2 *>(pair_grads),
-                                          p, ys, grad_out, out, STU, V, blank, io_bf16),
+                                          p, ys, grad_out, out, STU, V, blank, io_bf16, hat),
+             RNNT_STATUS_GRADS_BLANK_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+// rnnt_loss_pruned's (N,T,S,V) window rows of 4- or 2-byte elements on the full (N,T,U) lattice
+static int logits_pruned_forward_any(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                     const int *labels, const int *xn, const int *yn, const int *ranges, float *costs,
+                                     float *lse, float *pair_grads, int N, int T, int S, int U, int V,
+                                     int blank, float fastemit_lambda, int lse_mode, int elem_bytes, int rnnt_type,
+                                     float delay_penalty, int hat) {
+    if (!elem_ok(logits, elem_bytes) || !pruned_args_ok(N, T, S, U, V, blank) || !lse || !pairs_aligned(pair_grads) ||
+        !workspace_aligned16(workspace) || !path_type_ok(rnnt_type, delay_penalty, fastemit_lambda, U) ||
+        !hat_ok(hat, V))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    cudaStream_t s = (cudaStream_t)stream;
+    LossCall c = dense_call(xn, yn, N, T, U, costs, fastemit_lambda, lse_mode);
+    Workspace w;
+    if (!carve_ok(workspace, workspace_bytes, c.cells, N, &w)) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    // one pass over the window rows: their normalisers, and the full lattice's pairs ((kBig, kBig) off the windows)
+    RNNT_TRY(launch_lse_pairs_pruned(s, logits, labels, ranges, N, T, S, U, V, blank, w.pairs, lse, elem_bytes == 2,
+                                     hat),
+             RNNT_STATUS_GATHER_FAILED);
+    c.pairs = w.pairs; c.pair_grads = reinterpret_cast<float2 *>(pair_grads);
+    return run_typed(s, workspace, workspace_bytes, w, c, rnnt_type, delay_penalty, nullptr);
+}
+
+static int logits_pruned_backward_any(void *stream, const void *logits, const float *lse, const float *pair_grads,
+                                      const int *labels, const int *ranges, const float *grad_out, void *out, int N,
+                                      int T, int S, int U, int V, int blank, int elem_bytes, int hat) {
+    if (!elem_ok(logits, elem_bytes) || !elem_ok(out, elem_bytes) || !pruned_args_ok(N, T, S, U, V, blank) ||
+        !pairs_aligned(pair_grads) || !hat_ok(hat, V))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    RNNT_TRY(launch_expand_logits_pruned((cudaStream_t)stream, logits, lse, reinterpret_cast<const float2 *>(pair_grads),
+                                         labels, ranges, grad_out, out, N, T, S, U, V, blank, elem_bytes == 2, hat),
              RNNT_STATUS_GRADS_BLANK_FAILED);
     return RNNT_STATUS_SUCCESS;
 }
@@ -1000,34 +1083,72 @@ int rnnt_b200_logits_pruned_forward_ex(void *stream, void *workspace, size_t wor
                                        float *costs, float *lse, float *pair_grads, int N, int T, int S, int U, int V,
                                        int blank, float fastemit_lambda, int lse_mode, int elem_bytes, int rnnt_type,
                                        float delay_penalty) {
-    if ((elem_bytes != 4 && elem_bytes != 2) || (reinterpret_cast<uintptr_t>(logits) & (uintptr_t)(elem_bytes - 1)) ||
-        !pruned_args_ok(N, T, S, U, V, blank) || !lse || !pairs_aligned(pair_grads) ||
-        !workspace_aligned16(workspace) || !path_type_ok(rnnt_type, delay_penalty, fastemit_lambda, U))
-        return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0) return RNNT_STATUS_SUCCESS;
-    cudaStream_t s = (cudaStream_t)stream;
-    LossCall c = dense_call(xn, yn, N, T, U, costs, fastemit_lambda, lse_mode);
-    Workspace w;
-    if (!carve_ok(workspace, workspace_bytes, c.cells, N, &w)) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
-    // one pass over the window rows: their normalisers, and the full lattice's pairs ((kBig, kBig) off the windows)
-    RNNT_TRY(launch_lse_pairs_pruned(s, logits, labels, ranges, N, T, S, U, V, blank, w.pairs, lse, elem_bytes == 2),
-             RNNT_STATUS_GATHER_FAILED);
-    c.pairs = w.pairs; c.pair_grads = reinterpret_cast<float2 *>(pair_grads);
-    return run_typed(s, workspace, workspace_bytes, w, c, rnnt_type, delay_penalty, nullptr);
+    return logits_pruned_forward_any(stream, workspace, workspace_bytes, logits, labels, xn, yn, ranges, costs, lse,
+                                     pair_grads, N, T, S, U, V, blank, fastemit_lambda, lse_mode, elem_bytes,
+                                     rnnt_type, delay_penalty, 0);
 }
 
 int rnnt_b200_logits_pruned_backward(void *stream, const void *logits, const float *lse, const float *pair_grads,
                                      const int *labels, const int *ranges, const float *grad_out, void *out, int N,
                                      int T, int S, int U, int V, int blank, int elem_bytes) {
-    if ((elem_bytes != 4 && elem_bytes != 2) ||
-        ((reinterpret_cast<uintptr_t>(logits) | reinterpret_cast<uintptr_t>(out)) & (uintptr_t)(elem_bytes - 1)) ||
-        !pruned_args_ok(N, T, S, U, V, blank) || !pairs_aligned(pair_grads))
-        return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0) return RNNT_STATUS_SUCCESS;
-    RNNT_TRY(launch_expand_logits_pruned((cudaStream_t)stream, logits, lse, reinterpret_cast<const float2 *>(pair_grads),
-                                         labels, ranges, grad_out, out, N, T, S, U, V, blank, elem_bytes == 2),
-             RNNT_STATUS_GRADS_BLANK_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    return logits_pruned_backward_any(stream, logits, lse, pair_grads, labels, ranges, grad_out, out, N, T, S, U, V,
+                                      blank, elem_bytes, 0);
+}
+
+// HAT twins of the from-logits entries: the same drivers and workspaces, the HAT normalisation in the logits passes
+
+int rnnt_b200_logits_hat_forward(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                 const int *labels, const int *xn, const int *yn, float *costs, float *lse,
+                                 float *pair_grads, int N, int T, int U, int V, int blank, float fastemit_lambda,
+                                 int lse_mode, int elem_bytes, int rnnt_type, float delay_penalty) {
+    if (!elem_ok(logits, elem_bytes)) return RNNT_STATUS_INVALID_ARGUMENT;
+    return logits_forward_any(stream, workspace, workspace_bytes, logits, labels, xn, yn, costs, lse, pair_grads, N, T,
+                              U, V, blank, fastemit_lambda, lse_mode, elem_bytes == 2, rnnt_type, delay_penalty, 1);
+}
+
+int rnnt_b200_logits_hat_backward(void *stream, const void *logits, const float *lse, const float *pair_grads,
+                                  const int *labels, const float *grad_out, void *out, int N, int T, int U, int V,
+                                  int blank, int elem_bytes) {
+    if (!elem_ok(logits, elem_bytes) || !elem_ok(out, elem_bytes)) return RNNT_STATUS_INVALID_ARGUMENT;
+    return logits_backward_any(stream, logits, lse, pair_grads, labels, grad_out, out, N, T, U, V, blank,
+                               elem_bytes == 2, 1);
+}
+
+int rnnt_b200_logits_compact_hat_forward(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                         const int *ys, const int *xn, const int *yn, float *costs, float *lse,
+                                         float *pair_grads, int64_t *prefix, int *totals, int64_t STU, int N, int V,
+                                         int blank, float fastemit_lambda, int lse_mode, int max_T, int max_U,
+                                         int elem_bytes) {
+    if (!elem_ok(logits, elem_bytes)) return RNNT_STATUS_INVALID_ARGUMENT;
+    return logits_compact_forward_any(stream, workspace, workspace_bytes, logits, ys, xn, yn, costs, lse, pair_grads,
+                                      prefix, totals, STU, N, V, blank, fastemit_lambda, lse_mode, max_T, max_U,
+                                      elem_bytes == 2, 1);
+}
+
+int rnnt_b200_logits_compact_hat_backward(void *stream, const void *logits, const float *lse, const float *pair_grads,
+                                          const int *ys, const int *xn, const int *yn, const int64_t *prefix,
+                                          const float *grad_out, void *out, int64_t STU, int N, int V, int blank,
+                                          int elem_bytes) {
+    if (!elem_ok(logits, elem_bytes) || !elem_ok(out, elem_bytes)) return RNNT_STATUS_INVALID_ARGUMENT;
+    return logits_compact_backward_any(stream, logits, lse, pair_grads, ys, xn, yn, prefix, grad_out, out, STU, N, V,
+                                       blank, elem_bytes == 2, 1);
+}
+
+int rnnt_b200_logits_pruned_hat_forward(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                        const int *labels, const int *xn, const int *yn, const int *ranges,
+                                        float *costs, float *lse, float *pair_grads, int N, int T, int S, int U, int V,
+                                        int blank, float fastemit_lambda, int lse_mode, int elem_bytes, int rnnt_type,
+                                        float delay_penalty) {
+    return logits_pruned_forward_any(stream, workspace, workspace_bytes, logits, labels, xn, yn, ranges, costs, lse,
+                                     pair_grads, N, T, S, U, V, blank, fastemit_lambda, lse_mode, elem_bytes,
+                                     rnnt_type, delay_penalty, 1);
+}
+
+int rnnt_b200_logits_pruned_hat_backward(void *stream, const void *logits, const float *lse, const float *pair_grads,
+                                         const int *labels, const int *ranges, const float *grad_out, void *out, int N,
+                                         int T, int S, int U, int V, int blank, int elem_bytes) {
+    return logits_pruned_backward_any(stream, logits, lse, pair_grads, labels, ranges, grad_out, out, N, T, S, U, V,
+                                      blank, elem_bytes, 1);
 }
 
 size_t rnnt_b200_tdt_workspace_bytes(int N, int T, int U, int num_durations) {
@@ -1485,33 +1606,30 @@ size_t rnnt_b200_align_logits_workspace_bytes(int64_t cells, int N, int T, int U
 int rnnt_b200_align_logits_dense(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
                                  const int *labels, const int *xn, const int *yn, float *scores, int *frames, int N,
                                  int T, int U, int V, int blank, int elem_bytes, int rnnt_type, float delay_penalty) {
-    if ((elem_bytes != 4 && elem_bytes != 2) || !dense_args_ok(N, T, U, V, blank) ||
-        (reinterpret_cast<uintptr_t>(logits) & (uintptr_t)(elem_bytes - 1)) ||
-        !path_type_ok(rnnt_type, delay_penalty, 0.0f, U) || !scores || !frames || !workspace_aligned16(workspace))
-        return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0) return RNNT_STATUS_SUCCESS;
-    AlignCall c = {};
-    c.p = {xn, yn, nullptr, nullptr, N, T, U, 0};
-    c.T = T; c.U = U; c.cells = (int64_t)N * T * U;
-    c.lp = logits; c.labels = labels; c.V = V; c.blank = blank; c.io_bf16 = elem_bytes == 2;
-    c.scores = scores; c.frames = frames;
-    return run_align_logits((cudaStream_t)stream, workspace, workspace_bytes, c, rnnt_type, delay_penalty);
+    return align_logits_dense_any(stream, workspace, workspace_bytes, logits, labels, xn, yn, scores, frames, N, T, U,
+                                  V, blank, elem_bytes, rnnt_type, delay_penalty, 0);
 }
 
 int rnnt_b200_align_logits_compact(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
                                    const int *labels, const int *xn, const int *yn, float *scores, int *frames,
                                    int64_t STU, int N, int V, int blank, int elem_bytes, int max_T, int max_U) {
-    if ((elem_bytes != 4 && elem_bytes != 2) || !compact_args_ok(N, STU, V, blank) || max_T <= 0 || max_U <= 0 ||
-        (reinterpret_cast<uintptr_t>(logits) & (uintptr_t)(elem_bytes - 1)) || !scores || !frames ||
-        !workspace_aligned16(workspace))
-        return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0) return RNNT_STATUS_SUCCESS;
-    AlignCall c = {};
-    c.p = {xn, yn, nullptr, nullptr, N, 0, 0, 1};
-    c.T = max_T; c.U = max_U; c.cells = STU;
-    c.lp = logits; c.labels = labels; c.V = V; c.blank = blank; c.io_bf16 = elem_bytes == 2;
-    c.scores = scores; c.frames = frames;
-    return run_align_logits((cudaStream_t)stream, workspace, workspace_bytes, c, 0, 0.0f);
+    return align_logits_compact_any(stream, workspace, workspace_bytes, logits, labels, xn, yn, scores, frames, STU, N,
+                                    V, blank, elem_bytes, max_T, max_U, 0);
+}
+
+int rnnt_b200_align_logits_hat_dense(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                     const int *labels, const int *xn, const int *yn, float *scores, int *frames,
+                                     int N, int T, int U, int V, int blank, int elem_bytes, int rnnt_type,
+                                     float delay_penalty) {
+    return align_logits_dense_any(stream, workspace, workspace_bytes, logits, labels, xn, yn, scores, frames, N, T, U,
+                                  V, blank, elem_bytes, rnnt_type, delay_penalty, 1);
+}
+
+int rnnt_b200_align_logits_hat_compact(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
+                                       const int *labels, const int *xn, const int *yn, float *scores, int *frames,
+                                       int64_t STU, int N, int V, int blank, int elem_bytes, int max_T, int max_U) {
+    return align_logits_compact_any(stream, workspace, workspace_bytes, logits, labels, xn, yn, scores, frames, STU, N,
+                                    V, blank, elem_bytes, max_T, max_U, 1);
 }
 
 int rnnt_b200_compact_totals(void *stream, const int *xn, const int *yn, int N, int64_t *scratch, int *totals) {

@@ -80,6 +80,9 @@ const T *optional_arg(const c10::optional<at::Tensor> &t, Dt dt, const at::Tenso
 }
 
 void check_blank(int blank, int64_t V) { TORCH_CHECK(blank >= 0 && blank < V, "blank must be in [0, V)"); }
+// the HAT normalisation (hat = true) needs a label column besides the blank
+void check_hat(bool hat, int64_t V) { TORCH_CHECK(!hat || V >= 2, "hat needs V >= 2"); }
+int elem_bytes(const at::Tensor &xs) { return xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4; }
 
 void check4(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
             bool allow_bf16 = false) {
@@ -366,9 +369,11 @@ std::tuple<at::Tensor, at::Tensor> rnnt_gather_forward(const at::Tensor &xs, con
 std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_logits_forward(const at::Tensor &xs, const at::Tensor &ys,
                                                                    const at::Tensor &xn, const at::Tensor &yn,
                                                                    int blank, float fastemit_lambda, bool want_grads,
-                                                                   int lse_mode, int rnnt_type, double delay_penalty) {
+                                                                   int lse_mode, int rnnt_type, double delay_penalty,
+                                                                   bool hat) {
     const auto [N, T, U, V, bf16, guard] = dense_front(xs, ys, xn, yn, true);
     check_blank(blank, V);
+    check_hat(hat, V);
     const auto f32 = xs.options().dtype(at::kFloat);
     at::Tensor costs = at::empty({N}, f32);
     at::Tensor lse = at::empty({N, T, U}, f32);
@@ -376,7 +381,13 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_logits_forward(const at::Ten
     if (N == 0) return std::make_tuple(costs, lse, pg);
     at::Tensor ws = workspace(xs, rnnt_b200_workspace_bytes(N * T * U, (int)N));
     float *pgp = want_grads ? pg.data_ptr<float>() : nullptr;
-    if (bf16)
+    if (hat)
+        check_status(rnnt_b200_logits_hat_forward(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
+                                                  ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
+                                                  costs.data_ptr<float>(), lse.data_ptr<float>(), pgp, (int)N, (int)T,
+                                                  (int)U, (int)V, blank, fastemit_lambda, lse_mode, bf16 ? 2 : 4,
+                                                  rnnt_type, (float)delay_penalty));
+    else if (bf16)
         check_status(rnnt_b200_logits_forward_bf16_ex(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(),
                                                       xs.data_ptr(), ys.data_ptr<int>(), xn.data_ptr<int>(),
                                                       yn.data_ptr<int>(), costs.data_ptr<float>(), lse.data_ptr<float>(),
@@ -393,7 +404,7 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_logits_forward(const at::Ten
 
 // d loss / d logits, of the dtype of xs (float32 or bfloat16)
 at::Tensor rnnt_logits_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &pair_grads,
-                                const at::Tensor &ys, const at::Tensor &grad_out, int blank) {
+                                const at::Tensor &ys, const at::Tensor &grad_out, int blank, bool hat) {
     check_arg(xs, Dt::F32orBF16, xs, {kAny, kAny, kAny, kAny},
               "xs must be a contiguous CUDA Float tensor of shape (N, T, U, V)");
     const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), V = xs.size(3);
@@ -403,9 +414,15 @@ at::Tensor rnnt_logits_backward(const at::Tensor &xs, const at::Tensor &lse, con
     check_arg(ys, Dt::I32, xs, {N, U - 1}, "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
     check_arg(grad_out, Dt::F32, xs, N, "grad_out must be a contiguous Float tensor of shape (N,)");
     check_blank(blank, V);
+    check_hat(hat, V);
     const c10::cuda::CUDAGuard guard(xs.device());
     at::Tensor out = at::empty_like(xs);
-    if (xs.scalar_type() == at::ScalarType::BFloat16)
+    if (hat)
+        check_status(rnnt_b200_logits_hat_backward(current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(),
+                                                   pair_grads.data_ptr<float>(), ys.data_ptr<int>(),
+                                                   grad_out.data_ptr<float>(), out.data_ptr(), (int)N, (int)T, (int)U,
+                                                   (int)V, blank, elem_bytes(xs)));
+    else if (xs.scalar_type() == at::ScalarType::BFloat16)
         check_status(rnnt_b200_logits_backward_bf16(current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(),
                                                     pair_grads.data_ptr<float>(), ys.data_ptr<int>(),
                                                     grad_out.data_ptr<float>(), out.data_ptr(), (int)N, (int)T, (int)U,
@@ -422,8 +439,10 @@ at::Tensor rnnt_logits_backward(const at::Tensor &xs, const at::Tensor &lse, con
 // rnnt_loss_compact: one 16-byte device->host copy, or none with hints (max_T, max_U > 0).
 std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor>
 rnnt_logits_compact_forward(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
-                            int blank, float fastemit_lambda, bool want_grads, int lse_mode, int max_T, int max_U) {
+                            int blank, float fastemit_lambda, bool want_grads, int lse_mode, int max_T, int max_U,
+                            bool hat) {
     const auto [N, STU, V, bf16, guard] = compact_front(xs, ys, xn, yn, blank, true);
+    check_hat(hat, V);
     void *stream = current_stream(xs);
     const auto f32 = xs.options().dtype(at::kFloat);
     at::Tensor costs = at::empty({N}, f32);
@@ -434,7 +453,12 @@ rnnt_logits_compact_forward(const at::Tensor &xs, const at::Tensor &ys, const at
     std::tie(max_T, max_U) = compact_bounds(stream, xs, ys, xn, yn, max_T, max_U, prefix.data_ptr<int64_t>());
     at::Tensor ws = workspace(xs, rnnt_b200_workspace_bytes(STU, (int)N));
     float *pgp = want_grads ? pg.data_ptr<float>() : nullptr;
-    if (bf16)
+    if (hat)
+        check_status(rnnt_b200_logits_compact_hat_forward(
+            stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(), ys.data_ptr<int>(), xn.data_ptr<int>(),
+            yn.data_ptr<int>(), costs.data_ptr<float>(), lse.data_ptr<float>(), pgp, prefix.data_ptr<int64_t>(), nullptr,
+            STU, (int)N, (int)V, blank, fastemit_lambda, lse_mode, max_T, max_U, bf16 ? 2 : 4));
+    else if (bf16)
         check_status(rnnt_b200_logits_compact_forward_bf16(
             stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(), ys.data_ptr<int>(), xn.data_ptr<int>(),
             yn.data_ptr<int>(), costs.data_ptr<float>(), lse.data_ptr<float>(), pgp, prefix.data_ptr<int64_t>(), nullptr,
@@ -450,7 +474,7 @@ rnnt_logits_compact_forward(const at::Tensor &xs, const at::Tensor &ys, const at
 // d loss / d compact logits, of the dtype of xs
 at::Tensor rnnt_logits_compact_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &pair_grads,
                                         const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
-                                        const at::Tensor &prefix, const at::Tensor &grad_out, int blank) {
+                                        const at::Tensor &prefix, const at::Tensor &grad_out, int blank, bool hat) {
     check_arg(xs, Dt::F32orBF16, xs, {kAny, kAny}, "xs must be a contiguous CUDA Float tensor of shape (STU, V)");
     const int64_t STU = xs.size(0), V = xs.size(1), N = xn.numel();
     check_arg(lse, Dt::F32, xs, STU, "lse must be a contiguous Float tensor of shape (STU,) on the device of xs");
@@ -463,10 +487,16 @@ at::Tensor rnnt_logits_compact_backward(const at::Tensor &xs, const at::Tensor &
     check_arg(prefix, Dt::I64, xs, 2 * N, "prefix must be a contiguous Long tensor of shape (2N,) on the device of xs");
     check_arg(grad_out, Dt::F32, xs, N, "grad_out must be a contiguous Float tensor of shape (N,)");
     check_blank(blank, V);
+    check_hat(hat, V);
     const c10::cuda::CUDAGuard guard(xs.device());
     at::Tensor out = at::empty_like(xs);
     if (N == 0 || STU == 0) return out;                 // empty tensors: nothing to write (and no data pointers)
-    if (xs.scalar_type() == at::ScalarType::BFloat16)
+    if (hat)
+        check_status(rnnt_b200_logits_compact_hat_backward(
+            current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(), pair_grads.data_ptr<float>(), ys.data_ptr<int>(),
+            xn.data_ptr<int>(), yn.data_ptr<int>(), prefix.data_ptr<int64_t>(), grad_out.data_ptr<float>(),
+            out.data_ptr(), STU, (int)N, (int)V, blank, elem_bytes(xs)));
+    else if (xs.scalar_type() == at::ScalarType::BFloat16)
         check_status(rnnt_b200_logits_compact_backward_bf16(
             current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(), pair_grads.data_ptr<float>(), ys.data_ptr<int>(),
             xn.data_ptr<int>(), yn.data_ptr<int>(), prefix.data_ptr<int64_t>(), grad_out.data_ptr<float>(),
@@ -486,13 +516,14 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_logits_pruned_forward(const 
                                                                           const at::Tensor &ranges, int blank,
                                                                           float fastemit_lambda, bool want_grads,
                                                                           int lse_mode, int rnnt_type,
-                                                                          double delay_penalty) {
+                                                                          double delay_penalty, bool hat) {
     check4(xs, ys, xn, yn, true);
     check_batch4(xs, xn, yn);
     TORCH_CHECK(ys.dim() == 2 && ys.size(0) == xs.size(0), "ys shape must be (N, U-1)");
     const int64_t N = xs.size(0), T = xs.size(1), S = xs.size(2), V = xs.size(3), U = ys.size(1) + 1;
     check_arg(ranges, Dt::I32, xs, {N, T}, "ranges must be a contiguous Int tensor of shape (N, T) on the device of xs");
     check_blank(blank, V);
+    check_hat(hat, V);
     const c10::cuda::CUDAGuard guard(xs.device());
     const auto f32 = xs.options().dtype(at::kFloat);
     at::Tensor costs = at::empty({N}, f32);
@@ -500,7 +531,8 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_logits_pruned_forward(const 
     at::Tensor pg = output(want_grads, {N, T, U, 2}, f32);
     if (N == 0) return std::make_tuple(costs, lse, pg);
     at::Tensor ws = workspace(xs, rnnt_b200_workspace_bytes(N * T * U, (int)N));
-    check_status(rnnt_b200_logits_pruned_forward_ex(
+    const auto forward = hat ? rnnt_b200_logits_pruned_hat_forward : rnnt_b200_logits_pruned_forward_ex;
+    check_status(forward(
         current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(), ys.data_ptr<int>(), xn.data_ptr<int>(),
         yn.data_ptr<int>(), ranges.data_ptr<int>(), costs.data_ptr<float>(), lse.data_ptr<float>(),
         want_grads ? pg.data_ptr<float>() : nullptr, (int)N, (int)T, (int)S, (int)U, (int)V, blank, fastemit_lambda,
@@ -511,7 +543,7 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_logits_pruned_forward(const 
 // d loss / d pruned logits (N,T,S,V), of the dtype of xs
 at::Tensor rnnt_logits_pruned_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &pair_grads,
                                        const at::Tensor &ys, const at::Tensor &ranges, const at::Tensor &grad_out,
-                                       int blank) {
+                                       int blank, bool hat) {
     check_arg(xs, Dt::F32orBF16, xs, {kAny, kAny, kAny, kAny},
               "xs must be a contiguous CUDA Float tensor of shape (N, T, S, V)");
     const int64_t N = xs.size(0), T = xs.size(1), S = xs.size(2), V = xs.size(3);
@@ -523,14 +555,15 @@ at::Tensor rnnt_logits_pruned_backward(const at::Tensor &xs, const at::Tensor &l
     check_arg(ranges, Dt::I32, xs, {N, T}, "ranges must be a contiguous Int tensor of shape (N, T) on the device of xs");
     check_arg(grad_out, Dt::F32, xs, N, "grad_out must be a contiguous Float tensor of shape (N,)");
     check_blank(blank, V);
+    check_hat(hat, V);
     const c10::cuda::CUDAGuard guard(xs.device());
     at::Tensor out = at::empty_like(xs);
     if (N == 0) return out;
-    check_status(rnnt_b200_logits_pruned_backward(current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(),
-                                                  pair_grads.data_ptr<float>(), ys.data_ptr<int>(),
-                                                  ranges.data_ptr<int>(), grad_out.data_ptr<float>(), out.data_ptr(),
-                                                  (int)N, (int)T, (int)S, (int)U, (int)V, blank,
-                                                  xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
+    const auto backward = hat ? rnnt_b200_logits_pruned_hat_backward : rnnt_b200_logits_pruned_backward;
+    check_status(backward(current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(), pair_grads.data_ptr<float>(),
+                          ys.data_ptr<int>(), ranges.data_ptr<int>(), grad_out.data_ptr<float>(), out.data_ptr(),
+                          (int)N, (int)T, (int)S, (int)U, (int)V, blank,
+                          xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
     return out;
 }
 
@@ -1108,17 +1141,18 @@ std::tuple<at::Tensor, at::Tensor> rnnt_align_compact(const at::Tensor &xs, cons
 // (scores (N) f32, frames (N,U-1) i32).  No host sync.
 std::tuple<at::Tensor, at::Tensor> rnnt_align_logits_dense(const at::Tensor &xs, const at::Tensor &ys,
                                                            const at::Tensor &xn, const at::Tensor &yn, int blank,
-                                                           int rnnt_type, double delay_penalty) {
+                                                           int rnnt_type, double delay_penalty, bool hat) {
     const auto [N, T, U, V, bf16, guard] = dense_front(xs, ys, xn, yn, true);
     check_blank(blank, V);
+    check_hat(hat, V);
     at::Tensor scores = at::empty({N}, xs.options().dtype(at::kFloat));
     at::Tensor frames = label_slots(N * (U - 1), xs).view({N, U - 1});
     if (N == 0) return std::make_tuple(scores, frames);
     at::Tensor ws = workspace(xs, rnnt_b200_align_logits_workspace_bytes(N * T * U, (int)N, (int)T, (int)U));
-    check_status(rnnt_b200_align_logits_dense(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
-                                              ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
-                                              scores.data_ptr<float>(), frames.data_ptr<int>(), (int)N, (int)T, (int)U,
-                                              (int)V, blank, bf16 ? 2 : 4, rnnt_type, (float)delay_penalty));
+    const auto align = hat ? rnnt_b200_align_logits_hat_dense : rnnt_b200_align_logits_dense;
+    check_status(align(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(), ys.data_ptr<int>(),
+                       xn.data_ptr<int>(), yn.data_ptr<int>(), scores.data_ptr<float>(), frames.data_ptr<int>(),
+                       (int)N, (int)T, (int)U, (int)V, blank, bf16 ? 2 : 4, rnnt_type, (float)delay_penalty));
     return std::make_tuple(scores, frames);
 }
 
@@ -1126,8 +1160,9 @@ std::tuple<at::Tensor, at::Tensor> rnnt_align_logits_dense(const at::Tensor &xs,
 // f32, frames (sum yn) i32).  The bounds are the hints when given (no host sync), else one 16-byte device->host copy.
 std::tuple<at::Tensor, at::Tensor> rnnt_align_logits_compact(const at::Tensor &xs, const at::Tensor &ys,
                                                              const at::Tensor &xn, const at::Tensor &yn, int blank,
-                                                             int max_T, int max_U) {
+                                                             int max_T, int max_U, bool hat) {
     const auto [N, STU, V, bf16, guard] = compact_front(xs, ys, xn, yn, blank, true);
+    check_hat(hat, V);
     void *stream = current_stream(xs);
     at::Tensor scores = at::empty({N}, xs.options().dtype(at::kFloat));
     at::Tensor frames = label_slots(ys.numel(), xs);
@@ -1136,10 +1171,10 @@ std::tuple<at::Tensor, at::Tensor> rnnt_align_logits_compact(const at::Tensor &x
     max_T = std::max(max_T, 1);              // lengths of 0 or less: the lattice is outside any bounds (score NaN)
     max_U = std::max(max_U, 1);
     at::Tensor ws = workspace(xs, rnnt_b200_align_logits_workspace_bytes(STU, (int)N, max_T, max_U));
-    check_status(rnnt_b200_align_logits_compact(stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
-                                                ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
-                                                scores.data_ptr<float>(), frames.data_ptr<int>(), STU, (int)N, (int)V,
-                                                blank, bf16 ? 2 : 4, max_T, max_U));
+    const auto align = hat ? rnnt_b200_align_logits_hat_compact : rnnt_b200_align_logits_compact;
+    check_status(align(stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(), ys.data_ptr<int>(), xn.data_ptr<int>(),
+                       yn.data_ptr<int>(), scores.data_ptr<float>(), frames.data_ptr<int>(), STU, (int)N, (int)V,
+                       blank, bf16 ? 2 : 4, max_T, max_U));
     return std::make_tuple(scores, frames);
 }
 
@@ -1164,21 +1199,22 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("rnnt_rescale_", &rnnt_rescale_, py::arg("grads"), py::arg("grad_out"), py::arg("applied") = py::none());
     m.def("rnnt_logits_forward", &rnnt_logits_forward, py::arg("xs"), py::arg("ys"), py::arg("xn"), py::arg("yn"),
           py::arg("blank") = 0, py::arg("fastemit_lambda") = 0.0, py::arg("want_grads") = true, py::arg("lse_mode") = 0,
-          py::arg("rnnt_type") = 0, py::arg("delay_penalty") = 0.0);
+          py::arg("rnnt_type") = 0, py::arg("delay_penalty") = 0.0, py::arg("hat") = false);
     m.def("rnnt_logits_backward", &rnnt_logits_backward, py::arg("xs"), py::arg("lse"), py::arg("pair_grads"),
-          py::arg("ys"), py::arg("grad_out"), py::arg("blank") = 0);
+          py::arg("ys"), py::arg("grad_out"), py::arg("blank") = 0, py::arg("hat") = false);
     m.def("rnnt_logits_compact_forward", &rnnt_logits_compact_forward, py::arg("xs"), py::arg("ys"), py::arg("xn"),
           py::arg("yn"), py::arg("blank") = 0, py::arg("fastemit_lambda") = 0.0, py::arg("want_grads") = true,
-          py::arg("lse_mode") = 0, py::arg("max_T") = 0, py::arg("max_U") = 0);
+          py::arg("lse_mode") = 0, py::arg("max_T") = 0, py::arg("max_U") = 0, py::arg("hat") = false);
     m.def("rnnt_logits_compact_backward", &rnnt_logits_compact_backward, py::arg("xs"), py::arg("lse"),
           py::arg("pair_grads"), py::arg("ys"), py::arg("xn"), py::arg("yn"), py::arg("prefix"), py::arg("grad_out"),
-          py::arg("blank") = 0);
+          py::arg("blank") = 0, py::arg("hat") = false);
     m.def("rnnt_logits_pruned_forward", &rnnt_logits_pruned_forward, py::arg("xs"), py::arg("ys"), py::arg("xn"),
           py::arg("yn"), py::arg("ranges"), py::arg("blank") = 0, py::arg("fastemit_lambda") = 0.0,
           py::arg("want_grads") = true, py::arg("lse_mode") = 0, py::arg("rnnt_type") = 0,
-          py::arg("delay_penalty") = 0.0);
+          py::arg("delay_penalty") = 0.0, py::arg("hat") = false);
     m.def("rnnt_logits_pruned_backward", &rnnt_logits_pruned_backward, py::arg("xs"), py::arg("lse"),
-          py::arg("pair_grads"), py::arg("ys"), py::arg("ranges"), py::arg("grad_out"), py::arg("blank") = 0);
+          py::arg("pair_grads"), py::arg("ys"), py::arg("ranges"), py::arg("grad_out"), py::arg("blank") = 0,
+          py::arg("hat") = false);
     m.def("rnnt_tdt_forward", &rnnt_tdt_forward, py::arg("xs"), py::arg("ys"), py::arg("xn"), py::arg("yn"),
           py::arg("durations"), py::arg("sigma") = 0.0, py::arg("blank") = 0, py::arg("want_grads") = true);
     m.def("rnnt_tdt_backward", &rnnt_tdt_backward, py::arg("xs"), py::arg("lse"), py::arg("grads"), py::arg("ys"),
@@ -1237,10 +1273,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("max_U") = 0);
     m.def("rnnt_align_logits_dense", &rnnt_align_logits_dense,
           "Viterbi forced alignment from logits on k2's lattices, dense layout.", py::arg("xs"), py::arg("ys"),
-          py::arg("xn"), py::arg("yn"), py::arg("blank") = 0, py::arg("rnnt_type") = 0, py::arg("delay_penalty") = 0.0);
+          py::arg("xn"), py::arg("yn"), py::arg("blank") = 0, py::arg("rnnt_type") = 0, py::arg("delay_penalty") = 0.0,
+          py::arg("hat") = false);
     m.def("rnnt_align_logits_compact", &rnnt_align_logits_compact,
           "Viterbi forced alignment from logits, compact layout.", py::arg("xs"), py::arg("ys"), py::arg("xn"),
-          py::arg("yn"), py::arg("blank") = 0, py::arg("max_T") = 0, py::arg("max_U") = 0);
+          py::arg("yn"), py::arg("blank") = 0, py::arg("max_T") = 0, py::arg("max_U") = 0, py::arg("hat") = false);
     m.def("set_lse_mode", [](int mode) { rnnt_b200_set_lse_mode(mode); }, py::arg("mode"));
     m.def("get_lse_mode", []() { return rnnt_b200_get_lse_mode(); });
     m.def("launch_count", []() { return rnnt_b200_launch_count(); });

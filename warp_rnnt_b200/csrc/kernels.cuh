@@ -63,26 +63,27 @@ cudaError_t launch_expand(cudaStream_t s, const Problem &p, const ExpandSrc &src
 
 // logits.cu -- loss from un-normalised logits (fused log_softmax forward / backward).  io_bf16: the logits (and the
 // gradient written by launch_expand_logits) are bf16, else float; lse, pairs, pg and grad_out are float either way.
+// hat: the HAT normalisation (logits.cu) in the k_*_hat kernels instead of log_softmax.
 cudaError_t launch_lse_pairs(cudaStream_t s, const void *x, const int *labels, int N, int T, int U, int V, int blank,
-                             float2 *pairs, float *lse, int io_bf16);
+                             float2 *pairs, float *lse, int io_bf16, int hat);
 cudaError_t launch_expand_logits(cudaStream_t s, const void *x, const float *lse, const float2 *pg, const int *labels,
                                  const float *grad_out, void *out, int N, int T, int U, int V, int blank,
-                                 int io_bf16);
+                                 int io_bf16, int hat);
 // ... the same two passes over compact (STU,V) logits in joint_pack's row order: p is the compact Problem (prefix sums
 // on the device), labels (sum yn), grad_out (N) or nullptr
 cudaError_t launch_lse_pairs_compact(cudaStream_t s, const void *x, const Problem &p, const int *labels, int64_t STU,
-                                     int V, int blank, float2 *pairs, float *lse, int io_bf16);
+                                     int V, int blank, float2 *pairs, float *lse, int io_bf16, int hat);
 cudaError_t launch_expand_logits_compact(cudaStream_t s, const void *x, const float *lse, const float2 *pg,
                                          const Problem &p, const int *labels, const float *grad_out, void *out,
-                                         int64_t STU, int V, int blank, int io_bf16);
+                                         int64_t STU, int V, int blank, int io_bf16, int hat);
 // ... and over rnnt_loss_pruned's (N,T,S,V) window rows: row (n,t,s) is cell (t, ranges[n,t] + s) of the full (N,T,U)
 // lattice.  The forward writes lse (N,T,S) and the full (N,T,U,2) pairs: every cell (kBig, kBig), then each window
 // row's pair at its cell (u in [0, U)); the backward writes (N,T,S,V) from the full (N,T,U,2) pair gradients.
 cudaError_t launch_lse_pairs_pruned(cudaStream_t s, const void *x, const int *labels, const int *ranges, int N, int T,
-                                    int S, int U, int V, int blank, float2 *pairs, float *lse, int io_bf16);
+                                    int S, int U, int V, int blank, float2 *pairs, float *lse, int io_bf16, int hat);
 cudaError_t launch_expand_logits_pruned(cudaStream_t s, const void *x, const float *lse, const float2 *pg,
                                         const int *labels, const int *ranges, const float *grad_out, void *out, int N,
-                                        int T, int S, int U, int V, int blank, int io_bf16);
+                                        int T, int S, int U, int V, int blank, int io_bf16, int hat);
 
 // simple.cu -- the simple (factorised-joint) loss: am (N,T,V) + lm (N,U,V), and the prune ranges of its lattice
 struct SimpleArgs {

@@ -21,6 +21,14 @@
 // float row of the same V (same SUB, same lanes, same groups of 4 -- a bf16 group is one 8-byte load where a float
 // group is a float4), so lse and pairs are bit for bit those of the float path on the widened logits; k_expand_logits
 // computes every element as the float kernel does and rounds it to bf16 once, on the store.
+//
+// HAT (the Hybrid Autoregressive Transducer's normalisation, k2's get_hat_logprobs): the same passes with a second
+// normalisation, a template flag on the row bodies, instantiated as kernels of their own (k_*_hat) so the softmax
+// kernels stay exactly as they are.  The blank is a sigmoid and the labels a softmax over the non-blank columns:
+//   lse   = lse_nb, the normaliser of the row with column B excluded by index (summed as a row whose x[B] is -inf)
+//   pairs = (logsigmoid(x[B]), x[y] - lse_nb + logsigmoid(-x[B])), logsigmoid(z) = min(z, 0) - log1p(exp(-|z|))
+//   grad  = gl ([v == y] - exp(x[v] - lse_nb)) at v != B, gb sigmoid(-x[B]) - gl sigmoid(x[B]) (+ gl if y == B) at B
+// and a row with pair gradients (0, 0) gets zeros, NaN at v != B when lse_nb is NaN and at B when x[B] is NaN.
 #include "common.cuh"
 #include "kernels.cuh"
 
@@ -51,7 +59,24 @@ __device__ __forceinline__ float4 ld_group4(const __nv_bfloat16 *row, int q) {
 // (kBig, kBig) before.  Again only the mapping differs: a row is summed exactly as the dense row of its values.
 enum { kRowsDense = 0, kRowsCompact = 1, kRowsPruned = 2 };
 
-template <typename IN, int SUB, bool VEC4, int ROWS>
+// HAT: group q of a row with its element at column `blank` (if any) set to -inf, as the sums read it
+__device__ __forceinline__ float4 hat_group4(float4 a, int q, int blank) {
+    const int k = blank - 4 * q;
+    a.x = k == 0 ? -INFINITY : a.x;
+    a.y = k == 1 ? -INFINITY : a.y;
+    a.z = k == 2 ? -INFINITY : a.z;
+    a.w = k == 3 ? -INFINITY : a.w;
+    return a;
+}
+
+// HAT: the (blank, label) log-probs of a row from its non-blank normaliser l, in the order include/rnnt_b200.h states
+template <typename IN>
+__device__ __forceinline__ float2 hat_pair(const IN *row, int blank, int lab, float l) {
+    const float xb = io_load(row + blank), sp = log1pf(expf(-fabsf(xb)));
+    return make_float2(fminf(xb, 0.0f) - sp, (io_load(row + lab) - l) + (fminf(-xb, 0.0f) - sp));
+}
+
+template <typename IN, int SUB, bool VEC4, int ROWS, bool HAT = false>
 __device__ __forceinline__ void
 lse_pairs_rows(const IN *__restrict__ x, const int *__restrict__ labels, int64_t cells, int V, int blank, int U,
                FastDiv divU, FastDiv divTU, float2 *__restrict__ pairs, float *__restrict__ lse_out, Problem lay,
@@ -82,13 +107,34 @@ lse_pairs_rows(const IN *__restrict__ x, const int *__restrict__ labels, int64_t
             // the whole row is one group per lane: max first (shuffles only), then ONE exp per element -- the online
             // merge below would spend two more exp per lane and shuffle round
             const bool has = sub < (V >> 2);
-            const float4 a = has ? ld_group4(row, sub) : make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
-            m = fmaxf(fmaxf(a.x, a.y), fmaxf(a.z, a.w));
+            if constexpr (HAT) {
+                // (the softmax branch below with the blank masked; kept apart so that branch compiles as it did)
+                const float4 a = hat_group4(
+                    has ? ld_group4(row, sub) : make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY), sub, blank);
+                m = fmaxf(fmaxf(a.x, a.y), fmaxf(a.z, a.w));
 #pragma unroll
-            for (int o = SUB / 2; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-            s = has ? (expf(a.x - m) + expf(a.y - m)) + (expf(a.z - m) + expf(a.w - m)) : 0.0f;
+                for (int o = SUB / 2; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+                s = has ? (expf(a.x - m) + expf(a.y - m)) + (expf(a.z - m) + expf(a.w - m)) : 0.0f;
+            } else {
+                const float4 a = has ? ld_group4(row, sub) : make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
+                m = fmaxf(fmaxf(a.x, a.y), fmaxf(a.z, a.w));
+#pragma unroll
+                for (int o = SUB / 2; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+                s = has ? (expf(a.x - m) + expf(a.y - m)) + (expf(a.z - m) + expf(a.w - m)) : 0.0f;
+            }
 #pragma unroll
             for (int o = SUB / 2; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+        } else if (VEC4 && HAT) {
+            // only the group that holds the blank is masked: one lane, one iteration, the selects loop-invariant
+            const int qb = blank >> 2;
+            for (int q = sub; q < (V >> 2); q += SUB) {
+                float4 a = ld_group4(row, q);
+                if (q == qb) a = hat_group4(a, qb, blank);
+                const float mx = fmaxf(fmaxf(a.x, a.y), fmaxf(a.z, a.w));
+                if (mx > m) { s = s * expf(m - mx); m = mx; }
+                const float mo = off();
+                s += (expf(a.x - mo) + expf(a.y - mo)) + (expf(a.z - mo) + expf(a.w - mo));
+            }
         } else if (VEC4) {
             for (int q = sub; q < (V >> 2); q += SUB) {
                 const float4 a = ld_group4(row, q);
@@ -100,10 +146,15 @@ lse_pairs_rows(const IN *__restrict__ x, const int *__restrict__ labels, int64_t
         } else if (SUB == 1) {
             // short unaligned rows: one thread per cell; neighbouring threads' rows share cache lines, so the pass over
             // v is served from L1 after the first touch
-            for (int v = 0; v < V; ++v) m = fmaxf(m, io_load(row + v));
-            for (int v = 0; v < V; ++v) s += expf(io_load(row + v) - m);
+            if constexpr (HAT) {
+                for (int v = 0; v < V; ++v) m = fmaxf(m, v == blank ? -INFINITY : io_load(row + v));
+                for (int v = 0; v < V; ++v) s += expf((v == blank ? -INFINITY : io_load(row + v)) - m);
+            } else {
+                for (int v = 0; v < V; ++v) m = fmaxf(m, io_load(row + v));
+                for (int v = 0; v < V; ++v) s += expf(io_load(row + v) - m);
+            }
         } else {
-            for (int v = sub; v < V; v += SUB) add(io_load(row + v));
+            for (int v = sub; v < V; v += SUB) add(HAT && v == blank ? -INFINITY : io_load(row + v));
         }
         if (SUB > 1 && !(VEC4 && (V >> 2) <= SUB)) {
 #pragma unroll
@@ -126,7 +177,8 @@ lse_pairs_rows(const IN *__restrict__ x, const int *__restrict__ labels, int64_t
                 lse_out[cell] = l;
                 if (u >= 0 && u < U) {
                     lab = (u < U - 1) ? labels[(int64_t)n * (U - 1) + u] : blank;
-                    pairs[(int64_t)nt * U + u] = make_float2(io_load(row + blank) - l, io_load(row + lab) - l);
+                    if constexpr (HAT) pairs[(int64_t)nt * U + u] = hat_pair(row, blank, lab, l);
+                    else pairs[(int64_t)nt * U + u] = make_float2(io_load(row + blank) - l, io_load(row + lab) - l);
                 }
                 continue;
             } else if constexpr (COMPACT) {
@@ -138,7 +190,8 @@ lse_pairs_rows(const IN *__restrict__ x, const int *__restrict__ labels, int64_t
                 divU.divmod(rem, t, u);
                 lab = ((int)u < U - 1) ? labels[(int64_t)n * (U - 1) + u] : blank;
             }
-            pairs[cell] = make_float2(io_load(row + blank) - l, io_load(row + lab) - l);
+            if constexpr (HAT) pairs[cell] = hat_pair(row, blank, lab, l);
+            else pairs[cell] = make_float2(io_load(row + blank) - l, io_load(row + lab) - l);
             lse_out[cell] = l;
         }
     }
@@ -160,6 +213,15 @@ k_lse_pairs_pruned(const IN *__restrict__ x, const int *__restrict__ labels, con
                    float *__restrict__ lse_out) {
     lse_pairs_rows<IN, SUB, VEC4, kRowsPruned>(x, labels, rows, V, blank, U, divS, divT, pairs, lse_out, Problem{},
                                                ranges);
+}
+
+// the HAT twins of k_lse_pairs and k_lse_pairs_pruned (ROWS: kRowsDense, kRowsCompact or kRowsPruned)
+template <typename IN, int SUB, bool VEC4, int ROWS>
+__global__ void __launch_bounds__(kLogitThreads)
+k_lse_pairs_hat(const IN *__restrict__ x, const int *__restrict__ labels, const int *__restrict__ ranges, int64_t cells,
+                int V, int blank, int U, FastDiv divU, FastDiv divTU, float2 *__restrict__ pairs,
+                float *__restrict__ lse_out, Problem lay) {
+    lse_pairs_rows<IN, SUB, VEC4, ROWS, true>(x, labels, cells, V, blank, U, divU, divTU, pairs, lse_out, lay, ranges);
 }
 
 // every cell of the full (cells,2) pairs (kBig, kBig): an edge out of a cell that no window row covers is removed
@@ -207,7 +269,7 @@ __device__ __forceinline__ void st_logit_grads(__nv_bfloat16 *p, const float (&e
 // PRUNED: the rows are the (N,T,S,V) windows, divU divides by S and divTU by T as in k_lse_pairs; row (n,t,s) takes
 // (gb, gl) from the full (N,T,U,2) pair gradients at cell (t, u = ranges[n,t] + s), and a row with u outside [0, U) is
 // a padding row (pair gradients (0, 0)).
-template <typename IO, int VEC, int ROWS>
+template <typename IO, int VEC, int ROWS, bool HAT = false>
 __device__ __forceinline__ void
 expand_logits_rows(const IO *__restrict__ x, const float *__restrict__ lse, const float2 *__restrict__ pg,
                    const int *__restrict__ labels, const float *__restrict__ grad_out, IO *__restrict__ out,
@@ -248,6 +310,15 @@ expand_logits_rows(const IO *__restrict__ x, const float *__restrict__ lse, cons
             const float z = (lse[row] == lse[row]) ? 0.0f : NAN;
 #pragma unroll
             for (int k = 0; k < VEC; ++k) e[k] = z;
+            if constexpr (HAT) {
+                // HAT: the blank column's normaliser is its own logit (0 * sigmoid(x[B]))
+                if ((unsigned)(blank - v0) < (unsigned)VEC) {
+                    const float xb = io_load(x + f + (blank - v0));
+#pragma unroll
+                    for (int k = 0; k < VEC; ++k)
+                        if (v0 + k == blank) e[k] = (xb == xb) ? 0.0f : NAN;
+                }
+            }
         } else {
             int lab;
             float sc;
@@ -269,11 +340,28 @@ expand_logits_rows(const IO *__restrict__ x, const float *__restrict__ lse, cons
             const float l = lse[row], tot = q.x + q.y;
             float xv[VEC];
             ld_logits<VEC>(x + f, xv);
+            if constexpr (HAT) {
+                // the others: log_softmax's backward over v != B for gl; the blank (at most one per vector, computed
+                // once outside the unrolled loop): gb sigmoid(-x[B]) - gl sigmoid(x[B])
+                float eb = 0.0f;
+                if ((unsigned)(blank - v0) < (unsigned)VEC) {
+                    const float xb = io_load(x + f + (blank - v0));
+                    const float r = expf(-fabsf(xb)), big = 1.0f / (1.0f + r), small = r * big;
+                    const bool pos = xb >= 0.0f;
+                    eb = ((blank == lab ? q.y : 0.0f) + (q.x * (pos ? small : big) - q.y * (pos ? big : small))) * sc;
+                }
 #pragma unroll
-            for (int k = 0; k < VEC; ++k) {
-                float gsel = (v0 + k == blank) ? q.x : 0.0f;
-                if (v0 + k == lab) gsel += q.y;
-                e[k] = (gsel - expf(xv[k] - l) * tot) * sc;
+                for (int k = 0; k < VEC; ++k) {
+                    const float gsel = (v0 + k == lab) ? q.y : 0.0f;
+                    e[k] = (v0 + k == blank) ? eb : (gsel - expf(xv[k] - l) * q.y) * sc;
+                }
+            } else {
+#pragma unroll
+                for (int k = 0; k < VEC; ++k) {
+                    float gsel = (v0 + k == blank) ? q.x : 0.0f;
+                    if (v0 + k == lab) gsel += q.y;
+                    e[k] = (gsel - expf(xv[k] - l) * tot) * sc;
+                }
             }
         }
         st_logit_grads<VEC>(out + f, e);
@@ -302,13 +390,24 @@ k_expand_logits_pruned(const IO *__restrict__ x, const float *__restrict__ lse, 
                                              stride_rows, stride_v, Problem{}, ranges);
 }
 
+// the HAT twin of k_expand_logits and k_expand_logits_pruned (ROWS: kRowsDense, kRowsCompact or kRowsPruned)
+template <typename IO, int VEC, int ROWS>
+__global__ void __launch_bounds__(kLogitThreads)
+k_expand_logits_hat(const IO *__restrict__ x, const float *__restrict__ lse, const float2 *__restrict__ pg,
+                    const int *__restrict__ labels, const int *__restrict__ ranges, const float *__restrict__ grad_out,
+                    IO *__restrict__ out, int64_t cells, int V, int blank, int U, FastDiv divU, FastDiv divTU,
+                    int64_t stride_rows, int stride_v, Problem lay) {
+    expand_logits_rows<IO, VEC, ROWS, true>(x, lse, pg, labels, grad_out, out, cells, V, blank, U, divU, divTU,
+                                            stride_rows, stride_v, lay, ranges);
+}
+
 // compact grids: compact_gx (kernels.cuh)
 // lay == nullptr: dense (N,T,U,V) logits; else the compact (STU,V) rows of lattices lay->N, lay->T = lay->U = 0.
 // ranges != nullptr: the pruned (N,T,S,V) rows of windows ranges (N,T) on the full (N,T,U) lattice.
 template <typename IN>
 static cudaError_t lse_pairs_as(cudaStream_t s, const IN *x, const int *labels, int N, int T, int U, int V, int blank,
-                                float2 *pairs, float *lse, const Problem *lay, int64_t STU, const int *ranges = nullptr,
-                                int S = 0) {
+                                float2 *pairs, float *lse, const Problem *lay, int64_t STU, const int *ranges,
+                                int S, bool hat) {
     const int64_t cells = lay ? STU : (int64_t)N * T * (ranges ? S : U);
     if (cells <= 0 || N <= 0) return cudaSuccess;
     // pruned: the row -> (n*T + t, s) -> (n, t) divisions
@@ -328,7 +427,10 @@ static cudaError_t lse_pairs_as(cudaStream_t s, const IN *x, const int *labels, 
     const dim3 grid = lay ? dim3(compact_gx(STU, N, per_block * kCompactIters), N)
                           : dim3((unsigned)min((cells + per_block - 1) / per_block, (int64_t)sms * 16));
 #define RNNT_LSE_LAUNCH(SUB, VEC)                                                                                          \
-    (lay ? k_lse_pairs<IN, SUB, VEC, true><<<grid, kLogitThreads, 0, s>>>(x, labels, cells, V, blank, U, divU, divTU, pairs, lse, p) \
+    (hat ? (lay ? k_lse_pairs_hat<IN, SUB, VEC, kRowsCompact><<<grid, kLogitThreads, 0, s>>>(x, labels, ranges, cells, V, blank, U, divU, divTU, pairs, lse, p) \
+            : ranges ? k_lse_pairs_hat<IN, SUB, VEC, kRowsPruned><<<grid, kLogitThreads, 0, s>>>(x, labels, ranges, cells, V, blank, U, divU, divTU, pairs, lse, p) \
+                : k_lse_pairs_hat<IN, SUB, VEC, kRowsDense><<<grid, kLogitThreads, 0, s>>>(x, labels, ranges, cells, V, blank, U, divU, divTU, pairs, lse, p)) \
+     : lay ? k_lse_pairs<IN, SUB, VEC, true><<<grid, kLogitThreads, 0, s>>>(x, labels, cells, V, blank, U, divU, divTU, pairs, lse, p) \
      : ranges ? k_lse_pairs_pruned<IN, SUB, VEC><<<grid, kLogitThreads, 0, s>>>(x, labels, ranges, cells, V, blank, U, divU, divTU, pairs, lse) \
          : k_lse_pairs<IN, SUB, VEC><<<grid, kLogitThreads, 0, s>>>(x, labels, cells, V, blank, U, divU, divTU, pairs, lse, p))
     if (vec4) { if (sub == 8) RNNT_LSE_LAUNCH(8, true); else RNNT_LSE_LAUNCH(32, true); }
@@ -341,24 +443,28 @@ static cudaError_t lse_pairs_as(cudaStream_t s, const IN *x, const int *labels, 
 }
 
 cudaError_t launch_lse_pairs(cudaStream_t s, const void *x, const int *labels, int N, int T, int U, int V, int blank,
-                             float2 *pairs, float *lse, int io_bf16) {
+                             float2 *pairs, float *lse, int io_bf16, int hat) {
     if (io_bf16)
-        return lse_pairs_as(s, static_cast<const __nv_bfloat16 *>(x), labels, N, T, U, V, blank, pairs, lse, nullptr, 0);
-    return lse_pairs_as(s, static_cast<const float *>(x), labels, N, T, U, V, blank, pairs, lse, nullptr, 0);
+        return lse_pairs_as(s, static_cast<const __nv_bfloat16 *>(x), labels, N, T, U, V, blank, pairs, lse, nullptr, 0,
+                            nullptr, 0, hat);
+    return lse_pairs_as(s, static_cast<const float *>(x), labels, N, T, U, V, blank, pairs, lse, nullptr, 0, nullptr, 0,
+                        hat);
 }
 
 cudaError_t launch_lse_pairs_compact(cudaStream_t s, const void *x, const Problem &p, const int *labels, int64_t STU,
-                                     int V, int blank, float2 *pairs, float *lse, int io_bf16) {
+                                     int V, int blank, float2 *pairs, float *lse, int io_bf16, int hat) {
     if (io_bf16)
-        return lse_pairs_as(s, static_cast<const __nv_bfloat16 *>(x), labels, p.N, 0, 0, V, blank, pairs, lse, &p, STU);
-    return lse_pairs_as(s, static_cast<const float *>(x), labels, p.N, 0, 0, V, blank, pairs, lse, &p, STU);
+        return lse_pairs_as(s, static_cast<const __nv_bfloat16 *>(x), labels, p.N, 0, 0, V, blank, pairs, lse, &p, STU,
+                            nullptr, 0, hat);
+    return lse_pairs_as(s, static_cast<const float *>(x), labels, p.N, 0, 0, V, blank, pairs, lse, &p, STU, nullptr, 0,
+                        hat);
 }
 
 // lay, ranges: as for lse_pairs_as
 template <typename IO>
 static cudaError_t expand_logits_as(cudaStream_t s, const IO *x, const float *lse, const float2 *pg, const int *labels,
                                     const float *grad_out, IO *out, int N, int T, int U, int V, int blank,
-                                    const Problem *lay, int64_t STU, const int *ranges = nullptr, int S = 0) {
+                                    const Problem *lay, int64_t STU, const int *ranges, int S, bool hat) {
     const int64_t cells = lay ? STU : (int64_t)N * T * (ranges ? S : U);
     if (cells <= 0 || N <= 0) return cudaSuccess;
     const FastDiv divU((uint32_t)max(ranges ? S : U, 1)), divTU((uint32_t)max(ranges ? T : T * U, 1));
@@ -378,7 +484,10 @@ static cudaError_t expand_logits_as(cudaStream_t s, const IO *x, const float *ls
     const int64_t srows = stride / V;
     const int sv = (int)(stride - srows * V);
 #define RNNT_EXPAND_LAUNCH(VEC)                                                                                            \
-    (lay ? k_expand_logits<IO, VEC, true><<<grid, kLogitThreads, 0, s>>>(x, lse, pg, labels, grad_out, out, cells, V, blank, U, divU, divTU, srows, sv, p) \
+    (hat ? (lay ? k_expand_logits_hat<IO, VEC, kRowsCompact><<<grid, kLogitThreads, 0, s>>>(x, lse, pg, labels, ranges, grad_out, out, cells, V, blank, U, divU, divTU, srows, sv, p) \
+            : ranges ? k_expand_logits_hat<IO, VEC, kRowsPruned><<<grid, kLogitThreads, 0, s>>>(x, lse, pg, labels, ranges, grad_out, out, cells, V, blank, U, divU, divTU, srows, sv, p) \
+                : k_expand_logits_hat<IO, VEC, kRowsDense><<<grid, kLogitThreads, 0, s>>>(x, lse, pg, labels, ranges, grad_out, out, cells, V, blank, U, divU, divTU, srows, sv, p)) \
+     : lay ? k_expand_logits<IO, VEC, true><<<grid, kLogitThreads, 0, s>>>(x, lse, pg, labels, grad_out, out, cells, V, blank, U, divU, divTU, srows, sv, p) \
      : ranges ? k_expand_logits_pruned<IO, VEC><<<grid, kLogitThreads, 0, s>>>(x, lse, pg, labels, ranges, grad_out, out, cells, V, blank, U, divU, divTU, srows, sv) \
          : k_expand_logits<IO, VEC><<<grid, kLogitThreads, 0, s>>>(x, lse, pg, labels, grad_out, out, cells, V, blank, U, divU, divTU, srows, sv, p))
     if constexpr (sizeof(IO) == 2) {
@@ -397,40 +506,42 @@ static cudaError_t expand_logits_as(cudaStream_t s, const IO *x, const float *ls
 }
 
 cudaError_t launch_expand_logits(cudaStream_t s, const void *x, const float *lse, const float2 *pg, const int *labels,
-                                 const float *grad_out, void *out, int N, int T, int U, int V, int blank, int io_bf16) {
+                                 const float *grad_out, void *out, int N, int T, int U, int V, int blank, int io_bf16,
+                                 int hat) {
     if (io_bf16)
         return expand_logits_as(s, static_cast<const __nv_bfloat16 *>(x), lse, pg, labels, grad_out,
-                                static_cast<__nv_bfloat16 *>(out), N, T, U, V, blank, nullptr, 0);
+                                static_cast<__nv_bfloat16 *>(out), N, T, U, V, blank, nullptr, 0, nullptr, 0, hat);
     return expand_logits_as(s, static_cast<const float *>(x), lse, pg, labels, grad_out, static_cast<float *>(out), N, T,
-                            U, V, blank, nullptr, 0);
+                            U, V, blank, nullptr, 0, nullptr, 0, hat);
 }
 
 cudaError_t launch_expand_logits_compact(cudaStream_t s, const void *x, const float *lse, const float2 *pg,
                                          const Problem &p, const int *labels, const float *grad_out, void *out,
-                                         int64_t STU, int V, int blank, int io_bf16) {
+                                         int64_t STU, int V, int blank, int io_bf16, int hat) {
     if (io_bf16)
         return expand_logits_as(s, static_cast<const __nv_bfloat16 *>(x), lse, pg, labels, grad_out,
-                                static_cast<__nv_bfloat16 *>(out), p.N, 0, 0, V, blank, &p, STU);
+                                static_cast<__nv_bfloat16 *>(out), p.N, 0, 0, V, blank, &p, STU, nullptr, 0, hat);
     return expand_logits_as(s, static_cast<const float *>(x), lse, pg, labels, grad_out, static_cast<float *>(out), p.N,
-                            0, 0, V, blank, &p, STU);
+                            0, 0, V, blank, &p, STU, nullptr, 0, hat);
 }
 
 cudaError_t launch_lse_pairs_pruned(cudaStream_t s, const void *x, const int *labels, const int *ranges, int N, int T,
-                                    int S, int U, int V, int blank, float2 *pairs, float *lse, int io_bf16) {
+                                    int S, int U, int V, int blank, float2 *pairs, float *lse, int io_bf16, int hat) {
     if (io_bf16)
         return lse_pairs_as(s, static_cast<const __nv_bfloat16 *>(x), labels, N, T, U, V, blank, pairs, lse, nullptr, 0,
-                            ranges, S);
-    return lse_pairs_as(s, static_cast<const float *>(x), labels, N, T, U, V, blank, pairs, lse, nullptr, 0, ranges, S);
+                            ranges, S, hat);
+    return lse_pairs_as(s, static_cast<const float *>(x), labels, N, T, U, V, blank, pairs, lse, nullptr, 0, ranges, S,
+                        hat);
 }
 
 cudaError_t launch_expand_logits_pruned(cudaStream_t s, const void *x, const float *lse, const float2 *pg,
                                         const int *labels, const int *ranges, const float *grad_out, void *out, int N,
-                                        int T, int S, int U, int V, int blank, int io_bf16) {
+                                        int T, int S, int U, int V, int blank, int io_bf16, int hat) {
     if (io_bf16)
         return expand_logits_as(s, static_cast<const __nv_bfloat16 *>(x), lse, pg, labels, grad_out,
-                                static_cast<__nv_bfloat16 *>(out), N, T, U, V, blank, nullptr, 0, ranges, S);
+                                static_cast<__nv_bfloat16 *>(out), N, T, U, V, blank, nullptr, 0, ranges, S, hat);
     return expand_logits_as(s, static_cast<const float *>(x), lse, pg, labels, grad_out, static_cast<float *>(out), N, T,
-                            U, V, blank, nullptr, 0, ranges, S);
+                            U, V, blank, nullptr, 0, ranges, S, hat);
 }
 
 }  // namespace rnnt
