@@ -762,17 +762,6 @@ static bool tdt_durations(const int *durations, int D, TdtDurations *out) {
     out->dmax = durations[D - 1];
     return out->dmax > 0;
 }
-static bool tdt_args_ok(int N, int T, int U, int V, int D, int blank, int elem_bytes, const void *logits) {
-    return (elem_bytes == 4 || elem_bytes == 2) && !(reinterpret_cast<uintptr_t>(logits) & (uintptr_t)(elem_bytes - 1)) &&
-           N >= 0 && T >= 1 && U >= 1 && V >= 1 && (int64_t)V + D < ((int64_t)1 << 22) &&
-           (int64_t)N * T * U < ((int64_t)1 << 31) && blank >= 0 && blank < V;
-}
-// the compact layout: N <= 65535 (the normaliser's grid holds one CTA row per lattice), STU < 2^31 in place of N*T*U
-static bool tdt_compact_args_ok(int N, int64_t STU, int V, int D, int blank, int elem_bytes, const void *logits) {
-    return (elem_bytes == 4 || elem_bytes == 2) && !(reinterpret_cast<uintptr_t>(logits) & (uintptr_t)(elem_bytes - 1)) &&
-           N >= 0 && N <= 65535 && STU >= 0 && STU < ((int64_t)1 << 31) && V >= 1 &&
-           (int64_t)V + D < ((int64_t)1 << 22) && blank >= 0 && blank < V;
-}
 // Multi-blank: B big blanks with durations strictly increasing in [2, 16] (so B <= 15), in the durations' place
 static bool mb_durations(const int *durations, int B, TdtDurations *out) {
     if (!durations || B < 1 || B > kTdtMaxD - 2) return false;
@@ -786,12 +775,18 @@ static bool mb_durations(const int *durations, int B, TdtDurations *out) {
     out->dmax = durations[B - 1];
     return true;
 }
-// the row is V logits: the standard blank at `blank`, big blank i at blank - 1 - i, so blank in [B, V)
-static bool mb_args_ok(int N, int T, int U, int V, int B, int blank, int elem_bytes, const void *logits) {
-    return tdt_args_ok(N, T, U, V, 0, blank, elem_bytes, logits) && blank >= B;
-}
-static bool mb_compact_args_ok(int N, int64_t STU, int V, int B, int blank, int elem_bytes, const void *logits) {
-    return tdt_compact_args_ok(N, STU, V, 0, blank, elem_bytes, logits) && blank >= B;
+// The arguments every TDT or multi-blank call (mb) takes, dense or compact: the family's durations into dur, the
+// logits' element size and alignment, the row and the blank, sigma finite and >= 0, then the layout's sizes.  A TDT row
+// is V token logits then D duration logits, blank in [0, V); a multi-blank row is V logits, the standard blank at
+// `blank` and big blank i at blank - 1 - i, so blank in [B, V).  Dense: T, U >= 1 and N*T*U < 2^31; compact: STU < 2^31
+// in place of N*T*U, and N <= 65535 (the normaliser's grid holds one CTA row per lattice).
+static bool tdt_args_ok(bool mb, bool compact, const int *durations, int D, float sigma, int N, int64_t STU, int T,
+                        int U, int V, int blank, int elem_bytes, const void *logits, TdtDurations *dur) {
+    return (mb ? mb_durations(durations, D, dur) : tdt_durations(durations, D, dur)) && elem_ok(logits, elem_bytes) &&
+           V >= 1 && (int64_t)V + (mb ? 0 : D) < ((int64_t)1 << 22) && blank >= (mb ? D : 0) && blank < V &&
+           std::isfinite(sigma) && sigma >= 0.0f && N >= 0 &&
+           (compact ? N <= 65535 && STU >= 0 && STU < ((int64_t)1 << 31)
+                    : T >= 1 && U >= 1 && (int64_t)N * T * U < ((int64_t)1 << 31));
 }
 // cells: N*T*U (dense) or STU (compact); the compact call also takes 4 ints for the totals it does not return
 struct TdtWorkspace { float *lp, *alpha, *beta, *ll; int *status, *totals; size_t bytes; };
@@ -842,6 +837,90 @@ static TdtAlignWorkspace carve_tdt_align(void *base, int64_t cells, int N, int D
     w.totals = (int *)take(4 * sizeof(int));
     w.bytes = off;
     return w;
+}
+
+// The TDT and multi-blank calls (mb), dense (N,T,U) or compact (STU rows, T and U the bounds max_T, max_U).  Nothing
+// is launched before a refusal: the arguments first, then the N == 0 return, then the workspace.  The TDT lse is
+// (cells,2) (lse_tok, lse_dur) pairs, read and written as float2; the multi-blank lse is one float per cell.
+
+// the loss: the compact prefix sums into prefix (and totals, or the workspace's), then launch_tdt_forward
+static int tdt_forward_any(bool mb, bool compact, void *stream, void *workspace, size_t workspace_bytes,
+                           const void *logits, const int *labels, const int *xn, const int *yn, const int *durations,
+                           int D, float sigma, float *costs, float *lse, float *grads, int64_t *prefix, int *totals,
+                           int64_t STU, int N, int T, int U, int V, int blank, int elem_bytes) {
+    TdtDurations dur;
+    if (!tdt_args_ok(mb, compact, durations, D, sigma, N, STU, T, U, V, blank, elem_bytes, logits, &dur) || !costs ||
+        !lse || (!mb && !pairs_aligned(lse)) || !workspace_aligned16(workspace) ||
+        (compact && (!prefix || T < 1 || U < 1)))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    const TdtWorkspace w = carve_tdt(workspace, compact ? STU : (int64_t)N * T * U, N, D, compact);
+    if (!workspace || workspace_bytes < w.bytes) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    cudaStream_t s = (cudaStream_t)stream;
+    TdtFwd c = {};
+    if (compact) {
+        RNNT_TRY(launch_prefix(s, xn, yn, N, prefix, prefix + N, totals ? totals : w.totals),
+                 RNNT_STATUS_GATHER_FAILED);
+        c.mem_pref = prefix; c.lab_pref = prefix + N; c.STU = STU;
+    }
+    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = costs; c.pg = grads;
+    c.lp = w.lp; c.alpha = w.alpha; c.beta = w.beta; c.ll = w.ll; c.status = w.status;
+    c.N = N; c.T = T; c.U = U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur; c.io_bf16 = elem_bytes == 2;
+    c.multiblank = mb;
+    if (mb) c.lse_mb = lse; else c.lse = reinterpret_cast<float2 *>(lse);
+    RNNT_TRY(launch_tdt_forward(s, c), RNNT_STATUS_WARP_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+// the gradient (T, U: 0 when compact; yn and prefix: compact only)
+static int tdt_backward_any(bool mb, bool compact, void *stream, const void *logits, const float *lse,
+                            const float *grads, const int *labels, const int *yn, const int *durations, int D,
+                            const int64_t *prefix, const float *grad_out, void *out, int64_t STU, int N, int T, int U,
+                            int V, int blank, int elem_bytes) {
+    TdtDurations dur;
+    if (!tdt_args_ok(mb, compact, durations, D, 0.0f, N, STU, T, U, V, blank, elem_bytes, logits, &dur) ||
+        !elem_ok(out, elem_bytes) || !lse || (!mb && !pairs_aligned(lse)) || !grads || !out || (compact && !prefix))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0 || (compact && STU == 0)) return RNNT_STATUS_SUCCESS;
+    TdtBwd c = {};
+    if (compact) {
+        c.yn = yn; c.mem_pref = prefix; c.lab_pref = prefix + N; c.STU = STU;
+    }
+    c.x = logits; c.pg = grads; c.labels = labels; c.grad_out = grad_out; c.out = out;
+    c.N = N; c.T = T; c.U = U; c.V = V; c.D = D; c.blank = blank; c.io_bf16 = elem_bytes == 2;
+    c.multiblank = mb;
+    if (mb) c.lse_mb = lse; else c.lse = reinterpret_cast<const float2 *>(lse);
+    RNNT_TRY(launch_tdt_backward((cudaStream_t)stream, c), RNNT_STATUS_GRADS_BLANK_FAILED);
+    return RNNT_STATUS_SUCCESS;
+}
+
+// the Viterbi alignment: the compact prefix sums into the workspace, then launch_tdt_align, whose third output is
+// the label durations, or launch_mb_align, whose third output is the blank counts
+static int tdt_align_any(bool mb, bool compact, void *stream, void *workspace, size_t workspace_bytes,
+                         const void *logits, const int *labels, const int *xn, const int *yn, const int *durations,
+                         int D, float sigma, float *scores, int *frames, int *third, int64_t STU, int N, int T, int U,
+                         int V, int blank, int elem_bytes) {
+    TdtDurations dur;
+    if (!tdt_args_ok(mb, compact, durations, D, sigma, N, STU, T, U, V, blank, elem_bytes, logits, &dur) || !scores ||
+        !frames || !third || !workspace_aligned16(workspace) || (compact && (T < 1 || U < 1)))
+        return RNNT_STATUS_INVALID_ARGUMENT;
+    if (N == 0) return RNNT_STATUS_SUCCESS;
+    const TdtAlignWorkspace w = carve_tdt_align(workspace, compact ? STU : (int64_t)N * T * U, N, D);
+    if (!workspace || workspace_bytes < w.bytes) return RNNT_STATUS_WORKSPACE_TOO_SMALL;
+    cudaStream_t s = (cudaStream_t)stream;
+    TdtFwd c = {};
+    if (compact) {
+        RNNT_TRY(launch_prefix(s, xn, yn, N, w.prefix, w.prefix + N, w.totals), RNNT_STATUS_GATHER_FAILED);
+        c.mem_pref = w.prefix; c.lab_pref = w.prefix + N; c.STU = STU;
+    }
+    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = scores;
+    c.lp = w.lp; c.alpha = w.alpha; c.status = w.status;
+    c.N = N; c.T = T; c.U = U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur; c.io_bf16 = elem_bytes == 2;
+    c.multiblank = mb;
+    if (mb) c.lse_mb = (float *)w.lse; else c.lse = w.lse;
+    const auto align = mb ? launch_mb_align : launch_tdt_align;
+    RNNT_TRY(align(s, c, w.dec, frames, third), RNNT_STATUS_WARP_FAILED);
+    return RNNT_STATUS_SUCCESS;
 }
 
 extern "C" {
@@ -1159,38 +1238,16 @@ int rnnt_b200_tdt_forward(void *stream, void *workspace, size_t workspace_bytes,
                           const int *xn, const int *yn, const int *durations, int num_durations, float sigma,
                           float *costs, float *lse, float *grads, int N, int T, int U, int V, int blank,
                           int elem_bytes) {
-    TdtDurations dur;
-    if (!tdt_durations(durations, num_durations, &dur) || !tdt_args_ok(N, T, U, V, num_durations, blank, elem_bytes, logits) ||
-        !std::isfinite(sigma) || sigma < 0.0f || !costs || !lse || !pairs_aligned(lse) ||
-        !workspace_aligned16(workspace))
-        return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0) return RNNT_STATUS_SUCCESS;
-    if (!workspace || workspace_bytes < rnnt_b200_tdt_workspace_bytes(N, T, U, num_durations))
-        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
-    const TdtWorkspace w = carve_tdt(workspace, (int64_t)N * T * U, N, num_durations, false);
-    TdtFwd c = {};
-    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = costs;
-    c.lse = reinterpret_cast<float2 *>(lse); c.pg = grads;
-    c.lp = w.lp; c.alpha = w.alpha; c.beta = w.beta; c.ll = w.ll; c.status = w.status;
-    c.N = N; c.T = T; c.U = U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur; c.io_bf16 = elem_bytes == 2;
-    RNNT_TRY(launch_tdt_forward((cudaStream_t)stream, c), RNNT_STATUS_WARP_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    return tdt_forward_any(false, false, stream, workspace, workspace_bytes, logits, labels, xn, yn, durations,
+                           num_durations, sigma, costs, lse, grads, nullptr, nullptr, 0, N, T, U, V, blank,
+                           elem_bytes);
 }
 
 int rnnt_b200_tdt_backward(void *stream, const void *logits, const float *lse, const float *grads, const int *labels,
                            const int *durations, int num_durations, const float *grad_out, void *out, int N, int T,
                            int U, int V, int blank, int elem_bytes) {
-    TdtDurations dur;
-    if (!tdt_durations(durations, num_durations, &dur) || !tdt_args_ok(N, T, U, V, num_durations, blank, elem_bytes, logits) ||
-        (reinterpret_cast<uintptr_t>(out) & (uintptr_t)(elem_bytes - 1)) || !lse || !pairs_aligned(lse) || !grads ||
-        !out)
-        return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0) return RNNT_STATUS_SUCCESS;
-    TdtBwd c = {};
-    c.x = logits; c.lse = reinterpret_cast<const float2 *>(lse); c.pg = grads; c.labels = labels; c.grad_out = grad_out;
-    c.out = out; c.N = N; c.T = T; c.U = U; c.V = V; c.D = num_durations; c.blank = blank; c.io_bf16 = elem_bytes == 2;
-    RNNT_TRY(launch_tdt_backward((cudaStream_t)stream, c), RNNT_STATUS_GRADS_BLANK_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    return tdt_backward_any(false, false, stream, logits, lse, grads, labels, nullptr, durations, num_durations,
+                            nullptr, grad_out, out, 0, N, T, U, V, blank, elem_bytes);
 }
 
 size_t rnnt_b200_tdt_compact_workspace_bytes(int64_t STU, int N, int num_durations) {
@@ -1202,46 +1259,17 @@ int rnnt_b200_tdt_compact_forward(void *stream, void *workspace, size_t workspac
                                   int num_durations, float sigma, float *costs, float *lse, float *grads,
                                   int64_t *prefix, int *totals, int64_t STU, int N, int V, int blank, int elem_bytes,
                                   int max_T, int max_U) {
-    TdtDurations dur;
-    if (!tdt_durations(durations, num_durations, &dur) ||
-        !tdt_compact_args_ok(N, STU, V, num_durations, blank, elem_bytes, logits) || !std::isfinite(sigma) ||
-        sigma < 0.0f || !costs || !lse || !pairs_aligned(lse) || !workspace_aligned16(workspace) || !prefix ||
-        max_T < 1 || max_U < 1)
-        return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0) return RNNT_STATUS_SUCCESS;
-    if (!workspace || workspace_bytes < rnnt_b200_tdt_compact_workspace_bytes(STU, N, num_durations))
-        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
-    cudaStream_t s = (cudaStream_t)stream;
-    const TdtWorkspace w = carve_tdt(workspace, STU, N, num_durations, true);
-    RNNT_TRY(launch_prefix(s, xn, yn, N, prefix, prefix + N, totals ? totals : w.totals), RNNT_STATUS_GATHER_FAILED);
-    TdtFwd c = {};
-    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = costs;
-    c.mem_pref = prefix; c.lab_pref = prefix + N; c.STU = STU;
-    c.lse = reinterpret_cast<float2 *>(lse); c.pg = grads;
-    c.lp = w.lp; c.alpha = w.alpha; c.beta = w.beta; c.ll = w.ll; c.status = w.status;
-    c.N = N; c.T = max_T; c.U = max_U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur;
-    c.io_bf16 = elem_bytes == 2;
-    RNNT_TRY(launch_tdt_forward(s, c), RNNT_STATUS_WARP_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    return tdt_forward_any(false, true, stream, workspace, workspace_bytes, logits, labels, xn, yn, durations,
+                           num_durations, sigma, costs, lse, grads, prefix, totals, STU, N, max_T, max_U, V, blank,
+                           elem_bytes);
 }
 
 int rnnt_b200_tdt_compact_backward(void *stream, const void *logits, const float *lse, const float *grads,
                                    const int *labels, const int *yn, const int *durations, int num_durations,
                                    const int64_t *prefix, const float *grad_out, void *out, int64_t STU, int N, int V,
                                    int blank, int elem_bytes) {
-    TdtDurations dur;
-    if (!tdt_durations(durations, num_durations, &dur) ||
-        !tdt_compact_args_ok(N, STU, V, num_durations, blank, elem_bytes, logits) ||
-        (reinterpret_cast<uintptr_t>(out) & (uintptr_t)(elem_bytes - 1)) || !lse || !pairs_aligned(lse) || !grads ||
-        !out || !prefix)
-        return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0 || STU == 0) return RNNT_STATUS_SUCCESS;
-    TdtBwd c = {};
-    c.x = logits; c.lse = reinterpret_cast<const float2 *>(lse); c.pg = grads; c.labels = labels; c.grad_out = grad_out;
-    c.yn = yn; c.mem_pref = prefix; c.lab_pref = prefix + N; c.STU = STU;
-    c.out = out; c.N = N; c.V = V; c.D = num_durations; c.blank = blank; c.io_bf16 = elem_bytes == 2;
-    RNNT_TRY(launch_tdt_backward((cudaStream_t)stream, c), RNNT_STATUS_GRADS_BLANK_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    return tdt_backward_any(false, true, stream, logits, lse, grads, labels, yn, durations, num_durations, prefix,
+                            grad_out, out, STU, N, 0, 0, V, blank, elem_bytes);
 }
 
 size_t rnnt_b200_tdt_align_workspace_bytes(int64_t cells, int N, int num_durations) {
@@ -1252,77 +1280,31 @@ int rnnt_b200_tdt_align_dense(void *stream, void *workspace, size_t workspace_by
                               const int *labels, const int *xn, const int *yn, const int *durations, int num_durations,
                               float sigma, float *scores, int *frames, int *label_durations, int N, int T, int U,
                               int V, int blank, int elem_bytes) {
-    TdtDurations dur;
-    if (!tdt_durations(durations, num_durations, &dur) || !tdt_args_ok(N, T, U, V, num_durations, blank, elem_bytes, logits) ||
-        !std::isfinite(sigma) || sigma < 0.0f || !scores || !frames || !label_durations ||
-        !workspace_aligned16(workspace))
-        return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0) return RNNT_STATUS_SUCCESS;
-    const int64_t cells = (int64_t)N * T * U;
-    if (!workspace || workspace_bytes < rnnt_b200_tdt_align_workspace_bytes(cells, N, num_durations))
-        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
-    const TdtAlignWorkspace w = carve_tdt_align(workspace, cells, N, num_durations);
-    TdtFwd c = {};
-    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = scores;
-    c.lse = w.lse; c.lp = w.lp; c.alpha = w.alpha; c.status = w.status;
-    c.N = N; c.T = T; c.U = U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur; c.io_bf16 = elem_bytes == 2;
-    RNNT_TRY(launch_tdt_align((cudaStream_t)stream, c, w.dec, frames, label_durations), RNNT_STATUS_WARP_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    return tdt_align_any(false, false, stream, workspace, workspace_bytes, logits, labels, xn, yn, durations,
+                         num_durations, sigma, scores, frames, label_durations, 0, N, T, U, V, blank, elem_bytes);
 }
 
 int rnnt_b200_tdt_align_compact(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
                                 const int *labels, const int *xn, const int *yn, const int *durations,
                                 int num_durations, float sigma, float *scores, int *frames, int *label_durations,
                                 int64_t STU, int N, int V, int blank, int elem_bytes, int max_T, int max_U) {
-    TdtDurations dur;
-    if (!tdt_durations(durations, num_durations, &dur) ||
-        !tdt_compact_args_ok(N, STU, V, num_durations, blank, elem_bytes, logits) || !std::isfinite(sigma) ||
-        sigma < 0.0f || !scores || !frames || !label_durations || !workspace_aligned16(workspace) || max_T < 1 ||
-        max_U < 1)
-        return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0) return RNNT_STATUS_SUCCESS;
-    if (!workspace || workspace_bytes < rnnt_b200_tdt_align_workspace_bytes(STU, N, num_durations))
-        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
-    cudaStream_t s = (cudaStream_t)stream;
-    const TdtAlignWorkspace w = carve_tdt_align(workspace, STU, N, num_durations);
-    RNNT_TRY(launch_prefix(s, xn, yn, N, w.prefix, w.prefix + N, w.totals), RNNT_STATUS_GATHER_FAILED);
-    TdtFwd c = {};
-    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = scores;
-    c.mem_pref = w.prefix; c.lab_pref = w.prefix + N; c.STU = STU;
-    c.lse = w.lse; c.lp = w.lp; c.alpha = w.alpha; c.status = w.status;
-    c.N = N; c.T = max_T; c.U = max_U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur;
-    c.io_bf16 = elem_bytes == 2;
-    RNNT_TRY(launch_tdt_align(s, c, w.dec, frames, label_durations), RNNT_STATUS_WARP_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    return tdt_align_any(false, true, stream, workspace, workspace_bytes, logits, labels, xn, yn, durations,
+                         num_durations, sigma, scores, frames, label_durations, STU, N, max_T, max_U, V, blank,
+                         elem_bytes);
 }
 
 // The multi-blank alignment carves the TDT alignment's workspace with D = B; its lse is one float per cell, held in
 // the first half of the lse slot.
 size_t rnnt_b200_multiblank_align_workspace_bytes(int64_t cells, int N, int num_big_blanks) {
-    return carve_tdt_align(nullptr, cells, N, num_big_blanks).bytes;
+    return rnnt_b200_tdt_align_workspace_bytes(cells, N, num_big_blanks);
 }
 
 int rnnt_b200_multiblank_align_dense(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
                                      const int *labels, const int *xn, const int *yn, const int *big_blank_durations,
                                      int num_big_blanks, float sigma, float *scores, int *frames, int *blank_counts,
                                      int N, int T, int U, int V, int blank, int elem_bytes) {
-    TdtDurations dur;
-    if (!mb_durations(big_blank_durations, num_big_blanks, &dur) ||
-        !mb_args_ok(N, T, U, V, num_big_blanks, blank, elem_bytes, logits) || !std::isfinite(sigma) || sigma < 0.0f ||
-        !scores || !frames || !blank_counts || !workspace_aligned16(workspace))
-        return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0) return RNNT_STATUS_SUCCESS;
-    const int64_t cells = (int64_t)N * T * U;
-    if (!workspace || workspace_bytes < rnnt_b200_multiblank_align_workspace_bytes(cells, N, num_big_blanks))
-        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
-    const TdtAlignWorkspace w = carve_tdt_align(workspace, cells, N, num_big_blanks);
-    TdtFwd c = {};
-    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = scores;
-    c.multiblank = true; c.lse_mb = (float *)w.lse;
-    c.lp = w.lp; c.alpha = w.alpha; c.status = w.status;
-    c.N = N; c.T = T; c.U = U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur; c.io_bf16 = elem_bytes == 2;
-    RNNT_TRY(launch_mb_align((cudaStream_t)stream, c, w.dec, frames, blank_counts), RNNT_STATUS_WARP_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    return tdt_align_any(true, false, stream, workspace, workspace_bytes, logits, labels, xn, yn, big_blank_durations,
+                         num_big_blanks, sigma, scores, frames, blank_counts, 0, N, T, U, V, blank, elem_bytes);
 }
 
 int rnnt_b200_multiblank_align_compact(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
@@ -1330,75 +1312,34 @@ int rnnt_b200_multiblank_align_compact(void *stream, void *workspace, size_t wor
                                        const int *big_blank_durations, int num_big_blanks, float sigma, float *scores,
                                        int *frames, int *blank_counts, int64_t STU, int N, int V, int blank,
                                        int elem_bytes, int max_T, int max_U) {
-    TdtDurations dur;
-    if (!mb_durations(big_blank_durations, num_big_blanks, &dur) ||
-        !mb_compact_args_ok(N, STU, V, num_big_blanks, blank, elem_bytes, logits) || !std::isfinite(sigma) ||
-        sigma < 0.0f || !scores || !frames || !blank_counts || !workspace_aligned16(workspace) || max_T < 1 ||
-        max_U < 1)
-        return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0) return RNNT_STATUS_SUCCESS;
-    if (!workspace || workspace_bytes < rnnt_b200_multiblank_align_workspace_bytes(STU, N, num_big_blanks))
-        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
-    cudaStream_t s = (cudaStream_t)stream;
-    const TdtAlignWorkspace w = carve_tdt_align(workspace, STU, N, num_big_blanks);
-    RNNT_TRY(launch_prefix(s, xn, yn, N, w.prefix, w.prefix + N, w.totals), RNNT_STATUS_GATHER_FAILED);
-    TdtFwd c = {};
-    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = scores;
-    c.mem_pref = w.prefix; c.lab_pref = w.prefix + N; c.STU = STU;
-    c.multiblank = true; c.lse_mb = (float *)w.lse;
-    c.lp = w.lp; c.alpha = w.alpha; c.status = w.status;
-    c.N = N; c.T = max_T; c.U = max_U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur;
-    c.io_bf16 = elem_bytes == 2;
-    RNNT_TRY(launch_mb_align(s, c, w.dec, frames, blank_counts), RNNT_STATUS_WARP_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    return tdt_align_any(true, true, stream, workspace, workspace_bytes, logits, labels, xn, yn, big_blank_durations,
+                         num_big_blanks, sigma, scores, frames, blank_counts, STU, N, max_T, max_U, V, blank,
+                         elem_bytes);
 }
 
 size_t rnnt_b200_multiblank_workspace_bytes(int N, int T, int U, int num_big_blanks) {
-    return carve_tdt(nullptr, (int64_t)max(N, 0) * max(T, 0) * max(U, 0), N, num_big_blanks, false).bytes;
+    return rnnt_b200_tdt_workspace_bytes(N, T, U, num_big_blanks);
 }
 
 int rnnt_b200_multiblank_forward(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
                                  const int *labels, const int *xn, const int *yn, const int *big_blank_durations,
                                  int num_big_blanks, float sigma, float *costs, float *lse, float *grads, int N, int T,
                                  int U, int V, int blank, int elem_bytes) {
-    TdtDurations dur;
-    if (!mb_durations(big_blank_durations, num_big_blanks, &dur) ||
-        !mb_args_ok(N, T, U, V, num_big_blanks, blank, elem_bytes, logits) || !std::isfinite(sigma) || sigma < 0.0f ||
-        !costs || !lse || !workspace_aligned16(workspace))
-        return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0) return RNNT_STATUS_SUCCESS;
-    if (!workspace || workspace_bytes < rnnt_b200_multiblank_workspace_bytes(N, T, U, num_big_blanks))
-        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
-    const TdtWorkspace w = carve_tdt(workspace, (int64_t)N * T * U, N, num_big_blanks, false);
-    TdtFwd c = {};
-    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = costs;
-    c.multiblank = true; c.lse_mb = lse; c.pg = grads;
-    c.lp = w.lp; c.alpha = w.alpha; c.beta = w.beta; c.ll = w.ll; c.status = w.status;
-    c.N = N; c.T = T; c.U = U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur; c.io_bf16 = elem_bytes == 2;
-    RNNT_TRY(launch_tdt_forward((cudaStream_t)stream, c), RNNT_STATUS_WARP_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    return tdt_forward_any(true, false, stream, workspace, workspace_bytes, logits, labels, xn, yn,
+                           big_blank_durations, num_big_blanks, sigma, costs, lse, grads, nullptr, nullptr, 0, N, T, U,
+                           V, blank, elem_bytes);
 }
 
 int rnnt_b200_multiblank_backward(void *stream, const void *logits, const float *lse, const float *grads,
                                   const int *labels, const int *big_blank_durations, int num_big_blanks,
                                   const float *grad_out, void *out, int N, int T, int U, int V, int blank,
                                   int elem_bytes) {
-    TdtDurations dur;
-    if (!mb_durations(big_blank_durations, num_big_blanks, &dur) ||
-        !mb_args_ok(N, T, U, V, num_big_blanks, blank, elem_bytes, logits) ||
-        (reinterpret_cast<uintptr_t>(out) & (uintptr_t)(elem_bytes - 1)) || !lse || !grads || !out)
-        return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0) return RNNT_STATUS_SUCCESS;
-    TdtBwd c = {};
-    c.x = logits; c.multiblank = true; c.lse_mb = lse; c.pg = grads; c.labels = labels; c.grad_out = grad_out;
-    c.out = out; c.N = N; c.T = T; c.U = U; c.V = V; c.D = num_big_blanks; c.blank = blank;
-    c.io_bf16 = elem_bytes == 2;
-    RNNT_TRY(launch_tdt_backward((cudaStream_t)stream, c), RNNT_STATUS_GRADS_BLANK_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    return tdt_backward_any(true, false, stream, logits, lse, grads, labels, nullptr, big_blank_durations,
+                            num_big_blanks, nullptr, grad_out, out, 0, N, T, U, V, blank, elem_bytes);
 }
 
 size_t rnnt_b200_multiblank_compact_workspace_bytes(int64_t STU, int N, int num_big_blanks) {
-    return carve_tdt(nullptr, STU, N, num_big_blanks, true).bytes;
+    return rnnt_b200_tdt_compact_workspace_bytes(STU, N, num_big_blanks);
 }
 
 int rnnt_b200_multiblank_compact_forward(void *stream, void *workspace, size_t workspace_bytes, const void *logits,
@@ -1406,44 +1347,17 @@ int rnnt_b200_multiblank_compact_forward(void *stream, void *workspace, size_t w
                                          const int *big_blank_durations, int num_big_blanks, float sigma,
                                          float *costs, float *lse, float *grads, int64_t *prefix, int *totals,
                                          int64_t STU, int N, int V, int blank, int elem_bytes, int max_T, int max_U) {
-    TdtDurations dur;
-    if (!mb_durations(big_blank_durations, num_big_blanks, &dur) ||
-        !mb_compact_args_ok(N, STU, V, num_big_blanks, blank, elem_bytes, logits) || !std::isfinite(sigma) ||
-        sigma < 0.0f || !costs || !lse || !workspace_aligned16(workspace) || !prefix || max_T < 1 || max_U < 1)
-        return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0) return RNNT_STATUS_SUCCESS;
-    if (!workspace || workspace_bytes < rnnt_b200_multiblank_compact_workspace_bytes(STU, N, num_big_blanks))
-        return RNNT_STATUS_WORKSPACE_TOO_SMALL;
-    cudaStream_t s = (cudaStream_t)stream;
-    const TdtWorkspace w = carve_tdt(workspace, STU, N, num_big_blanks, true);
-    RNNT_TRY(launch_prefix(s, xn, yn, N, prefix, prefix + N, totals ? totals : w.totals), RNNT_STATUS_GATHER_FAILED);
-    TdtFwd c = {};
-    c.x = logits; c.labels = labels; c.xn = xn; c.yn = yn; c.costs = costs;
-    c.mem_pref = prefix; c.lab_pref = prefix + N; c.STU = STU;
-    c.multiblank = true; c.lse_mb = lse; c.pg = grads;
-    c.lp = w.lp; c.alpha = w.alpha; c.beta = w.beta; c.ll = w.ll; c.status = w.status;
-    c.N = N; c.T = max_T; c.U = max_U; c.V = V; c.blank = blank; c.sigma = sigma; c.dur = dur;
-    c.io_bf16 = elem_bytes == 2;
-    RNNT_TRY(launch_tdt_forward(s, c), RNNT_STATUS_WARP_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    return tdt_forward_any(true, true, stream, workspace, workspace_bytes, logits, labels, xn, yn,
+                           big_blank_durations, num_big_blanks, sigma, costs, lse, grads, prefix, totals, STU, N,
+                           max_T, max_U, V, blank, elem_bytes);
 }
 
 int rnnt_b200_multiblank_compact_backward(void *stream, const void *logits, const float *lse, const float *grads,
                                           const int *labels, const int *yn, const int *big_blank_durations,
                                           int num_big_blanks, const int64_t *prefix, const float *grad_out, void *out,
                                           int64_t STU, int N, int V, int blank, int elem_bytes) {
-    TdtDurations dur;
-    if (!mb_durations(big_blank_durations, num_big_blanks, &dur) ||
-        !mb_compact_args_ok(N, STU, V, num_big_blanks, blank, elem_bytes, logits) ||
-        (reinterpret_cast<uintptr_t>(out) & (uintptr_t)(elem_bytes - 1)) || !lse || !grads || !out || !prefix)
-        return RNNT_STATUS_INVALID_ARGUMENT;
-    if (N == 0 || STU == 0) return RNNT_STATUS_SUCCESS;
-    TdtBwd c = {};
-    c.x = logits; c.multiblank = true; c.lse_mb = lse; c.pg = grads; c.labels = labels; c.grad_out = grad_out;
-    c.yn = yn; c.mem_pref = prefix; c.lab_pref = prefix + N; c.STU = STU;
-    c.out = out; c.N = N; c.V = V; c.D = num_big_blanks; c.blank = blank; c.io_bf16 = elem_bytes == 2;
-    RNNT_TRY(launch_tdt_backward((cudaStream_t)stream, c), RNNT_STATUS_GRADS_BLANK_FAILED);
-    return RNNT_STATUS_SUCCESS;
+    return tdt_backward_any(true, true, stream, logits, lse, grads, labels, yn, big_blank_durations, num_big_blanks,
+                            prefix, grad_out, out, STU, N, 0, 0, V, blank, elem_bytes);
 }
 
 void rnnt_b200_debug_last_tdt_launch(int32_t *out) {

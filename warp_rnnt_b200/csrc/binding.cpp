@@ -567,233 +567,67 @@ at::Tensor rnnt_logits_pruned_backward(const at::Tensor &xs, const at::Tensor &l
     return out;
 }
 
-// TDT loss from (N,T,U,V+D) logits, float32 or bfloat16, D = durations.size(): (costs (N), lse (N,T,U,2),
-// grads (N,T,U,2+D) or empty), all float32.  No host sync.
-std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_tdt_forward(const at::Tensor &xs, const at::Tensor &ys,
-                                                                const at::Tensor &xn, const at::Tensor &yn,
-                                                                const std::vector<int> &durations, double sigma,
-                                                                int blank, bool want_grads) {
-    check4(xs, ys, xn, yn, true);
-    check_batch4(xs, xn, yn);
-    const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), D = (int64_t)durations.size();
-    check_arg(ys, Dt::I32, xs, {N, U - 1}, "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
-    TORCH_CHECK(D >= 1 && xs.size(3) > D, "xs must have more than len(durations) logits per cell (V + D)");
-    const int64_t V = xs.size(3) - D;
-    check_blank(blank, V);
-    const c10::cuda::CUDAGuard guard(xs.device());
-    const auto f32 = xs.options().dtype(at::kFloat);
-    at::Tensor costs = at::empty({N}, f32);
-    at::Tensor lse = at::empty({N, T, U, 2}, f32);
-    at::Tensor pg = output(want_grads, {N, T, U, 2 + D}, f32);
-    if (N == 0) return std::make_tuple(costs, lse, pg);
-    at::Tensor ws = workspace(xs, rnnt_b200_tdt_workspace_bytes((int)N, (int)T, (int)U, (int)D));
-    check_status(rnnt_b200_tdt_forward(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
-                                       ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(), durations.data(),
-                                       (int)D, (float)sigma, costs.data_ptr<float>(), lse.data_ptr<float>(),
-                                       want_grads ? pg.data_ptr<float>() : nullptr, (int)N, (int)T, (int)U, (int)V,
-                                       blank, xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
-    return std::make_tuple(costs, lse, pg);
+// ---- TDT and multi-blank --------------------------------------------------------------------------------------
+// The Token-and-Duration Transducer (TDT) and the multi-blank transducer share their kernels and the signatures of
+// their C ABI calls; a Lattice holds what differs.  D = durations.size().  A TDT row is V token logits then D duration
+// logits, blank in [0, V), and its lse holds (lse_tok, lse_dur) per cell; a multi-blank row is V logits with the D big
+// blanks below the standard blank, blank in [D, V), and its lse one float per cell.
+struct Lattice {
+    bool multiblank;
+    const char *row_cell, *row_row;           // the row must hold more than D logits: dense, compact
+    const char *blank_range;
+    const char *xs4, *lse4, *grads4;          // the dense backward's tensors
+    const char *xs2, *lse2, *grads2;          // the compact backward's tensors
+    decltype(&rnnt_b200_tdt_workspace_bytes) workspace_bytes;
+    decltype(&rnnt_b200_tdt_forward) forward;
+    decltype(&rnnt_b200_tdt_backward) backward;
+    decltype(&rnnt_b200_tdt_compact_workspace_bytes) compact_workspace_bytes;
+    decltype(&rnnt_b200_tdt_compact_forward) compact_forward;
+    decltype(&rnnt_b200_tdt_compact_backward) compact_backward;
+    decltype(&rnnt_b200_tdt_align_workspace_bytes) align_workspace_bytes;
+    decltype(&rnnt_b200_tdt_align_dense) align_dense;
+    decltype(&rnnt_b200_tdt_align_compact) align_compact;
+};
+
+const Lattice kTdt = {
+    false, "xs must have more than len(durations) logits per cell (V + D)",
+    "xs must have more than len(durations) logits per row (V + D)", "blank must be in [0, V)",
+    "xs must be a contiguous CUDA Float tensor of shape (N, T, U, V+D)",
+    "lse must be a contiguous Float tensor of shape (N, T, U, 2) on the device of xs",
+    "grads must be a contiguous Float tensor of shape (N, T, U, 2+D) on the device of xs",
+    "xs must be a contiguous CUDA Float tensor of shape (STU, V+D)",
+    "lse must be a contiguous Float tensor of shape (STU, 2) on the device of xs",
+    "grads must be a contiguous Float tensor of shape (STU, 2+D) on the device of xs",
+    rnnt_b200_tdt_workspace_bytes, rnnt_b200_tdt_forward, rnnt_b200_tdt_backward,
+    rnnt_b200_tdt_compact_workspace_bytes, rnnt_b200_tdt_compact_forward, rnnt_b200_tdt_compact_backward,
+    rnnt_b200_tdt_align_workspace_bytes, rnnt_b200_tdt_align_dense, rnnt_b200_tdt_align_compact};
+
+const Lattice kMultiblank = {
+    true, "xs must have more than len(big_blank_durations) logits per cell",
+    "xs must have more than len(big_blank_durations) logits per cell", "blank must be in [len(big_blank_durations), V)",
+    "xs must be a contiguous CUDA Float tensor of shape (N, T, U, V)",
+    "lse must be a contiguous Float tensor of shape (N, T, U) on the device of xs",
+    "grads must be a contiguous Float tensor of shape (N, T, U, 2+B) on the device of xs",
+    "xs must be a contiguous CUDA Float tensor of shape (STU, V)",
+    "lse must be a contiguous Float tensor of shape (STU,) on the device of xs",
+    "grads must be a contiguous Float tensor of shape (STU, 2+B) on the device of xs",
+    rnnt_b200_multiblank_workspace_bytes, rnnt_b200_multiblank_forward, rnnt_b200_multiblank_backward,
+    rnnt_b200_multiblank_compact_workspace_bytes, rnnt_b200_multiblank_compact_forward,
+    rnnt_b200_multiblank_compact_backward, rnnt_b200_multiblank_align_workspace_bytes,
+    rnnt_b200_multiblank_align_dense, rnnt_b200_multiblank_align_compact};
+
+// V of a row of W logits, after the row (message `row`) and the blank are checked
+int64_t lattice_tokens(const Lattice &F, int64_t W, int64_t D, int blank, const char *row) {
+    TORCH_CHECK(D >= 1 && W > D, row);
+    const int64_t V = F.multiblank ? W : W - D;
+    TORCH_CHECK(blank >= (F.multiblank ? D : 0) && blank < V, F.blank_range);
+    return V;
 }
 
-// d loss / d TDT logits (N,T,U,V+D), of the dtype of xs
-at::Tensor rnnt_tdt_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &grads, const at::Tensor &ys,
-                             const std::vector<int> &durations, const at::Tensor &grad_out, int blank) {
-    check_arg(xs, Dt::F32orBF16, xs, {kAny, kAny, kAny, kAny},
-              "xs must be a contiguous CUDA Float tensor of shape (N, T, U, V+D)");
-    const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), D = (int64_t)durations.size();
-    TORCH_CHECK(D >= 1 && xs.size(3) > D, "xs must have more than len(durations) logits per cell (V + D)");
-    const int64_t V = xs.size(3) - D;
-    check_arg(lse, Dt::F32, xs, {N, T, U, 2}, "lse must be a contiguous Float tensor of shape (N, T, U, 2) on the device of xs");
-    check_arg(grads, Dt::F32, xs, {N, T, U, 2 + D},
-              "grads must be a contiguous Float tensor of shape (N, T, U, 2+D) on the device of xs");
-    check_arg(ys, Dt::I32, xs, {N, U - 1}, "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
-    check_arg(grad_out, Dt::F32, xs, N, "grad_out must be a contiguous Float tensor of shape (N,)");
-    check_blank(blank, V);
-    const c10::cuda::CUDAGuard guard(xs.device());
-    at::Tensor out = at::empty_like(xs);
-    if (N == 0) return out;
-    check_status(rnnt_b200_tdt_backward(current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(), grads.data_ptr<float>(),
-                                        ys.data_ptr<int>(), durations.data(), (int)D, grad_out.data_ptr<float>(),
-                                        out.data_ptr(), (int)N, (int)T, (int)U, (int)V, blank,
-                                        xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
-    return out;
-}
-
-// TDT loss from compact (STU,V+D) logits in joint_pack's row order, float32 or bfloat16, labels (sum yn): (costs (N),
-// lse (STU,2), grads (STU,2+D) or empty, prefix (2N) int64 = {mem_pref, lab_pref} for the backward).  Shapes are
-// validated as in rnnt_loss_compact: one 16-byte device->host copy, or none with hints (max_T, max_U > 0).
-std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor>
-rnnt_tdt_compact_forward(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
-                         const std::vector<int> &durations, double sigma, int blank, bool want_grads, int max_T,
-                         int max_U) {
-    const auto [N, STU, W, bf16, guard] = compact_front(xs, ys, xn, yn, blank, true);
-    const int64_t D = (int64_t)durations.size();
-    TORCH_CHECK(D >= 1 && W > D, "xs must have more than len(durations) logits per row (V + D)");
-    check_blank(blank, W - D);
-    void *stream = current_stream(xs);
-    const auto f32 = xs.options().dtype(at::kFloat);
-    at::Tensor costs = at::empty({N}, f32);
-    at::Tensor lse = at::empty({STU, 2}, f32);
-    at::Tensor pg = output(want_grads, {STU, 2 + D}, f32);
-    at::Tensor prefix = at::empty({2 * N}, xs.options().dtype(at::kLong));
-    if (N == 0) return std::make_tuple(costs, lse, pg, prefix);
-    std::tie(max_T, max_U) = compact_bounds(stream, xs, ys, xn, yn, max_T, max_U, prefix.data_ptr<int64_t>());
-    // a batch whose lengths are all 0: bounds of 1 (its lattices are invalid either way)
-    max_T = std::max(max_T, 1);
-    max_U = std::max(max_U, 1);
-    at::Tensor ws = workspace(xs, rnnt_b200_tdt_compact_workspace_bytes(STU, (int)N, (int)D));
-    check_status(rnnt_b200_tdt_compact_forward(stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
-                                               ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
-                                               durations.data(), (int)D, (float)sigma, costs.data_ptr<float>(),
-                                               lse.data_ptr<float>(), want_grads ? pg.data_ptr<float>() : nullptr,
-                                               prefix.data_ptr<int64_t>(), nullptr, STU, (int)N, (int)(W - D), blank,
-                                               bf16 ? 2 : 4, max_T, max_U));
-    return std::make_tuple(costs, lse, pg, prefix);
-}
-
-// d loss / d compact TDT logits (STU,V+D), of the dtype of xs
-at::Tensor rnnt_tdt_compact_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &grads,
-                                     const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
-                                     const at::Tensor &prefix, const std::vector<int> &durations,
-                                     const at::Tensor &grad_out, int blank) {
-    check_arg(xs, Dt::F32orBF16, xs, {kAny, kAny}, "xs must be a contiguous CUDA Float tensor of shape (STU, V+D)");
-    const int64_t STU = xs.size(0), W = xs.size(1), N = xn.numel(), D = (int64_t)durations.size();
-    TORCH_CHECK(D >= 1 && W > D, "xs must have more than len(durations) logits per row (V + D)");
-    check_arg(lse, Dt::F32, xs, {STU, 2}, "lse must be a contiguous Float tensor of shape (STU, 2) on the device of xs");
-    check_arg(grads, Dt::F32, xs, {STU, 2 + D},
-              "grads must be a contiguous Float tensor of shape (STU, 2+D) on the device of xs");
-    TORCH_CHECK(is_arg(ys, Dt::I32, xs), "ys must be a contiguous Int tensor on the device of xs");
-    const char *lengths = "xn and yn must be contiguous Int tensors of shape (N,) on the device of xs";
-    check_arg(xn, Dt::I32, xs, N, lengths);
-    check_arg(yn, Dt::I32, xs, N, lengths);
-    check_arg(prefix, Dt::I64, xs, 2 * N, "prefix must be a contiguous Long tensor of shape (2N,) on the device of xs");
-    check_arg(grad_out, Dt::F32, xs, N, "grad_out must be a contiguous Float tensor of shape (N,)");
-    check_blank(blank, W - D);
-    const c10::cuda::CUDAGuard guard(xs.device());
-    at::Tensor out = at::empty_like(xs);
-    if (N == 0 || STU == 0) return out;                 // empty tensors: nothing to write (and no data pointers)
-    check_status(rnnt_b200_tdt_compact_backward(current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(),
-                                                grads.data_ptr<float>(), ys.data_ptr<int>(), yn.data_ptr<int>(),
-                                                durations.data(), (int)D, prefix.data_ptr<int64_t>(),
-                                                grad_out.data_ptr<float>(), out.data_ptr(), STU, (int)N, (int)(W - D),
-                                                blank, xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
-    return out;
-}
-
-// Multi-blank: B = big_blank_durations.size() big blanks in the row of V, the standard blank in [B, V)
-void check_multiblank(int64_t B, int blank, int64_t V) {
-    TORCH_CHECK(B >= 1 && V > B, "xs must have more than len(big_blank_durations) logits per cell");
-    TORCH_CHECK(blank >= B && blank < V, "blank must be in [len(big_blank_durations), V)");
-}
-
-// Multi-blank transducer loss from (N,T,U,V) logits, float32 or bfloat16, B = durations.size(): (costs (N),
-// lse (N,T,U), grads (N,T,U,2+B) or empty), all float32.  No host sync.
-std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_multiblank_forward(const at::Tensor &xs, const at::Tensor &ys,
-                                                                       const at::Tensor &xn, const at::Tensor &yn,
-                                                                       const std::vector<int> &durations,
-                                                                       double sigma, int blank, bool want_grads) {
-    check4(xs, ys, xn, yn, true);
-    check_batch4(xs, xn, yn);
-    const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), V = xs.size(3), B = (int64_t)durations.size();
-    check_arg(ys, Dt::I32, xs, {N, U - 1}, "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
-    check_multiblank(B, blank, V);
-    const c10::cuda::CUDAGuard guard(xs.device());
-    const auto f32 = xs.options().dtype(at::kFloat);
-    at::Tensor costs = at::empty({N}, f32);
-    at::Tensor lse = at::empty({N, T, U}, f32);
-    at::Tensor pg = output(want_grads, {N, T, U, 2 + B}, f32);
-    if (N == 0) return std::make_tuple(costs, lse, pg);
-    at::Tensor ws = workspace(xs, rnnt_b200_multiblank_workspace_bytes((int)N, (int)T, (int)U, (int)B));
-    check_status(rnnt_b200_multiblank_forward(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
-                                              ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
-                                              durations.data(), (int)B, (float)sigma, costs.data_ptr<float>(),
-                                              lse.data_ptr<float>(), want_grads ? pg.data_ptr<float>() : nullptr,
-                                              (int)N, (int)T, (int)U, (int)V, blank,
-                                              xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
-    return std::make_tuple(costs, lse, pg);
-}
-
-// d loss / d multi-blank logits (N,T,U,V), of the dtype of xs
-at::Tensor rnnt_multiblank_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &grads,
-                                    const at::Tensor &ys, const std::vector<int> &durations,
-                                    const at::Tensor &grad_out, int blank) {
-    check_arg(xs, Dt::F32orBF16, xs, {kAny, kAny, kAny, kAny},
-              "xs must be a contiguous CUDA Float tensor of shape (N, T, U, V)");
-    const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), V = xs.size(3), B = (int64_t)durations.size();
-    check_multiblank(B, blank, V);
-    check_arg(lse, Dt::F32, xs, {N, T, U}, "lse must be a contiguous Float tensor of shape (N, T, U) on the device of xs");
-    check_arg(grads, Dt::F32, xs, {N, T, U, 2 + B},
-              "grads must be a contiguous Float tensor of shape (N, T, U, 2+B) on the device of xs");
-    check_arg(ys, Dt::I32, xs, {N, U - 1}, "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
-    check_arg(grad_out, Dt::F32, xs, N, "grad_out must be a contiguous Float tensor of shape (N,)");
-    const c10::cuda::CUDAGuard guard(xs.device());
-    at::Tensor out = at::empty_like(xs);
-    if (N == 0) return out;
-    check_status(rnnt_b200_multiblank_backward(current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(),
-                                               grads.data_ptr<float>(), ys.data_ptr<int>(), durations.data(), (int)B,
-                                               grad_out.data_ptr<float>(), out.data_ptr(), (int)N, (int)T, (int)U,
-                                               (int)V, blank, xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
-    return out;
-}
-
-// Multi-blank loss from compact (STU,V) logits in joint_pack's row order, float32 or bfloat16, labels (sum yn):
-// (costs (N), lse (STU), grads (STU,2+B) or empty, prefix (2N) int64 for the backward).  Shapes are validated as in
-// rnnt_tdt_compact_forward: one 16-byte device->host copy, or none with hints (max_T, max_U > 0).
-std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor>
-rnnt_multiblank_compact_forward(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn,
-                                const at::Tensor &yn, const std::vector<int> &durations, double sigma, int blank,
-                                bool want_grads, int max_T, int max_U) {
-    const auto [N, STU, V, bf16, guard] = compact_front(xs, ys, xn, yn, blank, true);
-    const int64_t B = (int64_t)durations.size();
-    check_multiblank(B, blank, V);
-    void *stream = current_stream(xs);
-    const auto f32 = xs.options().dtype(at::kFloat);
-    at::Tensor costs = at::empty({N}, f32);
-    at::Tensor lse = at::empty({STU}, f32);
-    at::Tensor pg = output(want_grads, {STU, 2 + B}, f32);
-    at::Tensor prefix = at::empty({2 * N}, xs.options().dtype(at::kLong));
-    if (N == 0) return std::make_tuple(costs, lse, pg, prefix);
-    std::tie(max_T, max_U) = compact_bounds(stream, xs, ys, xn, yn, max_T, max_U, prefix.data_ptr<int64_t>());
-    // a batch whose lengths are all 0: bounds of 1 (its lattices are invalid either way)
-    max_T = std::max(max_T, 1);
-    max_U = std::max(max_U, 1);
-    at::Tensor ws = workspace(xs, rnnt_b200_multiblank_compact_workspace_bytes(STU, (int)N, (int)B));
-    check_status(rnnt_b200_multiblank_compact_forward(stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
-                                                      ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
-                                                      durations.data(), (int)B, (float)sigma, costs.data_ptr<float>(),
-                                                      lse.data_ptr<float>(),
-                                                      want_grads ? pg.data_ptr<float>() : nullptr,
-                                                      prefix.data_ptr<int64_t>(), nullptr, STU, (int)N, (int)V, blank,
-                                                      bf16 ? 2 : 4, max_T, max_U));
-    return std::make_tuple(costs, lse, pg, prefix);
-}
-
-// d loss / d compact multi-blank logits (STU,V), of the dtype of xs
-at::Tensor rnnt_multiblank_compact_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &grads,
-                                            const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
-                                            const at::Tensor &prefix, const std::vector<int> &durations,
-                                            const at::Tensor &grad_out, int blank) {
-    check_arg(xs, Dt::F32orBF16, xs, {kAny, kAny}, "xs must be a contiguous CUDA Float tensor of shape (STU, V)");
-    const int64_t STU = xs.size(0), V = xs.size(1), N = xn.numel(), B = (int64_t)durations.size();
-    check_multiblank(B, blank, V);
-    check_arg(lse, Dt::F32, xs, {STU}, "lse must be a contiguous Float tensor of shape (STU,) on the device of xs");
-    check_arg(grads, Dt::F32, xs, {STU, 2 + B},
-              "grads must be a contiguous Float tensor of shape (STU, 2+B) on the device of xs");
-    TORCH_CHECK(is_arg(ys, Dt::I32, xs), "ys must be a contiguous Int tensor on the device of xs");
-    const char *lengths = "xn and yn must be contiguous Int tensors of shape (N,) on the device of xs";
-    check_arg(xn, Dt::I32, xs, N, lengths);
-    check_arg(yn, Dt::I32, xs, N, lengths);
-    check_arg(prefix, Dt::I64, xs, 2 * N, "prefix must be a contiguous Long tensor of shape (2N,) on the device of xs");
-    check_arg(grad_out, Dt::F32, xs, N, "grad_out must be a contiguous Float tensor of shape (N,)");
-    const c10::cuda::CUDAGuard guard(xs.device());
-    at::Tensor out = at::empty_like(xs);
-    if (N == 0 || STU == 0) return out;                 // empty tensors: nothing to write (and no data pointers)
-    check_status(rnnt_b200_multiblank_compact_backward(current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(),
-                                                       grads.data_ptr<float>(), ys.data_ptr<int>(), yn.data_ptr<int>(),
-                                                       durations.data(), (int)B, prefix.data_ptr<int64_t>(),
-                                                       grad_out.data_ptr<float>(), out.data_ptr(), STU, (int)N, (int)V,
-                                                       blank, xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
-    return out;
+// the shape of lse on the given cells
+std::vector<int64_t> lse_sizes(const Lattice &F, std::vector<int64_t> cells) {
+    if (!F.multiblank) cells.push_back(2);
+    return cells;
 }
 
 // An (n,) int32 output of the TDT alignment: a view of at least one element, so that the C ABI, which refuses NULL
@@ -802,112 +636,168 @@ at::Tensor label_slots(int64_t n, const at::Tensor &like) {
     return at::empty({std::max<int64_t>(n, 1)}, like.options().dtype(at::kInt)).narrow(0, 0, n);
 }
 
-// Viterbi alignment on the TDT lattice, dense (N,T,U,V+D) f32 or bf16 logits: (scores (N) f32, frames (N,U-1) i32,
-// label durations (N,U-1) i32).  No host sync.
-std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_tdt_align_dense(const at::Tensor &xs, const at::Tensor &ys,
-                                                                    const at::Tensor &xn, const at::Tensor &yn,
-                                                                    const std::vector<int> &durations, double sigma,
-                                                                    int blank) {
+// the alignment's third output: TDT's label durations, shaped like frames, or multi-blank's blank counts (N, 1 + D)
+at::Tensor align_third(const Lattice &F, const at::Tensor &frames, int64_t N, int64_t D) {
+    if (F.multiblank) return at::empty({N, 1 + D}, frames.options());
+    return label_slots(frames.numel(), frames).view(frames.sizes());
+}
+
+// Loss from (N,T,U,V+D) TDT or (N,T,U,V) multi-blank logits, float32 or bfloat16: (costs (N), lse (N,T,U,2) or
+// (N,T,U), grads (N,T,U,2+D) or empty), all float32.  No host sync.
+template <const Lattice &F>
+std::tuple<at::Tensor, at::Tensor, at::Tensor> lattice_forward(const at::Tensor &xs, const at::Tensor &ys,
+                                                               const at::Tensor &xn, const at::Tensor &yn,
+                                                               const std::vector<int> &durations, double sigma,
+                                                               int blank, bool want_grads) {
     check4(xs, ys, xn, yn, true);
     check_batch4(xs, xn, yn);
     const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), D = (int64_t)durations.size();
     check_arg(ys, Dt::I32, xs, {N, U - 1}, "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
-    TORCH_CHECK(D >= 1 && xs.size(3) > D, "xs must have more than len(durations) logits per cell (V + D)");
-    const int64_t V = xs.size(3) - D;
-    check_blank(blank, V);
+    const int64_t V = lattice_tokens(F, xs.size(3), D, blank, F.row_cell);
     const c10::cuda::CUDAGuard guard(xs.device());
-    at::Tensor scores = at::empty({N}, xs.options().dtype(at::kFloat));
-    at::Tensor frames = label_slots(N * (U - 1), xs).view({N, U - 1});
-    at::Tensor fdur = label_slots(N * (U - 1), xs).view({N, U - 1});
-    if (N == 0) return std::make_tuple(scores, frames, fdur);
-    at::Tensor ws = workspace(xs, rnnt_b200_tdt_align_workspace_bytes(N * T * U, (int)N, (int)D));
-    check_status(rnnt_b200_tdt_align_dense(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
-                                           ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
-                                           durations.data(), (int)D, (float)sigma, scores.data_ptr<float>(),
-                                           frames.data_ptr<int>(), fdur.data_ptr<int>(), (int)N, (int)T, (int)U,
-                                           (int)V, blank, xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
-    return std::make_tuple(scores, frames, fdur);
+    const auto f32 = xs.options().dtype(at::kFloat);
+    at::Tensor costs = at::empty({N}, f32);
+    at::Tensor lse = at::empty(lse_sizes(F, {N, T, U}), f32);
+    at::Tensor pg = output(want_grads, {N, T, U, 2 + D}, f32);
+    if (N == 0) return std::make_tuple(costs, lse, pg);
+    at::Tensor ws = workspace(xs, F.workspace_bytes((int)N, (int)T, (int)U, (int)D));
+    check_status(F.forward(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(), ys.data_ptr<int>(),
+                           xn.data_ptr<int>(), yn.data_ptr<int>(), durations.data(), (int)D, (float)sigma,
+                           costs.data_ptr<float>(), lse.data_ptr<float>(), want_grads ? pg.data_ptr<float>() : nullptr,
+                           (int)N, (int)T, (int)U, (int)V, blank, elem_bytes(xs)));
+    return std::make_tuple(costs, lse, pg);
 }
 
-// Viterbi alignment on the TDT lattice, compact (STU,V+D) f32 or bf16 logits in joint_pack's row order, labels
-// (sum yn): (scores (N) f32, frames (sum yn) i32, label durations (sum yn) i32).  The bounds are the hints when given
-// (no host sync), else one 16-byte device->host copy, as in rnnt_tdt_compact_forward.
-std::tuple<at::Tensor, at::Tensor, at::Tensor>
-rnnt_tdt_align_compact(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
-                       const std::vector<int> &durations, double sigma, int blank, int max_T, int max_U) {
+// d loss / d logits (N,T,U,V+D) or (N,T,U,V), of the dtype of xs
+template <const Lattice &F>
+at::Tensor lattice_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &grads, const at::Tensor &ys,
+                            const std::vector<int> &durations, const at::Tensor &grad_out, int blank) {
+    check_arg(xs, Dt::F32orBF16, xs, {kAny, kAny, kAny, kAny}, F.xs4);
+    const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), D = (int64_t)durations.size();
+    const int64_t V = lattice_tokens(F, xs.size(3), D, blank, F.row_cell);
+    check_arg(lse, Dt::F32, xs, lse_sizes(F, {N, T, U}), F.lse4);
+    check_arg(grads, Dt::F32, xs, {N, T, U, 2 + D}, F.grads4);
+    check_arg(ys, Dt::I32, xs, {N, U - 1}, "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
+    check_arg(grad_out, Dt::F32, xs, N, "grad_out must be a contiguous Float tensor of shape (N,)");
+    const c10::cuda::CUDAGuard guard(xs.device());
+    at::Tensor out = at::empty_like(xs);
+    if (N == 0) return out;
+    check_status(F.backward(current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(), grads.data_ptr<float>(),
+                            ys.data_ptr<int>(), durations.data(), (int)D, grad_out.data_ptr<float>(), out.data_ptr(),
+                            (int)N, (int)T, (int)U, (int)V, blank, elem_bytes(xs)));
+    return out;
+}
+
+// Loss from compact (STU,V+D) TDT or (STU,V) multi-blank logits in joint_pack's row order, float32 or bfloat16, labels
+// (sum yn): (costs (N), lse (STU,2) or (STU), grads (STU,2+D) or empty, prefix (2N) int64 = {mem_pref, lab_pref} for
+// the backward).  Shapes are validated as in rnnt_loss_compact: one 16-byte device->host copy, or none with hints
+// (max_T, max_U > 0).
+template <const Lattice &F>
+std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor>
+lattice_compact_forward(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
+                        const std::vector<int> &durations, double sigma, int blank, bool want_grads, int max_T,
+                        int max_U) {
     const auto [N, STU, W, bf16, guard] = compact_front(xs, ys, xn, yn, blank, true);
-    const int64_t D = (int64_t)durations.size();
-    TORCH_CHECK(D >= 1 && W > D, "xs must have more than len(durations) logits per row (V + D)");
-    check_blank(blank, W - D);
+    const int64_t D = (int64_t)durations.size(), V = lattice_tokens(F, W, D, blank, F.row_row);
     void *stream = current_stream(xs);
-    at::Tensor scores = at::empty({N}, xs.options().dtype(at::kFloat));
-    at::Tensor frames = label_slots(ys.numel(), xs);
-    at::Tensor fdur = label_slots(ys.numel(), xs);
-    if (N == 0) return std::make_tuple(scores, frames, fdur);
-    std::tie(max_T, max_U) = compact_bounds(stream, xs, ys, xn, yn, max_T, max_U, nullptr);
+    const auto f32 = xs.options().dtype(at::kFloat);
+    at::Tensor costs = at::empty({N}, f32);
+    at::Tensor lse = at::empty(lse_sizes(F, {STU}), f32);
+    at::Tensor pg = output(want_grads, {STU, 2 + D}, f32);
+    at::Tensor prefix = at::empty({2 * N}, xs.options().dtype(at::kLong));
+    if (N == 0) return std::make_tuple(costs, lse, pg, prefix);
+    std::tie(max_T, max_U) = compact_bounds(stream, xs, ys, xn, yn, max_T, max_U, prefix.data_ptr<int64_t>());
     // a batch whose lengths are all 0: bounds of 1 (its lattices are invalid either way)
     max_T = std::max(max_T, 1);
     max_U = std::max(max_U, 1);
-    at::Tensor ws = workspace(xs, rnnt_b200_tdt_align_workspace_bytes(STU, (int)N, (int)D));
-    check_status(rnnt_b200_tdt_align_compact(stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
-                                             ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
-                                             durations.data(), (int)D, (float)sigma, scores.data_ptr<float>(),
-                                             frames.data_ptr<int>(), fdur.data_ptr<int>(), STU, (int)N, (int)(W - D),
-                                             blank, bf16 ? 2 : 4, max_T, max_U));
-    return std::make_tuple(scores, frames, fdur);
+    at::Tensor ws = workspace(xs, F.compact_workspace_bytes(STU, (int)N, (int)D));
+    check_status(F.compact_forward(stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(), ys.data_ptr<int>(),
+                                   xn.data_ptr<int>(), yn.data_ptr<int>(), durations.data(), (int)D, (float)sigma,
+                                   costs.data_ptr<float>(), lse.data_ptr<float>(),
+                                   want_grads ? pg.data_ptr<float>() : nullptr, prefix.data_ptr<int64_t>(), nullptr,
+                                   STU, (int)N, (int)V, blank, bf16 ? 2 : 4, max_T, max_U));
+    return std::make_tuple(costs, lse, pg, prefix);
 }
 
-// Viterbi alignment on the multi-blank lattice, dense (N,T,U,V) f32 or bf16 logits, B = durations.size(): (scores (N)
-// f32, frames (N,U-1) i32, blank counts (N,1+B) i32).  No host sync.
-std::tuple<at::Tensor, at::Tensor, at::Tensor> rnnt_multiblank_align_dense(const at::Tensor &xs, const at::Tensor &ys,
-                                                                           const at::Tensor &xn, const at::Tensor &yn,
-                                                                           const std::vector<int> &durations,
-                                                                           double sigma, int blank) {
+// d loss / d compact logits (STU,V+D) or (STU,V), of the dtype of xs
+template <const Lattice &F>
+at::Tensor lattice_compact_backward(const at::Tensor &xs, const at::Tensor &lse, const at::Tensor &grads,
+                                    const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
+                                    const at::Tensor &prefix, const std::vector<int> &durations,
+                                    const at::Tensor &grad_out, int blank) {
+    check_arg(xs, Dt::F32orBF16, xs, {kAny, kAny}, F.xs2);
+    const int64_t STU = xs.size(0), N = xn.numel(), D = (int64_t)durations.size();
+    const int64_t V = lattice_tokens(F, xs.size(1), D, blank, F.row_row);
+    if (F.multiblank)                                   // STU floats of any shape
+        check_arg(lse, Dt::F32, xs, STU, F.lse2);
+    else
+        check_arg(lse, Dt::F32, xs, {STU, 2}, F.lse2);
+    check_arg(grads, Dt::F32, xs, {STU, 2 + D}, F.grads2);
+    TORCH_CHECK(is_arg(ys, Dt::I32, xs), "ys must be a contiguous Int tensor on the device of xs");
+    const char *lengths = "xn and yn must be contiguous Int tensors of shape (N,) on the device of xs";
+    check_arg(xn, Dt::I32, xs, N, lengths);
+    check_arg(yn, Dt::I32, xs, N, lengths);
+    check_arg(prefix, Dt::I64, xs, 2 * N, "prefix must be a contiguous Long tensor of shape (2N,) on the device of xs");
+    check_arg(grad_out, Dt::F32, xs, N, "grad_out must be a contiguous Float tensor of shape (N,)");
+    const c10::cuda::CUDAGuard guard(xs.device());
+    at::Tensor out = at::empty_like(xs);
+    if (N == 0 || STU == 0) return out;                 // empty tensors: nothing to write (and no data pointers)
+    check_status(F.compact_backward(current_stream(xs), xs.data_ptr(), lse.data_ptr<float>(), grads.data_ptr<float>(),
+                                    ys.data_ptr<int>(), yn.data_ptr<int>(), durations.data(), (int)D,
+                                    prefix.data_ptr<int64_t>(), grad_out.data_ptr<float>(), out.data_ptr(), STU,
+                                    (int)N, (int)V, blank, elem_bytes(xs)));
+    return out;
+}
+
+// Viterbi alignment, dense (N,T,U,V+D) TDT or (N,T,U,V) multi-blank f32 or bf16 logits: (scores (N) f32, frames (N,U-1)
+// i32, and TDT's label durations (N,U-1) i32 or multi-blank's blank counts (N,1+D) i32).  No host sync.
+template <const Lattice &F>
+std::tuple<at::Tensor, at::Tensor, at::Tensor> lattice_align_dense(const at::Tensor &xs, const at::Tensor &ys,
+                                                                   const at::Tensor &xn, const at::Tensor &yn,
+                                                                   const std::vector<int> &durations, double sigma,
+                                                                   int blank) {
     check4(xs, ys, xn, yn, true);
     check_batch4(xs, xn, yn);
-    const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), V = xs.size(3), B = (int64_t)durations.size();
+    const int64_t N = xs.size(0), T = xs.size(1), U = xs.size(2), D = (int64_t)durations.size();
     check_arg(ys, Dt::I32, xs, {N, U - 1}, "ys must be a contiguous Int tensor of shape (N, U-1) on the device of xs");
-    check_multiblank(B, blank, V);
+    const int64_t V = lattice_tokens(F, xs.size(3), D, blank, F.row_cell);
     const c10::cuda::CUDAGuard guard(xs.device());
     at::Tensor scores = at::empty({N}, xs.options().dtype(at::kFloat));
     at::Tensor frames = label_slots(N * (U - 1), xs).view({N, U - 1});
-    at::Tensor counts = at::empty({N, 1 + B}, xs.options().dtype(at::kInt));
-    if (N == 0) return std::make_tuple(scores, frames, counts);
-    at::Tensor ws = workspace(xs, rnnt_b200_multiblank_align_workspace_bytes(N * T * U, (int)N, (int)B));
-    check_status(rnnt_b200_multiblank_align_dense(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
-                                                  ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
-                                                  durations.data(), (int)B, (float)sigma, scores.data_ptr<float>(),
-                                                  frames.data_ptr<int>(), counts.data_ptr<int>(), (int)N, (int)T,
-                                                  (int)U, (int)V, blank,
-                                                  xs.scalar_type() == at::ScalarType::BFloat16 ? 2 : 4));
-    return std::make_tuple(scores, frames, counts);
+    at::Tensor third = align_third(F, frames, N, D);
+    if (N == 0) return std::make_tuple(scores, frames, third);
+    at::Tensor ws = workspace(xs, F.align_workspace_bytes(N * T * U, (int)N, (int)D));
+    check_status(F.align_dense(current_stream(xs), ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(), ys.data_ptr<int>(),
+                               xn.data_ptr<int>(), yn.data_ptr<int>(), durations.data(), (int)D, (float)sigma,
+                               scores.data_ptr<float>(), frames.data_ptr<int>(), third.data_ptr<int>(), (int)N, (int)T,
+                               (int)U, (int)V, blank, elem_bytes(xs)));
+    return std::make_tuple(scores, frames, third);
 }
 
-// Viterbi alignment on the multi-blank lattice, compact (STU,V) f32 or bf16 logits in joint_pack's row order, labels
-// (sum yn): (scores (N) f32, frames (sum yn) i32, blank counts (N,1+B) i32).  The bounds are the hints when given (no
-// host sync), else one 16-byte device->host copy, as in rnnt_multiblank_compact_forward.
+// Viterbi alignment, compact (STU,V+D) TDT or (STU,V) multi-blank f32 or bf16 logits in joint_pack's row order, labels
+// (sum yn): (scores (N) f32, frames (sum yn) i32, and TDT's label durations (sum yn) i32 or multi-blank's blank counts
+// (N,1+D) i32).  The bounds are the hints when given (no host sync), else one 16-byte device->host copy.
+template <const Lattice &F>
 std::tuple<at::Tensor, at::Tensor, at::Tensor>
-rnnt_multiblank_align_compact(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
-                              const std::vector<int> &durations, double sigma, int blank, int max_T, int max_U) {
-    const auto [N, STU, V, bf16, guard] = compact_front(xs, ys, xn, yn, blank, true);
-    const int64_t B = (int64_t)durations.size();
-    check_multiblank(B, blank, V);
+lattice_align_compact(const at::Tensor &xs, const at::Tensor &ys, const at::Tensor &xn, const at::Tensor &yn,
+                      const std::vector<int> &durations, double sigma, int blank, int max_T, int max_U) {
+    const auto [N, STU, W, bf16, guard] = compact_front(xs, ys, xn, yn, blank, true);
+    const int64_t D = (int64_t)durations.size(), V = lattice_tokens(F, W, D, blank, F.row_row);
     void *stream = current_stream(xs);
     at::Tensor scores = at::empty({N}, xs.options().dtype(at::kFloat));
     at::Tensor frames = label_slots(ys.numel(), xs);
-    at::Tensor counts = at::empty({N, 1 + B}, xs.options().dtype(at::kInt));
-    if (N == 0) return std::make_tuple(scores, frames, counts);
+    at::Tensor third = align_third(F, frames, N, D);
+    if (N == 0) return std::make_tuple(scores, frames, third);
     std::tie(max_T, max_U) = compact_bounds(stream, xs, ys, xn, yn, max_T, max_U, nullptr);
     // a batch whose lengths are all 0: bounds of 1 (its lattices are invalid either way)
     max_T = std::max(max_T, 1);
     max_U = std::max(max_U, 1);
-    at::Tensor ws = workspace(xs, rnnt_b200_multiblank_align_workspace_bytes(STU, (int)N, (int)B));
-    check_status(rnnt_b200_multiblank_align_compact(stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(),
-                                                    ys.data_ptr<int>(), xn.data_ptr<int>(), yn.data_ptr<int>(),
-                                                    durations.data(), (int)B, (float)sigma, scores.data_ptr<float>(),
-                                                    frames.data_ptr<int>(), counts.data_ptr<int>(), STU, (int)N,
-                                                    (int)V, blank, bf16 ? 2 : 4, max_T, max_U));
-    return std::make_tuple(scores, frames, counts);
+    at::Tensor ws = workspace(xs, F.align_workspace_bytes(STU, (int)N, (int)D));
+    check_status(F.align_compact(stream, ws.data_ptr(), (size_t)ws.numel(), xs.data_ptr(), ys.data_ptr<int>(),
+                                 xn.data_ptr<int>(), yn.data_ptr<int>(), durations.data(), (int)D, (float)sigma,
+                                 scores.data_ptr<float>(), frames.data_ptr<int>(), third.data_ptr<int>(), STU, (int)N,
+                                 (int)V, blank, bf16 ? 2 : 4, max_T, max_U));
+    return std::make_tuple(scores, frames, third);
 }
 
 // am (N,T,V) and lm (N,U,V): dtypes, then contiguity and device, then shapes; then ys, xn and yn
@@ -1215,37 +1105,37 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("rnnt_logits_pruned_backward", &rnnt_logits_pruned_backward, py::arg("xs"), py::arg("lse"),
           py::arg("pair_grads"), py::arg("ys"), py::arg("ranges"), py::arg("grad_out"), py::arg("blank") = 0,
           py::arg("hat") = false);
-    m.def("rnnt_tdt_forward", &rnnt_tdt_forward, py::arg("xs"), py::arg("ys"), py::arg("xn"), py::arg("yn"),
+    m.def("rnnt_tdt_forward", &lattice_forward<kTdt>, py::arg("xs"), py::arg("ys"), py::arg("xn"), py::arg("yn"),
           py::arg("durations"), py::arg("sigma") = 0.0, py::arg("blank") = 0, py::arg("want_grads") = true);
-    m.def("rnnt_tdt_backward", &rnnt_tdt_backward, py::arg("xs"), py::arg("lse"), py::arg("grads"), py::arg("ys"),
+    m.def("rnnt_tdt_backward", &lattice_backward<kTdt>, py::arg("xs"), py::arg("lse"), py::arg("grads"), py::arg("ys"),
           py::arg("durations"), py::arg("grad_out"), py::arg("blank") = 0);
-    m.def("rnnt_tdt_compact_forward", &rnnt_tdt_compact_forward, py::arg("xs"), py::arg("ys"), py::arg("xn"),
+    m.def("rnnt_tdt_compact_forward", &lattice_compact_forward<kTdt>, py::arg("xs"), py::arg("ys"), py::arg("xn"),
           py::arg("yn"), py::arg("durations"), py::arg("sigma"), py::arg("blank"), py::arg("want_grads"),
           py::arg("max_T") = 0, py::arg("max_U") = 0);
-    m.def("rnnt_tdt_compact_backward", &rnnt_tdt_compact_backward, py::arg("xs"), py::arg("lse"), py::arg("grads"),
+    m.def("rnnt_tdt_compact_backward", &lattice_compact_backward<kTdt>, py::arg("xs"), py::arg("lse"), py::arg("grads"),
           py::arg("ys"), py::arg("xn"), py::arg("yn"), py::arg("prefix"), py::arg("durations"), py::arg("grad_out"),
           py::arg("blank"));
-    m.def("rnnt_multiblank_forward", &rnnt_multiblank_forward, py::arg("xs"), py::arg("ys"), py::arg("xn"),
+    m.def("rnnt_multiblank_forward", &lattice_forward<kMultiblank>, py::arg("xs"), py::arg("ys"), py::arg("xn"),
           py::arg("yn"), py::arg("big_blank_durations"), py::arg("sigma"), py::arg("blank"), py::arg("want_grads") = true);
-    m.def("rnnt_multiblank_backward", &rnnt_multiblank_backward, py::arg("xs"), py::arg("lse"), py::arg("grads"),
+    m.def("rnnt_multiblank_backward", &lattice_backward<kMultiblank>, py::arg("xs"), py::arg("lse"), py::arg("grads"),
           py::arg("ys"), py::arg("big_blank_durations"), py::arg("grad_out"), py::arg("blank"));
-    m.def("rnnt_multiblank_compact_forward", &rnnt_multiblank_compact_forward, py::arg("xs"), py::arg("ys"),
+    m.def("rnnt_multiblank_compact_forward", &lattice_compact_forward<kMultiblank>, py::arg("xs"), py::arg("ys"),
           py::arg("xn"), py::arg("yn"), py::arg("big_blank_durations"), py::arg("sigma"), py::arg("blank"),
           py::arg("want_grads"), py::arg("max_T") = 0, py::arg("max_U") = 0);
-    m.def("rnnt_multiblank_compact_backward", &rnnt_multiblank_compact_backward, py::arg("xs"), py::arg("lse"),
+    m.def("rnnt_multiblank_compact_backward", &lattice_compact_backward<kMultiblank>, py::arg("xs"), py::arg("lse"),
           py::arg("grads"), py::arg("ys"), py::arg("xn"), py::arg("yn"), py::arg("prefix"),
           py::arg("big_blank_durations"), py::arg("grad_out"), py::arg("blank"));
-    m.def("rnnt_tdt_align_dense", &rnnt_tdt_align_dense, "Viterbi forced alignment on the TDT lattice, dense layout.",
-          py::arg("xs"), py::arg("ys"), py::arg("xn"), py::arg("yn"), py::arg("durations"), py::arg("sigma") = 0.0,
-          py::arg("blank") = 0);
-    m.def("rnnt_tdt_align_compact", &rnnt_tdt_align_compact,
+    m.def("rnnt_tdt_align_dense", &lattice_align_dense<kTdt>,
+          "Viterbi forced alignment on the TDT lattice, dense layout.", py::arg("xs"), py::arg("ys"), py::arg("xn"),
+          py::arg("yn"), py::arg("durations"), py::arg("sigma") = 0.0, py::arg("blank") = 0);
+    m.def("rnnt_tdt_align_compact", &lattice_align_compact<kTdt>,
           "Viterbi forced alignment on the TDT lattice, compact layout.", py::arg("xs"), py::arg("ys"), py::arg("xn"),
           py::arg("yn"), py::arg("durations"), py::arg("sigma") = 0.0, py::arg("blank") = 0, py::arg("max_T") = 0,
           py::arg("max_U") = 0);
-    m.def("rnnt_multiblank_align_dense", &rnnt_multiblank_align_dense,
+    m.def("rnnt_multiblank_align_dense", &lattice_align_dense<kMultiblank>,
           "Viterbi forced alignment on the multi-blank lattice, dense layout.", py::arg("xs"), py::arg("ys"),
           py::arg("xn"), py::arg("yn"), py::arg("big_blank_durations"), py::arg("sigma"), py::arg("blank"));
-    m.def("rnnt_multiblank_align_compact", &rnnt_multiblank_align_compact,
+    m.def("rnnt_multiblank_align_compact", &lattice_align_compact<kMultiblank>,
           "Viterbi forced alignment on the multi-blank lattice, compact layout.", py::arg("xs"), py::arg("ys"),
           py::arg("xn"), py::arg("yn"), py::arg("big_blank_durations"), py::arg("sigma"), py::arg("blank"),
           py::arg("max_T") = 0, py::arg("max_U") = 0);
